@@ -2,6 +2,7 @@
 """bench.py -- rays/sec of the SDF volume-rendering hot path (BASELINE.json metric), one workload per invocation.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--precision bf16x3|bf16|fp32]
+                  [--dump-outputs DIR]
 
 Workloads (BASELINE.json configs; the default is the headline the metric is quoted on):
   neus-facto-dtu65-4096x128   configs[1]: DTU-scan65-shaped rays, 4096 rays x 128 samples per GPU, neus-facto SDFField (hash L=16 F=2
@@ -21,6 +22,9 @@ value   : whole-job rays/s, inputs resident in HBM, CUDA-event time (max over ra
 e2e     : same metric through the public module API with HOST (pinned) ray buffers: H2D of the rays and D2H of the rendered
           rgb / depth / normal / accumulation inside the timed region (the headline workload replays one CUDA graph per step).
 roofline: the dominant kernel against the measured peak of MEASURED_PEAKS.json (burst peak: the kernel is event-timed alone).
+--dump-outputs DIR: after the timed steps, what the timed path returned in its last step (rank 0) is written as DIR/<name>.npy in
+          float32: the rendered rgb / depth / normal / accumulation, or for the training workload the loss and a fixed, seeded sample
+          of the updated parameters.  Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 cpu_baseline / --impl reference: the CPU oracle port (oracle/, a restatement of the reference's torch-CPU path, pinned to the
           unmodified reference by tests/golden) on a bounded sample of the same workload, all host threads.
 """
@@ -90,23 +94,8 @@ def oracle_of(field, spec=None):
     return OracleField(spec, sd)
 
 
-def read_traffic(workload, precision):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel from the committed `ncu --set full` capture."""
-    for name in (f"r02_ncu_{workload}_{precision}_summary.json", f"r02_ncu_field_tc_{precision}_summary.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if not os.path.exists(p):
-            continue
-        try:
-            with open(p) as fh:
-                d = json.load(fh)
-
-            def mb(k):
-                v, u = float(d[k]["value"]), d[k]["unit"]
-                return v * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}[u]
-            return mb("dram__bytes_read.sum") + mb("dram__bytes_write.sum")
-        except Exception:  # noqa: BLE001
-            return None
-    return None
+# NVIDIA's H100 SXM data sheet (700 W card): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s -- used when no measured peaks are present
+H100_DATASHEET = {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}
 
 
 def read_peaks():
@@ -114,13 +103,21 @@ def read_peaks():
     if os.path.exists(p):
         with open(p) as fh:
             d = json.load(fh)
-        return {"bf16_tflops": d.get("bf16_tflops", 1590.0), "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 1400.0),
-                "hbm_gbs": d.get("hbm_gbs", 6650.0), "source": "measured"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+        return {"bf16_tflops": d.get("bf16_tflops", H100_DATASHEET["bf16_tflops"]), "hbm_gbs": d.get("hbm_gbs", H100_DATASHEET["hbm_gbs"]), "source": "measured"}
+    return {**H100_DATASHEET, "source": "H100 SXM data sheet"}
+
+
+def dump_outputs(outdir, arrays):
+    """--dump-outputs: each tensor as <outdir>/<name>.npy, float32."""
+    import numpy as np
+
+    os.makedirs(outdir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(outdir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -302,6 +299,7 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="A/B: e2e without CUDA-graph replay")
     ap.add_argument("--no-train-section", action="store_true", help="skip the training-step section (angelo-train-8192 with the NCCL gradient all-reduce) of the headline line")
     ap.add_argument("--table-dtype", default="fp32", choices=["fp32", "fp16"], help="fp16 = gather from a half-precision copy (tiny-cuda-nn's storage)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write what the timed path returned in its last step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -328,7 +326,7 @@ def main():
 
     precision = args.precision
     if precision == "auto":
-        precision = "bf16x3"   # tcgen05 path at parity-grade precision (bf16 split, fp32 accumulate); fp32 / bf16 via --precision
+        precision = "bf16x3"   # tensor-core path at parity-grade precision (bf16 split, fp32 accumulate); fp32 / bf16 via --precision
     wl = args.workload
     white = torch.ones(3, device=dev)
     H = sb.FieldHeadNames
@@ -433,7 +431,7 @@ def main():
         flop_per_launch = FLOP_PER_SAMPLE_BAKED * R * 48
         cfg = {"workload": wl, "rays_per_gpu": R, "samples_per_ray": 48, "sampler": "ProposalNetworkSampler(256, 96 -> 48), 2 HashMLPDensityFields, eval",
                "field": "bakedsdf SDFField: L-inf contraction, off-axis PE deg 8 (371-wide input), diffuse / tint / reflections / n.v, L16 F2 T2^19", "precision": precision,
-               "step": "proposal sampler -> SDFField.render (generic engine: per-layer tcgen05 Linear kernels + compositing kernels)"}
+               "step": "proposal sampler -> SDFField.render (generic engine: per-layer tensor-core Linear kernels + compositing kernels)"}
         kernel = "sdfb200_field_render (k_tc_linear x layers + elementwise + k_render_alphas)"
         cpu_sample = 64
 
@@ -443,7 +441,7 @@ def main():
     cam_d = cam.view(-1, 1).to(dev)
     pix = torch.ones(R, 1, device=dev)
     dev_in = [t.to(dev) for t in host]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > the 50 MB L2
 
     def barrier():
         if world > 1:
@@ -472,6 +470,8 @@ def main():
             pairs.append((e0, e1))
         barrier()
         launches = sb._lib.launch_count() - launches0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {k: v for k, v in last.items() if torch.is_tensor(v)})
         dev_ms = sum(a.elapsed_time(b) for a, b in pairs)
         fld_ms = sum(a.elapsed_time(b) for a, b in field_ms)
         if wl == "volsdf-errorbounded-4096":
@@ -532,7 +532,7 @@ def main():
     train = None
     if wl == WORKLOAD and not args.no_train_section:
         torch.cuda.empty_cache()
-        train = train_section(world, rank)
+        train = train_section(world, rank, steps=args.steps, warmup=args.warmup)
         barrier()
     times = torch.tensor([dev_ms, e2e_ms, fld_ms], device=dev, dtype=torch.float64)
     if world > 1:
@@ -559,7 +559,7 @@ def main():
             "e2e": {"value": e2e, "unit": "rays/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "gpu_launches": int(launches),
             "roofline": {"bound": "tensor", "achieved": achieved_tflops, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-                         "frac": achieved_tflops / peaks["bf16_tflops"], "traffic": read_traffic(wl, precision), "peak_source": peaks["source"] + " bf16_tflops (burst)",
+                         "frac": achieved_tflops / peaks["bf16_tflops"], "traffic": None, "peak_source": peaks["source"] + " bf16_tflops (burst)",
                          "kernel": kernel, "ms_per_launch": fld_ms / args.steps, "algorithmic_flop_per_launch": flop_per_launch},
             "cpu_baseline": cpu, "clocks": clk,
         }  # fmt: skip

@@ -1,5 +1,5 @@
 /*
- * sdfb200.h -- C ABI of the B200-native SDF volume-rendering hot path (sdfstudio drop-in).
+ * sdfb200.h -- C ABI of the H100-native SDF volume-rendering hot path (sdfstudio drop-in).
  *
  * The reference (autonomousvision/sdfstudio) has NO native/FFI boundary on this path: its plug points are Python
  * nn.Modules (SURVEY.md section 8b).  This header is the C-ABI *underneath* those modules; every entry point names the
@@ -44,8 +44,8 @@ enum { SDFB200_SPACING_UNIFORM = 0, SDFB200_SPACING_LINDISP = 1, SDFB200_SPACING
        SDFB200_SPACING_PIECEWISE = 4, SDFB200_SPACING_IDENTITY = 5 /* bins already euclidean */ };
 enum { SDFB200_BG_COLOR = 0, SDFB200_BG_LAST_SAMPLE = 1, SDFB200_BG_PER_RAY = 2 };
 enum { SDFB200_PRECISION_FP32 = 0,      /* CUDA-core fp32 FMA (exact-fp32 reference numerics)            */
-       SDFB200_PRECISION_BF16X3 = 1,    /* tcgen05 bf16 split a0*w0 + a1*w0 + a0*w1, fp32 accumulate      */
-       SDFB200_PRECISION_BF16 = 2 };    /* tcgen05 single bf16 pass (fast mode; reported with PSNR-vs-ref) */
+       SDFB200_PRECISION_BF16X3 = 1,    /* wgmma bf16 split a0*w0 + a1*w0 + a0*w1, fp32 accumulate        */
+       SDFB200_PRECISION_BF16 = 2 };    /* wgmma single bf16 pass (fast mode; reported with PSNR-vs-ref)   */
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Multi-resolution grid.  Replaces tinycudann.Encoding(HashGrid) as configured at
@@ -354,7 +354,7 @@ int sdfb200_weights_backward(const float* alphas_or_density, const float* euclid
 
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Training path: dense-layer GEMMs on tcgen05 (bf16x3 = parity grade, bf16 = fast), fp32 row-major in / out.  They replace the ATen /
+ * Training path: dense-layer GEMMs on wgmma (bf16x3 = parity grade, bf16 = fast), fp32 row-major in / out.  They replace the ATen /
  * cuBLAS matmuls autograd runs for every nn.Linear of SDFField when the reference trains (sdf_field.py:400-409 through
  * engine/trainer.py:319-323): forward Y = X W^T (+ bias, activation), input gradient dX = dY W, weight gradient dW = dY^T X.  The set is
  * closed under differentiation (each one's backward is the other two), which is what the eikonal term's double backward needs

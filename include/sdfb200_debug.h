@@ -1,5 +1,5 @@
 /*
- * sdfb200_debug.h -- validation hooks of the tcgen05 building blocks.  NOT part of the product library: these entry points are
+ * sdfb200_debug.h -- validation hooks of the tensor-core (wgmma) building blocks.  NOT part of the product library: these entry points are
  * compiled into libsdfb200_dbg.so only (sdfstudio_b200/build.py build_debug), which the -m gpu building-block tests load.
  */
 #ifndef SDFB200_DEBUG_H_
@@ -10,14 +10,15 @@ extern "C" {
 #endif
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Debug / validation hook (no reference counterpart): one CTA computes D[128,Np] = A[128,K] W[N,K]^T with the tcgen05
- * machinery of the fused field kernel (bf16 split planes, SS- or TS-mode A operand, bulk-copy weight ring).
- * K % 32 == 0, K <= 256, N <= 256, Np = N rounded up to 16.  scratch: >= (K/32)*planes*Np*64 bytes.
+ * Debug / validation hook (no reference counterpart): one CTA computes D[128,Np] = A[128,K] W[N,K]^T with the wgmma
+ * machinery of the tensor-core kernels (bf16 split planes, A operand in shared memory (mode_ts = 0) or in registers
+ * (mode_ts = 1), bulk-copy weight ring).  K % 32 == 0, K <= 256, N <= 256, Np = N rounded up to 16.
+ * scratch: >= (K/32)*planes*Np64*64 bytes, Np64 = N rounded up to 64.
  * ------------------------------------------------------------------------------------------------------------- */
 int sdfb200_debug_tc_gemm(const float* A, const float* W, int32_t K, int32_t N, int32_t mode_ts, int32_t planes, float* D,
                           void* scratch, void* stream);
 
-/* Building-block test of the generic tcgen05 Linear (csrc/tc_linear.cu): Y[M, Np] = epi(X[M, Kp] W[Np, Kp]^T + bias) with
+/* Building-block test of the generic tensor-core Linear (csrc/tc_linear.cu): Y[M, Np] = epi(X[M, Kp] W[Np, Kp]^T + bias) with
  * epi 0 none / 1 softplus(beta 100) / 2 relu / 3 multiply by softplus'(aux) (no bias); planes 1 = bf16, 2 = bf16x3.
  * All dims padded to 16; scratch >= 256 KiB. */
 int sdfb200_debug_tc_linear(int32_t planes, int32_t epi, const float* X, int32_t ldx, const float* W, const float* bias, float* Y,

@@ -1,4 +1,4 @@
-"""sdfstudio_b200 -- B200-native drop-in for sdfstudio's per-ray SDF volume-rendering hot path.
+"""sdfstudio_b200 -- H100-native drop-in for sdfstudio's per-ray SDF volume-rendering hot path.
 
 Host side mirrors the reference's plug points (SURVEY.md section 8b):
   encoding.Encoding            <- tinycudann.Encoding (HashGrid)        nerfstudio/fields/sdf_field.py:230-241
@@ -6,7 +6,7 @@ Host side mirrors the reference's plug points (SURVEY.md section 8b):
   ray_samplers.*               <- nerfstudio.model_components.ray_samplers
   renderers.*                  <- nerfstudio.model_components.renderers
   rays.*                       <- nerfstudio.cameras.rays (containers + alpha/density -> weights)
-All arithmetic runs in libsdfb200.so (CUDA, sm_100a) behind the C ABI of include/sdfb200.h.  No CPU / PyTorch fallback.
+All arithmetic runs in libsdfb200.so (CUDA, sm_90a) behind the C ABI of include/sdfb200.h.  No CPU / PyTorch fallback.
 """
 from . import _lib  # noqa: F401
 from . import cameras, meshing  # noqa: F401

@@ -121,7 +121,7 @@ _PROTOS = {
     "sdfb200_field_render": (C.c_int, [C.POINTER(FieldDesc), _vp, _vp, C.POINTER(FieldIn), C.POINTER(FieldOut), C.POINTER(FieldRender), _vp, _sz, _vp]),
 }
 EXPORTED_SYMBOLS = tuple(_PROTOS)
-# validation hooks of the tcgen05 building blocks: libsdfb200_dbg.so only (include/sdfb200_debug.h), never loaded by the product
+# validation hooks of the tensor-core building blocks: libsdfb200_dbg.so only (include/sdfb200_debug.h), never loaded by the product
 _DEBUG_PROTOS = {
     "sdfb200_debug_tc_linear": (C.c_int, [_i32, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _i32, _i32, _vp, _vp]),
     "sdfb200_debug_tc_gemm": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),

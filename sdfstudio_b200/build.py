@@ -1,4 +1,4 @@
-"""Builds libsdfb200.so (sm_100a) in-tree with nvcc.  `python -m sdfstudio_b200.build [--force]`."""
+"""Builds libsdfb200.so (sm_90a) in-tree with nvcc.  `python -m sdfstudio_b200.build [--force]`."""
 import os
 import subprocess
 import sys
@@ -10,7 +10,7 @@ LIB_DEBUG = os.path.join(HERE, "libsdfb200_dbg.so")   # product objects + the bu
 SOURCES = ["api.cu", "grid_encode.cu", "field_simt.cu", "field_tc.cu", "field_tc_p2_torch.cu", "field_tc_p2_tcnn.cu", "field_tc_p1_torch.cu", "field_tc_p1_tcnn.cu", "tc_linear.cu", "tc_wgrad.cu", "samplers.cu", "render.cu", "render_backward.cu", "density_field.cu", "rays_gen.cu"]
 DEBUG_SOURCES = ["tc_test.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
          "-Xptxas", "-v"]
 
 

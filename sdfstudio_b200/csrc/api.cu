@@ -35,7 +35,7 @@ static int plan_or_fail(const sdfb200_field_t* f, FieldPlan& p) {
   const int rc = make_field_plan(*f, p);
   if (rc) return fail(SDFB200_EINVAL, "inconsistent field descriptor%s (plan error %lld)", "", (long long)rc);
   // tensor-core precisions: the fused kernel (field_tc.cu) for the neus-facto shape family, otherwise the generic kernels with the
-  // tcgen05 Linear (tc_linear.cu) as their GEMM engine -- no extra packed section for the latter
+  // tensor-core Linear (tc_linear.cu) as their GEMM engine -- no extra packed section for the latter
   if (f->precision != SDFB200_PRECISION_FP32 && field_tc_supported(*f, p)) {
     p.tc_bytes = field_tc_packed_bytes(*f, p);
     p.total_bytes = p.tc_off + p.tc_bytes;
@@ -208,7 +208,7 @@ extern "C" int sdfb200_field_render(const sdfb200_field_t* f, const void* packed
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Training path: the three GEMMs autograd needs for a Linear layer (forward / input gradient / weight gradient), closed under
-// differentiation (the backward of each is made of the other two), on the tcgen05 kernels of tc_linear.cu / tc_wgrad.cu.
+// differentiation (the backward of each is made of the other two), on the tensor-core kernels of tc_linear.cu / tc_wgrad.cu.
 // ---------------------------------------------------------------------------------------------------------------------
 static int gemm_planes(int32_t precision) { return precision == SDFB200_PRECISION_BF16 ? 1 : 2; }
 

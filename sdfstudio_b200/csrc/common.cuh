@@ -1,4 +1,4 @@
-// Shared helpers for the sdfb200 kernels (sm_100a only).
+// Shared helpers for the sdfb200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -50,7 +50,26 @@ inline int launched(const char* name) {
     }                                                                                               \
   } while (0)
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;   // H100 SXM: sizes the per-CTA workspaces of the persistent kernels
+
+// CTAs of a persistent launch: the SM count of the current device (114 on the H100 PCIe part), at most kNumSMs (the workspace bound).
+// Queried once per device: the samplers launch the field kernel many times per step and the attribute query is not free.
+inline int persistent_ctas() {
+  static std::atomic<int> cached[64];   // per device ordinal, 0 = not queried yet
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    cudaGetLastError();   // do not leave the failed query behind for the next launch check
+    return kNumSMs;
+  }
+  if (dev >= 0 && dev < 64 && (n = cached[dev].load(std::memory_order_relaxed)) > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+    cudaGetLastError();
+    return kNumSMs;
+  }
+  n = n < kNumSMs ? n : kNumSMs;
+  if (dev >= 0 && dev < 64) cached[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
 
 __host__ __device__ inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 __host__ __device__ inline int round_up(int a, int b) { return (a + b - 1) / b * b; }

@@ -10,7 +10,7 @@
 namespace sdfb200 {
 
 constexpr int kPad = 16;               // every K / N dimension is padded to a multiple of 16 (zero filled)
-constexpr int64_t kChunkPoints = 148 * 4 * 128;  // points per pass of the generic path (bounds the workspace): 4 full waves of 128-row tiles on 148 SMs
+constexpr int64_t kChunkPoints = 132 * 4 * 128;  // points per pass of the generic path (bounds the workspace): 4 full waves of 128-row tiles on 132 SMs
 
 inline int pad16(int v) { return (v + kPad - 1) / kPad * kPad; }
 

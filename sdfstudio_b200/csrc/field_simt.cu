@@ -1,5 +1,5 @@
 // Generic fp32 (CUDA-core) evaluation of the SDF field: any layer count / skip connection / head combination of
-// SDFFieldConfig.  This is the exact-fp32 path (SDFB200_PRECISION_FP32) and the reference for the tcgen05 path.
+// SDFFieldConfig.  This is the exact-fp32 path (SDFB200_PRECISION_FP32) and the reference for the tensor-core path.
 //
 // Stages (each a kernel; activations live in the caller's workspace, chunked so they stay L2-resident):
 //   k_field_inputs   positions (o + d*t), SceneContraction, NeRF PE           sdf_field.py:623-631, encodings.py:167-208
@@ -223,7 +223,7 @@ __global__ void __launch_bounds__(256) k_sgemm(const float* __restrict__ X, int 
   }
 }
 
-// GEMM engine of the current field call: 0 planes = the exact-fp32 CUDA-core kernel below; 1 / 2 = the generic tcgen05 Linear
+// GEMM engine of the current field call: 0 planes = the exact-fp32 CUDA-core kernel below; 1 / 2 = the generic tensor-core Linear
 // (bf16 / bf16x3, csrc/tc_linear.cu) with `scratch` for its packed weight chunk.  Set by field_forward_fp32 for the duration of a call.
 struct GemmEngine { int planes; void* scratch; };
 static thread_local GemmEngine g_gemm = {0, nullptr};

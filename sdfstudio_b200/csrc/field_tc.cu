@@ -6,8 +6,8 @@
 namespace sdfb200 {
 using namespace tc;
 
-// pack fp32 W (row n, column k at W[rowmap(n)*ldw + colmap(k)]) into bf16 split planes: K-blocked, N split in two halves (one per
-// CTA of a pair), canonical K-major no-swizzle layout inside a half:  [K-block][half][plane][k/8][row in half][8 bf16]
+// pack fp32 W (row n, column k at W[rowmap(n)*ldw + colmap(k)]) into bf16 split planes: K-blocked, canonical K-major no-swizzle
+// layout:  [K-block][plane][k/8][row][8 bf16]
 struct IdxMap { short src[kInK]; };   // packed index -> source index (-1 = zero); identity when unused
 __global__ void k_tc_pack(const float* __restrict__ W, int ldw, int N, int K, int Np, int nblocks, int kblk, int planes, int use_colmap, const IdxMap colmap,
                           int use_rowmap, const IdxMap rowmap, __nv_bfloat16* __restrict__ out) {
@@ -22,10 +22,9 @@ __global__ void k_tc_pack(const float* __restrict__ W, int ldw, int N, int K, in
   const float w = (ns >= 0 && ks >= 0) ? W[(size_t)ns * ldw + ks] : 0.f;
   const __nv_bfloat16 hi = __float2bfloat16_rn(w);
   const __nv_bfloat16 lo = __float2bfloat16_rn(w - __bfloat162float(hi));
-  const int nh = Np / 2, half = n / nh, nl = n - half * nh;
-  const size_t plane_elems = (size_t)nh * kblk;
-  const size_t base = ((size_t)b * 2 + half) * planes * plane_elems;
-  const size_t off = (size_t)(kk / 8) * (nh * 8) + (size_t)nl * 8 + (kk % 8);
+  const size_t plane_elems = (size_t)Np * kblk;
+  const size_t base = (size_t)b * planes * plane_elems;
+  const size_t off = (size_t)(kk / 8) * (Np * 8) + (size_t)n * 8 + (kk % 8);
   out[base + off] = hi;
   if (planes > 1) out[base + plane_elems + off] = lo;
 }
@@ -61,8 +60,8 @@ struct TcPlan {
 
 static void make_tc_plan(const sdfb200_field_t& f, const FieldPlan& p, TcPlan& t) {
   t.planes = f.precision == SDFB200_PRECISION_BF16X3 ? 2 : 1;
-  const int np[L_COUNT] = {256, 256, 256, kInK, 256, 256, 256};
-  const int kdim[L_COUNT] = {kInK, 256, 256, 256, 256, kInK, 256};
+  const int np[L_COUNT] = {256, 256, 256, 128, 256, 256, 256};           // B0: the 96 input rows padded to an n64 multiple
+  const int kdim[L_COUNT] = {kInK, 256, 256, 256, kInK, 256, 256};
   size_t off = p.tc_off;
   for (int l = 0; l < L_COUNT; ++l) {
     t.layer[l].w_off = off;
@@ -149,14 +148,6 @@ int field_tc_pack(const sdfb200_field_t& f, const FieldPlan& p, char* blob, cuda
   return 0;
 }
 
-// grid size: two CTAs per cluster, one cluster per TPC; never more clusters than can be co-resident (the tile loop is static)
-static int tc_max_pairs() {
-  static int cached = 0;
-  if (cached) return cached;
-  cached = kNumSMs / 2;
-  return cached;
-}
-
 int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* blob, const void* table, const sdfb200_field_in_t& in,
                      const sdfb200_field_out_t& out, const TcRender* rnd, float* ws, size_t ws_floats, cudaStream_t st) {
   const int64_t N = in.n_rays * (int64_t)in.n_samples;
@@ -183,7 +174,6 @@ int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* b
   a.in_dim = p.in_dim; a.pe_dim = p.pe_dim; a.grid_dim = p.grid_dim; a.app_dim = f.appearance_dim; a.use_n_dot_v = f.use_n_dot_v;
   a.mode = sdf_only ? 0 : 1;
   a.n_samples = in.n_samples; a.has_bins = in.bins != nullptr; a.n_points = N; a.n_tiles = (int)ceil_div(N, 128);
-  a.n_tile_pairs = (a.n_tiles + 1) / 2;
   a.rgb_padding = f.rgb_padding; a.cos_anneal = in.cos_anneal_ratio;
   a.origins = in.origins; a.directions = in.directions; a.bins = in.bins; a.appearance = in.appearance; a.variance = in.variance; a.beta = in.beta;
   a.beta_min = in.beta_min; a.table = table; a.blob = blob;
@@ -191,13 +181,13 @@ int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* b
   a.b_c0 = t.bc_off; a.b_c1 = p.col[1].b_off; a.w_c2 = p.col[2].w_off; a.b_c2 = p.col[2].b_off;
   a.scratch = reinterpret_cast<char*>(ws); a.scratch_per_cta = per_cta; a.out = out;
   if (render) a.rnd = *rnd; else { a.rnd = TcRender{}; a.rnd.enabled = 0; }
-  const int pairs = a.n_tile_pairs < tc_max_pairs() ? a.n_tile_pairs : tc_max_pairs();
-  const int grid = 2 * pairs;
-  const size_t smem = 2 * (size_t)t.planes * (kInK / 8) * 2048 + (size_t)kStages * t.planes * 128 * kKB * 2 + (6 * 128 + 9 * 256 + 32 + 12) * 4 + 1024;
+  // persistent CTAs, one per SM (the static tile loop needs no co-residency, but more CTAs than SMs would only add a tail wave)
+  const int ctas = persistent_ctas();
+  const int grid = a.n_tiles < ctas ? a.n_tiles : ctas;
+  const size_t smem = (size_t)t.planes * kAPlane + (size_t)kStages * t.planes * 256 * kKB * 2 + (9 * 256 + 7 * 128 + 32 + 12) * 4 + 1024;
   const bool torch_layout = f.grid.layout == SDFB200_GRID_TORCH;
   if (t.planes == 2) return torch_layout ? launch_field_tc_p2_torch(a, grid, smem, st) : launch_field_tc_p2_tcnn(a, grid, smem, st);
   return torch_layout ? launch_field_tc_p1_torch(a, grid, smem, st) : launch_field_tc_p1_tcnn(a, grid, smem, st);
-  return 0;
 }
 
 }  // namespace sdfb200

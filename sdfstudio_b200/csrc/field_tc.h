@@ -6,24 +6,12 @@
 namespace sdfb200 {
 
 
-constexpr int kEpiWarps = 8;
+constexpr int kEpiWarps = 8;                                 // two warpgroups: MMAs + epilogues, 64 tile rows each
 constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kGatherWarps = 4;                              // hash-grid part of the encode: one thread per point
-#ifndef TCV_ALU_WARPS
-#define TCV_ALU_WARPS 2
-#endif
-constexpr int kAluWarps = TCV_ALU_WARPS;                     // 0: the gather warps also write the PE / x / static colour columns; 2: two extra warps do (two points per thread)
-constexpr int kEncWarps = kGatherWarps + kAluWarps;
-constexpr int kWarpProducer = kEpiWarps + kEncWarps;         // 14
-constexpr int kWarpMma = kWarpProducer + 1;                  // 15
-constexpr int kTcThreads = (kWarpMma + 1) * 32;              // 512: register allocation rounds the warp count up to a multiple of 4 anyway
-#ifndef TCV_STAGES
-#define TCV_STAGES 4
-#endif
-constexpr int kStages = TCV_STAGES;      // weight ring depth (16 KB per stage and CTA at two planes).  4, not 7: the 48 KB go to L1 (carve-out 228 -> 196 KB), which
-                                         // the hash gathers of the coarse levels need more than the MMA issuer needs look-ahead (A/B: 7 -> 1.59 ms, 4 -> 1.47 ms)
-constexpr int kKB = 32;           // K per streamed weight block of the 256-row layers (one 16 KB stage per CTA at two planes)
-constexpr int kKBMax = 64;        // the 96-row layer streams K blocks of 64 (12 KB): deeper prefetch in bytes for the short layers
+constexpr int kTcThreads = kEpiThreads;
+constexpr int kStages = 2;        // weight ring depth (32 KB per stage at two planes, next to the 128 KB A operand)
+constexpr int kKB = 32;           // K per streamed weight block of the 256-row layers (one 32 KB stage at two planes)
+constexpr int kKBMax = 64;        // the 128-row layer (96 live rows) streams K blocks of 64: a full stage
 constexpr int kMaxGridDim = 32;
 constexpr int kMaxPe = 60;        // PE columns (2 * 3 * degree), degree <= 10
 constexpr int kPeRows = 64;       // rows reserved for the PE jacobian in the scratch
@@ -31,15 +19,17 @@ constexpr int kInK = 96;          // padded K of the two small-K operands (geo i
 constexpr float kHalfPiF = 1.5707963267948966f;
 // kernel order of the geo input columns (K = 96): [grid features 0..31 | PE | x(3) | zero padding] -- every group of four hash
 // levels is one aligned 16-byte operand chunk.  W0 (columns) and W0^T (rows) are permuted accordingly at pack time.
-// per-CTA scratch: softplus'(z1) unorm16 [64 KB] | h2 planes [P x 64 KB] | 2 x input jacobian (PE [64][128] f32 | grid [96][128] f32)
+constexpr uint32_t kAPlane = 32 * 2048;   // one bf16 plane of the A operand: [K/8 = 32][128 rows][16 B]
+// per-CTA scratch: softplus'(z1) unorm16 [64 KB] | h2 planes [P x 64 KB] | input jacobian (PE [64][128] f32 | grid [96][128] f32)
 constexpr size_t kJRBytes = (size_t)(kPeRows + kMaxGridDim * 3) * 128 * 4;
-__host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 + (size_t)planes * 65536 + 2 * kJRBytes; }
+__host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 + (size_t)planes * 65536 + kJRBytes; }
 
-enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0H, L_C0MISC, L_C1, L_COUNT };
+// layers in the order the kernel runs them (and the producer streams them)
+enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
 
 struct TcLayer {
   unsigned long long w_off;  // byte offset of the packed planes inside the blob
-  int Np;                    // rows of the weight tile (UMMA N); each CTA of a pair holds Np / 2 of them
+  int Np;                    // rows of the weight tile (MMA N, a multiple of 64)
   int nkb;                   // number of K blocks
   int kblk;                  // K per block (32 or 64)
 };
@@ -49,7 +39,7 @@ struct TcArgs {
   TcLayer layer[L_COUNT];
   int use_grid, pe_degree, use_pe, contraction, in_dim, pe_dim, grid_dim, app_dim, use_n_dot_v;
   int mode;  // 0: sdf only (G0, G1)   1: everything
-  int n_samples, has_bins, n_tiles, n_tile_pairs;
+  int n_samples, has_bins, n_tiles;
   long long n_points;
   float rgb_padding, cos_anneal;
   const float *origins, *directions, *bins, *appearance, *variance, *beta, *beta_min;
@@ -63,7 +53,7 @@ struct TcArgs {
   TcRender rnd;
 };
 
-// one launcher per instantiation; grid = 2 x CTA pairs
+// one launcher per instantiation
 int launch_field_tc_p2_torch(const TcArgs& a, int grid, size_t smem, cudaStream_t st);
 int launch_field_tc_p2_tcnn(const TcArgs& a, int grid, size_t smem, cudaStream_t st);
 int launch_field_tc_p1_torch(const TcArgs& a, int grid, size_t smem, cudaStream_t st);

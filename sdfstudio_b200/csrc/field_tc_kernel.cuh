@@ -1,30 +1,28 @@
-// Fused tcgen05 evaluation of the SDF field (SDFB200_PRECISION_BF16X3 / _BF16) for the neus-facto family of shapes:
+// Fused tensor-core evaluation of the SDF field (SDFB200_PRECISION_BF16X3 / _BF16) for the neus-facto family of shapes:
 // geo MLP in-256-256-(1+256), colour MLP cin-256-256-3, analytic d sdf/dx, 2-feature hash grid (fp32 or fp16 table),
 // optionally followed IN THE SAME KERNEL by the per-ray compositing (alpha / density -> transmittance -> weights -> rgb, depth,
 // normal, accumulation: cameras/rays.py:131-230, model_components/renderers.py:53-118,171-261,284-295).
 //
-// Persistent CTA PAIRS (cluster of 2, tcgen05 cta_group::2): every CTA walks its own 128-point tiles, one MMA covers the two
-// tiles of a pair (M = 256) and each CTA streams only HALF of every weight tile (rows [0,N/2) / [N/2,N) of the B operand).
+// Persistent CTAs, one 128-point tile at a time.  Two warpgroups own 64 rows of the tile each and run every layer as wgmma
+// m64n64k16 (accumulator in registers, A operand in shared memory, weights streamed by a producer warp through a shared-memory
+// ring filled by 1-D bulk copies from a pre-packed image).  A warpgroup only reads and writes its own rows of the A operand, so the
+// two warpgroups meet only at the weight ring and at the per-point heads / compositing.
 // Per tile (everything stays on chip except three L2-resident spills):
-//   encode   4 gather warps (one thread per point), decoupled from the compute warps and one tile ahead: position,
-//            contraction, hash gathers (+ jacobian), PE -> bf16 split planes in smem (double buffered)
-//   G0 G1    h = softplus_100(W a + b)       accumulator in TMEM (256 cols), converted IN PLACE into the next layer's A operand
-//            (bf16 planes, K step j at columns 16 j (hi) / 16 j + 8 (lo) of the accumulator it came from); the two 256-column halves
-//            of TMEM (X, Y) alternate as accumulator / A operand from layer to layer, and the next layer's MMAs TRAIL the epilogue:
-//            every 32 converted columns (one streamed K block) are handed to the MMA issuer (a_rdy[0..7]), so the tensor pipe runs under
-//            the epilogue
+//   encode   one thread per point for position, contraction, hash gathers (+ jacobian), one for PE
+//            -> bf16 split planes of the geo input (A operand columns 0..95)
+//   G0 G1    h = softplus_100(W a + b), epilogue in registers, written over the A operand as the next layer's input
 //   sdf      fp32 dot of h2 with row 0 of W2 on CUDA cores (exact fp32: the SDF drives NeuS alpha / Laplace density)
 //   (no G2)  the geo feature is linear in h2, so colour layer 0 is pre-multiplied at pack time: Wc = Wgf W2', and h2 itself
-//            (bf16 planes) takes the L2-resident round trip across the reverse sweep
+//            (bf16 planes) takes an L2-resident round trip across the reverse sweep
 //   B1 B0    reverse sweep: g2 = W2[0,:]*sp'(z2), g1 = (W1^T g2)*sp'(z1), gin = W0^T g1;  sp'(z1) spilled at G0
 //   grad     d sdf/dx = gin_x + PE jacobian + grid jacobian / 4      (what autograd computes at sdf_field.py:647-654)
-//   C0 C1    relu MLP on [x, dir-enc, grad, geo feature, appearance]; last 256->3 layer as fp32 dots; sigmoid + padding
+//   C0 C1    relu MLP on [x, dir-enc, grad, geo feature, appearance] (misc columns first, h2 accumulated onto them);
+//            last 256->3 layer as fp32 dots; sigmoid + padding
 //   heads    Laplace density, NeuS alpha, occupancy, normals; optional per-sample outputs
 //   render   (fused mode) segmented prefix product over the rays of the tile in double, weights, per-ray sums
-// MMA = tcgen05.mma kind::f16 (bf16 x bf16 -> fp32).  bf16x3: a0*w0 + a1*w0 + a0*w1 with a = a0+a1, w = w0+w1
-// (error ~2^-16 relative, fp32 accumulate).  Weights stream through a shared-memory ring filled by 1-D bulk copies (UBLKCP)
-// from a pre-packed image.  Warp roles: 0-7 epilogues (2 threads per row: the 16-column chunks 2 i + q of iteration i), 8-11 hash gathers, 12-13 PE / colour
-// input columns, 14 weight producer, 15 MMA issuer (leader CTA) / weight-arrival relay (peer CTA).
+// MMA = wgmma bf16 x bf16 -> fp32.  bf16x3: a0*w0 + a1*w0 + a0*w1 with a = a0+a1, w = w0+w1 (error ~2^-16 relative, fp32 accumulate).
+// 256 threads: the accumulator alone takes 128 registers per thread, so no warp is spent on a separate producer role (a ninth
+// warp would cap every thread at 168 registers); thread 0 keeps the weight ring filled between its own MMAs.
 #pragma once
 #include "field_tc.h"
 #include "grid.cuh"
@@ -87,62 +85,38 @@ __device__ __forceinline__ PointGeom point_geom(const TcArgs& a, long long p) {
   return g;
 }
 
-// one 16-byte chunk (8 consecutive K columns of one row) of a small-K smem operand, all planes: layout [plane][k/8][row][8]
+// one 16-byte chunk (8 consecutive K columns of one row) of the A operand, all planes: layout [plane][k/8][row][8]
 template <int P>
 __device__ __forceinline__ void store_chunk(uint8_t* inA, int row, int chunk, const float (&v)[8]) {
   uint32_t hi[4], lo[4];
 #pragma unroll
   for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hi[e], lo[e]);
   *reinterpret_cast<uint4*>(inA + (size_t)chunk * 2048 + row * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-  if (P > 1) *reinterpret_cast<uint4*>(inA + (kInK / 8) * 2048 + (size_t)chunk * 2048 + row * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+  if (P > 1) *reinterpret_cast<uint4*>(inA + kAPlane + (size_t)chunk * 2048 + row * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
 
 // accurate sin / sincos as real calls: one copy of the (long) range-reduction code instead of one per call site -- the roles of this
 // kernel share the SM's instruction cache, and `no instruction` stalls were 20 % of all samples with everything inlined
-// L2 eviction priorities (0 normal, 1 evict_first, 2 evict_last) of the hash table and of the per-CTA scratch spills (A/B measured, DESIGN.md)
-// 1: the hash gathers of the NEXT tile start only after this tile's E1 (the two softplus epilogues spill 64 + 128 KB through the same L1
-// request queue the gathers saturate; keeping them apart costs nothing because the gathers need < half of a tile's time)
-#ifndef TCV_GATHER_AFTER_E1
-#define TCV_GATHER_AFTER_E1 1
-#endif
-// pause (ns) of a gather thread after each hash level (spreads the gathers over the tile).  0 since the MMAs trail the epilogues: a tile is
-// short enough now that the encode of the next tile (~45 k cycles of gathers) must not be stretched (A/B: 600 -> 1.47 ms, 0 -> 1.44 ms)
-#ifndef TCV_GATHER_NAP
-#define TCV_GATHER_NAP 0
-#endif
-// epilogue waits for an MMA phase: 1 = plain spin on try_wait (shortest wake-up; the phases are short now that the MMAs trail the epilogues)
-#ifndef TCV_EPI_SPIN
-#define TCV_EPI_SPIN 0
-#endif
-#if TCV_EPI_SPIN
-#define EPI_WAIT(bar, par) mbar_wait(bar, par)
-#else
-#define EPI_WAIT(bar, par) mbar_wait_backoff(bar, par)
-#endif
+// L2 eviction priority (0 normal, 1 evict_first, 2 evict_last) of the hash-table gathers
 #ifndef TCV_POL_TABLE
 #define TCV_POL_TABLE 2
-#endif
-#ifndef TCV_POL_SCRATCH
-#define TCV_POL_SCRATCH 1
 #endif
 
 static __device__ __noinline__ void sincos_call(float x, float* s, float* c) { sincosf(x, s, c); }
 static __device__ __noinline__ float sin_call(float x) { return sinf(x); }
 
-// store one bf16 element (split into P planes) of a small-K smem operand: layout [plane][k/8][row][8]
+// store one bf16 element (split into P planes) of the A operand: layout [plane][k/8][row][8]
 template <int P>
 __device__ __forceinline__ void store_in(uint8_t* inA, int row, int col, float v) {
   const __nv_bfloat16 hi = __float2bfloat16_rn(v);
   const uint32_t off = (uint32_t)(col >> 3) * 2048u + (uint32_t)row * 16u + (uint32_t)(col & 7) * 2u;
   *reinterpret_cast<__nv_bfloat16*>(inA + off) = hi;
-  if (P > 1) *reinterpret_cast<__nv_bfloat16*>(inA + (kInK / 8) * 2048 + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
+  if (P > 1) *reinterpret_cast<__nv_bfloat16*>(inA + kAPlane + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
 // Hash-grid part of the geo input of one tile (gather warps, one thread per point).  Outputs: operand chunks 0..3 (bf16 planes,
 // kernel column order: four levels = one aligned 16-byte chunk) and, in the per-CTA global scratch, the grid jacobian
-// [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  Measured on B200 (same-box A/B, DESIGN.md): neither two levels of
-// gathers in flight per thread nor lane pairs sharing the 128-byte line of the two x-neighbours change the gather rate, so the
-// plain one-level-at-a-time form (smallest code) is used.
+// [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  One level at a time (smallest code).
 template <int P, int LAYOUT>
 __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int row, uint8_t* inA, uint8_t* enc, uint64_t pol_table) {
   float* Jg = reinterpret_cast<float*>(enc) + kPeRows * 128;
@@ -161,7 +135,6 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
       level_prepare<LAYOUT>(a.grid, l, x01, y01, z01, c);
       level_fetch_rt2(a.grid, a.table, c, tv, pol_table);
       level_finish<2, LAYOUT>(a.grid, c, tv, o, dj);
-      if (TCV_GATHER_NAP > 0 && a.mode != 0) __nanosleep(TCV_GATHER_NAP);
     }
     store_in<P>(inA, row, 2 * l, o[0]);
     store_in<P>(inA, row, 2 * l + 1, o[1]);
@@ -191,7 +164,7 @@ __device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int ro
 #pragma unroll 1
   for (int ch = 4; ch < kInK / 8; ++ch) {
     *reinterpret_cast<uint4*>(inA + (size_t)ch * 2048 + row * 16) = z4;
-    if (P > 1) *reinterpret_cast<uint4*>(inA + (kInK / 8) * 2048 + (size_t)ch * 2048 + row * 16) = z4;
+    if (P > 1) *reinterpret_cast<uint4*>(inA + kAPlane + (size_t)ch * 2048 + row * 16) = z4;
   }
 #pragma unroll 1
   for (int i = 0; i < a.pe_dim; ++i) {                       // sin(x 2^k) | sin(x 2^k + pi/2)   (encodings.py:194-198)
@@ -222,7 +195,7 @@ __device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, in
 #pragma unroll 1
   for (int ch = 1; ch < kInK / 8; ++ch) {
     *reinterpret_cast<uint4*>(inA + (size_t)ch * 2048 + row * 16) = z4;
-    if (P > 1) *reinterpret_cast<uint4*>(inA + (kInK / 8) * 2048 + (size_t)ch * 2048 + row * 16) = z4;
+    if (P > 1) *reinterpret_cast<uint4*>(inA + kAPlane + (size_t)ch * 2048 + row * 16) = z4;
   }
   store_in<P>(inA, row, 8 + 0, g.px); store_in<P>(inA, row, 8 + 1, g.py); store_in<P>(inA, row, 8 + 2, g.pz);
   // direction encoding: sin(d 2^k) | sin(d 2^k + pi/2), k = 0..3, then d itself (NeRFEncoding(4, include_input), encodings.py:167-208)
@@ -242,48 +215,105 @@ __device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, in
 }
 
 #ifdef SDFB200_TC_TIMING
-// stamps of CTA 0: [0,16) epilogue thread 0, [16,20) gather thread 0, [20,28) MMA thread (time at which layer L starts issuing)
+// stamps of CTA 0, thread 0, first 16 tiles: [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring order), [15] tile end
 __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
 #define TC_STAMP(k)                                                                                                  \
   do {                                                                                                               \
-    if (blockIdx.x == 0 && lane == 0 && tile_no >= 0 && tile_no < 16) g_tc_timing[tile_no * 32 + (k)] = clock64();                   \
+    if (blockIdx.x == 0 && tid == 0 && tile_no >= 0 && tile_no < 16) g_tc_timing[tile_no * 32 + (k)] = clock64();                   \
   } while (0)
 #else
 #define TC_STAMP(k) do { } while (0)
 #endif
 
+// Weight ring producer (thread 0 of the CTA, between its own MMAs): walks every K-block of every layer of every tile of this CTA in
+// consumption order and issues the bulk copy of block j once its slot has been released (all 8 consumer warps are through block
+// j - kStages, which only needs earlier blocks: no cycle).
+struct RingCursor { int tile, L, kb; uint32_t j; };
+template <int P>
+__device__ __forceinline__ void produce_until(RingCursor& pr, uint32_t upto, const TcArgs& a, int nlayers, uint8_t* ring, uint32_t stage_bytes,
+                                              uint64_t* full, uint64_t* empty) {
+  while (pr.j <= upto && pr.tile < a.n_tiles) {
+    const TcLayer& ly = a.layer[pr.L];
+    const uint32_t bytes = (uint32_t)P * ly.Np * ly.kblk * 2;
+    const int s = pr.j % kStages;
+    mbar_wait(&empty[s], ((pr.j / kStages) & 1) ^ 1);
+    mbar_arrive_expect_tx(&full[s], bytes);
+    bulk_g2s(ring + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(a.blob) + ly.w_off + (size_t)pr.kb * bytes, bytes, &full[s]);
+    ++pr.j;
+    if (++pr.kb == ly.nkb) {
+      pr.kb = 0;
+      if (++pr.L == nlayers) { pr.L = 0; pr.tile += gridDim.x; }
+    }
+  }
+}
+
+// All MMAs of one layer for the 64 rows of a warpgroup: acc (+)= A[rows, K] W^T, the weight K-blocks taken from the ring in order.
+// Every consumer warp releases a ring slot once its own MMAs on it are complete (empty barrier count = 8 warps).
+template <int P>
+__device__ __forceinline__ void layer_mma(float (&acc)[4][32], const TcLayer& ly, bool zero, uint32_t a_base, uint8_t* ring, uint32_t stage_bytes,
+                                          uint64_t* full, uint64_t* empty, uint32_t& it, int lane, bool producer, RingCursor& pr, const TcArgs& a,
+                                          int nlayers) {
+  if (zero) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+  }
+  const int nch = ly.Np / 64;
+  const uint32_t lbo_b = (uint32_t)ly.Np * 16, plane_b = (uint32_t)ly.Np * ly.kblk * 2;
+  const int ksteps = ly.kblk / 16;
+  for (int kb = 0; kb < ly.nkb; ++kb, ++it) {
+    if (producer) produce_until<P>(pr, it + kStages - 1, a, nlayers, ring, stage_bytes, full, empty);
+    __syncwarp();
+    const int s = it % kStages;
+    mbar_wait(&full[s], (it / kStages) & 1);
+    const uint32_t wbase = smem_u32(ring + (size_t)s * stage_bytes);
+    wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+    wg_arrive();
+    for (int j = 0; j < ksteps; ++j) {
+      const int kstep = kb * ksteps + j;
+      const uint64_t a0 = make_smem_desc(a_base + kstep * 2 * 2048, 2048, 128);
+      const uint64_t a1 = make_smem_desc(a_base + kAPlane + kstep * 2 * 2048, 2048, 128);
+      wgmma_kstep_ss<P, 4>(acc, a0, a1, wbase + j * 2 * lbo_b, plane_b, lbo_b, nch);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+  }
+}
+
+// accumulator element pair (c, i), i even: columns col, col + 1 of row `row` -> one 4-byte unit of each A plane
+template <int P>
+__device__ __forceinline__ void store_pair(uint8_t* abuf, int col, int row, float v0, float v1) {
+  uint32_t hi, lo;
+  split2(v0, v1, hi, lo);
+  const uint32_t off = (uint32_t)(col >> 3) * 2048u + (uint32_t)row * 16u + (uint32_t)(col & 7) * 2u;
+  *reinterpret_cast<uint32_t*>(abuf + off) = hi;
+  if (P > 1) *reinterpret_cast<uint32_t*>(abuf + kAPlane + off) = lo;
+}
+
 template <int P, int LAYOUT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constant__ TcArgs a) {
+__global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constant__ TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  constexpr uint32_t kInBytes = (uint32_t)P * (kInK / 8) * 2048;       // small-K operand (all planes), double buffered
-  constexpr uint32_t kStageBytes = (uint32_t)P * 128 * kKB * 2;        // this CTA's half of one weight K-block, all planes
-  uint8_t* inA0 = smem;
-  uint8_t* ring = smem + 2 * kInBytes;
+  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;        // one weight K-block, all planes (the 128-row layer: K blocks of 64)
+  uint8_t* abuf = smem;                                                // A operand of every layer: [P][32 chunks][128 rows][16 B]
+  uint8_t* ring = smem + P * kAPlane;
   float* fbuf = reinterpret_cast<float*>(ring + kStages * kStageBytes);
-  float* red = fbuf;                  // [3][2][128] partial sums
-  float* prm = fbuf + 6 * 128;        // [9][256] biases / fp32 weight rows used by the epilogues
-  float* racc = prm + 9 * 256;        // [8][4] per-ray accumulators of the fused compositing (rays spanning several warps)
+  float* prm = fbuf;                  // [9][256] biases / fp32 weight rows used by the epilogues
+  float* hs = prm + 9 * 256;          // [7][128] per-row inputs of the heads: sdf, gradient (3), raw rgb (3)
+  float* racc = hs + 7 * 128;         // [8][4] per-ray accumulators of the fused compositing (rays spanning several warps)
   float* lastrgb = racc + 32;         // [4][3]
-  __shared__ uint64_t full[kStages], empty[kStages], peer_full[kStages], dfull, g0done, a_rdy[8], x_free, c0_ready, in_ready, misc_ready, e1done;
+  __shared__ uint64_t full[kStages], empty[kStages];
   __shared__ double wtot[4];
-  __shared__ uint32_t tmem_base_s;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int npairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
+  const int nlayers = a.mode == 0 ? 2 : L_COUNT;
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); mbar_init(&peer_full[s], 1); }
-    mbar_init(&dfull, 1);
-    mbar_init(&g0done, 1);
-    for (int g = 0; g < 8; ++g) mbar_init(&a_rdy[g], 2 * kEpiWarps);
-    mbar_init(&x_free, 2 * kEpiWarps);
-    mbar_init(&c0_ready, 2 * kEpiWarps);
-    mbar_init(&e1done, kEpiWarps);
-    mbar_init(&in_ready, 2 * kEncWarps);
-    mbar_init(&misc_ready, 2 * (kAluWarps > 0 ? kAluWarps : kGatherWarps));
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kEpiWarps); }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc2<512>(&tmem_base_s);
   {
     const char* blob = a.blob;
     const float* src[9] = {reinterpret_cast<const float*>(blob + a.b_g0), reinterpret_cast<const float*>(blob + a.b_g1),
@@ -294,625 +324,386 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kTcThreads, 1) k_fie
     for (int i = tid; i < 9 * 256; i += kTcThreads) prm[i] = src[i >> 8][i & 255];
     if (tid < 44) racc[tid] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();                      // barriers of both CTAs initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
-  // two 256-column regions; per layer one is the accumulator and the other holds the A operand (the previous accumulator, converted in place):
-  //   G0: D=X | G1: A=X D=Y | B1: A=Y D=X | B0: A=X D=Y[0,96) | C0H (+C0MISC): A=X (h2 reloaded) D=Y | C1: A=Y D=X
-  const uint32_t x_tmem = tmem;
-  const uint32_t y_tmem = tmem + 256;
-  const int nphase_layers = a.mode == 0 ? 2 : L_COUNT;
-  // leader-side barriers that both CTAs arrive on
-  const uint32_t a_rdy_r0 = mapa_shared(smem_u32(&a_rdy[0]), 0);      // a_rdy[g] of the leader CTA: + 8 g
-  const uint32_t x_free_r = mapa_shared(smem_u32(&x_free), 0);
-  const uint32_t c0_ready_r = mapa_shared(smem_u32(&c0_ready), 0);
-  const uint32_t in_ready_r = mapa_shared(smem_u32(&in_ready), 0);
-  const uint32_t misc_ready_r = mapa_shared(smem_u32(&misc_ready), 0);
 
-  if (warp == kWarpProducer) {
-    // ============================== weight producer (this CTA's half of every weight tile) ==============================
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tp = pair; tp < a.n_tile_pairs; tp += npairs) {
-        for (int L = 0; L < nphase_layers; ++L) {
-          const TcLayer ly = a.layer[L];
-          const uint32_t bytes = (uint32_t)P * (ly.Np / 2) * ly.kblk * 2;
-          const uint8_t* src = reinterpret_cast<const uint8_t*>(a.blob) + ly.w_off + (size_t)rank * bytes;
-          for (int kb = 0; kb < ly.nkb; ++kb, ++it) {
-            const int s = it % kStages;
-            mbar_wait(&empty[s], ((it / kStages) & 1) ^ 1);
-            mbar_arrive_expect_tx(&full[s], bytes);
-            bulk_g2s(ring + (size_t)s * kStageBytes, src + (size_t)kb * 2 * bytes, bytes, &full[s]);
+  // ============================== two warpgroups, 64 rows of the tile each ==============================
+  const int wg = warp >> 2, t = tid & 127;
+  const int wrow0 = wg * 64;
+  const int r0 = wrow0 + (t >> 5) * 16 + ((t & 31) >> 2);   // the thread's accumulator rows: r0, r0 + 8
+  const int cq = (t & 3) * 2;                                // column offset inside every 8-column block
+  const int wg_bar = 1 + wg;                                 // named barrier of this warpgroup
+  const uint32_t a_base = smem_u32(abuf) + wrow0 * 16;
+  const char* blob = a.blob;
+  const float* p_bg0 = prm;             // smem copies (broadcast loads instead of one LDG per element)
+  const float* p_bg1 = prm + 256;
+  const float* p_wg2 = prm + 768;       // row 0 of the last geo layer
+  const float* p_bc0 = prm + 1024;
+  const float* p_bc1 = prm + 1280;
+  const float* p_wc2 = prm + 1536;      // [3][256]
+  const float sdf_bias = __ldg(reinterpret_cast<const float*>(blob + a.b_g2));
+  const float* b_c2 = reinterpret_cast<const float*>(blob + a.b_c2);
+  char* scr = a.scratch + (size_t)blockIdx.x * a.scratch_per_cta;
+  uint32_t* sig_s = reinterpret_cast<uint32_t*>(scr);                       // [64 units][256 threads]: softplus'(z1) as 2 x unorm16
+  uint32_t* gf_s = reinterpret_cast<uint32_t*>(scr + 65536);                // [P][64 units][256 threads]: h2 as bf16x2 planes
+  uint8_t* enc_s = reinterpret_cast<uint8_t*>(scr + 65536 + (size_t)P * 65536);   // input jacobian: PE [64][128] f32 | grid [96][128] f32
+  const float* Jpe = reinterpret_cast<const float*>(enc_s);
+  const float* Jg = Jpe + kPeRows * 128;
+  const uint64_t pol_table = l2_policy(TCV_POL_TABLE);
+  const uint64_t pol_keep = l2_policy_evict_normal();
+  uint32_t it = 0;
+  const bool producer = tid == 0;
+  RingCursor pr{(int)blockIdx.x, 0, 0, 0u};
+  float acc[4][32];
+#define SYNC_A()                \
+  do {                          \
+    fence_async_smem();         \
+    named_sync(wg_bar, 128);    \
+  } while (0)
+#define LAYER(L, zero)                                                                                 \
+  do {                                                                                                 \
+    layer_mma<P>(acc, a.layer[L], zero, a_base, ring, kStageBytes, full, empty, it, lane, producer, pr, a, nlayers); \
+    named_sync(wg_bar, 128); /* every warp of the warpgroup is done reading this layer's A operand */  \
+    TC_STAMP(1 + (L));                                                                                 \
+  } while (0)
+
+  int tile_no = -1;
+  for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
+    ++tile_no;
+    TC_STAMP(0);
+    // ---------------- encode: thread t < 64 hash gathers of row wrow0 + t, thread t >= 64 PE / x of row wrow0 + t - 64 ----------------
+    {
+      const int row = wrow0 + (t & 63);
+      if (t < 64) {
+        encode_tile_grid<P, LAYOUT>(a, tile, row, abuf, enc_s, pol_table);
+        const long long p = (long long)tile * 128 + row;
+        if (p < a.n_points) {
+          const PointGeom g = point_geom(a, p);
+          if (a.out.points_norm) a.out.points_norm[p] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(g.px, g.px), __fmul_rn(g.py, g.py)), __fmul_rn(g.pz, g.pz)));
+          if (a.out.points) { a.out.points[p * 3] = g.px; a.out.points[p * 3 + 1] = g.py; a.out.points[p * 3 + 2] = g.pz; }
+        }
+      } else {
+        encode_tile_pe<P>(a, tile, row, abuf, enc_s);
+      }
+    }
+    SYNC_A();
+
+    // ---------------- G0 -> E0: h1 = softplus(z1) -> A ; softplus'(z1) -> scratch ----------------
+    LAYER(L_G0, true);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int col = c * 64 + (i >> 2) * 8 + cq, row = r0 + 8 * ((i >> 1) & 1);
+        const float2 b2 = *reinterpret_cast<const float2*>(p_bg0 + col);
+        float h0, h1, s0, s1;
+        softplus100_fast(acc[c][i] + b2.x, h0, s0);
+        softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
+        store_pair<P>(abuf, col, row, h0, h1);
+        if (a.mode != 0) sig_s[(c * 16 + (i >> 1)) * 256 + tid] = __float2uint_rn(s0 * 65535.0f) | (__float2uint_rn(s1 * 65535.0f) << 16);
+      }
+    }
+    SYNC_A();
+
+    // ---------------- G1 -> E1: sdf = W2[0,:] . h2 + b (fp32) ; h2 -> scratch planes ; g2 = W2[0,:] * softplus'(z2) -> A ----------------
+    LAYER(L_G1, true);
+    float sp[2] = {0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int col = c * 64 + (i >> 2) * 8 + cq, h = (i >> 1) & 1, row = r0 + 8 * h;
+        const float2 b2 = *reinterpret_cast<const float2*>(p_bg1 + col);
+        const float2 w2 = *reinterpret_cast<const float2*>(p_wg2 + col);
+        float h0, h1, s0, s1;
+        softplus100_fast(acc[c][i] + b2.x, h0, s0);
+        softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
+        sp[h] = fmaf(w2.x, h0, sp[h]);
+        sp[h] = fmaf(w2.y, h1, sp[h]);
+        if (a.mode != 0) {
+          uint32_t hi, lo;
+          split2(h0, h1, hi, lo);
+          const int u = (c * 16 + (i >> 1)) * 256 + tid;
+          gf_s[u] = hi;
+          if (P > 1) gf_s[64 * 256 + u] = lo;
+          store_pair<P>(abuf, col, row, w2.x * s0, w2.y * s1);
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      sp[h] += __shfl_xor_sync(0xffffffffu, sp[h], 1);
+      sp[h] += __shfl_xor_sync(0xffffffffu, sp[h], 2);
+    }
+    if ((t & 3) < 2) {
+      const int h = t & 1, row = r0 + 8 * h;
+      const float sdf = sp[h] + sdf_bias;
+      const long long p = (long long)tile * 128 + row;
+      if (p < a.n_points && a.out.sdf) a.out.sdf[p] = sdf;
+      hs[row] = sdf;
+    }
+    if (a.mode == 0) continue;
+    SYNC_A();
+
+    // ---------------- B1 -> EB1: g1 = (W1^T g2) * softplus'(z1) -> A ----------------
+    LAYER(L_B1, true);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int col = c * 64 + (i >> 2) * 8 + cq, row = r0 + 8 * ((i >> 1) & 1);
+        const uint32_t sw = sig_s[(c * 16 + (i >> 1)) * 256 + tid];
+        const float s0 = (float)(sw & 0xFFFFu) * (1.0f / 65535.0f), s1 = (float)(sw >> 16) * (1.0f / 65535.0f);
+        store_pair<P>(abuf, col, row, acc[c][i] * s0, acc[c][i + 1] * s1);
+      }
+    }
+    SYNC_A();
+
+    // ---------------- B0 -> EB0: gin (96 cols, kernel order) . input jacobian -> d sdf / dx ----------------
+    LAYER(L_B0, true);
+    const int deg = a.pe_degree, half = 3 * deg;
+    float gr[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = c * 64 + (i >> 2) * 8 + cq + (i & 1), h = (i >> 1) & 1, row = r0 + 8 * h;
+        const float g = acc[c][i];
+        if (col < 32) {
+          if (col < a.grid_dim) {
+#pragma unroll
+            for (int d3 = 0; d3 < 3; ++d3) gr[h][d3] = fmaf(g, ld_stream_f1(Jg + (col * 3 + d3) * 128 + row, pol_keep), gr[h][d3]);
+          }
+        } else {
+          // PE column i -> axis (i mod 3 deg) / deg, factor 2^k cos(arg) ; x column -> its own axis, factor 1
+          const int ip = col - 32;
+          if (ip < a.pe_dim) {
+            const int ia = ip >= half ? ip - half : ip;
+            const int ax = ia < deg ? 0 : (ia < 2 * deg ? 1 : 2);
+            const float tv = g * ld_stream_f1(Jpe + ip * 128 + row, pol_keep);
+            gr[h][0] += ax == 0 ? tv : 0.f; gr[h][1] += ax == 1 ? tv : 0.f; gr[h][2] += ax == 2 ? tv : 0.f;
+          } else if (ip - a.pe_dim < 3) {
+            const int ax = ip - a.pe_dim;
+            gr[h][0] += ax == 0 ? g : 0.f; gr[h][1] += ax == 1 ? g : 0.f; gr[h][2] += ax == 2 ? g : 0.f;
           }
         }
       }
     }
-  } else if (warp == kWarpMma) {
-    if (rank != 0) {
-      // ============================== peer CTA: forward "my half of stage s has landed" to the leader ==============================
-      if (lane == 0) {
-        uint32_t it = 0;
-        for (int tp = pair; tp < a.n_tile_pairs; tp += npairs)
-          for (int L = 0; L < nphase_layers; ++L)
-            for (int kb = 0; kb < a.layer[L].nkb; ++kb, ++it) {
-              const int s = it % kStages;
-              mbar_wait(&full[s], (it / kStages) & 1);
-              mbar_arrive_remote(mapa_shared(smem_u32(&peer_full[s]), 0));
-            }
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int d3 = 0; d3 < 3; ++d3) {
+        gr[h][d3] += __shfl_xor_sync(0xffffffffu, gr[h][d3], 1);
+        gr[h][d3] += __shfl_xor_sync(0xffffffffu, gr[h][d3], 2);
       }
-    } else if (lane == 0) {
-      // ============================== MMA issuer (leader CTA, one thread) ==============================
-      uint32_t it = 0, par_a = 0, par_in = 0, par_misc = 0, par_x = 0, par_c0 = 0;
-      int tile_no = -1;
-      for (int tp = pair; tp < a.n_tile_pairs; tp += npairs) {
-        ++tile_no;
-        const uint32_t in_base = smem_u32(inA0 + (tile_no & 1) * kInBytes);
-        for (int L = 0; L < nphase_layers; ++L) {
-          const bool a_in_smem = (L == L_G0 || L == L_C0MISC);
-          if (L == L_C0MISC) {                                   // accumulates onto C0H; static columns from the gather warps, chunk 0 (gradient) from EB0
-            mbar_wait_cluster(&misc_ready, par_misc); par_misc ^= 1;
-            mbar_wait_cluster(&c0_ready, par_c0); par_c0 ^= 1;
-          } else if (L == L_G0) {
-            mbar_wait_cluster(&x_free, par_x); par_x ^= 1;      // both CTAs: region X drained (EC1 / sdf-only E1 of the previous tile)
-            mbar_wait_cluster(&in_ready, par_in); par_in ^= 1;
-          }
-          if (a_in_smem) tc_fence_after();
-          TC_STAMP(20 + L);
-          const TcLayer ly = a.layer[L];
-          const uint32_t d_tmem = (L == L_G0 || L == L_B1 || L == L_C1) ? x_tmem : y_tmem;
-          const uint32_t a_tmem = (L == L_G1 || L == L_B0 || L == L_C0H) ? x_tmem : y_tmem;
-          const int groups_per_kb = 8 / ly.nkb;                  // TS layers: K = 256 arrives in 8 groups of 32 columns, handed over one by one by the epilogue
-          const uint32_t idesc = make_idesc_bf16(256, ly.Np);
-          const uint32_t lbo_b = (uint32_t)(ly.Np / 2) * 16, plane_b = (uint32_t)(ly.Np / 2) * ly.kblk * 2;
-          const int ksteps = ly.kblk / 16;
-          uint32_t acc = (L == L_C0MISC) ? 1u : 0u;
-          for (int kb = 0; kb < ly.nkb; ++kb, ++it) {
-            const int s = it % kStages;
-            if (!a_in_smem)
-              for (int g = kb * groups_per_kb; g < (kb + 1) * groups_per_kb; ++g) mbar_wait_cluster(&a_rdy[g], par_a);   // both CTAs: these A columns are in place
-            mbar_wait(&full[s], (it / kStages) & 1);
-            mbar_wait_cluster(&peer_full[s], (it / kStages) & 1);
-            tc_fence_after();
-            const uint32_t wbase = smem_u32(ring + (size_t)s * kStageBytes);
-#pragma unroll 2
-            for (int j = 0; j < ksteps; ++j) {
-              const int kstep = kb * ksteps + j;
-              const uint64_t b0 = make_smem_desc(wbase + j * 2 * lbo_b, lbo_b, 128);
-              const uint64_t b1 = make_smem_desc(wbase + plane_b + j * 2 * lbo_b, lbo_b, 128);
-              if (a_in_smem) {
-                const uint64_t a0 = make_smem_desc(in_base + kstep * 2 * 2048, 2048, 128);
-                mma_ss2(d_tmem, a0, b0, idesc, acc);
-                acc = 1;
-                if (P > 1) {
-                  const uint64_t a1 = make_smem_desc(in_base + (kInK / 8) * 2048 + kstep * 2 * 2048, 2048, 128);
-                  mma_ss2(d_tmem, a1, b0, idesc, 1);
-                  mma_ss2(d_tmem, a0, b1, idesc, 1);
-                }
-              } else {
-                mma_ts2(d_tmem, a_tmem + kstep * 16, b0, idesc, acc);
-                acc = 1;
-                if (P > 1) {
-                  mma_ts2(d_tmem, a_tmem + kstep * 16 + 8, b0, idesc, 1);
-                  mma_ts2(d_tmem, a_tmem + kstep * 16, b1, idesc, 1);
-                }
-              }
-            }
-            mma_commit2(&empty[s]);
-          }
-          if (!a_in_smem) par_a ^= 1;
-          if (L == L_G0) mma_commit2(&g0done);               // the geo input of this tile has been consumed (gather warps)
-          if (L != L_C0H) mma_commit2(&dfull);               // C0H is completed by C0MISC
-        }
-        TC_STAMP(27);
-      }
+    // colour misc operand over the (consumed) A columns 0..95: chunk 0 = [grad(3), n.v, 0 x4] (sdf_field.py:572-584; columns re-ordered
+    // at pack time) from the thread pair that owns the row, chunks 1..11 = [x, dir-enc, dir, appearance] one thread per row
+    if ((t & 3) < 2) {
+      const int h = t & 1, row = r0 + 8 * h;
+      const long long p_raw = (long long)tile * 128 + row;
+      const PointGeom pg = point_geom(a, p_raw < a.n_points ? p_raw : a.n_points - 1);
+      const float grx = gr[h][0], gry = gr[h][1], grz = gr[h][2];
+      const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
+      const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? (grx / gn) * pg.dx + (gry / gn) * pg.dy + (grz / gn) * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
+      store_chunk<P>(abuf, row, 0, c0v);
+      hs[128 + row] = grx; hs[256 + row] = gry; hs[384 + row] = grz;
     }
-  } else if (warp >= kEpiWarps) {
-    // ============================== encode warps, one tile ahead of the compute warps ==============================
-    // warps 8-11: hash gathers (one thread per point); warps 12-13: PE / x columns and the static colour columns (two points per thread)
-    // (kAluWarps == 0: the four gather warps do all of it, one point per thread -- the PE / colour ALU work then spreads evenly over the
-    //  four SM sub-partitions instead of slowing down the epilogue warps that share a scheduler with the two extra warps)
-    const bool alu = kAluWarps > 0 && warp >= kEpiWarps + kGatherWarps;
-    const int row = alu ? (warp - kEpiWarps - kGatherWarps) * 32 + lane : (warp - kEpiWarps) * 32 + lane;
-    uint8_t* enc_s = reinterpret_cast<uint8_t*>(a.scratch + (size_t)blockIdx.x * a.scratch_per_cta) + 65536 + (size_t)P * 65536;
-    const uint64_t pol_table = l2_policy(TCV_POL_TABLE);
-    auto encode = [&](int tile, uint8_t* inA, uint8_t* enc) {
-      if (alu) { encode_tile_pe<P>(a, tile, row, inA, enc); encode_tile_pe<P>(a, tile, row + 64, inA, enc); }
-      else {
-        encode_tile_grid<P, LAYOUT>(a, tile, row, inA, enc, pol_table);
-        if (kAluWarps == 0) encode_tile_pe<P>(a, tile, row, inA, enc);
-      }
-      fence_async_smem();
-      __threadfence_block();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(in_ready_r);
-    };
-    int tile_no = -1;
-    encode(2 * pair + (int)rank, inA0, enc_s);
-    for (int tp = pair; tp < a.n_tile_pairs; tp += npairs) {
-      ++tile_no;
-      const int tile = 2 * tp + (int)rank;
-      const int buf = tile_no & 1;
-      if (warp == kEpiWarps) TC_STAMP(16);
-      mbar_wait_backoff(&g0done, tile_no & 1);              // G0 of this tile is complete (hence every MMA of the previous tile)
-      if (warp == kEpiWarps) TC_STAMP(17);
-      if (a.mode != 0 && (alu || kAluWarps == 0)) {
-        colour_static_tile<P>(a, tile, row, inA0 + buf * kInBytes);
-        if (alu) colour_static_tile<P>(a, tile, row + 64, inA0 + buf * kInBytes);
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(misc_ready_r);
-      }
-      if (warp == kEpiWarps) TC_STAMP(18);
-      if (TCV_GATHER_AFTER_E1 && !alu && a.mode != 0) mbar_wait_backoff(&e1done, tile_no & 1);   // this CTA's E1 (h2 spill) is through
-      if (tp + npairs < a.n_tile_pairs) encode(tile + 2 * npairs, inA0 + (buf ^ 1) * kInBytes, enc_s + (size_t)(buf ^ 1) * kJRBytes);
-      if (warp == kEpiWarps) TC_STAMP(19);
-    }
-  } else {
-    // ============================== epilogue warps (8): thread (row, q) owns accumulator columns [128 q, 128 q + 128) ==============================
-    const int wq = warp & 3;                              // TMEM lane quadrant
-    const int row = wq * 32 + lane;                       // tile row == TMEM lane
-    const int q = warp >> 2;                              // column half
-    const uint32_t lane_addr = (uint32_t)(wq * 32) << 16;
-    const char* blob = a.blob;
-    const float* p_bg0 = prm;             // smem copies (broadcast LDS.128 instead of one LDG per element)
-    const float* p_bg1 = prm + 256;
-    const float* p_wg2 = prm + 768;       // row 0 of the last geo layer
-    const float* p_bc0 = prm + 1024;
-    const float* p_bc1 = prm + 1280;
-    const float* p_wc2 = prm + 1536;      // [3][256]
-    const float sdf_bias = __ldg(reinterpret_cast<const float*>(blob + a.b_g2));
-    const float* b_c2 = reinterpret_cast<const float*>(blob + a.b_c2);
-    uint8_t* sig_s = reinterpret_cast<uint8_t*>(a.scratch + (size_t)blockIdx.x * a.scratch_per_cta);   // [32 units][128 rows][16 B]
-    uint8_t* gf_s = sig_s + 65536;                                                                      // [P][32 units][128][16 B]
-    uint8_t* enc_s = gf_s + (size_t)P * 65536;                                                          // 2 x input jacobian
-    uint32_t dpar = 0;
-    const uint64_t pol_stream = l2_policy(TCV_POL_SCRATCH);
-    const uint64_t pol_keep = l2_policy_evict_normal();
-    // hand 32 converted A columns (K group g = this iteration's chunk of both column-half threads) to the MMA issuer
-    auto sub_arrive = [&](int g) {
-      tc_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(a_rdy_r0 + 8 * g);
-    };
-    auto x_arrive = [&]() {
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(x_free_r);
-    };
+    if (t < 64) colour_static_tile<P>(a, tile, wrow0 + t, abuf);
+    SYNC_A();
 
-    int tile_no = -1;
-    for (int tp = pair; tp < a.n_tile_pairs; tp += npairs) {
-      ++tile_no;
-      const int tile = 2 * tp + (int)rank;
-      if (warp == 0) TC_STAMP(0);
-      const int buf = tile_no & 1;
-      uint8_t* inA = inA0 + buf * kInBytes;               // geo input now, colour operand later
-      const uint8_t* enc_cur = enc_s + (size_t)buf * kJRBytes;
+    // ---------------- C0: misc columns, then h2 (reloaded from the scratch) accumulated onto them ----------------
+    LAYER(L_C0MISC, true);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int col = c * 64 + (i >> 2) * 8 + cq, row = r0 + 8 * ((i >> 1) & 1);
+        const int u = (c * 16 + (i >> 1)) * 256 + tid;
+        const uint32_t off = (uint32_t)(col >> 3) * 2048u + (uint32_t)row * 16u + (uint32_t)(col & 7) * 2u;
+        *reinterpret_cast<uint32_t*>(abuf + off) = gf_s[u];
+        if (P > 1) *reinterpret_cast<uint32_t*>(abuf + kAPlane + off) = gf_s[64 * 256 + u];
+      }
+    }
+    SYNC_A();
+    LAYER(L_C0H, false);
+    // ---------------- EC0: relu -> A ----------------
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int col = c * 64 + (i >> 2) * 8 + cq, row = r0 + 8 * ((i >> 1) & 1);
+        const float2 b2 = *reinterpret_cast<const float2*>(p_bc0 + col);
+        store_pair<P>(abuf, col, row, fmaxf(acc[c][i] + b2.x, 0.f), fmaxf(acc[c][i + 1] + b2.y, 0.f));
+      }
+    }
+    SYNC_A();
+
+    // ---------------- C1 -> EC1: relu, last colour layer (256 -> 3) as fp32 dots ----------------
+    LAYER(L_C1, true);
+    {
+      float rr[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int col = c * 64 + (i >> 2) * 8 + cq + (i & 1), h = (i >> 1) & 1;
+          const float v = fmaxf(acc[c][i] + p_bc1[col], 0.f);
+          rr[h][0] = fmaf(p_wc2[col], v, rr[h][0]);
+          rr[h][1] = fmaf(p_wc2[256 + col], v, rr[h][1]);
+          rr[h][2] = fmaf(p_wc2[512 + col], v, rr[h][2]);
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          rr[h][k] += __shfl_xor_sync(0xffffffffu, rr[h][k], 1);
+          rr[h][k] += __shfl_xor_sync(0xffffffffu, rr[h][k], 2);
+        }
+      if ((t & 3) < 2) {
+        const int h = t & 1, row = r0 + 8 * h;
+        hs[512 + row] = rr[h][0]; hs[640 + row] = rr[h][1]; hs[768 + row] = rr[h][2];
+      }
+    }
+    named_sync(3, kEpiThreads);      // both warpgroups' head inputs are in `hs`
+
+    if (wg == 0) {
+      // ---------------- per-point heads: thread = tile row ----------------
+      const int row = t, wq = warp;
       const long long p_raw = (long long)tile * 128 + row;
       const bool valid = p_raw < a.n_points;
       const long long p = valid ? p_raw : a.n_points - 1;
       const PointGeom pg = point_geom(a, p);
-      const float px = pg.px, py = pg.py, pz = pg.pz, dirx = pg.dx, diry = pg.dy, dirz = pg.dz, delta = pg.delta;
-      if (q == 0 && valid) {
-        if (a.out.points_norm) a.out.points_norm[p] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
-        if (a.out.points) { a.out.points[p * 3] = px; a.out.points[p * 3 + 1] = py; a.out.points[p * 3 + 2] = pz; }
-      }
-      if (tile_no == 0 || a.mode == 0) x_arrive();        // region X is free (later tiles: signalled at the end of EC1 of the previous tile)
-      if (warp == 0) TC_STAMP(1);
-
-      // ---------------- E0: h1 = softplus(z1) -> A planes ; softplus'(z1) -> scratch ----------------
-      EPI_WAIT(&dfull, dpar); dpar ^= 1; tc_fence_after();
-      if (warp == 0) TC_STAMP(2);
-      // thread (row, q) converts the 16-column chunks 2 i + q, i = 0..7: after every iteration 32 more columns (one K group) are done
-#pragma unroll 1
-      for (int cc = 0; cc < 8; ++cc) {
-        const int col0 = (2 * cc + q) * 16;
-        uint32_t v[16];
-        tmem_ld16(x_tmem + lane_addr + col0, v);
-        tc_wait_ld();
-        uint32_t hi[8], lo[8];
-        float sg[16];
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const float4 b4 = *reinterpret_cast<const float4*>(p_bg0 + col0 + j);
-          float h0, h1, h2, h3;
-          softplus100_fast(__uint_as_float(v[j]) + b4.x, h0, sg[j]);
-          softplus100_fast(__uint_as_float(v[j + 1]) + b4.y, h1, sg[j + 1]);
-          softplus100_fast(__uint_as_float(v[j + 2]) + b4.z, h2, sg[j + 2]);
-          softplus100_fast(__uint_as_float(v[j + 3]) + b4.w, h3, sg[j + 3]);
-          split2(h0, h1, hi[j >> 1], lo[j >> 1]);
-          split2(h2, h3, hi[(j >> 1) + 1], lo[(j >> 1) + 1]);
-        }
-        tmem_st8(x_tmem + lane_addr + col0, hi);
-        if (P > 1) tmem_st8(x_tmem + lane_addr + col0 + 8, lo);
-        sub_arrive(cc);
-        if (a.mode != 0) {
-#pragma unroll
-          for (int u8 = 0; u8 < 2; ++u8) {
-            // 8 values -> 8 x unorm16 (one 16-byte unit per thread): absolute error 2^-17
-            uint32_t pk[4];
-#pragma unroll
-            for (int e2 = 0; e2 < 4; ++e2) {
-              const uint32_t lo16 = __float2uint_rn(sg[u8 * 8 + 2 * e2] * 65535.0f), hi16 = __float2uint_rn(sg[u8 * 8 + 2 * e2 + 1] * 65535.0f);
-              pk[e2] = lo16 | (hi16 << 16);
-            }
-            st_stream(sig_s + ((size_t)((col0 >> 3) + u8) * 128 + row) * 16, make_uint4(pk[0], pk[1], pk[2], pk[3]), pol_stream);
-          }
-        }
-      }
-      if (warp == 0) TC_STAMP(3);
-
-      // ---------------- E1: h2 -> scratch planes (colour layer 0 input) ; sdf = W2[0,:] . h2 + b (fp32) ;
-      //                      g2 = W2[0,:] * softplus'(z2) -> A planes (seed of the reverse sweep)
-      EPI_WAIT(&dfull, dpar); dpar ^= 1; tc_fence_after();
-      if (warp == 0) TC_STAMP(4);
-      float sdf_part = 0.f;
-#pragma unroll 1
-      for (int cc = 0; cc < 8; ++cc) {
-        const int col0 = (2 * cc + q) * 16;
-        uint32_t v[16];
-        tmem_ld16(y_tmem + lane_addr + col0, v);
-        tc_wait_ld();
-        uint32_t hi[8], lo[8], ghi[8], glo[8];
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const float4 b4 = *reinterpret_cast<const float4*>(p_bg1 + col0 + j);
-          const float4 w4 = *reinterpret_cast<const float4*>(p_wg2 + col0 + j);
-          float h0, h1, h2, h3, s0, s1, s2, s3;
-          softplus100_fast(__uint_as_float(v[j]) + b4.x, h0, s0);
-          softplus100_fast(__uint_as_float(v[j + 1]) + b4.y, h1, s1);
-          softplus100_fast(__uint_as_float(v[j + 2]) + b4.z, h2, s2);
-          softplus100_fast(__uint_as_float(v[j + 3]) + b4.w, h3, s3);
-          sdf_part = fmaf(w4.x, h0, sdf_part); sdf_part = fmaf(w4.y, h1, sdf_part);
-          sdf_part = fmaf(w4.z, h2, sdf_part); sdf_part = fmaf(w4.w, h3, sdf_part);
-          split2(h0, h1, hi[j >> 1], lo[j >> 1]);
-          split2(h2, h3, hi[(j >> 1) + 1], lo[(j >> 1) + 1]);
-          if (a.mode != 0) {
-            split2(w4.x * s0, w4.y * s1, ghi[j >> 1], glo[j >> 1]);
-            split2(w4.z * s2, w4.w * s3, ghi[(j >> 1) + 1], glo[(j >> 1) + 1]);
-          }
-        }
-        if (a.mode != 0) {
-#pragma unroll
-          for (int u8 = 0; u8 < 2; ++u8) {
-            const size_t unit = ((size_t)((col0 >> 3) + u8) * 128 + row) * 16;
-            st_stream(gf_s + unit, make_uint4(hi[4 * u8], hi[4 * u8 + 1], hi[4 * u8 + 2], hi[4 * u8 + 3]), pol_stream);
-            if (P > 1) st_stream(gf_s + 65536 + unit, make_uint4(lo[4 * u8], lo[4 * u8 + 1], lo[4 * u8 + 2], lo[4 * u8 + 3]), pol_stream);
-          }
-          tmem_st8(y_tmem + lane_addr + col0, ghi);
-          if (P > 1) tmem_st8(y_tmem + lane_addr + col0 + 8, glo);
-          sub_arrive(cc);
-        }
-      }
-      red[q * 128 + row] = sdf_part;
-      if (a.mode == 0) tc_fence_before();
-      if (TCV_GATHER_AFTER_E1 && a.mode != 0 && lane == 0) mbar_arrive(&e1done);
-      if (warp == 0) TC_STAMP(5);
-      named_sync(2, kEpiThreads);
-      const float sdf = (red[row] + red[128 + row]) + sdf_bias;
-      if (q == 0 && valid && a.out.sdf) a.out.sdf[p] = sdf;
-      if (a.mode == 0) {
-        named_sync(2, kEpiThreads);  // `red` is reused by the next tile
-        continue;
-      }
-
-      // ---------------- EB1: g1 = (W1^T g2) * softplus'(z1) -> A planes ----------------
-      // softplus'(z1) does not depend on this phase's MMA: all 16 units are in flight before the wait
-      {
-        uint4 sp[16];
-#pragma unroll
-        for (int u = 0; u < 16; ++u) sp[u] = ld_stream_u4(sig_s + ((size_t)((2 * (u >> 1) + q) * 2 + (u & 1)) * 128 + row) * 16, pol_stream);   // units of chunk 2 i + q
-        EPI_WAIT(&dfull, dpar); dpar ^= 1; tc_fence_after();
-        TC_STAMP(8);
-#pragma unroll
-        for (int cc = 0; cc < 8; ++cc) {
-          const int col0 = (2 * cc + q) * 16;
-          uint32_t v[16];
-          tmem_ld16(x_tmem + lane_addr + col0, v);
-          tc_wait_ld();
-          uint32_t hi[8], lo[8];
-          const uint32_t spw[8] = {sp[2 * cc].x, sp[2 * cc].y, sp[2 * cc].z, sp[2 * cc].w, sp[2 * cc + 1].x, sp[2 * cc + 1].y, sp[2 * cc + 1].z, sp[2 * cc + 1].w};
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float s0 = (float)(spw[j] & 0xFFFFu) * (1.0f / 65535.0f), s1 = (float)(spw[j] >> 16) * (1.0f / 65535.0f);
-            split2(__uint_as_float(v[2 * j]) * s0, __uint_as_float(v[2 * j + 1]) * s1, hi[j], lo[j]);
-          }
-          tmem_st8(x_tmem + lane_addr + col0, hi);
-          if (P > 1) tmem_st8(x_tmem + lane_addr + col0 + 8, lo);
-          sub_arrive(cc);
-        }
-      }
-      TC_STAMP(9);
-
-      // ---------------- EB0: gin (96 cols, kernel order) . input jacobian -> d sdf / dx ; gradient chunk of the colour operand ;
-      //                       h2 planes back into the A operand for colour layer 0
-      // thread (row, q) owns the operand chunks {0,1,4,5,8} (q = 0) / {2,3,6,7} (q = 1): two grid chunks + its share of PE / x
-      // (chunks 9..11 are zero padding).  The jacobian does not depend on this phase's MMA: the first chunk is fetched before the wait.
-      const float* Jpe = reinterpret_cast<const float*>(enc_cur);
-      const float* Jg = Jpe + kPeRows * 128;
-      const int deg = a.pe_degree, half = 3 * deg;
-      float gx = 0.f, gy = 0.f, gz = 0.f;
-      {
-        // the jacobian does not depend on this phase's MMA: every entry is in flight before the wait
-        float jg[48];                       // grid chunks 2q, 2q+1: [col][3]
-        float jp[24];                       // PE / x chunks: 4+2q, 5+2q (and 8 for q = 0): one factor per column
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int cg = q * 16 + j;
-          const bool on = cg < a.grid_dim;
-#pragma unroll
-          for (int d3 = 0; d3 < 3; ++d3) jg[j * 3 + d3] = on ? ld_stream_f1(Jg + (cg * 3 + d3) * 128 + row, pol_keep) : 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 24; ++j) {
-          const int i = j < 16 ? q * 16 + j : 32 + (j - 16);        // PE index (kernel column 32 + i)
-          const bool is_pe = i < a.pe_dim && (j < 16 || q == 0);
-          const int xj = i - a.pe_dim;
-          jp[j] = is_pe ? ld_stream_f1(Jpe + i * 128 + row, pol_keep) : ((xj >= 0 && xj < 3 && (j < 16 || q == 0)) ? 1.f : 0.f);
-        }
-        EPI_WAIT(&dfull, dpar); dpar ^= 1; tc_fence_after();
-        TC_STAMP(10);
-        uint32_t gin_v[8];
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          tmem_ld8(y_tmem + lane_addr + (2 * q + c) * 8, gin_v);
-          tc_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float g = __uint_as_float(gin_v[j]);
-            gx = fmaf(g, jg[(c * 8 + j) * 3 + 0], gx); gy = fmaf(g, jg[(c * 8 + j) * 3 + 1], gy); gz = fmaf(g, jg[(c * 8 + j) * 3 + 2], gz);
-          }
-        }
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          if (c < 2 || q == 0) {
-            const int ck = c < 2 ? 4 + 2 * q + c : 8;
-            tmem_ld8(y_tmem + lane_addr + ck * 8, gin_v);
-            tc_wait_ld();
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int i = ck * 8 + j - 32;
-              // axis of this column: PE column i -> (i mod 3 deg) / deg ; x column -> its own index
-              const int ia = i >= half ? i - half : i;
-              const int ax = i < a.pe_dim ? (ia < deg ? 0 : (ia < 2 * deg ? 1 : 2)) : i - a.pe_dim;
-              const float t = __uint_as_float(gin_v[j]) * jp[c * 8 + j];
-              gx += ax == 0 ? t : 0.f; gy += ax == 1 ? t : 0.f; gz += ax == 2 ? t : 0.f;
-            }
-          }
-        }
-      }
-      red[(0 * 2 + q) * 128 + row] = gx; red[(1 * 2 + q) * 128 + row] = gy; red[(2 * 2 + q) * 128 + row] = gz;
-      // h2 planes back into region X as the A operand of colour layer 0 (B0, whose A operand X held, is complete; the gin columns of Y
-      // have been read above, so C0H may overwrite Y).  Two batches of 8 units (all L2 loads of a batch in flight together); a batch covers
-      // the K groups 2 hb, 2 hb + 1: thread (row, q) brings the units 8 g + 4 q .. + 3 of each group g.
-#pragma unroll 1
-      for (int hb = 0; hb < 2; ++hb) {
-        uint4 gh[8], gl[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int un = 8 * (2 * hb + (u >> 2)) + 4 * q + (u & 3);
-          const size_t unit = ((size_t)un * 128 + row) * 16;
-          gh[u] = ld_stream_u4(gf_s + unit, pol_stream);
-          if (P > 1) gl[u] = ld_stream_u4(gf_s + 65536 + unit, pol_stream);
-        }
-#pragma unroll
-        for (int u = 0; u < 8; u += 2) {
-          const int un = 8 * (2 * hb + (u >> 2)) + 4 * q + (u & 3);      // even: K step un / 2 at columns 16 (un / 2)
-          const uint32_t h8[8] = {gh[u].x, gh[u].y, gh[u].z, gh[u].w, gh[u + 1].x, gh[u + 1].y, gh[u + 1].z, gh[u + 1].w};
-          tmem_st8(x_tmem + lane_addr + (un >> 1) * 16, h8);
-          if (P > 1) {
-            const uint32_t l8[8] = {gl[u].x, gl[u].y, gl[u].z, gl[u].w, gl[u + 1].x, gl[u + 1].y, gl[u + 1].z, gl[u + 1].w};
-            tmem_st8(x_tmem + lane_addr + (un >> 1) * 16 + 8, l8);
-          }
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) sub_arrive(4 * hb + g);
-      }
-      named_sync(2, kEpiThreads);
-      const float grx = red[(0 * 2 + 0) * 128 + row] + red[(0 * 2 + 1) * 128 + row];
-      const float gry = red[(1 * 2 + 0) * 128 + row] + red[(1 * 2 + 1) * 128 + row];
-      const float grz = red[(2 * 2 + 0) * 128 + row] + red[(2 * 2 + 1) * 128 + row];
+      const float dirx = pg.dx, diry = pg.dy, dirz = pg.dz, delta = pg.delta;
+      const float sdf = hs[row], grx = hs[128 + row], gry = hs[256 + row], grz = hs[384 + row];
       const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
       const float nx = grx / gn, ny = gry / gn, nz = grz / gn;
-      if (q == 0) {
-        // chunk 0 of the colour operand: [grad(3), n.v, 0, 0, 0, 0]   (sdf_field.py:572-584; columns re-ordered at pack time)
-        const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? nx * dirx + ny * diry + nz * dirz : 0.f, 0.f, 0.f, 0.f, 0.f};
-        store_chunk<P>(inA, row, 0, c0v);
+      float rgbv[3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float raw = hs[512 + c * 128 + row] + __ldg(b_c2 + c);
+        rgbv[c] = sigmoidf_(raw) * (1.f + 2.f * a.rgb_padding) - a.rgb_padding;
       }
-      // chunk 0 of the colour operand (gradient, n.v) is in shared memory: C0MISC may run
-      fence_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(c0_ready_r);
-      if (warp == 0) TC_STAMP(11);
-
-      // ---------------- EC0: relu -> A planes ----------------
-      EPI_WAIT(&dfull, dpar); dpar ^= 1; tc_fence_after();
-      if (warp == 0) TC_STAMP(12);
-#pragma unroll 1
-      for (int cc = 0; cc < 8; ++cc) {
-        const int col0 = (2 * cc + q) * 16;
-        uint32_t v[16];
-        tmem_ld16(y_tmem + lane_addr + col0, v);
-        tc_wait_ld();
-        uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int j = 0; j < 16; j += 2) {
-          const float2 b2 = *reinterpret_cast<const float2*>(p_bc0 + col0 + j);
-          split2(fmaxf(__uint_as_float(v[j]) + b2.x, 0.f), fmaxf(__uint_as_float(v[j + 1]) + b2.y, 0.f), hi[j >> 1], lo[j >> 1]);
-        }
-        tmem_st8(y_tmem + lane_addr + col0, hi);
-        if (P > 1) tmem_st8(y_tmem + lane_addr + col0 + 8, lo);
-        sub_arrive(cc);
+      float density = 0.f, alpha = 0.f;
+      if (a.out.density || (a.rnd.enabled && a.rnd.from_density)) {
+        const float beta = fabsf(__ldg(a.beta)) + __ldg(a.beta_min);
+        const float sg = sdf > 0.f ? 1.f : (sdf < 0.f ? -1.f : 0.f);
+        density = (1.0f / beta) * (0.5f + 0.5f * sg * expm1f(-fabsf(sdf) / beta));
       }
-      if (warp == 0) TC_STAMP(13);
-
-      // ---------------- EC1: relu, last colour layer (256 -> 3) as fp32 dots ----------------
-      EPI_WAIT(&dfull, dpar); dpar ^= 1; tc_fence_after();
-      if (warp == 0) TC_STAMP(14);
-      {
-        float r0 = 0.f, r1 = 0.f, r2 = 0.f;
-#pragma unroll 1
-        for (int cc = 0; cc < 8; ++cc) {
-          const int col0 = q * 128 + cc * 16;
-          uint32_t v[16];
-          tmem_ld16(x_tmem + lane_addr + col0, v);
-          tc_wait_ld();
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            // broadcast LDS.128: one shared-memory instruction per four columns and operand row instead of one per element
-            const float4 b4 = *reinterpret_cast<const float4*>(p_bc1 + col0 + j);
-            const float4 w0 = *reinterpret_cast<const float4*>(p_wc2 + col0 + j);
-            const float4 w1 = *reinterpret_cast<const float4*>(p_wc2 + 256 + col0 + j);
-            const float4 w2 = *reinterpret_cast<const float4*>(p_wc2 + 512 + col0 + j);
-            const float c0 = fmaxf(__uint_as_float(v[j]) + b4.x, 0.f), c1 = fmaxf(__uint_as_float(v[j + 1]) + b4.y, 0.f);
-            const float c2 = fmaxf(__uint_as_float(v[j + 2]) + b4.z, 0.f), c3 = fmaxf(__uint_as_float(v[j + 3]) + b4.w, 0.f);
-            r0 = fmaf(w0.x, c0, r0); r0 = fmaf(w0.y, c1, r0); r0 = fmaf(w0.z, c2, r0); r0 = fmaf(w0.w, c3, r0);
-            r1 = fmaf(w1.x, c0, r1); r1 = fmaf(w1.y, c1, r1); r1 = fmaf(w1.z, c2, r1); r1 = fmaf(w1.w, c3, r1);
-            r2 = fmaf(w2.x, c0, r2); r2 = fmaf(w2.y, c1, r2); r2 = fmaf(w2.z, c2, r2); r2 = fmaf(w2.w, c3, r2);
-          }
-        }
-        named_sync(2, kEpiThreads);   // everyone has consumed the gradient partials in `red`
-        red[(0 * 2 + q) * 128 + row] = r0; red[(1 * 2 + q) * 128 + row] = r1; red[(2 * 2 + q) * 128 + row] = r2;
+      if (a.out.alpha || (a.rnd.enabled && !a.rnd.from_density)) {
+        const float inv_s = fminf(fmaxf(expf(__ldg(a.variance) * 10.0f), 1e-6f), 1e6f);
+        const float true_cos = dirx * grx + diry * gry + dirz * grz;
+        const float iter_cos = -(fmaxf(-true_cos * 0.5f + 0.5f, 0.f) * (1.0f - a.cos_anneal) + fmaxf(-true_cos, 0.f) * a.cos_anneal);
+        const float prev_cdf = sigmoidf_((sdf - iter_cos * delta * 0.5f) * inv_s), next_cdf = sigmoidf_((sdf + iter_cos * delta * 0.5f) * inv_s);
+        alpha = fminf(fmaxf((prev_cdf - next_cdf + 1e-5f) / (prev_cdf + 1e-5f), 0.f), 1.f);
       }
-      // the accumulator and the A planes are drained: the next tile's G0 may start while the heads / compositing of this tile run
-      if (tp + npairs < a.n_tile_pairs) x_arrive(); else tc_fence_before();
-      named_sync(2, kEpiThreads);
-      if (q == 0) {
-        // ---------------- per-point heads ----------------
-        float rgbv[3];
+      if (valid) {
+        if (a.out.rgb) { a.out.rgb[p * 3] = rgbv[0]; a.out.rgb[p * 3 + 1] = rgbv[1]; a.out.rgb[p * 3 + 2] = rgbv[2]; }
+        if (a.out.gradients) { a.out.gradients[p * 3] = grx; a.out.gradients[p * 3 + 1] = gry; a.out.gradients[p * 3 + 2] = grz; }
+        if (a.out.normals) { a.out.normals[p * 3] = nx; a.out.normals[p * 3 + 1] = ny; a.out.normals[p * 3 + 2] = nz; }
+        if (a.out.density) a.out.density[p] = density;
+        if (a.out.occupancy) a.out.occupancy[p] = sigmoidf_(-10.0f * sdf);
+        if (a.out.alpha) a.out.alpha[p] = alpha;
+      }
+      if (a.rnd.enabled) {
+        // ---------------- fused compositing: the tile holds 128 / S whole rays; row -> (ray, sample) = (row / S, row % S) ----------------
+        const int S = a.n_samples;
+        const int s_idx = row % S;
+        const int rl = row / S;                                   // ray within the tile
+        const bool dens = a.rnd.from_density != 0;
+        // factor by which the transmittance drops across this sample: 1 - alpha + 1e-7 (rays.py:204-206), or as an exponent
+        // delta * sigma for the density form (rays.py:160-170)
+        const float dd = valid ? __fmul_rn(delta, density) : 0.f;
+        double f = dens ? (double)dd : (valid ? (double)__fadd_rn(__fsub_rn(1.0f, alpha), 1e-7f) : 1.0);
+        double incl = f;
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const float raw = (red[(c * 2 + 0) * 128 + row] + red[(c * 2 + 1) * 128 + row]) + __ldg(b_c2 + c);
-          rgbv[c] = sigmoidf_(raw) * (1.f + 2.f * a.rgb_padding) - a.rgb_padding;
+        for (int d = 1; d < 32; d <<= 1) {
+          const double o = __shfl_up_sync(0xffffffffu, incl, d);
+          if (lane >= d && s_idx >= d) incl = dens ? incl + o : incl * o;
         }
-        float density = 0.f, alpha = 0.f;
-        if (a.out.density || (a.rnd.enabled && a.rnd.from_density)) {
-          const float beta = fabsf(__ldg(a.beta)) + __ldg(a.beta_min);
-          const float sg = sdf > 0.f ? 1.f : (sdf < 0.f ? -1.f : 0.f);
-          density = (1.0f / beta) * (0.5f + 0.5f * sg * expm1f(-fabsf(sdf) / beta));
+        double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+        if (lane == 0 || s_idx == 0) excl = dens ? 0.0 : 1.0;
+        if (lane == 31) wtot[wq] = incl;
+        named_sync(4, 128);
+        if (S > 32) {
+          const int first = (wq * 32 / S) * (S / 32);
+          for (int w2 = first; w2 < wq; ++w2) excl = dens ? excl + wtot[w2] : excl * wtot[w2];
         }
-        if (a.out.alpha || (a.rnd.enabled && !a.rnd.from_density)) {
-          const float inv_s = fminf(fmaxf(expf(__ldg(a.variance) * 10.0f), 1e-6f), 1e6f);
-          const float true_cos = dirx * grx + diry * gry + dirz * grz;
-          const float iter_cos = -(fmaxf(-true_cos * 0.5f + 0.5f, 0.f) * (1.0f - a.cos_anneal) + fmaxf(-true_cos, 0.f) * a.cos_anneal);
-          const float prev_cdf = sigmoidf_((sdf - iter_cos * delta * 0.5f) * inv_s), next_cdf = sigmoidf_((sdf + iter_cos * delta * 0.5f) * inv_s);
-          alpha = fminf(fmaxf((prev_cdf - next_cdf + 1e-5f) / (prev_cdf + 1e-5f), 0.f), 1.f);
+        const float T = dens ? expf(-(float)excl) : (float)excl;
+        const float al = dens ? __fsub_rn(1.0f, expf(-dd)) : alpha;
+        const float w = valid ? __fmul_rn(al, T) : 0.f;
+        const float mid = __fdiv_rn(__fadd_rn(pg.t0, pg.t1), 2.0f);            // (starts + ends) / 2, renderers.py:247
+        if (valid && a.rnd.weights) a.rnd.weights[p] = w;
+        float vs[8] = {w, w * rgbv[0], w * rgbv[1], w * rgbv[2], w * nx, w * ny, w * nz, w * mid};
+        float smin = valid ? mid : INFINITY, smax = valid ? mid : -INFINITY;
+        const int span = S < 32 ? S : 32;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          if (d < span) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) vs[k] += __shfl_down_sync(0xffffffffu, vs[k], d);
+          }
+          smin = fminf(smin, __shfl_xor_sync(0xffffffffu, smin, d));
+          smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, d));
         }
-        if (valid) {
-          if (a.out.rgb) { a.out.rgb[p * 3] = rgbv[0]; a.out.rgb[p * 3 + 1] = rgbv[1]; a.out.rgb[p * 3 + 2] = rgbv[2]; }
-          if (a.out.gradients) { a.out.gradients[p * 3] = grx; a.out.gradients[p * 3 + 1] = gry; a.out.gradients[p * 3 + 2] = grz; }
-          if (a.out.normals) { a.out.normals[p * 3] = nx; a.out.normals[p * 3 + 1] = ny; a.out.normals[p * 3 + 2] = nz; }
-          if (a.out.density) a.out.density[p] = density;
-          if (a.out.occupancy) a.out.occupancy[p] = sigmoidf_(-10.0f * sdf);
-          if (a.out.alpha) a.out.alpha[p] = alpha;
+        if (a.rnd.steps_minmax && lane == 0 && smin <= smax) { atomic_min_float(a.rnd.steps_minmax, smin); atomic_max_float(a.rnd.steps_minmax + 1, smax); }
+        if (S > 32) {
+          if (lane == 0) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) atomicAdd(&racc[k * 4 + rl], vs[k]);
+          }
+          if (s_idx == S - 1) { lastrgb[rl * 3] = rgbv[0]; lastrgb[rl * 3 + 1] = rgbv[1]; lastrgb[rl * 3 + 2] = rgbv[2]; }
+          named_sync(4, 128);
+          if (s_idx == 0) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { vs[k] = racc[k * 4 + rl]; racc[k * 4 + rl] = 0.f; }
+          }
         }
-        if (a.rnd.enabled) {
-          // ---------------- fused compositing: the tile holds 128 / S whole rays; row -> (ray, sample) = (row / S, row % S) ----------------
-          const int S = a.n_samples;
-          const int s_idx = row % S;
-          const int rl = row / S;                                   // ray within the tile
-          const bool dens = a.rnd.from_density != 0;
-          // factor by which the transmittance drops across this sample: 1 - alpha + 1e-7 (rays.py:204-206), or as an exponent
-          // delta * sigma for the density form (rays.py:160-170)
-          const float dd = valid ? __fmul_rn(delta, density) : 0.f;
-          double f = dens ? (double)dd : (valid ? (double)__fadd_rn(__fsub_rn(1.0f, alpha), 1e-7f) : 1.0);
-          double incl = f;
+        // transmittance after the last sample (alphas: transmittance[:, -1] = bg_transmittance, neus.py:101) / before it (densities: volsdf.py:67-68)
+        double tot;
+        float lr, lg, lb;
+        if (S > 32) {
+          const int first = (wq * 32 / S) * (S / 32);
+          tot = dens ? 0.0 : 1.0;
+          const int nw = dens ? S / 32 - 1 : S / 32;
+          for (int w2 = first; w2 < first + nw; ++w2) tot = dens ? tot + wtot[w2] : tot * wtot[w2];
+          lr = lastrgb[rl * 3]; lg = lastrgb[rl * 3 + 1]; lb = lastrgb[rl * 3 + 2];
+        } else {
+          const int last = (lane - s_idx) + S - 1;
+          tot = __shfl_sync(0xffffffffu, dens ? excl : incl, last);
+          lr = __shfl_sync(0xffffffffu, rgbv[0], last); lg = __shfl_sync(0xffffffffu, rgbv[1], last); lb = __shfl_sync(0xffffffffu, rgbv[2], last);
+        }
+        if (S > 32 && dens) {
+          // exclusive sum at the last sample of the ray = transmittance exponent before the last sample; it lives in the last warp of the ray
+          if (s_idx == S - 1) wtot[wq] = excl;       // (wtot of the ray's last warp is no longer needed by anyone else)
+          named_sync(4, 128);
+          tot = wtot[(wq * 32 / S) * (S / 32) + S / 32 - 1];
+        }
+        const long long ray = (long long)tile * (128 / S) + rl;
+        if (s_idx == 0 && ray * S < a.n_points) {
+          const float acc = vs[0];
+          if (a.rnd.rgb) {
+            float bgc[3] = {0.f, 0.f, 0.f};
+            if (a.rnd.bg_mode == SDFB200_BG_COLOR) { bgc[0] = a.rnd.bg[0]; bgc[1] = a.rnd.bg[1]; bgc[2] = a.rnd.bg[2]; }
+            else if (a.rnd.bg_mode == SDFB200_BG_PER_RAY) { bgc[0] = a.rnd.bg[ray * 3]; bgc[1] = a.rnd.bg[ray * 3 + 1]; bgc[2] = a.rnd.bg[ray * 3 + 2]; }
+            else { bgc[0] = lr; bgc[1] = lg; bgc[2] = lb; }
+            const float rem = 1.0f - acc;
+            const float o[3] = {vs[1] + bgc[0] * rem, vs[2] + bgc[1] * rem, vs[3] + bgc[2] * rem};
 #pragma unroll
-          for (int d = 1; d < 32; d <<= 1) {
-            const double o = __shfl_up_sync(0xffffffffu, incl, d);
-            if (lane >= d && s_idx >= d) incl = dens ? incl + o : incl * o;
+            for (int c = 0; c < 3; ++c) a.rnd.rgb[ray * 3 + c] = a.rnd.clamp01 ? fminf(fmaxf(o[c], 0.f), 1.f) : o[c];
           }
-          double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-          if (lane == 0 || s_idx == 0) excl = dens ? 0.0 : 1.0;
-          if (lane == 31) wtot[wq] = incl;
-          named_sync(3, 128);
-          if (S > 32) {
-            const int first = (wq * 32 / S) * (S / 32);
-            for (int w2 = first; w2 < wq; ++w2) excl = dens ? excl + wtot[w2] : excl * wtot[w2];
-          }
-          const float T = dens ? expf(-(float)excl) : (float)excl;
-          const float al = dens ? __fsub_rn(1.0f, expf(-dd)) : alpha;
-          const float w = valid ? __fmul_rn(al, T) : 0.f;
-          const float mid = __fdiv_rn(__fadd_rn(pg.t0, pg.t1), 2.0f);            // (starts + ends) / 2, renderers.py:247
-          if (valid && a.rnd.weights) a.rnd.weights[p] = w;
-          float vs[8] = {w, w * rgbv[0], w * rgbv[1], w * rgbv[2], w * nx, w * ny, w * nz, w * mid};
-          float smin = valid ? mid : INFINITY, smax = valid ? mid : -INFINITY;
-          const int span = S < 32 ? S : 32;
-#pragma unroll
-          for (int d = 1; d < 32; d <<= 1) {
-            if (d < span) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k) vs[k] += __shfl_down_sync(0xffffffffu, vs[k], d);
-            }
-            smin = fminf(smin, __shfl_xor_sync(0xffffffffu, smin, d));
-            smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, d));
-          }
-          if (a.rnd.steps_minmax && lane == 0 && smin <= smax) { atomic_min_float(a.rnd.steps_minmax, smin); atomic_max_float(a.rnd.steps_minmax + 1, smax); }
-          if (S > 32) {
-            if (lane == 0) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k) atomicAdd(&racc[k * 4 + rl], vs[k]);
-            }
-            if (s_idx == S - 1) { lastrgb[rl * 3] = rgbv[0]; lastrgb[rl * 3 + 1] = rgbv[1]; lastrgb[rl * 3 + 2] = rgbv[2]; }
-            named_sync(3, 128);
-            if (s_idx == 0) {
-#pragma unroll
-              for (int k = 0; k < 8; ++k) { vs[k] = racc[k * 4 + rl]; racc[k * 4 + rl] = 0.f; }
-            }
-          }
-          // transmittance after the last sample (alphas: transmittance[:, -1] = bg_transmittance, neus.py:101) / before it (densities: volsdf.py:67-68)
-          double tot;
-          float lr, lg, lb;
-          if (S > 32) {
-            const int first = (wq * 32 / S) * (S / 32);
-            tot = dens ? 0.0 : 1.0;
-            const int nw = dens ? S / 32 - 1 : S / 32;
-            for (int w2 = first; w2 < first + nw; ++w2) tot = dens ? tot + wtot[w2] : tot * wtot[w2];
-            lr = lastrgb[rl * 3]; lg = lastrgb[rl * 3 + 1]; lb = lastrgb[rl * 3 + 2];
-          } else {
-            const int last = (lane - s_idx) + S - 1;
-            tot = __shfl_sync(0xffffffffu, dens ? excl : incl, last);
-            lr = __shfl_sync(0xffffffffu, rgbv[0], last); lg = __shfl_sync(0xffffffffu, rgbv[1], last); lb = __shfl_sync(0xffffffffu, rgbv[2], last);
-          }
-          if (S > 32 && dens) {
-            // exclusive sum at the last sample of the ray = transmittance exponent before the last sample; it lives in the last warp of the ray
-            if (s_idx == S - 1) wtot[wq] = excl;       // (wtot of the ray's last warp is no longer needed by anyone else)
-            named_sync(3, 128);
-            tot = wtot[(wq * 32 / S) * (S / 32) + S / 32 - 1];
-          }
-          const long long ray = (long long)tile * (128 / S) + rl;
-          if (s_idx == 0 && ray * S < a.n_points) {
-            const float acc = vs[0];
-            if (a.rnd.rgb) {
-              float bgc[3] = {0.f, 0.f, 0.f};
-              if (a.rnd.bg_mode == SDFB200_BG_COLOR) { bgc[0] = a.rnd.bg[0]; bgc[1] = a.rnd.bg[1]; bgc[2] = a.rnd.bg[2]; }
-              else if (a.rnd.bg_mode == SDFB200_BG_PER_RAY) { bgc[0] = a.rnd.bg[ray * 3]; bgc[1] = a.rnd.bg[ray * 3 + 1]; bgc[2] = a.rnd.bg[ray * 3 + 2]; }
-              else { bgc[0] = lr; bgc[1] = lg; bgc[2] = lb; }
-              const float rem = 1.0f - acc;
-              const float o[3] = {vs[1] + bgc[0] * rem, vs[2] + bgc[1] * rem, vs[3] + bgc[2] * rem};
-#pragma unroll
-              for (int c = 0; c < 3; ++c) a.rnd.rgb[ray * 3 + c] = a.rnd.clamp01 ? fminf(fmaxf(o[c], 0.f), 1.f) : o[c];
-            }
-            if (a.rnd.accumulation) a.rnd.accumulation[ray] = acc;
-            if (a.rnd.normal) { a.rnd.normal[ray * 3] = vs[4]; a.rnd.normal[ray * 3 + 1] = vs[5]; a.rnd.normal[ray * 3 + 2] = vs[6]; }
-            if (a.rnd.depth) a.rnd.depth[ray] = vs[7] / (acc + 1e-10f);
-            if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)tot) : (float)tot;
-          }
+          if (a.rnd.accumulation) a.rnd.accumulation[ray] = acc;
+          if (a.rnd.normal) { a.rnd.normal[ray * 3] = vs[4]; a.rnd.normal[ray * 3 + 1] = vs[5]; a.rnd.normal[ray * 3 + 2] = vs[6]; }
+          if (a.rnd.depth) a.rnd.depth[ray] = vs[7] / (acc + 1e-10f);
+          if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)tot) : (float)tot;
         }
       }
-      named_sync(2, kEpiThreads);     // `red` / `racc` are rewritten by the next tile
-      if (warp == 0) TC_STAMP(15);
     }
-    tc_fence_before();
+    named_sync(3, kEpiThreads);     // `hs` / `racc` are rewritten by the next tile
+    TC_STAMP(15);
   }
-  __syncthreads();
-  cluster_sync_all();                 // no CTA of the pair may release its TMEM / exit while the other one's MMAs could still touch it
-  if (warp == 0) tmem_dealloc2<512>(tmem);
+#undef SYNC_A
+#undef LAYER
 }
-
 
 template <int P, int LAYOUT>
 static int launch_field_tc(const TcArgs& a, int grid, size_t smem, cudaStream_t st) {

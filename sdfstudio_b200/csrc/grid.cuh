@@ -62,7 +62,7 @@ struct TableLoad<__half, F> {
 };
 
 // L2 eviction-priority policies (createpolicy): the hash table is re-read by every tile -> evict_last; streaming
-// scratch of the fused kernel -> evict_first, so that it does not push the table out of the 126 MB L2.
+// scratch -> evict_first, so that it pushes as little of the table out of L2 as possible.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));

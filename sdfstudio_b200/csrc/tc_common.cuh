@@ -1,11 +1,12 @@
-// sm_100a primitives used by the tensor-core field kernel: mbarrier, 1-D bulk async copy (TMA engine, UBLKCP),
-// tcgen05 alloc / mma (SS and TS) / commit / ld / st / fences, UMMA shared-memory + instruction descriptors.
+// sm_90a primitives of the tensor-core kernels: mbarrier, 1-D bulk async copy (TMA engine), wgmma (warpgroup MMA with the
+// accumulator in registers, A from shared memory or registers, B from shared memory) and its shared-memory descriptors.
 //
-// Operand layout convention (both A-in-smem and B): the canonical K-major NO-SWIZZLE layout
+// Operand layout convention (A in smem and B): the canonical K-major NO-SWIZZLE layout
 //     element (row r, k)  ->  byte  (k/8) * LBO + (r/8) * SBO + (r%8) * 16 + (k%8) * 2        (bf16)
 // with SBO = 128 (8 rows x 16 B, i.e. rows are consecutive 16-byte units) and LBO = rows * 16.
-// So a tile is stored as [k-chunk of 8][row][8 bf16]; advancing one UMMA K step (16) moves the start by 2*LBO.
-// Weights are pre-packed in global memory in exactly this order, so a stage is filled by one 1-D bulk copy.
+// So a tile is stored as [k-chunk of 8][row][8 bf16]; advancing one MMA K step (16) moves the start by 2*LBO, advancing 64 rows
+// (one m64 / n64 block) moves it by 1024 bytes.  Weights are pre-packed in global memory in exactly this order, so a stage is
+// filled by one 1-D bulk copy.
 #pragma once
 #include "common.cuh"
 
@@ -52,142 +53,69 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// make generic-proxy writes to shared memory visible to the async proxy (UMMA operand reads)
+// make generic-proxy writes to shared memory visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- tcgen05 ----------------------------------------------------------------------------------------------------
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]          (kind::f16: bf16 x bf16 -> fp32)
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// ---- wgmma (warpgroup MMA, sm_90a) -------------------------------------------------------------------------------
+// All 128 threads of a warpgroup issue these together.  The accumulator lives in registers; for m64nN thread t of the warpgroup
+// holds rows 16 (t/32) + (t%32)/4 (+8) and, per 8-column block j, columns 8 j + 2 (t%4) (+1):
+//     d[4 j + 2 h + e]  =  D(row 16 (t/32) + (t%32)/4 + 8 h, column 8 j + 2 (t%4) + e)
+__device__ __forceinline__ void wg_arrive() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs (cute::warpgroup_fence_operand)
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32-bit, 16 consecutive columns: thread t of warp w gets TMEM lane 32*(w%4)+t, columns [col, col+16)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+// D[64 x 64] += A[smem desc, 64 x 16] * B[smem desc, 64 x 16]^T   (bf16 x bf16 -> fp32, both K-major)
+__device__ __forceinline__ void wgmma64_ss(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-        "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(1)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-               "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-
-
-// ---- CTA pairs (cluster of 2, tcgen05 cta_group::2) ---------------------------------------------------------------
-// One MMA covers M = 256 rows: 128 from each CTA of the pair (its own A operand, its own accumulator in its own TMEM, lane = row)
-// and N columns whose B operand is split in halves: rows [0, N/2) of the weight tile come from the leader CTA's shared memory,
-// rows [N/2, N) from the peer's -- each CTA streams only half of the weights.  Only the leader (cluster rank 0) issues MMAs;
-// completion is multicast to the mbarriers of both CTAs.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> shared::cluster address of the same variable in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-// Arrive on an mbarrier of another CTA of the cluster.  Default (.release.cta) semantics, like cutlass::arch::ClusterBarrier::arrive:
-// what crosses the CTA boundary here is tensor memory (ordered by tcgen05.fence::before/after_thread_sync around the barrier) and
-// shared memory read by the async proxy (fence.proxy.async before the arrive) -- no global-memory hand-off needs cluster scope.
-// (.release.cluster / .acquire.cluster make ptxas emit a full memory barrier per arrive and an L1 invalidation, CCTL.IVALL, per
-// wait: measured as membar stalls and a 13 % L1 hit rate for the coarse hash levels.)
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void mma_ss2(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 64] += A[registers, 64 x 16] * B[smem desc, 64 x 16]^T.  a: the m16n8k16-style fragment of the thread's rows
+// (a[0] = (r, 2c..2c+1), a[1] = (r+8, 2c..), a[2] = (r, 2c+8..), a[3] = (r+8, 2c+8..), r = 16 (t/32) + (t%32)/4, c = t%4)
+__device__ __forceinline__ void wgmma64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1)
       : "memory");
-}
-__device__ __forceinline__ void mma_ts2(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the mbarrier at this shared-memory offset in BOTH CTAs of the pair once all previously issued MMAs have completed
-__device__ __forceinline__ void mma_commit2(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"(mask)
-               : "memory");
 }
 
 // ---- descriptors -------------------------------------------------------------------------------------------------
-// shared-memory matrix descriptor, K-major, no swizzle (cute::UMMA::SmemDescriptor, version 1)
+// wgmma shared-memory matrix descriptor, K-major, no swizzle (layout type 0): LBO = byte distance between the two 8 x 16-byte core
+// matrices of one K step (K direction), SBO = byte distance between 8-row groups (M / N direction)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  return d;                // base_offset = 0, lbo_mode = 0, layout_type = SWIZZLE_NONE (0)
+  return d;                // base_offset = 0, layout_type = SWIZZLE_NONE (0)
 }
-// instruction descriptor for kind::f16, A = B = bf16, D = fp32, both K-major (cute::UMMA::InstrDescriptor)
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) /* D fp32 */ | (1u << 7) /* A bf16 */ | (1u << 10) /* B bf16 */ | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+
+// one K step (16) of a 64-row warpgroup tile against NCH 64-row blocks of B, bf16 (P = 1) or bf16x3 (P = 2: a0 w0 + a1 w0 + a0 w1):
+// a0 / a1 = descriptors of the A planes, b_addr = shared address of plane 0 of B at this K step, b_plane = byte distance of plane 1,
+// lbo_b = B's K-direction core-matrix stride.  Only the first nch (<= NCH, warp-uniform) blocks are issued.
+template <int P, int NCH>
+__device__ __forceinline__ void wgmma_kstep_ss(float (&acc)[NCH][32], uint64_t a0, uint64_t a1, uint32_t b_addr, uint32_t b_plane, uint32_t lbo_b, int nch) {
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+    if (c < nch) {
+      const uint64_t b0 = make_smem_desc(b_addr + c * 1024, lbo_b, 128);
+      wgmma64_ss(acc[c], a0, b0);
+      if (P > 1) {
+        wgmma64_ss(acc[c], a1, b0);
+        wgmma64_ss(acc[c], a0, make_smem_desc(b_addr + b_plane + c * 1024, lbo_b, 128));
+      }
+    }
+  }
 }
 
 // ---- streaming (evict_first) global accesses for the per-CTA scratch ------------------------------------------------

@@ -1,10 +1,9 @@
 // Generic tensor-core Linear for the field shapes the fused kernel does not cover (bakedsdf / angelo / stock volsdf ...):
 //   Y[M, n0:n0+Nc] = epi( X[M, k0:k0+Kc] * W[n0:n0+Nc, k0:k0+Kc]^T (+ partial sums) + bias )
-// One CTA per 128-row tile, the machinery of the fused field kernel (and of the sdfb200_debug_tc_gemm building-block test):
-// 16 warps stage the fp32 activations as bf16 split planes straight into TMEM (A operand, TS mode; two 128-column halves, the MMAs of the
-// first half run while the second is staged), one warp streams the
-// pre-packed weight K-blocks through a 3-stage shared-memory ring with 1-D bulk copies, one thread issues tcgen05.mma (bf16x3 =
-// a0 w0 + a1 w0 + a0 w1, fp32 accumulate in TMEM), the 16 warps read D back and apply the epilogue of k_sgemm (field_simt.cu).
+// One CTA per 128-row tile: two warpgroups (64 rows each) stage the fp32 activations as bf16 split planes in shared memory, one warp
+// streams the pre-packed weight K-blocks through a 2-stage shared-memory ring with 1-D bulk copies, and each warpgroup runs wgmma
+// m64n64k16 over its rows (bf16x3 = a0 w0 + a1 w0 + a0 w1, fp32 accumulate in registers), then applies the epilogue of k_sgemm
+// (field_simt.cu) straight from the accumulator registers.
 // K > 256 / N > 256 are chunked by the host wrapper (partial sums round-trip through Y).
 #include "tc_common.cuh"
 #include "tc_linear.h"
@@ -14,14 +13,10 @@ using namespace tc;
 
 namespace {
 constexpr int kKBL = 32;          // K per streamed weight block
-constexpr int kStagesL = 3;
-constexpr int kThreadsL = 576;    // 16 staging / epilogue warps + weight producer + MMA issuer
-constexpr int kEpiL = 512;
-constexpr int kLdS = 132;                                  // padded row stride (floats) of the transposition tile
+constexpr int kStagesL = 2;
+constexpr int kThreadsL = 288;    // two MMA / epilogue warpgroups + weight producer
+constexpr uint32_t kAPlaneL = 32 * 2048;                          // one plane of the A operand: [K/8 (<= 32)][128 rows][16 B]
 constexpr uint32_t kRingBytesL = kStagesL * 2 * 256 * kKBL * 2;   // weight ring at its largest (2 planes, N = 256)
-constexpr uint32_t kStageTileBytesL = 128 * kLdS * 4;
-
-__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // softplus_100 / its derivative through MUFU ex2 / lg2 (same formulas as the fused kernel, field_tc.cu): ~10 instructions instead of
 // the ~100 of log1pf(expf(.)) -- at 64 elements per thread the accurate versions cost more than the tensor-core GEMM they follow
@@ -53,7 +48,7 @@ __global__ void k_tcl_pack(const float* __restrict__ W, int ldw, int N, int K, i
 struct LinArgs {
   const float* X; int ldx; long long M;
   int Kc32, Kvalid;                 // K of this chunk rounded up to 32 / columns of X actually present
-  const __nv_bfloat16* Wp; int Ncp; // packed weights of this chunk, N of this chunk (multiple of 16, <= 256)
+  const __nv_bfloat16* Wp; int Ncp, Np64;   // packed weights of this chunk (Np64 rows), N of this chunk (multiple of 16, <= 256)
   const float* bias;                // already offset by n0 (may be NULL)
   float* Y; int ldy; int n0;
   int accumulate, final_chunk;      // add the partial sums already in Y / apply bias + activation
@@ -63,185 +58,113 @@ struct LinArgs {
 template <int P, int EPI>
 __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t full[kStagesL], empty[kStagesL], dfull;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t full[kStagesL], empty[kStagesL];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nblocks = a.Kc32 / kKBL;
-  const uint32_t stage_bytes = (uint32_t)P * a.Ncp * kKBL * 2;
+  const uint32_t stage_bytes = (uint32_t)P * a.Np64 * kKBL * 2;
+  uint8_t* a_smem = smem;                               // [P][K/8][128][16 B]
+  uint8_t* ring = smem + P * kAPlaneL;
+  const long long m0 = (long long)blockIdx.x * 128;
   if (tid == 0) {
-    for (int s = 0; s < kStagesL; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(&dfull, 1);
+    for (int s = 0; s < kStagesL; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc<512>(&tmem_base_s);
-  tc_fence_before();
+  if (tid < 256) {
+    // stage A: thread (row, chunk) converts 8 consecutive columns of one row (rows fastest: conflict-free 16-byte smem stores)
+    const int chunks = a.Kc32 / 8;
+    for (int u = tid; u < chunks * 128; u += 256) {
+      const int r = u & 127, ch = u >> 7, k = ch * 8;
+      const long long m = m0 + r;
+      float v[8];
+      if (m < a.M && k + 8 <= a.Kvalid) {
+        const float4 x0 = __ldg(reinterpret_cast<const float4*>(a.X + m * (long long)a.ldx + k));
+        const float4 x1 = __ldg(reinterpret_cast<const float4*>(a.X + m * (long long)a.ldx + k + 4));
+        v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
+      } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) v[e] = (m < a.M && k + e < a.Kvalid) ? __ldg(a.X + m * (long long)a.ldx + k + e) : 0.f;
+      }
+      uint32_t hi[4], lo[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hi[e], lo[e]);
+      *reinterpret_cast<uint4*>(a_smem + (size_t)ch * 2048 + r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+      if (P > 1) *reinterpret_cast<uint4*>(a_smem + kAPlaneL + (size_t)ch * 2048 + r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    }
+    fence_async_smem();
+  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
-  const uint32_t d_tmem = tmem;             // accumulator: columns [0, 256)
-  const uint32_t a_tmem = tmem + 256;       // A plane p at columns 256 + 128 p
-  const long long m0 = (long long)blockIdx.x * 128;
 
-  if (warp == 16) {
+  if (warp == 8) {
     // ---------------- weight producer ----------------
     if (lane == 0) {
       for (int b = 0; b < nblocks; ++b) {
         const int s = b % kStagesL;
         mbar_wait(&empty[s], ((b / kStagesL) & 1) ^ 1);
         mbar_arrive_expect_tx(&full[s], stage_bytes);
-        bulk_g2s(smem + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(a.Wp) + (size_t)b * stage_bytes, stage_bytes, &full[s]);
+        bulk_g2s(ring + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(a.Wp) + (size_t)b * stage_bytes, stage_bytes, &full[s]);
       }
     }
-  } else if (warp == 17) {
-    // ---------------- MMA issuer ----------------
-    // the A operand is staged in two 128-column halves: the MMAs of the first four K blocks run while the second half is still being
-    // converted (barrier 1: columns [0,128) staged, barrier 3: columns [128,256) staged)
-    bar_sync(1, kEpiL + 32);
-    tc_fence_after();
-    {
-      const uint32_t idesc = make_idesc_bf16(128, a.Ncp);
-      const uint32_t lbo_b = (uint32_t)a.Ncp * 16, plane_b = (uint32_t)a.Ncp * kKBL * 2;
-      uint32_t acc = 0;
-      for (int b = 0; b < nblocks; ++b) {
-        if (b == 128 / kKBL) {               // warp-uniform: the whole warp takes part in the named barrier (reconverge first: bar.sync is .aligned)
-          __syncwarp();
-          bar_sync(3, kEpiL + 32);
-          tc_fence_after();
-        }
-        if (lane != 0) continue;
-        const int s = b % kStagesL;
-        mbar_wait(&full[s], (b / kStagesL) & 1);
-        tc_fence_after();
-        const uint32_t wbase = smem_u32(smem + (size_t)s * stage_bytes);
-#pragma unroll
-        for (int j = 0; j < kKBL / 16; ++j) {
-          const int kstep = b * (kKBL / 16) + j;
-          const uint64_t b0 = make_smem_desc(wbase + j * 2 * lbo_b, lbo_b, 128);
-          mma_ts(d_tmem, a_tmem + kstep * 8, b0, idesc, acc);
-          acc = 1;
-          if (P > 1) {
-            const uint64_t b1 = make_smem_desc(wbase + plane_b + j * 2 * lbo_b, lbo_b, 128);
-            mma_ts(d_tmem, a_tmem + 128 + kstep * 8, b0, idesc, 1);
-            mma_ts(d_tmem, a_tmem + kstep * 8, b1, idesc, 1);
-          }
-        }
-        mma_commit(&empty[s]);
-      }
-      if (lane == 0) mma_commit(&dfull);
-    }
-  } else {
-    // ---------------- 16 warps: stage A, then the epilogue ----------------
-    // Global memory is touched with one row per warp instruction (32 lanes x 16 contiguous bytes); the transposition to the
-    // "lane = row" view that tcgen05.st / tcgen05.ld need goes through a padded shared-memory tile (row stride kLdS floats:
-    // conflict-free for both access patterns).  A row-per-lane global pattern costs 32 L1 wavefronts per instruction instead of 4.
-    float* stg = reinterpret_cast<float*>(smem + kRingBytesL);
-    const int row = (warp & 3) * 32 + lane;               // tile row == TMEM lane
-    const int q = warp >> 2;
-    const uint32_t lane_addr = (uint32_t)((warp & 3) * 32) << 16;
-    // register double buffer: the 8 row loads of the NEXT 128-column half are in flight while the current half is converted
-    float4 t[8];
-    auto load_half = [&](int kbase) {
-      const int kcols = a.Kc32 - kbase < 128 ? a.Kc32 - kbase : 128;
-      const int k = kbase + lane * 4;
-      const bool colok = lane * 4 < kcols && k < a.Kvalid;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const long long m = m0 + warp + 16 * i;
-        t[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (colok && m < a.M) t[i] = __ldg(reinterpret_cast<const float4*>(a.X + m * (long long)a.ldx + k));
-      }
-    };
-    load_half(0);
-    for (int kbase = 0; kbase < a.Kc32; kbase += 128) {
-      const int kcols = a.Kc32 - kbase < 128 ? a.Kc32 - kbase : 128;          // multiple of 32
-#pragma unroll
-      for (int i = 0; i < 8; ++i) *reinterpret_cast<float4*>(stg + (warp + 16 * i) * kLdS + lane * 4) = t[i];
-      if (kbase + 128 < a.Kc32) load_half(kbase + 128);
-      bar_sync(2, kEpiL);
-      for (int g = q; g < kcols / 16; g += 4) {
-        float v[16];
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          const float4 u = *reinterpret_cast<const float4*>(stg + row * kLdS + g * 16 + j4 * 4);
-          v[j4 * 4] = u.x; v[j4 * 4 + 1] = u.y; v[j4 * 4 + 2] = u.z; v[j4 * 4 + 3] = u.w;
-        }
-        uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) split2(v[2 * j], v[2 * j + 1], hi[j], lo[j]);
-        tmem_st8(a_tmem + lane_addr + kbase / 2 + g * 8, hi);
-        if (P > 1) tmem_st8(a_tmem + 128 + lane_addr + kbase / 2 + g * 8, lo);
-      }
-      // this half of the A operand is in TMEM: hand it to the MMA issuer (which also orders the reuse of the transposition tile)
-      tc_wait_st();
-      tc_fence_before();
-      bar_sync(kbase == 0 ? 1 : 3, kEpiL + 32);
-    }
-    mbar_wait_backoff(&dfull, 0);
-    tc_fence_after();
-    for (int nbase = 0; nbase < a.Ncp; nbase += 128) {
-      const int ncols = a.Ncp - nbase < 128 ? a.Ncp - nbase : 128;            // multiple of 16
-      for (int g = q; g < ncols / 16; g += 4) {
-        uint32_t v[16];
-        tmem_ld16(d_tmem + lane_addr + nbase + g * 16, v);
-        tc_wait_ld();
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4)
-          *reinterpret_cast<float4*>(stg + row * kLdS + g * 16 + j4 * 4) =
-              make_float4(__uint_as_float(v[j4 * 4]), __uint_as_float(v[j4 * 4 + 1]), __uint_as_float(v[j4 * 4 + 2]), __uint_as_float(v[j4 * 4 + 3]));
-      }
-      bar_sync(2, kEpiL);
-      if (lane * 4 < ncols) {
-        const int n = nbase + lane * 4;                     // column inside this N chunk
-        float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (a.final_chunk && EPI != TCL_MUL_DSOFTPLUS && a.bias != nullptr) bv = __ldg(reinterpret_cast<const float4*>(a.bias + n));
-        const float b4[4] = {bv.x, bv.y, bv.z, bv.w};
-        // operands that come from global memory (previous partial sums, softplus' source) are fetched for all 8 rows of this warp first
-        const bool want_aux = a.final_chunk && EPI == TCL_MUL_DSOFTPLUS && a.n0 + n < a.aux_cols;
-        float4 pv[8], hv[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const long long m = m0 + warp + 16 * i;
-          pv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          hv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (m < a.M) {
-            if (a.accumulate) pv[i] = *reinterpret_cast<const float4*>(a.Y + m * (long long)a.ldy + a.n0 + n);
-            if (want_aux) hv[i] = __ldg(reinterpret_cast<const float4*>(a.aux + m * (long long)a.ldaux + a.n0 + n));
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int r = warp + 16 * i;
-          const long long m = m0 + r;
-          if (m < a.M) {
-            const float4 d4 = *reinterpret_cast<const float4*>(stg + r * kLdS + lane * 4);
-            float y[4] = {d4.x + pv[i].x, d4.y + pv[i].y, d4.z + pv[i].z, d4.w + pv[i].w};
-            if (a.final_chunk) {
-              if (EPI == TCL_MUL_DSOFTPLUS) {
-                if (want_aux) {
-                  const float hh[4] = {hv[i].x, hv[i].y, hv[i].z, hv[i].w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j)
-                    if (a.n0 + n + j < a.aux_cols) y[j] *= tcl_dsoftplus_from_h(hh[j]);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  y[j] += b4[j];
-                  if (EPI == TCL_SOFTPLUS) y[j] = tcl_softplus100(y[j]);
-                  if (EPI == TCL_RELU) y[j] = fmaxf(y[j], 0.f);
-                }
-              }
-            }
-            *reinterpret_cast<float4*>(a.Y + m * (long long)a.ldy + a.n0 + n) = make_float4(y[0], y[1], y[2], y[3]);
-          }
-        }
-      }
-      bar_sync(2, kEpiL);
-    }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<512>(tmem);
+  // ---------------- two warpgroups: MMAs over 64 rows each, then the epilogue from the accumulator registers ----------------
+  const int wg = warp >> 2, t = tid & 127;
+  const int rw = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c2 = (t & 3) * 2;      // first of the thread's two rows (+8), column offset
+  const int nch = a.Np64 / 64;
+  float acc[4][32];
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+  const uint32_t lbo_b = (uint32_t)a.Np64 * 16, plane_b = (uint32_t)a.Np64 * kKBL * 2;
+  const uint32_t abase = smem_u32(a_smem) + wg * 64 * 16;
+  for (int b = 0; b < nblocks; ++b) {
+    const int s = b % kStagesL;
+    mbar_wait(&full[s], (b / kStagesL) & 1);
+    const uint32_t wbase = smem_u32(ring + (size_t)s * stage_bytes);
+    wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+    wg_arrive();
+#pragma unroll
+    for (int j = 0; j < kKBL / 16; ++j) {
+      const int kstep = b * (kKBL / 16) + j;
+      const uint64_t a0 = make_smem_desc(abase + kstep * 2 * 2048, 2048, 128);
+      const uint64_t a1 = make_smem_desc(abase + kAPlaneL + kstep * 2 * 2048, 2048, 128);
+      wgmma_kstep_ss<P, 4>(acc, a0, a1, wbase + j * 2 * lbo_b, plane_b, lbo_b, nch);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+    if (t == 0) mbar_arrive(&empty[s]);
+  }
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int n = c * 64 + (i >> 2) * 8 + c2;           // column inside this N chunk (even; n + 1 < Ncp when n < Ncp)
+      const long long m = m0 + rw + 8 * ((i >> 1) & 1);
+      if (c < nch && n < a.Ncp && m < a.M) {
+        float y[2] = {acc[c][i], acc[c][i + 1]};
+        float2* yp = reinterpret_cast<float2*>(a.Y + m * (long long)a.ldy + a.n0 + n);
+        if (a.accumulate) { const float2 pv = *yp; y[0] += pv.x; y[1] += pv.y; }
+        if (a.final_chunk) {
+          if (EPI == TCL_MUL_DSOFTPLUS) {
+#pragma unroll
+            for (int j = 0; j < 2; ++j)
+              if (a.n0 + n + j < a.aux_cols) y[j] *= tcl_dsoftplus_from_h(__ldg(a.aux + m * (long long)a.ldaux + a.n0 + n + j));
+          } else {
+            const float2 bv = a.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(a.bias + n)) : make_float2(0.f, 0.f);
+            const float b2[2] = {bv.x, bv.y};
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              y[j] += b2[j];
+              if (EPI == TCL_SOFTPLUS) y[j] = tcl_softplus100(y[j]);
+              if (EPI == TCL_RELU) y[j] = fmaxf(y[j], 0.f);
+            }
+          }
+        }
+        *yp = make_float2(y[0], y[1]);
+      }
+    }
+  }
 }
 
 template <int P>
@@ -282,17 +205,18 @@ int tc_gemm_ex(int planes, int epi, const float* X, int ldx, const float* W, int
     for (int k0 = 0; k0 < Kp; k0 += 256) {
       const int Kc = Kp - k0 < 256 ? Kp - k0 : 256;
       const int Kc32 = (Kc + 31) / 32 * 32, nblocks = Kc32 / kKBL;
-      const int tot = nblocks * Nc * kKBL;
+      const int Np64 = (Nc + 63) / 64 * 64;
+      const int tot = nblocks * Np64 * kKBL;
       const float* wsrc = trans_w ? W + (size_t)k0 * ldw + n0 : W + (size_t)n0 * ldw + k0;
       const int nv = Nw - n0 < Nc ? (Nw - n0 > 0 ? Nw - n0 : 0) : Nc, kv = Kw - k0 < Kc ? (Kw - k0 > 0 ? Kw - k0 : 0) : Kc;
-      k_tcl_pack<<<(tot + 255) / 256, 256, 0, st>>>(wsrc, ldw, nv, kv, Nc, nblocks, planes, trans_w, (__nv_bfloat16*)scratch);
+      k_tcl_pack<<<(tot + 255) / 256, 256, 0, st>>>(wsrc, ldw, nv, kv, Np64, nblocks, planes, trans_w, (__nv_bfloat16*)scratch);
       SDFB_LAUNCHED("k_tcl_pack");
       LinArgs a;
-      a.X = X + k0; a.ldx = ldx; a.M = M; a.Kc32 = Kc32; a.Kvalid = kv; a.Wp = (const __nv_bfloat16*)scratch; a.Ncp = Nc;
+      a.X = X + k0; a.ldx = ldx; a.M = M; a.Kc32 = Kc32; a.Kvalid = kv; a.Wp = (const __nv_bfloat16*)scratch; a.Ncp = Nc; a.Np64 = Np64;
       a.bias = bias ? bias + n0 : nullptr; a.Y = Y; a.ldy = ldy; a.n0 = n0; a.accumulate = k0 > 0; a.final_chunk = k0 + 256 >= Kp;
       a.aux = aux; a.ldaux = ldaux; a.aux_cols = aux_cols;
       if (epi != TCL_MUL_DSOFTPLUS && epi != TCL_NONE) SDFB_REQUIRE(bias != nullptr, "tc_gemm: bias is NULL");
-      const size_t smem = (size_t)kRingBytesL + kStageTileBytesL + 1024;
+      const size_t smem = (size_t)planes * kAPlaneL + kRingBytesL + 1024;
       const int r = planes == 2 ? launch_linear<2>(epi, a, smem, grid, st) : launch_linear<1>(epi, a, smem, grid, st);
       if (r) return r;
     }

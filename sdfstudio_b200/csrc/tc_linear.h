@@ -1,4 +1,4 @@
-// Generic tcgen05 Linear (csrc/tc_linear.cu): drop-in for sgemm() of field_simt.cu when the field runs at a tensor-core precision
+// Generic tensor-core Linear (csrc/tc_linear.cu): drop-in for sgemm() of field_simt.cu when the field runs at a tensor-core precision
 // but its shape is outside the fused kernel's family.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
-// Building-block test of the tcgen05 path (sdfb200_debug_tc_gemm): one CTA computes D[128,N] = A[128,K] * W[N,K]^T with
-// the exact machinery the fused field kernel uses -- bf16 split planes, canonical no-swizzle K-major operands, A either in
-// shared memory (SS) or in tensor memory (TS), weights streamed through a 2-stage ring by 1-D bulk copies, accumulator
-// in TMEM read back with tcgen05.ld.  Lets the descriptors / layouts be validated in isolation on the GPU.
+// Building-block test of the wgmma path (sdfb200_debug_tc_gemm): one CTA computes D[128,N] = A[128,K] * W[N,K]^T with
+// the machinery of the tensor-core kernels -- bf16 split planes, canonical no-swizzle K-major operands, A either in shared memory
+// (SS) or in registers (RS), weights streamed through a 2-stage ring by 1-D bulk copies, accumulator in registers (two warpgroups
+// of 64 rows).  Lets the descriptors / layouts be validated in isolation on the GPU.
 #include "tc_common.cuh"
 #include "../../include/sdfb200_debug.h"
 
@@ -28,139 +28,138 @@ __global__ void k_tc_pack_w(const float* __restrict__ W, int ldw, int N, int K, 
   if (planes > 1) out[base + plane_elems + off] = lo;
 }
 
-template <int P, bool TS>
-__global__ void __launch_bounds__(192, 1) k_tc_gemm_test(const float* __restrict__ A, const __nv_bfloat16* __restrict__ Wp, int K, int Np,
+template <int P, bool RS>
+__global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict__ A, const __nv_bfloat16* __restrict__ Wp, int K, int Np, int Np64,
                                                          float* __restrict__ D) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t full[2], empty[2], dfull;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t full[2], empty[2];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nblocks = K / kKB;
-  const uint32_t stage_bytes = (uint32_t)P * Np * kKB * 2;
+  const uint32_t stage_bytes = (uint32_t)P * Np64 * kKB * 2;
   uint8_t* a_smem = smem;                                        // [P][K/8][128][16 B]   (SS mode only)
-  uint8_t* w_smem = smem + (TS ? 0 : (size_t)P * K * 256);       // 2 stages
+  uint8_t* w_smem = smem + (RS ? 0 : (size_t)P * K * 256);       // 2 stages
   if (tid == 0) {
-    mbar_init(&full[0], 1); mbar_init(&full[1], 1); mbar_init(&empty[0], 1); mbar_init(&empty[1], 1); mbar_init(&dfull, 1);
+    mbar_init(&full[0], 1); mbar_init(&full[1], 1); mbar_init(&empty[0], 2); mbar_init(&empty[1], 2);
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc<512>(&tmem_base_s);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
-  const uint32_t d_tmem = tmem;             // columns [0, 256)
-  const uint32_t a_tmem = tmem + 256;       // plane p at columns 256 + 128 p
-
-  if (warp < 4) {
-    // ---- stage A as bf16 planes: thread r owns row r ----
-    const int r = tid;
-    const uint32_t lane_addr = (uint32_t)(warp * 32) << 16;
-    for (int k0 = 0; k0 < K; k0 += 16) {
+  if (!RS && tid < 256) {
+    // ---- stage A as bf16 planes: thread (r, half) converts half of row r ----
+    const int r = tid & 127;
+    for (int k0 = (tid >> 7) * 16; k0 < K; k0 += 32) {
       uint32_t hi[8], lo[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) split2(A[(size_t)r * K + k0 + 2 * j], A[(size_t)r * K + k0 + 2 * j + 1], hi[j], lo[j]);
-      if (TS) {
-        tmem_st8(a_tmem + lane_addr + k0 / 2, hi);
-        if (P > 1) tmem_st8(a_tmem + 128 + lane_addr + k0 / 2, lo);
-      } else {
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const uint32_t off = (uint32_t)((k0 / 8 + c) * 2048 + r * 16);
-          *reinterpret_cast<uint4*>(a_smem + off) = make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
-          if (P > 1) *reinterpret_cast<uint4*>(a_smem + (size_t)K * 256 + off) = make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
-        }
+      for (int c = 0; c < 2; ++c) {
+        const uint32_t off = (uint32_t)((k0 / 8 + c) * 2048 + r * 16);
+        *reinterpret_cast<uint4*>(a_smem + off) = make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
+        if (P > 1) *reinterpret_cast<uint4*>(a_smem + (size_t)K * 256 + off) = make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
       }
     }
-    if (TS) tc_wait_st();
-    else fence_async_smem();
-    tc_fence_before();
+    fence_async_smem();
   }
   __syncthreads();
-  tc_fence_after();
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8) {
     // ---- weight producer ----
-    for (int b = 0; b < nblocks; ++b) {
-      const int s = b & 1;
-      mbar_wait(&empty[s], ((b >> 1) & 1) ^ 1);
-      mbar_arrive_expect_tx(&full[s], stage_bytes);
-      bulk_g2s(w_smem + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(Wp) + (size_t)b * stage_bytes, stage_bytes, &full[s]);
+    if (lane == 0) {
+      for (int b = 0; b < nblocks; ++b) {
+        const int s = b & 1;
+        mbar_wait(&empty[s], ((b >> 1) & 1) ^ 1);
+        mbar_arrive_expect_tx(&full[s], stage_bytes);
+        bulk_g2s(w_smem + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(Wp) + (size_t)b * stage_bytes, stage_bytes, &full[s]);
+      }
     }
-  } else if (warp == 5 && lane == 0) {
-    // ---- MMA issuer ----
-    const uint32_t idesc = make_idesc_bf16(128, Np);
-    const uint32_t lbo_b = (uint32_t)Np * 16, plane_b = (uint32_t)Np * kKB * 2;
-    uint32_t acc = 0;
+  } else {
+    // ---- two warpgroups, 64 rows each ----
+    const int wg = warp >> 2, t = tid & 127;
+    const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c2 = (t & 3) * 2;
+    const int nch = Np64 / 64;
+    float acc[4][32];
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+    const uint32_t lbo_b = (uint32_t)Np64 * 16, plane_b = (uint32_t)Np64 * kKB * 2;
+    const uint32_t abase = smem_u32(a_smem) + wg * 64 * 16;
     for (int b = 0; b < nblocks; ++b) {
       const int s = b & 1;
       mbar_wait(&full[s], (b >> 1) & 1);
-      tc_fence_after();
       const uint32_t wbase = smem_u32(w_smem + (size_t)s * stage_bytes);
+      uint32_t afr[kKB / 16][2][4];
+      if (RS) {
+        // A fragments straight from global memory: rows r0 / r0 + 8, columns 2c, 2c + 1 (+8) of each K step
 #pragma unroll
-      for (int j = 0; j < kKB / 16; ++j) {
-        const int kstep = b * (kKB / 16) + j;  // global 16-wide K step
-        const uint64_t b0 = make_smem_desc(wbase + j * 2 * lbo_b, lbo_b, 128);
-        const uint64_t b1 = make_smem_desc(wbase + plane_b + j * 2 * lbo_b, lbo_b, 128);
-        if (TS) {
-          mma_ts(d_tmem, a_tmem + kstep * 8, b0, idesc, acc);
-          acc = 1;
-          if (P > 1) {
-            mma_ts(d_tmem, a_tmem + 128 + kstep * 8, b0, idesc, 1);
-            mma_ts(d_tmem, a_tmem + kstep * 8, b1, idesc, 1);
-          }
-        } else {
-          const uint32_t abase = smem_u32(a_smem);
-          const uint64_t a0 = make_smem_desc(abase + kstep * 2 * 2048, 2048, 128);
-          const uint64_t a1 = make_smem_desc(abase + (uint32_t)K * 256 + kstep * 2 * 2048, 2048, 128);
-          mma_ss(d_tmem, a0, b0, idesc, acc);
-          acc = 1;
-          if (P > 1) {
-            mma_ss(d_tmem, a1, b0, idesc, 1);
-            mma_ss(d_tmem, a0, b1, idesc, 1);
+        for (int j = 0; j < kKB / 16; ++j) {
+          const int k = b * kKB + j * 16 + c2;
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const float* src = A + (size_t)(r0 + 8 * (q & 1)) * K + k + 8 * (q >> 1);
+            split2(src[0], src[1], afr[j][0][q], afr[j][1][q]);
           }
         }
       }
-      mma_commit(&empty[s]);
-    }
-    mma_commit(&dfull);
-  }
-  if (warp < 4) {
-    mbar_wait(&dfull, 0);
-    tc_fence_after();
-    const uint32_t lane_addr = (uint32_t)(warp * 32) << 16;
-    for (int c0 = 0; c0 < Np; c0 += 16) {
-      uint32_t v[16];
-      tmem_ld16(d_tmem + lane_addr + c0, v);
-      tc_wait_ld();
+      wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+      wg_arrive();
 #pragma unroll
-      for (int j = 0; j < 16; ++j) D[(size_t)tid * Np + c0 + j] = __uint_as_float(v[j]);
+      for (int j = 0; j < kKB / 16; ++j) {
+        const int kstep = b * (kKB / 16) + j;  // global 16-wide K step
+        const uint32_t baddr = wbase + j * 2 * lbo_b;
+        if (RS) {
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            if (c < nch) {
+              const uint64_t b0 = make_smem_desc(baddr + c * 1024, lbo_b, 128);
+              wgmma64_rs(acc[c], afr[j][0], b0);
+              if (P > 1) {
+                wgmma64_rs(acc[c], afr[j][1], b0);
+                wgmma64_rs(acc[c], afr[j][0], make_smem_desc(baddr + plane_b + c * 1024, lbo_b, 128));
+              }
+            }
+          }
+        } else {
+          const uint64_t a0 = make_smem_desc(abase + kstep * 2 * 2048, 2048, 128);
+          const uint64_t a1 = make_smem_desc(abase + (uint32_t)K * 256 + kstep * 2 * 2048, 2048, 128);
+          wgmma_kstep_ss<P, 4>(acc, a0, a1, baddr, plane_b, lbo_b, nch);
+        }
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+      if (t == 0) mbar_arrive(&empty[s]);
     }
-    tc_fence_before();
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = c * 64 + (i >> 2) * 8 + c2 + (i & 1), row = r0 + 8 * ((i >> 1) & 1);
+        if (c < nch && col < Np) D[(size_t)row * Np + col] = acc[c][i];
+      }
+    }
   }
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<512>(tmem);
 }
 
 }  // namespace sdfb200
 
 using namespace sdfb200;
 
-// D[128,Np] = A[128,K] W[N,K]^T ; K % 32 == 0, K <= 256, Np = N rounded up to 16 <= 256.  scratch: >= K/32*planes*Np*64 B
+// D[128,Np] = A[128,K] W[N,K]^T ; K % 32 == 0, K <= 256, Np = N rounded up to 16 <= 256.  scratch: >= K/32*planes*Np64*64 B
+// (Np64 = N rounded up to 64: the weights are packed in whole n64 blocks)
 extern "C" int sdfb200_debug_tc_gemm(const float* A, const float* W, int32_t K, int32_t N, int32_t mode_ts, int32_t planes, float* D, void* scratch,
                                      void* stream) {
   SDFB_REQUIRE(A && W && D && scratch, "NULL pointer");
   SDFB_REQUIRE(K % 32 == 0 && K >= 32 && K <= 256 && N >= 1 && N <= 256 && (planes == 1 || planes == 2), "unsupported test shape");
-  const int Np = (N + 15) / 16 * 16;
+  const int Np = (N + 15) / 16 * 16, Np64 = (N + 63) / 64 * 64;
   const int nblocks = K / kKB;
   cudaStream_t st = (cudaStream_t)stream;
-  const int tot = nblocks * Np * kKB;
-  k_tc_pack_w<<<(tot + 255) / 256, 256, 0, st>>>(W, K, N, K, Np, nblocks, planes, (__nv_bfloat16*)scratch);
+  const int tot = nblocks * Np64 * kKB;
+  k_tc_pack_w<<<(tot + 255) / 256, 256, 0, st>>>(W, K, N, K, Np64, nblocks, planes, (__nv_bfloat16*)scratch);
   SDFB_LAUNCHED("k_tc_pack_w");
-  const size_t smem = (mode_ts ? 0 : (size_t)planes * K * 256) + 2 * (size_t)planes * Np * kKB * 2 + 1024;
+  const size_t smem = (mode_ts ? 0 : (size_t)planes * K * 256) + 2 * (size_t)planes * Np64 * kKB * 2 + 1024;
 #define LAUNCH(P_, TS_)                                                                                              \
   do {                                                                                                               \
     SDFB_CUDA(cudaFuncSetAttribute(k_tc_gemm_test<P_, TS_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    k_tc_gemm_test<P_, TS_><<<1, 192, smem, st>>>(A, (const __nv_bfloat16*)scratch, K, Np, D);                        \
+    k_tc_gemm_test<P_, TS_><<<1, 288, smem, st>>>(A, (const __nv_bfloat16*)scratch, K, Np, Np64, D);                        \
   } while (0)
   if (planes == 1 && !mode_ts) LAUNCH(1, false);
   else if (planes == 1 && mode_ts) LAUNCH(1, true);
@@ -171,7 +170,7 @@ extern "C" int sdfb200_debug_tc_gemm(const float* A, const float* W, int32_t K, 
   return 0;
 }
 
-// building-block test of the generic tcgen05 Linear (tc_linear.cu) against a reference GEMM: same arguments as the internal sgemm()
+// building-block test of the generic tensor-core Linear (tc_linear.cu) against a reference GEMM: same arguments as the internal sgemm()
 namespace sdfb200 {
 int tc_gemm(int planes, int epi, const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy, int64_t M, int Np, int Kp,
             const float* aux, int ldaux, int aux_cols, void* scratch, cudaStream_t st);

@@ -1,150 +1,113 @@
-// Weight-gradient GEMM of the training path on tcgen05:  C[N, K] = A[P, N]^T B[P, K]   (dW = dY^T X, reduction over the P points)
+// Weight-gradient GEMM of the training path on wgmma:  C[N, K] = A[P, N]^T B[P, K]   (dW = dY^T X, reduction over the P points)
 // (what autograd's mm backward computes for every nn.Linear of the reference's SDFField, nerfstudio/fields/sdf_field.py:400-409,
 // trained through engine/trainer.py:319-323).
 //
-// Persistent CTAs, each accumulating its share of the points in TMEM: both operands are "long" in the reduction dimension, so both are
-// staged TRANSPOSED into shared memory as bf16 split planes in the canonical K-major (here: point-major) no-swizzle layout
+// Persistent CTAs, each accumulating its share of the points in registers: both operands are "long" in the reduction dimension, so both
+// are staged TRANSPOSED into shared memory as bf16 split planes in the canonical K-major (here: point-major) no-swizzle layout
 //     element (row r, point m) -> (m/8) * LBO + r * 16 + (m%8) * 2,   LBO = rows * 16
-// by 16 staging warps (global reads coalesced along the row index: 32 lanes = 32 consecutive columns of one point's row; each thread
-// gathers 8 consecutive points of ONE column and writes one 16-byte unit per plane), and consumed in SS mode by one MMA-issuing
-// thread: D[n, k] += sum_m A[m, n] B[m, k] as M = 128 (rows n, two halves for N = 256), N = K columns, K = 16 points per instruction;
-// bf16x3 = a0 b0 + a1 b0 + a0 b1.  The per-CTA partial sums go to a workspace and are reduced by a second kernel in a fixed order
-// (deterministic, unlike atomics).  HBM-bound by construction: 2 KB of fp32 activations per point and layer against 6144 tensor cycles
-// per 128 points.
+// (global reads coalesced along the row index: 32 lanes = 32 consecutive columns of one point's row; each thread gathers 8 consecutive
+// points of ONE column and writes one 16-byte unit per plane), double buffered so that the loads of the next 32 points run under the
+// MMAs of the current ones.  Two warpgroups: D[n, k] += sum_m A[m, n] B[m, k] with warpgroup w owning the rows n in [64 w, 64 w + 64)
+// of a 128-row chunk, N = K columns in n64 blocks, K = 16 points per instruction; bf16x3 = a0 b0 + a1 b0 + a0 b1.  The per-CTA
+// partial sums go to a workspace and are reduced by a second kernel in a fixed order (deterministic, unlike atomics).
 #include "tc_common.cuh"
 
 namespace sdfb200 {
 using namespace tc;
 
 namespace {
-constexpr int kWgThreads = 544;     // 16 staging warps + MMA issuer
-constexpr int kWgStage = 512;
+constexpr int kWgThreads = 256;     // two warpgroups: staging + MMAs
 constexpr int kWgPts = 32;          // points per stage
-constexpr int kWgStages = 2;
-constexpr int kWgRows = 256;        // rows per operand tile (N or K chunk, zero padded)
-constexpr uint32_t kWgOpBytes = 2u * (kWgPts / 8) * kWgRows * 16;     // one operand, both planes: 32 KB
-constexpr uint32_t kWgStageBytes = 2 * kWgOpBytes;
+constexpr int kWgRowsA = 128;       // rows of the A operand tile (N chunk, zero padded)
+constexpr int kWgRowsB = 256;       // rows of the B operand tile (K chunk, zero padded)
+constexpr uint32_t kWgPlaneA = (kWgPts / 8) * kWgRowsA * 16;          // 8 KB
+constexpr uint32_t kWgPlaneB = (kWgPts / 8) * kWgRowsB * 16;          // 16 KB
+constexpr uint32_t kWgStageBytes = 2 * (kWgPlaneA + kWgPlaneB);       // both operands, both planes
 
 struct WgArgs {
   const float* A; long long lda;    // [P, >= n0 + Nc]
   const float* B; long long ldb;    // [P, >= k0 + Kc]
   long long P;
-  int Nc, Kc;                       // rows of this (n, k) chunk, <= 256; Kc padded to 16 for the MMA
+  int Nc, Kc;                       // rows of this (n, k) chunk: Nc <= 128, Kc <= 256
   float* partial;                   // [gridDim.x][256][256]
 };
 
 template <int PL>
 __global__ void __launch_bounds__(kWgThreads, 1) k_tc_wgrad(const WgArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t full[kWgStages], empty[kWgStages], done;
-  __shared__ uint32_t tmem_base_s;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (tid == 0) {
-    for (int s = 0; s < kWgStages; ++s) { mbar_init(&full[s], 16); mbar_init(&empty[s], 1); }
-    mbar_init(&done, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc<512>(&tmem_base_s);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const long long nblk = (a.P + kWgPts - 1) / kWgPts;
-  const int Kmma = (a.Kc + 15) / 16 * 16;
-  const int halves = a.Nc > 128 ? 2 : 1;
+  const int nch = (a.Kc + 63) / 64;
+  const int wg = warp >> 2, t = tid & 127;
+  const bool mma_rows = wg * 64 < a.Nc;          // warpgroup-uniform: this warpgroup's 64 rows hold live columns of A
 
-  if (warp == 16) {
-    // ---------------- MMA issuer ----------------
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(128, Kmma);
-      uint32_t it = 0;
-      bool first = true;
-      for (long long blk = blockIdx.x; blk < nblk; blk += gridDim.x, ++it) {
-        const int s = it % kWgStages;
-        mbar_wait(&full[s], (it / kWgStages) & 1);
-        tc_fence_after();
-        const uint32_t abase = smem_u32(smem + (size_t)s * kWgStageBytes);
-        const uint32_t bbase = abase + kWgOpBytes;
-        constexpr uint32_t lbo = kWgRows * 16, plane = (kWgPts / 8) * kWgRows * 16;
+  // thread (op, col) gathers 8 consecutive points of one column: 128 A columns + 256 B columns, 4 groups of 8 points per stage
+  auto stage = [&](long long blk, uint8_t* dst) {
+    const long long m0 = blk * kWgPts;
+    for (int u = tid; u < (kWgRowsA + kWgRowsB) * (kWgPts / 8); u += kWgThreads) {
+      const int cc = u % (kWgRowsA + kWgRowsB), g = u / (kWgRowsA + kWgRowsB);
+      const bool isA = cc < kWgRowsA;
+      const int col = isA ? cc : cc - kWgRowsA;
+      const float* src = isA ? a.A : a.B;
+      const long long ld = isA ? a.lda : a.ldb;
+      const bool live = col < (isA ? a.Nc : a.Kc);
+      float v[8];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (h < halves) {
-#pragma unroll
-            for (int j = 0; j < kWgPts / 16; ++j) {
-              const uint64_t a0 = make_smem_desc(abase + h * 128 * 16 + j * 2 * lbo, lbo, 128);
-              const uint64_t b0 = make_smem_desc(bbase + j * 2 * lbo, lbo, 128);
-              mma_ss(tmem + h * 256, a0, b0, idesc, (first && j == 0) ? 0u : 1u);
-              if (PL > 1) {
-                const uint64_t a1 = make_smem_desc(abase + plane + h * 128 * 16 + j * 2 * lbo, lbo, 128);
-                const uint64_t b1 = make_smem_desc(bbase + plane + j * 2 * lbo, lbo, 128);
-                mma_ss(tmem + h * 256, a1, b0, idesc, 1);
-                mma_ss(tmem + h * 256, a0, b1, idesc, 1);
-              }
-            }
-          }
-        }
-        first = false;
-        mma_commit(&empty[s]);
-      }
-      mma_commit(&done);
-    }
-  } else {
-    // ---------------- staging: thread (op, col) gathers 8 consecutive points of one column, 4 groups per stage ----------------
-    const int op = tid >> 8;                      // 0: A (dY), 1: B (X)
-    const int col = tid & 255;
-    const float* src = op == 0 ? a.A : a.B;
-    const long long ld = op == 0 ? a.lda : a.ldb;
-    const bool live = col < (op == 0 ? a.Nc : a.Kc);
-    uint32_t it = 0;
-    for (long long blk = blockIdx.x; blk < nblk; blk += gridDim.x, ++it) {
-      const int s = it % kWgStages;
-      const long long m0 = blk * kWgPts;
-      float v[kWgPts];
-#pragma unroll
-      for (int i = 0; i < kWgPts; ++i) {
-        const long long m = m0 + i;
+      for (int i = 0; i < 8; ++i) {
+        const long long m = m0 + g * 8 + i;
         v[i] = (live && m < a.P) ? __ldg(src + m * ld + col) : 0.f;
       }
-      mbar_wait(&empty[s], ((it / kWgStages) & 1) ^ 1);
-      uint8_t* dst = smem + (size_t)s * kWgStageBytes + (size_t)op * kWgOpBytes;
+      uint32_t hi[4], lo[4];
 #pragma unroll
-      for (int g = 0; g < kWgPts / 8; ++g) {
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) split2(v[g * 8 + 2 * e], v[g * 8 + 2 * e + 1], hi[e], lo[e]);
-        *reinterpret_cast<uint4*>(dst + (size_t)g * kWgRows * 16 + col * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        if (PL > 1) *reinterpret_cast<uint4*>(dst + (kWgPts / 8) * kWgRows * 16 + (size_t)g * kWgRows * 16 + col * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-      }
-      fence_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full[s]);
+      for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hi[e], lo[e]);
+      const int rows = isA ? kWgRowsA : kWgRowsB;
+      uint8_t* base = dst + (isA ? 0 : PL * kWgPlaneA) + (size_t)g * rows * 16 + col * 16;
+      *reinterpret_cast<uint4*>(base) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+      if (PL > 1) *reinterpret_cast<uint4*>(base + (isA ? kWgPlaneA : kWgPlaneB)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
     }
-    // ---------------- epilogue: partial sums of this CTA -> workspace ----------------
-    mbar_wait_backoff(&done, 0);
-    tc_fence_after();
-    const int wq = warp & 3, cq = warp >> 2;      // TMEM lane quadrant, column quarter
-    const int row = wq * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(wq * 32) << 16;
-    float* out = a.partial + (size_t)blockIdx.x * 256 * 256;
-    const bool any = blockIdx.x < nblk;           // a CTA without points wrote nothing into TMEM
-    for (int h = 0; h < halves; ++h) {
-      for (int c0 = cq * 64; c0 < cq * 64 + 64 && c0 < Kmma; c0 += 16) {
-        uint32_t d[16];
-        if (any) { tmem_ld16(tmem + h * 256 + lane_addr + c0, d); tc_wait_ld(); }
-        else {
+    fence_async_smem();
+  };
+
+  float acc[4][32];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) d[j] = 0u;
-        }
-        float* o = out + (size_t)(h * 128 + row) * 256 + c0;
+  for (int c = 0; c < 4; ++c)
 #pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4)
-          *reinterpret_cast<float4*>(o + j4 * 4) = make_float4(__uint_as_float(d[j4 * 4]), __uint_as_float(d[j4 * 4 + 1]), __uint_as_float(d[j4 * 4 + 2]), __uint_as_float(d[j4 * 4 + 3]));
-      }
-    }
-    tc_fence_before();
-  }
+    for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+  int it = 0;
+  if (blockIdx.x < nblk) stage(blockIdx.x, smem);
   __syncthreads();
-  if (warp == 0) tmem_dealloc<512>(tmem);
+  for (long long blk = blockIdx.x; blk < nblk; blk += gridDim.x, ++it) {
+    uint8_t* cur = smem + (size_t)(it & 1) * kWgStageBytes;
+    if (mma_rows) {
+      const uint32_t abase = smem_u32(cur) + wg * 64 * 16, bbase = smem_u32(cur + PL * kWgPlaneA);
+      wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+      wg_arrive();
+#pragma unroll
+      for (int j = 0; j < kWgPts / 16; ++j) {
+        const uint64_t a0 = make_smem_desc(abase + j * 2 * kWgRowsA * 16, kWgRowsA * 16, 128);
+        const uint64_t a1 = make_smem_desc(abase + kWgPlaneA + j * 2 * kWgRowsA * 16, kWgRowsA * 16, 128);
+        wgmma_kstep_ss<PL, 4>(acc, a0, a1, bbase + j * 2 * kWgRowsB * 16, kWgPlaneB, kWgRowsB * 16, nch);
+      }
+      wg_commit();
+    }
+    if (blk + gridDim.x < nblk) stage(blk + gridDim.x, smem + (size_t)((it + 1) & 1) * kWgStageBytes);
+    if (mma_rows) {
+      wg_wait<0>();
+      wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+    }
+    __syncthreads();
+  }
+  // ---------------- partial sums of this CTA -> workspace (zeros for a CTA without points) ----------------
+  float* out = a.partial + (size_t)blockIdx.x * 256 * 256;
+  const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c2 = (t & 3) * 2;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      const int n = r0 + 8 * ((i >> 1) & 1), k = c * 64 + (i >> 2) * 8 + c2;
+      if (c < nch) *reinterpret_cast<float2*>(out + (size_t)n * 256 + k) = make_float2(acc[c][i], acc[c][i + 1]);
+    }
+  }
 }
 
 // C[n0 + n, k0 + k] (+)= sum_g partial[g][n][k]   in a fixed order
@@ -169,12 +132,13 @@ int tc_wgrad(int planes, const float* A, long long lda, const float* B, long lon
   SDFB_REQUIRE(workspace_bytes >= tc_wgrad_workspace_bytes(), "tc_wgrad: workspace too small");
   SDFB_REQUIRE(N >= 1 && K >= 1 && P >= 0, "tc_wgrad: bad sizes");
   const long long nblk = (P + kWgPts - 1) / kWgPts;
-  const int grid = (int)(nblk < kNumSMs ? (nblk > 0 ? nblk : 1) : kNumSMs);
-  const size_t smem = (size_t)kWgStages * kWgStageBytes + 1024;
-  for (int n0 = 0; n0 < N; n0 += 256) {
+  const int ctas = persistent_ctas();
+  const int grid = (int)(nblk < ctas ? (nblk > 0 ? nblk : 1) : ctas);
+  const size_t smem = 2 * (size_t)kWgStageBytes + 1024;
+  for (int n0 = 0; n0 < N; n0 += kWgRowsA) {
     for (int k0 = 0; k0 < K; k0 += 256) {
       WgArgs a;
-      a.A = A + n0; a.lda = lda; a.B = B + k0; a.ldb = ldb; a.P = P; a.Nc = N - n0 < 256 ? N - n0 : 256; a.Kc = K - k0 < 256 ? K - k0 : 256;
+      a.A = A + n0; a.lda = lda; a.B = B + k0; a.ldb = ldb; a.P = P; a.Nc = N - n0 < kWgRowsA ? N - n0 : kWgRowsA; a.Kc = K - k0 < 256 ? K - k0 : 256;
       a.partial = (float*)workspace;
       if (planes == 2) {
         SDFB_CUDA(cudaFuncSetAttribute(k_tc_wgrad<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -1,4 +1,4 @@
-"""B200-native drop-in for ``nerfstudio.fields.density_fields.HashMLPDensityField`` (the proposal networks of
+"""H100-native drop-in for ``nerfstudio.fields.density_fields.HashMLPDensityField`` (the proposal networks of
 neus-facto / bakedsdf, density_fields.py:40-121): same constructor, ``get_density``, ``density_fn``.  The reference builds a
 ``tcnn.NetworkWithInputEncoding`` (HashGrid + FullyFusedMLP, ReLU, no biases, output activation None) and applies
 ``trunc_exp``; here one fused kernel (sdfb200_density_field_forward) does lookup + MLP + exp.

@@ -1,4 +1,4 @@
-"""Dense-layer GEMMs of the TRAINING path on the tcgen05 kernels (sdfb200_gemm_nt / _nn / _tn), as autograd Functions.
+"""Dense-layer GEMMs of the TRAINING path on the tensor-core (wgmma) kernels (sdfb200_gemm_nt / _nn / _tn), as autograd Functions.
 
 The reference trains through ATen autograd over ``nn.Linear`` (nerfstudio/fields/sdf_field.py:400-409 via engine/trainer.py:319-323),
 including the double backward of the eikonal term (``torch.autograd.grad(..., create_graph=True)``, sdf_field.py:646-655).  The three
@@ -176,7 +176,7 @@ class _LinearAct(torch.autograd.Function):
 
 
 def linear(x, weight, bias, act: int = 0, precision="bf16x3"):
-    """``act(F.linear(x, weight, bias))`` on the tcgen05 GEMMs: x [P, pad16(K)] (padding columns ignored), weight [N, K], bias [N]
+    """``act(F.linear(x, weight, bias))`` on the tensor-core GEMMs: x [P, pad16(K)] (padding columns ignored), weight [N, K], bias [N]
     -> [P, pad16(N)].  For act = 0 / relu the padding columns of the result are zero; for softplus they hold softplus(0) and must be
     sliced off or ignored by the consumer (the next layer's GEMM ignores them).  Differentiable to any order."""
     return _LinearAct.apply(x, weight, bias, act, precision)

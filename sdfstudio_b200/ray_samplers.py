@@ -1,4 +1,4 @@
-"""B200-native drop-ins for ``nerfstudio.model_components.ray_samplers`` (same class names, constructor arguments,
+"""H100-native drop-ins for ``nerfstudio.model_components.ray_samplers`` (same class names, constructor arguments,
 ``forward`` signatures and train/eval behaviour).  Every per-ray scan runs in libsdfb200.so (csrc/samplers.cu); the
 Python here only sequences kernels and draws the training-mode jitter with ``torch.rand`` in the reference's order.
 """

@@ -1,4 +1,4 @@
-"""B200-native drop-ins for ``nerfstudio.model_components.renderers`` (dense branch): RGBRenderer :42-118,
+"""H100-native drop-ins for ``nerfstudio.model_components.renderers`` (dense branch): RGBRenderer :42-118,
 AccumulationRenderer :171-197, DepthRenderer :200-261, SemanticRenderer :284-295.  The per-ray reductions run in
 libsdfb200.so (csrc/render.cu, sdfb200_render).  ``render_all`` composites every per-ray output SurfaceModel.get_outputs
 asks for (models/base_surface_model.py:300-310) in ONE kernel launch.

@@ -1,4 +1,4 @@
-"""B200-native drop-ins for ``nerfstudio.model_components.scene_colliders`` (:30-163): set ``nears`` / ``fars`` on a RayBundle.
+"""H100-native drop-ins for ``nerfstudio.model_components.scene_colliders`` (:30-163): set ``nears`` / ``fars`` on a RayBundle.
 One kernel launch (sdfb200_collide) instead of ~20 ATen elementwise ops."""
 import ctypes as C
 

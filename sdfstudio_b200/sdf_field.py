@@ -1,4 +1,4 @@
-"""B200-native drop-in for ``nerfstudio.fields.sdf_field`` (SDFField, SDFFieldConfig, LaplaceDensity,
+"""H100-native drop-in for ``nerfstudio.fields.sdf_field`` (SDFField, SDFFieldConfig, LaplaceDensity,
 SingleVarianceNetwork).  Same constructor, same methods, same parameter names/shapes (``glin{l}.weight_g/weight_v/bias``,
 ``clin{l}.*``, ``laplace_density.beta``, ``deviation_network.variance``, ``embedding_appearance.embedding.weight``) so a
 reference state_dict loads directly; the arithmetic runs in libsdfb200.so through sdfb200_field_forward.
@@ -84,7 +84,7 @@ class _EncodingInfo:
 
 @dataclass
 class SDFFieldConfig:
-    """Field-for-field copy of the reference config (sdf_field.py:121-185) + two B200 knobs at the end."""
+    """Field-for-field copy of the reference config (sdf_field.py:121-185) + two knobs of this package at the end."""
 
     _target: Type = field(default_factory=lambda: SDFField)
     num_layers: int = 8
@@ -117,11 +117,11 @@ class SDFFieldConfig:
     hash_features_per_level: int = 2
     hash_smoothstep: bool = True
     use_position_encoding: bool = True
-    # ---- B200 knobs (not in the reference) ----
+    # ---- knobs of this package (not in the reference) ----
     grid_layout: str = "tcnn"      # "tcnn" (checkpoint compatible) | "torch" (reference HashEncoding layout)
     precision: str = "fp32"        # "fp32" | "bf16x3" | "bf16"   (include/sdfb200.h SDFB200_PRECISION_*)
     table_dtype: str = "fp32"      # "fp32" | "fp16": gather from an fp16 copy of the table (tiny-cuda-nn's own storage precision)
-    train_gemm: str = "auto"       # training-mode dense layers: "auto" = tcgen05 GEMMs (linear_ops.py) unless precision == "fp32"; "aten" | "tc"
+    train_gemm: str = "auto"       # training-mode dense layers: "auto" = tensor-core GEMMs (linear_ops.py) unless precision == "fp32"; "aten" | "tc"
 
     def setup(self, **kwargs):
         return self._target(self, **kwargs)

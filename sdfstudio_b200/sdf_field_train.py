@@ -3,9 +3,9 @@
 What trains in the reference is ATen autograd over ``nn.Linear`` layers plus the ``tinycudann.Encoding`` operator
 (nerfstudio/fields/sdf_field.py:380-410, :614-689).  This module is that composition over this package's kernels: the grid operator
 (forward, backward, second-order backward for the eikonal term: sdfb200_grid_encode / _backward / _backward_backward, and their grouped
-forms for the seven taps of a numerical-gradient sample) and, at precision bf16x3 / bf16, the dense layers on the tcgen05 GEMMs of
+forms for the seven taps of a numerical-gradient sample) and, at precision bf16x3 / bf16, the dense layers on the tensor-core GEMMs of
 linear_ops.py (closed under differentiation); precision "fp32" keeps ATen matmuls, the reference's exact arithmetic.
-The fused tcgen05 kernel (csrc/field_tc_kernel.cuh) is the rendering / sampling path (everything under ``torch.no_grad``: the NeuS /
+The fused tensor-core kernel (csrc/field_tc_kernel.cuh) is the rendering / sampling path (everything under ``torch.no_grad``: the NeuS /
 error-bounded / UniSurf samplers, evaluation, mesh extraction).
 
 Functions take the SDFField module as first argument; SDFField dispatches here when autograd is recording in training mode.
@@ -39,7 +39,7 @@ def nerf_encoding(x, num_frequencies: int, max_exp: float, include_input: bool, 
 
 
 def _gemm_precision(field):
-    """None -> ATen matmuls (precision "fp32": exact reference arithmetic); otherwise the tcgen05 GEMMs of linear_ops at that precision."""
+    """None -> ATen matmuls (precision "fp32": exact reference arithmetic); otherwise the tensor-core GEMMs of linear_ops at that precision."""
     mode = getattr(field.config, "train_gemm", "auto")
     prec = getattr(field.config, "precision", "fp32")
     if mode == "aten" or (mode == "auto" and prec == "fp32"):

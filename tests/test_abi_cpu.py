@@ -181,7 +181,7 @@ def test_mirror_signatures_and_config_defaults_match_reference():
         assert cls is not None, f"{name} is not mirrored"
         params = [(n, p) for n, p in inspect.signature(cls.__init__).parameters.items() if n not in ("self", "kwargs", "args")]
         mine = [[n, None if p.default is inspect.Parameter.empty else plain(p.default)] for n, p in params]
-        # every reference parameter exists, in the same order, with the same default (extra trailing B200 keyword arguments are allowed)
+        # every reference parameter exists, in the same order, with the same default (extra trailing keyword arguments of this package are allowed)
         if mine[: len(sig)] != sig:
             problems.append((name, mine[: len(sig)], sig))
     assert not problems, problems
@@ -228,43 +228,72 @@ def test_proposal_network_checkpoint_layout_loads():
         checkpoint.load_density_field_checkpoint(wrong, ckpt, index=0)
 
 
-@pytest.mark.reference
-def test_reference_tensordataclasses_pass_through_the_host_side():
-    """The reference's own RayBundle / RaySamples (TensorDataclass objects with expanded stride-0 fields, cameras/rays.py:233-339) are what the
-    modules receive inside sdfstudio: the host-side accessors must read them, keep their TYPE when slicing / flattening, and rebuild the
-    [R, S+1] bin buffer the kernels take.  Structure only (no kernel runs on the CPU box)."""
-    from oracle import ref_import
+def test_foreign_tensordataclasses_pass_through_the_host_side():
+    """Inside sdfstudio the modules receive the reference's own RayBundle / RaySamples (TensorDataclass objects, cameras/rays.py:233-339),
+    not this package's classes.  Local stand-ins with the same fields and the same memory layout (a camera bundle [H, W, k]; starts / ends as
+    overlapping slices of one bin buffer; origins / directions stride-0 expanded over the samples, ray_samplers.py:119-125): the host-side
+    accessors must read them, keep their TYPE when flattening / slicing / sharding, and rebuild the [R, S+1] bin buffers the kernels take.
+    Structure only (no kernel runs)."""
+    import dataclasses
+    from typing import Optional
 
     import sdfstudio_b200 as sb
     from sdfstudio_b200 import parallel
 
-    ref = ref_import.ref_modules()
+    @dataclasses.dataclass
+    class ForeignRayBundle:
+        origins: torch.Tensor
+        directions: torch.Tensor
+        pixel_area: torch.Tensor
+        directions_norm: Optional[torch.Tensor] = None
+        camera_indices: Optional[torch.Tensor] = None
+        nears: Optional[torch.Tensor] = None
+        fars: Optional[torch.Tensor] = None
+        times: Optional[torch.Tensor] = None
+
+    @dataclasses.dataclass
+    class ForeignFrustums:
+        origins: torch.Tensor
+        directions: torch.Tensor
+        starts: torch.Tensor
+        ends: torch.Tensor
+
+    @dataclasses.dataclass
+    class ForeignRaySamples:
+        frustums: ForeignFrustums
+        spacing_starts: torch.Tensor
+        spacing_ends: torch.Tensor
+
     H, W, S = 5, 7, 9
     g = torch.Generator().manual_seed(2)
     d = torch.randn(H, W, 3, generator=g)
     d = d / d.norm(dim=-1, keepdim=True)
-    bundle = ref.RayBundle(origins=torch.randn(H, W, 3, generator=g), directions=d, pixel_area=torch.ones(H, W, 1), directions_norm=torch.ones(H, W, 1),
-                           camera_indices=torch.zeros(H, W, 1, dtype=torch.long), nears=torch.full((H, W, 1), 0.5), fars=torch.full((H, W, 1), 4.5))
+    bundle = ForeignRayBundle(origins=torch.randn(H, W, 3, generator=g), directions=d, pixel_area=torch.ones(H, W, 1), directions_norm=torch.ones(H, W, 1),
+                              camera_indices=torch.zeros(H, W, 1, dtype=torch.long), nears=torch.full((H, W, 1), 0.5), fars=torch.full((H, W, 1), 4.5))
     flat, hw = parallel.flatten_ray_bundle(bundle)
     assert hw == (H, W) and type(flat) is type(bundle) and flat.origins.shape == (H * W, 3) and flat.camera_indices.dtype == torch.long
-    assert torch.equal(flat.origins.view(H, W, 3), bundle.origins)
+    assert torch.equal(flat.origins.view(H, W, 3), bundle.origins) and flat.times is None
+    assert parallel.flatten_ray_bundle(flat) == (flat, None)
     part = parallel.slice_ray_bundle(flat, 3, 11)
     assert type(part) is type(bundle) and part.origins.shape == (8, 3) and torch.equal(part.fars, flat.fars[3:11])
     sh = parallel.shard_ray_bundle(flat, 1, 3)
-    assert sh.origins.shape[0] == parallel.shard_bounds(H * W, 1, 3)[1] - parallel.shard_bounds(H * W, 1, 3)[0]
-    # the reference sampler's RaySamples: starts / ends are overlapping slices of one bin buffer, origins / directions stride-0 expanded
-    rs = ref.ray_samplers.UniformSampler(num_samples=S).eval()(flat)
+    s0, s1 = parallel.shard_bounds(H * W, 1, 3)
+    assert type(sh) is type(bundle) and sh.origins.shape[0] == s1 - s0 and torch.equal(sh.directions, flat.directions[s0:s1])
+    # samples laid out like the reference's UniformSampler output
+    R = H * W
+    spacing = torch.linspace(0.0, 1.0, S + 1).expand(R, S + 1).contiguous()
+    euclid = (flat.nears + (flat.fars - flat.nears) * spacing).contiguous()
+    fr = ForeignFrustums(origins=flat.origins[:, None, :].expand(R, S, 3), directions=flat.directions[:, None, :].expand(R, S, 3),
+                         starts=euclid[:, :-1, None], ends=euclid[:, 1:, None])
+    rs = ForeignRaySamples(frustums=fr, spacing_starts=spacing[:, :-1, None], spacing_ends=spacing[:, 1:, None])
     assert rs.frustums.origins.stride()[1] == 0
     bins = sb.rays.bins_of(rs)
-    assert bins.shape == (H * W, S + 1) and bins.is_contiguous()
+    assert bins.shape == (R, S + 1) and bins.is_contiguous()
     assert torch.equal(bins[:, :-1], rs.frustums.starts[..., 0]) and torch.equal(bins[:, 1:], rs.frustums.ends[..., 0])
     sp = sb.rays.spacing_bins_of(rs)
     assert torch.equal(sp[:, :-1], rs.spacing_starts[..., 0]) and torch.equal(sp[:, -1], rs.spacing_ends[:, -1, 0])
     o2, d2 = sb.rays.rays_of(rs)
     assert o2.is_contiguous() and torch.equal(o2, flat.origins) and torch.equal(d2, flat.directions)
-    # FieldHeadNames of the reference compare equal to the product's keys (dicts returned by SDFField are indexed with either)
-    assert {h.value for h in ref.FieldHeadNames} >= {h.value for h in sb.FieldHeadNames} or all(
-        getattr(ref.FieldHeadNames, h.name).value == h.value for h in sb.FieldHeadNames)
 
 
 def test_grouped_grid_calls_reject_bad_groups_and_encoding_context_nests():

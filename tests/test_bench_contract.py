@@ -1,5 +1,5 @@
-"""CPU-only: the JSON lines bench.py printed on the B200 (committed under profiles/) carry every key of the driver's contract, and the
-derived fields are consistent with each other (value <-> ms_per_step, roofline.frac = achieved / peak, e2e bytes declared)."""
+"""CPU-only: the JSON lines bench.py printed on an H100 (committed under profiles/) carry every key of the benchmark's result format, and
+the derived fields are consistent with each other (value <-> ms_per_step, roofline.frac = achieved / peak, e2e bytes declared)."""
 import glob
 import json
 import os

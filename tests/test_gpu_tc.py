@@ -1,4 +1,4 @@
-"""-m gpu: tcgen05 building blocks (bf16 split-plane GEMM tile, SS and TS operand modes) against torch fp64."""
+"""-m gpu: tensor-core building blocks (bf16 split-plane wgmma GEMM tile, A operand in shared memory or in registers) against torch fp64."""
 import pytest
 import torch
 
@@ -17,7 +17,8 @@ def test_tc_gemm_tile(ts, planes, K, N):
     W = (torch.randn(N, K, generator=g) / K**0.5).cuda()
     Np = (N + 15) // 16 * 16
     D = torch.full((128, Np), float("nan"), device="cuda")
-    scratch = torch.zeros((K // 32) * planes * Np * 64, dtype=torch.uint8, device="cuda")
+    Np64 = (N + 63) // 64 * 64
+    scratch = torch.zeros((K // 32) * planes * Np64 * 64, dtype=torch.uint8, device="cuda")
     rc = lib.sdfb200_debug_tc_gemm(A.data_ptr(), W.data_ptr(), K, N, ts, planes, D.data_ptr(), scratch.data_ptr(), 0)
     assert rc == 0, lib.sdfb200_last_error_string()
     torch.cuda.synchronize()
@@ -136,7 +137,7 @@ def test_field_fp16_table_matches_oracle_on_the_same_quantised_table(precision):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# generic tcgen05 Linear (csrc/tc_linear.cu): the GEMM engine of every field shape outside the fused kernel's family
+# generic tensor-core Linear (csrc/tc_linear.cu): the GEMM engine of every field shape outside the fused kernel's family
 # ----------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("planes", [1, 2])
 @pytest.mark.parametrize("epi", [0, 1, 2, 3])
@@ -175,7 +176,7 @@ def test_tc_linear_matches_fp64(planes, epi, M, Kp, Np):
 
 @pytest.mark.parametrize("name", ["bakedsdf_small", "volsdf_stock", "angelo_small"])
 def test_generic_shapes_on_the_tensor_core_engine(name):
-    """Field shapes outside the fused family at precision='bf16x3': the generic kernels with tcgen05 GEMMs must sit at the fp32
+    """Field shapes outside the fused family at precision='bf16x3': the generic kernels with tensor-core GEMMs must sit at the fp32
     reference's own noise level, like the fused kernel does for neus-facto."""
     sb, field, rs, out, e64, (o, d, cam, eu, o64) = _run_case(name, "bf16x3")
     G = load_golden(name)

@@ -1,5 +1,5 @@
-"""-m gpu: the fused tcgen05 field kernel in the regime bench.py runs it in -- many 128-point tiles per persistent CTA
-(BASELINE configs[1]: 4096 rays x 128 samples, hash L=16 F=2 T=2^19, MLP 2x256, i.e. 4096 tiles on 148 CTAs = 27.7 tiles
+"""-m gpu: the fused tensor-core field kernel in the regime bench.py runs it in -- many 128-point tiles per persistent CTA
+(BASELINE configs[1]: 4096 rays x 128 samples, hash L=16 F=2 T=2^19, MLP 2x256, i.e. 4096 tiles on 132 CTAs = 31.0 tiles
 per CTA), the tile loop / operand double buffering / mbarrier phase carry-over included.  The oracle (fp64) is evaluated on a
 strided ray subset; rays are independent, so the subset pins the whole batch statistically while the oracle finishes in
 seconds.  Reference: nerfstudio/fields/sdf_field.py:614-689 (get_outputs), cameras/rays.py:194-230, renderers.py:53-118,215-261.
@@ -49,7 +49,7 @@ def _check_heads(sb, out, e32, e64, idx, tag, floor_rel=1e-4):
 @pytest.mark.parametrize("precision,table_dtype", [("bf16x3", "fp32"), ("bf16x3", "fp16")])
 def test_bench_config_multi_tile_parity(precision, table_dtype):
     """4096 rays x 128 samples at the benchmark's dtype: per-sample heads at the reference's fp32 noise level, rendered
-    RGB / depth within 1e-4 relative of the oracle, on every 16th ray (256 rays, spread over all 148 CTAs and all tile slots)."""
+    RGB / depth within 1e-4 relative of the oracle, on every 16th ray (256 rays, spread over all 132 CTAs and all tile slots)."""
     import sdfstudio_b200 as sb
     from sdfstudio_b200.synthetic import dtu_like_rays
 
@@ -101,15 +101,15 @@ def test_bench_config_fast_mode_psnr():
 
 @pytest.mark.parametrize("precision", ["bf16x3", "bf16"])
 def test_ragged_multi_tile_and_tile_boundaries(precision):
-    """N = 3 * 148 * 128 + 37 points (a ragged last tile after three full waves), S = 37 so that rays straddle tile boundaries:
+    """N = 3 * 132 * 128 + 39 points (a ragged last tile after three full waves), S = 37 so that rays straddle tile boundaries:
     (a) strided subset + the very last rays against the fp64 oracle, (b) a big call equals small calls bit for bit (the
     arithmetic of a row must not depend on which tile / CTA / buffer parity it lands in)."""
     import sdfstudio_b200 as sb
     from sdfstudio_b200.synthetic import dtu_like_rays
 
     field, o32, o64 = _bench_field(precision)
-    R, S = 1537, 37
-    assert R * S == 3 * 148 * 128 + 37
+    R, S = 1371, 37
+    assert R * S == 3 * 132 * 128 + 39
     o, d, cam, nears, fars = dtu_like_rays(R, 77)
     rb = make_bundle(o, d, cam, nears, fars)
     H = sb.FieldHeadNames

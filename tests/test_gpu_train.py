@@ -235,7 +235,7 @@ def _oracle_loss(of: OracleField, spec, o, d, cam, starts, deltas, bins, target,
 @pytest.mark.parametrize("case", ["neusfacto_c1", "bakedsdf_small"])
 def test_sdffield_training_step(case, gemm):
     """gemm="aten": dense layers through ATen (fp32, the reference's own arithmetic); gemm="tc": forward, input-gradient and
-    weight-gradient GEMMs -- incl. the eikonal double backward -- on the tcgen05 kernels (linear_ops.py, bf16x3)."""
+    weight-gradient GEMMs -- incl. the eikonal double backward -- on the tensor-core kernels (linear_ops.py, bf16x3)."""
     import sdfstudio_b200 as sb
 
     spec, kw, o, d, cam, nears, fars, oracle, field = build_case(case)
@@ -310,7 +310,7 @@ def test_sdffield_training_step(case, gemm):
 @pytest.mark.parametrize("P,N,K", [(1000, 256, 71), (4097, 257, 256), (333, 3, 256), (2500, 256, 321), (77, 16, 16)])
 @pytest.mark.parametrize("precision", ["bf16x3", "bf16"])
 def test_training_gemm_primitives(P, N, K, precision):
-    """sdfb200_gemm_nt / _nn / _tn (tcgen05) against fp64 matmuls: Y = X W^T, dX = dY W, dW = dY^T X."""
+    """sdfb200_gemm_nt / _nn / _tn (tensor cores) against fp64 matmuls: Y = X W^T, dX = dY W, dW = dY^T X."""
     from sdfstudio_b200 import linear_ops as lo
 
     g = torch.Generator().manual_seed(P + N + K)

@@ -1,4 +1,4 @@
-"""Field-call time of shapes OUTSIDE the fused kernel's family (generic kernels): exact-fp32 CUDA-core GEMMs vs the tcgen05 Linear
+"""Field-call time of shapes OUTSIDE the fused kernel's family (generic kernels): exact-fp32 CUDA-core GEMMs vs the tensor-core Linear
 engine (csrc/tc_linear.cu).  bakedsdf-shaped (off-axis PE deg 8, ref-nerf heads, L-inf contraction; SURVEY.md 8d config 5) and the stock
 volsdf / neus 8x256 MLP without grid (config 3).  Prints one JSON line per (shape, precision).
 

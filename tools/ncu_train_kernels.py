@@ -1,5 +1,5 @@
 """Driver for ncu captures of the training-step kernels at the angelo-train-8192 shapes: grouped grid forward / table-gradient scatter
-(7 taps per sample, ray-coherent samples, 2.1 GB table, 8 of 16 levels active), tcgen05 forward GEMM + weight-gradient GEMM.  Run under
+(7 taps per sample, ray-coherent samples, 2.1 GB table, 8 of 16 levels active), tensor-core forward GEMM + weight-gradient GEMM.  Run under
     ncu --set full --clock-control none -k regex:'k_grid_encode_grouped|k_grid_encode_bwd_grouped|k_tc_wgrad|k_tc_linear' -c 8 -o gpurun_out/r02_train python tools/ncu_train_kernels.py
 """
 import os

@@ -1,7 +1,7 @@
 """Context row (BASELINE.md section 3, optional): the headline step computed by the ORACLE modules (the restatement of the reference's
 PyTorch code: torch-layout HashEncoding, nn.Linear-style matmuls, autograd for the sdf gradient) placed on the GPU, i.e. the reference's
 pure-PyTorch path on ATen / cuBLAS kernels with TF32 matmuls like scripts/train.py:59.  NOT the tiny-cuda-nn path (that cannot be built
-here: no source, no network) -- it is what `use_tcnn=False`-style PyTorch code achieves on the same B200.
+here: no source, no network) -- it is what `use_tcnn=False`-style PyTorch code achieves on the same GPU.
     python tools/oracle_gpu_bench.py [--rays 4096] [--steps 10]"""
 import argparse
 import json

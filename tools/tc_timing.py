@@ -1,5 +1,6 @@
-"""Per-phase cycle breakdown of the fused tensor-core field kernel (CTA 0, first tiles): epilogue thread, gather thread and MMA
-issuer stamps.  Uses the timing build of the kernel inside libsdfb200_dbg.so (sdfstudio_b200/build.py)."""
+"""Per-phase cycle breakdown of the fused tensor-core field kernel (CTA 0, thread 0, first tiles): tile start, the end of every layer
+(its MMAs plus the epilogue that precedes the next one start with the next stamp) and the tile end.  Uses the timing build of the kernel
+inside libsdfb200_dbg.so (sdfstudio_b200/build.py).   usage: tools/tc_timing.py [precision] [log2T] [table dtype] [fused|unfused]"""
 import ctypes
 import os
 import sys
@@ -10,8 +11,7 @@ import torch  # noqa: E402
 
 from sdfstudio_b200 import _lib  # noqa: E402
 
-variant = sys.argv[5] if len(sys.argv) > 5 else None
-_lib.LIB_PATH = os.path.join(_lib.HERE, f"libsdfb200_v{variant}.so" if variant else "libsdfb200_dbg.so")     # same ABI + the stamped kernel
+_lib.LIB_PATH = os.path.join(_lib.HERE, "libsdfb200_dbg.so")     # same ABI + the stamped kernel
 import sdfstudio_b200 as sb  # noqa: E402
 from sdfstudio_b200.synthetic import dtu_like_rays, perturb_field_  # noqa: E402
 
@@ -46,15 +46,14 @@ with torch.no_grad():
         e1.record()
         torch.cuda.synchronize()
         ms.append(e0.elapsed_time(e1))
-print(f"variant {variant}: field call {sorted(ms)[len(ms)//2]:.3f} ms (median of 10, L2 flushed)")
+print(f"field call {sorted(ms)[len(ms)//2]:.3f} ms (median of 10, L2 flushed)")
 lib = _lib.load()
 lib.sdfb200_debug_tc_timing.argtypes = [ctypes.c_void_p]
 buf = (ctypes.c_longlong * 512)()
 assert lib.sdfb200_debug_tc_timing(buf) == 0
-names = ["start", "wait G0", "E0", "wait G1", "E1", "-", "-", "wait B1", "EB1", "wait B0", "EB0", "wait C0", "EC0", "wait C1", "EC1+heads"]
+# stamps written by the kernel (field_tc_kernel.cuh, TC_STAMP): [0] tile start, [1 + L] end of layer L in the order the kernel runs them,
+# [15] end of the tile (heads / compositing done); stamp 1 + L minus stamp L = the layer's MMAs + the epilogue before them
+layers = ["encode+G0", "E0+G1", "E1+B1", "EB1+B0", "EB0+C0 misc", "h2 reload+C0 h2", "EC0+C1"]
 for t in (5, 10):
     st = [buf[t * 32 + k] for k in range(32)]
-    tot = st[15] - st[0]
-    print(f"tile {t}: epilogue total {tot} cycles  " + "  ".join(f"{n} {st[i+1]-st[i]}" for i, n in enumerate(names) if n != "-"))
-    print(f"   gather: wait g0done {st[17]-st[16]}  colour cols {st[18]-st[17]}  encode next {st[19]-st[18]}   (loop start at +{st[16]-st[0]} of the epilogue's tile start)")
-    print("   mma issue start (relative to epilogue tile start): " + "  ".join(f"L{L} +{st[20+L]-st[0]}" for L in range(7)) + f"  done issuing +{st[27]-st[0]}")
+    print(f"tile {t}: total {st[15] - st[0]} cycles  " + "  ".join(f"{n} {st[L + 1] - st[L]}" for L, n in enumerate(layers)) + f"  EC1+heads {st[15] - st[7]}")

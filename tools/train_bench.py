@@ -25,7 +25,7 @@ def main():
     ap.add_argument("--samples", type=int, default=64)
     ap.add_argument("--importance", type=int, default=64)
     ap.add_argument("--precision", default="bf16x3", help="precision of the no_grad (sampler) kernels")
-    ap.add_argument("--train-gemm", default="auto", choices=["auto", "tc", "aten"], help="dense layers of the training path: tcgen05 GEMMs (linear_ops) or ATen")
+    ap.add_argument("--train-gemm", default="auto", choices=["auto", "tc", "aten"], help="dense layers of the training path: tensor-core GEMMs (linear_ops) or ATen")
     ap.add_argument("--no-tf32", action="store_true", help="keep ATen matmuls in fp32 (the reference trains with TF32, scripts/train.py:59)")
     args = ap.parse_args()
     dev = torch.device("cuda")

@@ -2,7 +2,7 @@
 (method_configs.py:404-432: hash L=16 F=8 T=2^22 base 64 max 4096, linear interpolation, one hidden geo layer 167-256-257, colour MLP 4x256,
 numerical gradients = 7 geo evaluations per sample, PE zeroed, appearance embedding, progressive level mask) at 8192 rays per GPU:
 
-    ProposalNetworkSampler (256, 96 -> 48 samples, two HashMLPDensityFields, no grad) -> SDFField training forward (tcgen05 GEMMs of
+    ProposalNetworkSampler (256, 96 -> 48 samples, two HashMLPDensityFields, no grad) -> SDFField training forward (tensor-core GEMMs of
     linear_ops.py + this package's twice-differentiable grid operator) -> alpha compositing -> rgb L1 + eikonal + curvature-free loss
     -> backward -> gradient all-reduce over NCCL (DistributedDataParallel, the reference's own wrapper: pipelines/base_pipeline.py:241-243)
     -> Adam.
@@ -132,6 +132,11 @@ def main(args):
         pairs.append((e0, e1))
     barrier()
     launches = sb._lib.launch_count() - launches0
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        # the loss of the last timed step and a fixed sample of the parameters it updated (the hash table alone is ~2 GB)
+        g = torch.Generator().manual_seed(0)
+        sample = torch.cat([p.detach().flatten()[torch.randint(0, p.numel(), (min(p.numel(), 4096),), generator=g).to(dev)] for p in field.parameters()])
+        bench.dump_outputs(args.dump_outputs, {"loss": loss.reshape(1), "params_sample": sample})
     dev_ms = sum(a.elapsed_time(b) for a, b in pairs)
     # end to end: host rays in, scalar loss out (the reference's train_iteration returns the loss dict to the host: trainer.py:319-327)
     loss_host = torch.empty((), dtype=torch.float32).pin_memory()
@@ -181,7 +186,7 @@ def main(args):
             "dtype": f"{precision} GEMMs (fp32 accumulate), fp32 table / optimizer", "data": "synthetic",
             "config": {"workload": "angelo-train-8192", "rays_per_gpu": R, "samples_per_ray": S_TRAIN,
                        "field": "neus-facto-angelo SDFField: hash L16 F8 T2^22 (2.1 GB fp32), geo 167-256-257, colour 4x256, numerical gradients (7 geo evaluations / sample), level mask 8/16",
-                       "step": "proposal sampler (no grad) -> field fwd (tcgen05 GEMMs + grid operator) -> compositing -> L1 + eikonal -> backward -> all-reduce -> Adam",
+                       "step": "proposal sampler (no grad) -> field fwd (tensor-core GEMMs + grid operator) -> compositing -> L1 + eikonal -> backward -> all-reduce -> Adam",
                        "parallelism": f"data parallel x{world}: ray shard per rank, DistributedDataParallel gradient all-reduce over NCCL inside the timed region",
                        "gradient_bytes": n_grad * 4, "allreduce_alone_ms": ar_ms, "l2": "flushed between timed steps (256 MiB write)"},
             "e2e": {"value": rays_total / (e2e_ms * 1e-3), "unit": "rays/s", "h2d_bytes_per_step": sum(t.numel() * 4 for t in host), "d2h_bytes_per_step": 4},
