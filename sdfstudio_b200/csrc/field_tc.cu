@@ -60,15 +60,14 @@ struct TcPlan {
 
 static void make_tc_plan(const sdfb200_field_t& f, const FieldPlan& p, TcPlan& t) {
   t.planes = f.precision == SDFB200_PRECISION_BF16X3 ? 2 : 1;
-  const int np[L_COUNT] = {256, 256, 256, 128, 256, 256, 256};           // B0: the 96 input rows padded to an n64 multiple
   const int kdim[L_COUNT] = {kInK, 256, 256, 256, kInK, 256, 256};
   size_t off = p.tc_off;
   for (int l = 0; l < L_COUNT; ++l) {
     t.layer[l].w_off = off;
-    t.layer[l].Np = np[l];
-    t.layer[l].kblk = np[l] <= 128 ? kKBMax : kKB;
+    t.layer[l].Np = tc_layer_np(l);
+    t.layer[l].kblk = tc_layer_kblk(l);
     t.layer[l].nkb = kdim[l] / t.layer[l].kblk;
-    off = align_up(off + tc_layer_bytes(t.planes, np[l], t.layer[l].nkb, t.layer[l].kblk), 256);
+    off = align_up(off + tc_layer_bytes(t.planes, t.layer[l].Np, t.layer[l].nkb, t.layer[l].kblk), 256);
   }
   t.wc_off = off;                       // fp32 [256][256]: Wgf * W2[1:,:]   (colour layer 0 applied to h2 directly)
   off = align_up(off + 256 * 256 * 4, 256);

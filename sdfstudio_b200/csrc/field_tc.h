@@ -6,12 +6,16 @@
 namespace sdfb200 {
 
 
-constexpr int kEpiWarps = 8;                                 // two warpgroups: MMAs + epilogues, 64 tile rows each
+constexpr int kEpiWarps = 8;                                 // two consumer warpgroups: MMAs + epilogues, 64 tile rows each
 constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kTcThreads = kEpiThreads;
-constexpr int kStages = 2;        // weight ring depth (32 KB per stage at two planes, next to the 128 KB A operand)
-constexpr int kKB = 32;           // K per streamed weight block of the 256-row layers (one 32 KB stage at two planes)
-constexpr int kKBMax = 64;        // the 128-row layer (96 live rows) streams K blocks of 64: a full stage
+constexpr int kTcThreads = kEpiThreads + 128;                // + one producer warpgroup (one thread streams the weights)
+// register split after setmaxnreg.  The launch gets 168 per thread (65536 / 384, rounded down to a multiple of 8); the consumers can
+// only take what the producer warpgroup gives back: 256 x (240 - 168) = 128 x (168 - 24)
+constexpr int kConsumerRegs = 240;
+constexpr int kProducerRegs = 24;
+static_assert(2 * (kConsumerRegs - 168) <= 168 - kProducerRegs, "setmaxnreg.inc would wait for registers nobody frees");
+constexpr int kStages = 5;        // weight ring depth (16 KB per stage at two planes, next to the 128 KB A operand)
+constexpr int kKB = 16;           // K per streamed weight block of the 256-row layers (one 16 KB stage at two planes)
 constexpr int kMaxGridDim = 32;
 constexpr int kMaxPe = 60;        // PE columns (2 * 3 * degree), degree <= 10
 constexpr int kPeRows = 64;       // rows reserved for the PE jacobian in the scratch
@@ -27,11 +31,22 @@ __host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 +
 // layers in the order the kernel runs them (and the producer streams them)
 enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
 
+// Weight tile of layer L: N rows (the MMA's N; B0's 96 input rows padded to 128) and the K per streamed block.  Every block is exactly
+// one ring stage (256 x kKB elements per plane): the pack plan, the producer and the MMAs all take the shapes from here.
+__host__ __device__ constexpr int tc_layer_np(int L) { return L == L_B0 ? 128 : 256; }
+__host__ __device__ constexpr int tc_layer_kblk(int L) { return kKB * 256 / tc_layer_np(L); }
+constexpr bool tc_blocks_fill_stages() {
+  for (int L = 0; L < L_COUNT; ++L)
+    if (tc_layer_np(L) * tc_layer_kblk(L) != 256 * kKB || tc_layer_kblk(L) % 16 != 0) return false;
+  return kInK % kKB == 0 && 256 % (2 * kKB) == 0;
+}
+static_assert(tc_blocks_fill_stages(), "every streamed weight block must be one full ring stage of whole K steps");
+
 struct TcLayer {
   unsigned long long w_off;  // byte offset of the packed planes inside the blob
   int Np;                    // rows of the weight tile (MMA N, a multiple of 64)
   int nkb;                   // number of K blocks
-  int kblk;                  // K per block (32 or 64)
+  int kblk;                  // K per block (tc_layer_kblk)
 };
 
 struct TcArgs {

@@ -3,10 +3,11 @@
 // optionally followed IN THE SAME KERNEL by the per-ray compositing (alpha / density -> transmittance -> weights -> rgb, depth,
 // normal, accumulation: cameras/rays.py:131-230, model_components/renderers.py:53-118,171-261,284-295).
 //
-// Persistent CTAs, one 128-point tile at a time.  Two warpgroups own 64 rows of the tile each and run every layer as wgmma
-// m64n64k16 (accumulator in registers, A operand in shared memory, weights streamed by a producer warp through a shared-memory
+// Persistent CTAs, one 128-point tile at a time.  Two consumer warpgroups own 64 rows of the tile each and run every layer as wgmma
+// m64n256k16 (m64n128k16 for B0; accumulator in registers, A operand in shared memory, weights streamed through a shared-memory
 // ring filled by 1-D bulk copies from a pre-packed image).  A warpgroup only reads and writes its own rows of the A operand, so the
-// two warpgroups meet only at the weight ring and at the per-point heads / compositing.
+// two warpgroups meet only at the weight ring and at the per-point heads / compositing.  A third warpgroup gives its registers to
+// the consumers (setmaxnreg) and keeps one thread filling the ring, so no consumer warpgroup stalls while a slot is being freed.
 // Per tile (everything stays on chip except three L2-resident spills):
 //   encode   one thread per point for position, contraction, hash gathers (+ jacobian), one for PE
 //            -> bf16 split planes of the geo input (A operand columns 0..95)
@@ -21,8 +22,6 @@
 //   heads    Laplace density, NeuS alpha, occupancy, normals; optional per-sample outputs
 //   render   (fused mode) segmented prefix product over the rays of the tile in double, weights, per-ray sums
 // MMA = wgmma bf16 x bf16 -> fp32.  bf16x3: a0*w0 + a1*w0 + a0*w1 with a = a0+a1, w = w0+w1 (error ~2^-16 relative, fp32 accumulate).
-// 256 threads: the accumulator alone takes 128 registers per thread, so no warp is spent on a separate producer role (a ninth
-// warp would cap every thread at 168 registers); thread 0 keeps the weight ring filled between its own MMAs.
 #pragma once
 #include "field_tc.h"
 #include "grid.cuh"
@@ -215,70 +214,80 @@ __device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, in
 }
 
 #ifdef SDFB200_TC_TIMING
-// stamps of CTA 0, thread 0, first 16 tiles: [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring order), [15] tile end
+// CTA 0, first 16 tiles, row = tile: clock64() of consumer thread 0 at [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring
+// order), [8] end of the encode, [15] tile end; cycle sums over the tile of [9] consumer thread 0 waiting for weights (full) and
+// [10] the producer waiting for a free ring slot (empty)
 __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
-#define TC_STAMP(k)                                                                                                  \
+#define TC_CLOCK() clock64()
+#define TC_PUT(tno, k, v)                                                                                            \
   do {                                                                                                               \
-    if (blockIdx.x == 0 && tid == 0 && tile_no >= 0 && tile_no < 16) g_tc_timing[tile_no * 32 + (k)] = clock64();                   \
+    if (blockIdx.x == 0 && (tno) >= 0 && (tno) < 16) g_tc_timing[(tno) * 32 + (k)] = (v);                            \
   } while (0)
 #else
-#define TC_STAMP(k) do { } while (0)
+#define TC_CLOCK() 0ll
+#define TC_PUT(tno, k, v) do { } while (0)
 #endif
+#define TC_STAMP(k) do { if (tid == 0) TC_PUT(tile_no, k, TC_CLOCK()); } while (0)
 
-// Weight ring producer (thread 0 of the CTA, between its own MMAs): walks every K-block of every layer of every tile of this CTA in
+// Weight ring producer (one thread of the producer warpgroup): walks every K-block of every layer of every tile of this CTA in
 // consumption order and issues the bulk copy of block j once its slot has been released (all 8 consumer warps are through block
-// j - kStages, which only needs earlier blocks: no cycle).
-struct RingCursor { int tile, L, kb; uint32_t j; };
+// j - kStages).  Every block of every layer is one full stage (tc_blocks_fill_stages).
 template <int P>
-__device__ __forceinline__ void produce_until(RingCursor& pr, uint32_t upto, const TcArgs& a, int nlayers, uint8_t* ring, uint32_t stage_bytes,
-                                              uint64_t* full, uint64_t* empty) {
-  while (pr.j <= upto && pr.tile < a.n_tiles) {
-    const TcLayer& ly = a.layer[pr.L];
-    const uint32_t bytes = (uint32_t)P * ly.Np * ly.kblk * 2;
-    const int s = pr.j % kStages;
-    mbar_wait(&empty[s], ((pr.j / kStages) & 1) ^ 1);
-    mbar_arrive_expect_tx(&full[s], bytes);
-    bulk_g2s(ring + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(a.blob) + ly.w_off + (size_t)pr.kb * bytes, bytes, &full[s]);
-    ++pr.j;
-    if (++pr.kb == ly.nkb) {
-      pr.kb = 0;
-      if (++pr.L == nlayers) { pr.L = 0; pr.tile += gridDim.x; }
+__device__ __forceinline__ void produce_all(const TcArgs& a, int nlayers, uint8_t* ring, uint64_t* full, uint64_t* empty) {
+  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;
+  uint32_t j = 0;
+  int tile_no = 0;
+  for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
+    long long waited = 0;
+    for (int L = 0; L < nlayers; ++L) {
+      const TcLayer& ly = a.layer[L];
+      for (int kb = 0; kb < ly.nkb; ++kb, ++j) {
+        const int s = j % kStages;
+        const long long w0 = TC_CLOCK();
+        mbar_wait(&empty[s], ((j / kStages) & 1) ^ 1);
+        waited += TC_CLOCK() - w0;
+        mbar_arrive_expect_tx(&full[s], kStageBytes);
+        bulk_g2s(ring + (size_t)s * kStageBytes, reinterpret_cast<const uint8_t*>(a.blob) + ly.w_off + (size_t)kb * kStageBytes, kStageBytes, &full[s]);
+      }
     }
+    TC_PUT(tile_no, 10, waited);
   }
 }
 
-// All MMAs of one layer for the 64 rows of a warpgroup: acc (+)= A[rows, K] W^T, the weight K-blocks taken from the ring in order.
-// Every consumer warp releases a ring slot once its own MMAs on it are complete (empty barrier count = 8 warps).
-template <int P>
-__device__ __forceinline__ void layer_mma(float (&acc)[4][32], const TcLayer& ly, bool zero, uint32_t a_base, uint8_t* ring, uint32_t stage_bytes,
-                                          uint64_t* full, uint64_t* empty, uint32_t& it, int lane, bool producer, RingCursor& pr, const TcArgs& a,
-                                          int nlayers) {
+// All MMAs of layer L for the 64 rows of a warpgroup: acc (+)= A[rows, K] W^T with one m64nN wgmma per product and K step (N = 256, or
+// 128 for B0: acc[0..1]), the weight K-blocks taken from the ring in order.  Every consumer warp releases a slot once its MMAs on it are
+// complete (empty barrier count = 8 warps).  Each block is drained before the next is issued: with the producer in its own warpgroup and
+// 5 stages, keeping one block in flight (wait_group 1) measured no faster.
+template <int P, int L>
+__device__ __forceinline__ void layer_mma(float (&acc)[4][32], const TcLayer& ly, bool zero, uint32_t a_base, const uint8_t* ring, uint64_t* full,
+                                          uint64_t* empty, uint32_t& it, int lane, long long& waited) {
+  constexpr int N = tc_layer_np(L);
+  constexpr int KSTEPS = tc_layer_kblk(L) / 16;              // K steps per ring stage
+  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;
+  constexpr uint32_t lbo_b = N * 16, plane_b = N * KSTEPS * 16 * 2;
+  float (&d)[N / 2] = *reinterpret_cast<float (*)[N / 2]>(&acc[0][0]);
   if (zero) {
 #pragma unroll
-    for (int c = 0; c < 4; ++c)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
   }
-  const int nch = ly.Np / 64;
-  const uint32_t lbo_b = (uint32_t)ly.Np * 16, plane_b = (uint32_t)ly.Np * ly.kblk * 2;
-  const int ksteps = ly.kblk / 16;
   for (int kb = 0; kb < ly.nkb; ++kb, ++it) {
-    if (producer) produce_until<P>(pr, it + kStages - 1, a, nlayers, ring, stage_bytes, full, empty);
-    __syncwarp();
     const int s = it % kStages;
+    const long long w0 = TC_CLOCK();
     mbar_wait(&full[s], (it / kStages) & 1);
-    const uint32_t wbase = smem_u32(ring + (size_t)s * stage_bytes);
-    wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+    waited += TC_CLOCK() - w0;
+    const uint32_t wbase = smem_u32(ring + (size_t)s * kStageBytes);
+    wg_fence_acc(d);
     wg_arrive();
-    for (int j = 0; j < ksteps; ++j) {
-      const int kstep = kb * ksteps + j;
+#pragma unroll
+    for (int j = 0; j < KSTEPS; ++j) {
+      const int kstep = kb * KSTEPS + j;
       const uint64_t a0 = make_smem_desc(a_base + kstep * 2 * 2048, 2048, 128);
       const uint64_t a1 = make_smem_desc(a_base + kAPlane + kstep * 2 * 2048, 2048, 128);
-      wgmma_kstep_ss<P, 4>(acc, a0, a1, wbase + j * 2 * lbo_b, plane_b, lbo_b, nch);
+      wgmma_kstep_wide_ss<P, N>(d, a0, a1, wbase + j * 2 * lbo_b, plane_b, lbo_b);
     }
     wg_commit();
     wg_wait<0>();
-    wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
+    wg_fence_acc(d);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
   }
@@ -297,7 +306,7 @@ __device__ __forceinline__ void store_pair(uint8_t* abuf, int col, int row, floa
 template <int P, int LAYOUT>
 __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constant__ TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;        // one weight K-block, all planes (the 128-row layer: K blocks of 64)
+  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;        // one weight K-block, all planes (the 128-row layer: K blocks of 32)
   uint8_t* abuf = smem;                                                // A operand of every layer: [P][32 chunks][128 rows][16 B]
   uint8_t* ring = smem + P * kAPlane;
   float* fbuf = reinterpret_cast<float*>(ring + kStages * kStageBytes);
@@ -326,6 +335,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   }
   __syncthreads();
 
+  // ============================== producer warpgroup: one thread streams the weights ==============================
+  if (tid >= kEpiThreads) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (tid == kEpiThreads) produce_all<P>(a, nlayers, ring, full, empty);
+    return;
+  }
+  setmaxnreg_inc<kConsumerRegs>();
+
   // ============================== two warpgroups, 64 rows of the tile each ==============================
   const int wg = warp >> 2, t = tid & 127;
   const int wrow0 = wg * 64;
@@ -351,8 +368,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   const uint64_t pol_table = l2_policy(TCV_POL_TABLE);
   const uint64_t pol_keep = l2_policy_evict_normal();
   uint32_t it = 0;
-  const bool producer = tid == 0;
-  RingCursor pr{(int)blockIdx.x, 0, 0, 0u};
+  long long waited = 0;
   float acc[4][32];
 #define SYNC_A()                \
   do {                          \
@@ -361,7 +377,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   } while (0)
 #define LAYER(L, zero)                                                                                 \
   do {                                                                                                 \
-    layer_mma<P>(acc, a.layer[L], zero, a_base, ring, kStageBytes, full, empty, it, lane, producer, pr, a, nlayers); \
+    layer_mma<P, L>(acc, a.layer[L], zero, a_base, ring, full, empty, it, lane, waited);               \
     named_sync(wg_bar, 128); /* every warp of the warpgroup is done reading this layer's A operand */  \
     TC_STAMP(1 + (L));                                                                                 \
   } while (0)
@@ -370,6 +386,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
     ++tile_no;
     TC_STAMP(0);
+    waited = 0;
     // ---------------- encode: thread t < 64 hash gathers of row wrow0 + t, thread t >= 64 PE / x of row wrow0 + t - 64 ----------------
     {
       const int row = wrow0 + (t & 63);
@@ -386,6 +403,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
       }
     }
     SYNC_A();
+    TC_STAMP(8);
 
     // ---------------- G0 -> E0: h1 = softplus(z1) -> A ; softplus'(z1) -> scratch ----------------
     LAYER(L_G0, true);
@@ -700,6 +718,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     }
     named_sync(3, kEpiThreads);     // `hs` / `racc` are rewritten by the next tile
     TC_STAMP(15);
+    if (tid == 0) TC_PUT(tile_no, 9, waited);
   }
 #undef SYNC_A
 #undef LAYER
