@@ -72,7 +72,6 @@ inline int persistent_ctas() {
 }
 
 __host__ __device__ inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
-__host__ __device__ inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
 
 // nn.Softplus(beta=100), threshold 20 (sdf_field.py:365)
 __device__ __forceinline__ float softplus100(float z) {

@@ -1,33 +1,12 @@
-// Host side of the fused tensor-core field kernel (csrc/field_tc_kernel.cuh): packed-weight plan, weight packing kernels,
-// launch dispatch.  See field_tc_kernel.cuh for the kernel itself.
+// Host side of the fused tensor-core field kernel (csrc/field_tc_kernel.cuh): packed-weight plan, weight packing (tc_pack,
+// tc_linear.cu), launch dispatch.  See field_tc_kernel.cuh for the kernel itself.
 #include "field_tc.h"
 #include "tc_common.cuh"
+#include "tc_linear.h"
 
 namespace sdfb200 {
 using namespace tc;
-
-// pack fp32 W (row n, column k at W[rowmap(n)*ldw + colmap(k)]) into bf16 split planes: K-blocked, canonical K-major no-swizzle
-// layout:  [K-block][plane][k/8][row][8 bf16]
-struct IdxMap { short src[kInK]; };   // packed index -> source index (-1 = zero); identity when unused
-__global__ void k_tc_pack(const float* __restrict__ W, int ldw, int N, int K, int Np, int nblocks, int kblk, int planes, int use_colmap, const IdxMap colmap,
-                          int use_rowmap, const IdxMap rowmap, __nv_bfloat16* __restrict__ out) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nblocks * Np * kblk) return;
-  const int kk = idx % kblk;
-  const int n = (idx / kblk) % Np;
-  const int b = idx / (kblk * Np);
-  const int k = b * kblk + kk;
-  const int ks = use_colmap ? (k < kInK ? colmap.src[k] : -1) : (k < K ? k : -1);
-  const int ns = use_rowmap ? (n < kInK ? rowmap.src[n] : -1) : (n < N ? n : -1);
-  const float w = (ns >= 0 && ks >= 0) ? W[(size_t)ns * ldw + ks] : 0.f;
-  const __nv_bfloat16 hi = __float2bfloat16_rn(w);
-  const __nv_bfloat16 lo = __float2bfloat16_rn(w - __bfloat162float(hi));
-  const size_t plane_elems = (size_t)Np * kblk;
-  const size_t base = (size_t)b * planes * plane_elems;
-  const size_t off = (size_t)(kk / 8) * (Np * 8) + (size_t)n * 8 + (kk % 8);
-  out[base + off] = hi;
-  if (planes > 1) out[base + plane_elems + off] = lo;
-}
+static_assert(sizeof(TcIdxMap) == kInK * sizeof(short), "one index map entry per column of the small-K operands");
 
 // colour layer 0 pre-multiplied with the (activation-free) last geo layer: Wc[o][k] = sum_j Wc0[o][33+j] W2[1+j][k],
 // bias[o] = bc0[o] + sum_j Wc0[o][33+j] b2[1+j]        (sdf_field.py:406-410 feeds :576-592)
@@ -60,13 +39,12 @@ struct TcPlan {
 
 static void make_tc_plan(const sdfb200_field_t& f, const FieldPlan& p, TcPlan& t) {
   t.planes = f.precision == SDFB200_PRECISION_BF16X3 ? 2 : 1;
-  const int kdim[L_COUNT] = {kInK, 256, 256, 256, kInK, 256, 256};
   size_t off = p.tc_off;
   for (int l = 0; l < L_COUNT; ++l) {
     t.layer[l].w_off = off;
     t.layer[l].Np = tc_layer_np(l);
     t.layer[l].kblk = tc_layer_kblk(l);
-    t.layer[l].nkb = kdim[l] / t.layer[l].kblk;
+    t.layer[l].nkb = tc_layer_k(l) / t.layer[l].kblk;
     off = align_up(off + tc_layer_bytes(t.planes, t.layer[l].Np, t.layer[l].nkb, t.layer[l].kblk), 256);
   }
   t.wc_off = off;                       // fp32 [256][256]: Wgf * W2[1:,:]   (colour layer 0 applied to h2 directly)
@@ -107,19 +85,13 @@ size_t field_tc_workspace_floats(const sdfb200_field_t& f, const FieldPlan&, int
 int field_tc_pack(const sdfb200_field_t& f, const FieldPlan& p, char* blob, cudaStream_t st) {
   TcPlan t;
   make_tc_plan(f, p, t);
-  IdxMap ident;
-  for (int i = 0; i < kInK; ++i) ident.src[i] = (short)i;
-  auto pack = [&](int L, const float* W, int ldw, int N, int K, const IdxMap* colmap, const IdxMap* rowmap) -> int {
+  auto pack = [&](int L, const float* W, int ldw, int N, int K, const TcIdxMap* colmap, const TcIdxMap* rowmap) -> int {
     const TcLayer& ly = t.layer[L];
-    const int tot = ly.nkb * ly.Np * ly.kblk;
-    k_tc_pack<<<(tot + 255) / 256, 256, 0, st>>>(W, ldw, N, K, ly.Np, ly.nkb, ly.kblk, t.planes, colmap != nullptr, colmap ? *colmap : ident, rowmap != nullptr,
-                                                 rowmap ? *rowmap : ident, (__nv_bfloat16*)(blob + ly.w_off));
-    SDFB_LAUNCHED("k_tc_pack");
-    return 0;
+    return tc_pack(W, ldw, 0, N, K, ly.Np, ly.kblk, ly.nkb, t.planes, rowmap, colmap, blob + ly.w_off, st);
   };
   const LayerPlan &g0 = p.geo[0], &g1 = p.geo[1], &g2 = p.geo[2], &c0 = p.col[0], &c1 = p.col[1];
   // geo input, kernel column order [grid(32) | PE | x | 0]  <-  reference order [x(3) | PE | grid]  (sdf_field.py:391-396)
-  IdxMap gin;
+  TcIdxMap gin;
   for (int i = 0; i < kInK; ++i) gin.src[i] = -1;
   for (int i = 0; i < p.grid_dim; ++i) gin.src[i] = (short)(3 + p.pe_dim + i);
   for (int i = 0; i < p.pe_dim; ++i) gin.src[32 + i] = (short)(3 + i);
@@ -136,7 +108,7 @@ int field_tc_pack(const sdfb200_field_t& f, const FieldPlan& p, char* blob, cuda
   if ((r = pack(L_C0H, (const float*)(blob + t.wc_off), 256, 256, 256, nullptr, nullptr))) return r;
   // misc operand, kernel order: chunk 0 = [grad(3), n.v, 0 x4] (written per tile by the epilogue), then the static part
   // [x(3), dir-enc(27), appearance] prepared by the gather warps
-  IdxMap cm;
+  TcIdxMap cm;
   for (int i = 0; i < kInK; ++i) cm.src[i] = -1;
   cm.src[0] = 30; cm.src[1] = 31; cm.src[2] = 32;
   if (f.use_n_dot_v) cm.src[3] = (short)(289 + f.appearance_dim);
@@ -190,6 +162,3 @@ int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* b
 }
 
 }  // namespace sdfb200
-
-
-

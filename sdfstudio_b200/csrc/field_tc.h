@@ -31,14 +31,16 @@ __host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 +
 // layers in the order the kernel runs them (and the producer streams them)
 enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
 
-// Weight tile of layer L: N rows (the MMA's N; B0's 96 input rows padded to 128) and the K per streamed block.  Every block is exactly
-// one ring stage (256 x kKB elements per plane): the pack plan, the producer and the MMAs all take the shapes from here.
+// Weight tile of layer L: N rows (the MMA's N; B0's 96 input rows padded to 128), K (the geo input and the colour misc operand are
+// kInK wide) and the K per streamed block.  Every block is exactly one ring stage (256 x kKB elements per plane): the pack plan, the
+// producer and the MMAs all take the shapes from here.
 __host__ __device__ constexpr int tc_layer_np(int L) { return L == L_B0 ? 128 : 256; }
+__host__ __device__ constexpr int tc_layer_k(int L) { return L == L_G0 || L == L_C0MISC ? kInK : 256; }
 __host__ __device__ constexpr int tc_layer_kblk(int L) { return kKB * 256 / tc_layer_np(L); }
 constexpr bool tc_blocks_fill_stages() {
   for (int L = 0; L < L_COUNT; ++L)
-    if (tc_layer_np(L) * tc_layer_kblk(L) != 256 * kKB || tc_layer_kblk(L) % 16 != 0) return false;
-  return kInK % kKB == 0 && 256 % (2 * kKB) == 0;
+    if (tc_layer_np(L) * tc_layer_kblk(L) != 256 * kKB || tc_layer_kblk(L) % 16 != 0 || tc_layer_k(L) % tc_layer_kblk(L) != 0) return false;
+  return true;
 }
 static_assert(tc_blocks_fill_stages(), "every streamed weight block must be one full ring stage of whole K steps");
 

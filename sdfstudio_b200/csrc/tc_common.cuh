@@ -42,11 +42,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// many-thread wait: back off between polls so the spinning warps do not eat the issue slots of the MMA / producer warps
-__device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity) {
-  while (!mbar_try_wait(bar, parity)) __nanosleep(40);
-}
-
 // ---- 1-D bulk async copy global -> shared (completes on an mbarrier with complete_tx) -----------------------------
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
@@ -155,29 +150,10 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 template <uint32_t R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// ---- streaming (evict_first) global accesses for the per-CTA scratch ------------------------------------------------
-__device__ __forceinline__ void st_stream(void* p, uint4 v, uint64_t pol) {
-  asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void st_stream(void* p, float4 v, uint64_t pol) {
-  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void st_stream(float* p, float v, uint64_t pol) {
-  asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(p), "f"(v), "l"(pol) : "memory");
-}
-__device__ __forceinline__ uint4 ld_stream_u4(const void* p, uint64_t pol) {
-  uint4 v;
-  asm volatile("ld.global.L2::cache_hint.v4.b32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol) : "memory");
-  return v;
-}
+// ---- L2-hinted global load (per-CTA scratch of the fused kernel) -------------------------------------------------
 __device__ __forceinline__ float ld_stream_f1(const float* p, uint64_t pol) {
   float v;
   asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol) : "memory");
-  return v;
-}
-__device__ __forceinline__ float4 ld_stream_f4(const void* p, uint64_t pol) {
-  float4 v;
-  asm volatile("ld.global.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol) : "memory");
   return v;
 }
 
@@ -193,8 +169,110 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t&
   const float ah = __uint_as_float(hi << 16), bh = __uint_as_float(hi & 0xFFFF0000u);
   lo = pack_bf16x2(a - ah, b - bh);
 }
-__device__ __forceinline__ float bf16lo_to_f32(uint32_t packed) { return __uint_as_float(packed << 16); }
-__device__ __forceinline__ float bf16hi_to_f32(uint32_t packed) { return __uint_as_float(packed & 0xFFFF0000u); }
+
+// ---- A operand in shared memory: [plane][k/8][128 rows][8 bf16], `plane` bytes apart ------------------------------------
+constexpr uint32_t kAChunk = 128 * 16;   // one 8-column chunk of a 128-row plane (the descriptor's LBO)
+// byte offset of element (row, col) inside one plane
+__device__ __forceinline__ uint32_t a_off(int row, int col) { return (uint32_t)(col >> 3) * kAChunk + (uint32_t)row * 16u + (uint32_t)(col & 7) * 2u; }
+// one element, split into P bf16 planes
+template <int P>
+__device__ __forceinline__ void store_a(uint8_t* a, uint32_t plane, int row, int col, float v) {
+  const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+  const uint32_t off = a_off(row, col);
+  *reinterpret_cast<__nv_bfloat16*>(a + off) = hi;
+  if (P > 1) *reinterpret_cast<__nv_bfloat16*>(a + plane + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
+}
+// two adjacent columns (an accumulator element pair): one 4-byte unit per plane, already split
+template <int P>
+__device__ __forceinline__ void store_a_pair(uint8_t* a, uint32_t plane, int row, int col, uint32_t hi, uint32_t lo) {
+  const uint32_t off = a_off(row, col);
+  *reinterpret_cast<uint32_t*>(a + off) = hi;
+  if (P > 1) *reinterpret_cast<uint32_t*>(a + plane + off) = lo;
+}
+template <int P>
+__device__ __forceinline__ void store_a_pair(uint8_t* a, uint32_t plane, int row, int col, float v0, float v1) {
+  uint32_t hi, lo;
+  split2(v0, v1, hi, lo);
+  store_a_pair<P>(a, plane, row, col, hi, lo);
+}
+// one 16-byte chunk (8 consecutive columns of one row), already split
+template <int P>
+__device__ __forceinline__ void store_a_chunk(uint8_t* a, uint32_t plane, int row, int chunk, uint4 hi, uint4 lo) {
+  *reinterpret_cast<uint4*>(a + (size_t)chunk * kAChunk + row * 16) = hi;
+  if (P > 1) *reinterpret_cast<uint4*>(a + plane + (size_t)chunk * kAChunk + row * 16) = lo;
+}
+template <int P>
+__device__ __forceinline__ void store_a_chunk(uint8_t* a, uint32_t plane, int row, int chunk, const float (&v)[8]) {
+  uint32_t hi[4], lo[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hi[e], lo[e]);
+  store_a_chunk<P>(a, plane, row, chunk, make_uint4(hi[0], hi[1], hi[2], hi[3]), make_uint4(lo[0], lo[1], lo[2], lo[3]));
+}
+// descriptor of one plane of a warpgroup's 64 rows (shared address `base`) at MMA K step `kstep`
+__device__ __forceinline__ uint64_t a_desc(uint32_t base, int kstep) { return make_smem_desc(base + kstep * 2 * kAChunk, kAChunk, 128); }
+
+// ---- accumulator fragment ---------------------------------------------------------------------------------------
+// Thread t of the warpgroup whose 64 rows start at row0 holds rows r0 = frag_row0(row0, t) and r0 + 8 and, in every 8-column block,
+// columns cq = frag_cq(t) and cq + 1.  Element i of n64 block c (the layout next to wgmma64_ss) sits at (frag_row(r0, i), frag_col(cq, c, i)).
+__device__ __forceinline__ int frag_row0(int row0, int t) { return row0 + (t >> 5) * 16 + ((t & 31) >> 2); }
+__device__ __forceinline__ int frag_cq(int t) { return (t & 3) * 2; }
+template <typename T>   // int, or long long for a global row index
+__device__ __forceinline__ T frag_row(T r0, int i) { return r0 + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int cq, int c, int i) { return c * 64 + (i >> 2) * 8 + cq + (i & 1); }
+
+// ---- weight ring ------------------------------------------------------------------------------------------------
+// S stages of `bytes` each; block j of the stream goes to slot j % S.  full[s] (count 1) completes when a block has landed in slot s,
+// empty[s] (count = the consumers' arrivals, set by the kernel) when the consumers have released it.  Both functions add the cycles
+// they spent waiting to *waited in the timing build of the fused kernel (tools/tc_timing.py).
+#ifdef SDFB200_TC_TIMING
+#define TC_CLOCK() clock64()
+#else
+#define TC_CLOCK() 0ll
+#endif
+// producer (one thread): once the slot of stream block j has been released, copy block kb of the packed image `blocks` into it
+template <int S>
+__device__ __forceinline__ void ring_fill(uint8_t* ring, uint64_t* full, uint64_t* empty, uint32_t j, const uint8_t* blocks, int kb, uint32_t bytes,
+                                          long long* waited = nullptr) {
+  const int s = j % S;
+  const long long w0 = TC_CLOCK();
+  mbar_wait(&empty[s], ((j / S) & 1) ^ 1);
+  if (waited) *waited += TC_CLOCK() - w0;
+  mbar_arrive_expect_tx(&full[s], bytes);
+  bulk_g2s(ring + (size_t)s * bytes, blocks + (size_t)kb * bytes, bytes, &full[s]);
+}
+// consumer: wait until block j is in its slot; returns the slot, which the caller releases (arrives on empty[slot]) when done with it
+template <int S>
+__device__ __forceinline__ int ring_wait(uint64_t* full, uint32_t j, long long* waited = nullptr) {
+  const int s = j % S;
+  const long long w0 = TC_CLOCK();
+  mbar_wait(&full[s], (j / S) & 1);
+  if (waited) *waited += TC_CLOCK() - w0;
+  return s;
+}
+
+// ---- fast softplus_100 ------------------------------------------------------------------------------------------
+// softplus_100 and its derivative through MUFU ex2 / lg2 / rcp: ~10 instructions instead of the ~100 of log1pf(expf(.)).  t = 100 z.
+// Absolute error ~1e-7 on h (the quantity that feeds the next layer), i.e. at the level of fp32 rounding of the reference's own
+// log1p(exp(.)).
+__device__ __forceinline__ float fast_ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float fast_lg2(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float fast_rcp(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ void softplus100_fast(float z, float& h, float& dsig) {
+  // exp(100 z) = 2^(z * 100 log2 e); log1p(e)/100 = lg2(1+e) * ln2/100.  For small e, 1+e rounds e to ~6e-8 absolute, i.e. an
+  // absolute error of ~4e-10 on h: irrelevant next to the bf16x3 operand rounding (2^-17 relative).
+  const float e = fast_ex2(fminf(z, 0.3f) * 144.26950408889634f);
+  const float u = 1.0f + e;
+  const bool lin = z > 0.2f;                                            // PyTorch's softplus threshold: beta*x > 20
+  h = lin ? z : fast_lg2(u) * 0.006931471805599453f;
+  dsig = lin ? 1.0f : e * fast_rcp(u);
+}
+__device__ __forceinline__ float softplus100_fast(float z) {
+  float h, dsig;
+  softplus100_fast(z, h, dsig);
+  return h;
+}
+// softplus_100'(z) from h = softplus_100(z):  sigma(100 z) = 1 - exp(-100 h)
+__device__ __forceinline__ float dsoftplus100_fast_from_h(float h) { return 1.0f - fast_ex2(h * -144.26950408889634f); }
 
 }  // namespace tc
 }  // namespace sdfb200

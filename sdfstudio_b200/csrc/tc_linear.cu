@@ -18,29 +18,22 @@ constexpr int kThreadsL = 288;    // two MMA / epilogue warpgroups + weight prod
 constexpr uint32_t kAPlaneL = 32 * 2048;                          // one plane of the A operand: [K/8 (<= 32)][128 rows][16 B]
 constexpr uint32_t kRingBytesL = kStagesL * 2 * 256 * kKBL * 2;   // weight ring at its largest (2 planes, N = 256)
 
-// softplus_100 / its derivative through MUFU ex2 / lg2 (same formulas as the fused kernel, field_tc.cu): ~10 instructions instead of
-// the ~100 of log1pf(expf(.)) -- at 64 elements per thread the accurate versions cost more than the tensor-core GEMM they follow
-__device__ __forceinline__ float tcl_ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float tcl_lg2(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float tcl_softplus100(float z) {
-  const float e = tcl_ex2(fminf(z, 0.3f) * 144.26950408889634f);
-  return z > 0.2f ? z : tcl_lg2(1.0f + e) * 0.006931471805599453f;
-}
-__device__ __forceinline__ float tcl_dsoftplus_from_h(float h) { return 1.0f - tcl_ex2(h * -144.26950408889634f); }
-
-// fp32 W[n, k] (row stride ldw) -> bf16 split planes [K-block][plane][k/8][n][8], zero padded to (Ncp, nblocks*32)
-// trans != 0: the source holds the matrix transposed (element (n, k) at W[k * ldw + n]) -- the dgrad GEMM dX = dY W packs W^T this way
-__global__ void k_tcl_pack(const float* __restrict__ W, int ldw, int N, int K, int Ncp, int nblocks, int planes, int trans, __nv_bfloat16* __restrict__ out) {
+// one thread per packed element of every plane; see tc_pack (tc_linear.h)
+__global__ void k_tc_pack(const float* __restrict__ W, int ldw, int trans, int N, int K, int Np, int kblk, int nblocks, int planes, int use_rowmap,
+                          const TcIdxMap rowmap, int use_colmap, const TcIdxMap colmap, __nv_bfloat16* __restrict__ out) {
+  constexpr int kMap = (int)(sizeof(TcIdxMap) / sizeof(short));
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= nblocks * Ncp * kKBL) return;
-  const int kk = idx % kKBL;
-  const int n = (idx / kKBL) % Ncp;
-  const int b = idx / (kKBL * Ncp);
-  const int k = b * kKBL + kk;
-  const float w = (n < N && k < K) ? (trans ? W[(size_t)k * ldw + n] : W[(size_t)n * ldw + k]) : 0.f;
+  if (idx >= nblocks * Np * kblk) return;
+  const int kk = idx % kblk;
+  const int n = (idx / kblk) % Np;
+  const int b = idx / (kblk * Np);
+  const int k = b * kblk + kk;
+  const int ks = use_colmap ? (k < kMap ? colmap.src[k] : -1) : (k < K ? k : -1);
+  const int ns = use_rowmap ? (n < kMap ? rowmap.src[n] : -1) : (n < N ? n : -1);
+  const float w = (ns >= 0 && ks >= 0) ? (trans ? W[(size_t)ks * ldw + ns] : W[(size_t)ns * ldw + ks]) : 0.f;
   const __nv_bfloat16 hi = __float2bfloat16_rn(w);
-  const size_t plane_elems = (size_t)Ncp * kKBL;
-  const size_t off = (size_t)b * planes * plane_elems + (size_t)(kk / 8) * (Ncp * 8) + (size_t)n * 8 + (kk % 8);
+  const size_t plane_elems = (size_t)Np * kblk;
+  const size_t off = (size_t)b * planes * plane_elems + (size_t)(kk / 8) * (Np * 8) + (size_t)n * 8 + (kk % 8);
   out[off] = hi;
   if (planes > 1) out[off + plane_elems] = __float2bfloat16_rn(w - __bfloat162float(hi));
 }
@@ -87,8 +80,8 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
       uint32_t hi[4], lo[4];
 #pragma unroll
       for (int e = 0; e < 4; ++e) split2(v[2 * e], v[2 * e + 1], hi[e], lo[e]);
-      *reinterpret_cast<uint4*>(a_smem + (size_t)ch * 2048 + r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-      if (P > 1) *reinterpret_cast<uint4*>(a_smem + kAPlaneL + (size_t)ch * 2048 + r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+      *reinterpret_cast<uint4*>(a_smem + (size_t)ch * kAChunk + r * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+      if (P > 1) *reinterpret_cast<uint4*>(a_smem + kAPlaneL + (size_t)ch * kAChunk + r * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
     }
     fence_async_smem();
   }
@@ -97,18 +90,14 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
   if (warp == 8) {
     // ---------------- weight producer ----------------
     if (lane == 0) {
-      for (int b = 0; b < nblocks; ++b) {
-        const int s = b % kStagesL;
-        mbar_wait(&empty[s], ((b / kStagesL) & 1) ^ 1);
-        mbar_arrive_expect_tx(&full[s], stage_bytes);
-        bulk_g2s(ring + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(a.Wp) + (size_t)b * stage_bytes, stage_bytes, &full[s]);
-      }
+      for (int b = 0; b < nblocks; ++b)
+        ring_fill<kStagesL>(ring, full, empty, b, reinterpret_cast<const uint8_t*>(a.Wp), b, stage_bytes);
     }
     return;
   }
   // ---------------- two warpgroups: MMAs over 64 rows each, then the epilogue from the accumulator registers ----------------
   const int wg = warp >> 2, t = tid & 127;
-  const int rw = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c2 = (t & 3) * 2;      // first of the thread's two rows (+8), column offset
+  const int rw = frag_row0(wg * 64, t), c2 = frag_cq(t);
   const int nch = a.Np64 / 64;
   float acc[4][32];
 #pragma unroll
@@ -118,17 +107,14 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
   const uint32_t lbo_b = (uint32_t)a.Np64 * 16, plane_b = (uint32_t)a.Np64 * kKBL * 2;
   const uint32_t abase = smem_u32(a_smem) + wg * 64 * 16;
   for (int b = 0; b < nblocks; ++b) {
-    const int s = b % kStagesL;
-    mbar_wait(&full[s], (b / kStagesL) & 1);
+    const int s = ring_wait<kStagesL>(full, b);
     const uint32_t wbase = smem_u32(ring + (size_t)s * stage_bytes);
     wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
     wg_arrive();
 #pragma unroll
     for (int j = 0; j < kKBL / 16; ++j) {
       const int kstep = b * (kKBL / 16) + j;
-      const uint64_t a0 = make_smem_desc(abase + kstep * 2 * 2048, 2048, 128);
-      const uint64_t a1 = make_smem_desc(abase + kAPlaneL + kstep * 2 * 2048, 2048, 128);
-      wgmma_kstep_ss<P, 4>(acc, a0, a1, wbase + j * 2 * lbo_b, plane_b, lbo_b, nch);
+      wgmma_kstep_ss<P, 4>(acc, a_desc(abase, kstep), a_desc(abase + kAPlaneL, kstep), wbase + j * 2 * lbo_b, plane_b, lbo_b, nch);
     }
     wg_commit();
     wg_wait<0>();
@@ -139,8 +125,8 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
-      const int n = c * 64 + (i >> 2) * 8 + c2;           // column inside this N chunk (even; n + 1 < Ncp when n < Ncp)
-      const long long m = m0 + rw + 8 * ((i >> 1) & 1);
+      const int n = frag_col(c2, c, i);                  // column inside this N chunk (even; n + 1 < Ncp when n < Ncp)
+      const long long m = frag_row(m0 + rw, i);
       if (c < nch && n < a.Ncp && m < a.M) {
         float y[2] = {acc[c][i], acc[c][i + 1]};
         float2* yp = reinterpret_cast<float2*>(a.Y + m * (long long)a.ldy + a.n0 + n);
@@ -149,14 +135,14 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
           if (EPI == TCL_MUL_DSOFTPLUS) {
 #pragma unroll
             for (int j = 0; j < 2; ++j)
-              if (a.n0 + n + j < a.aux_cols) y[j] *= tcl_dsoftplus_from_h(__ldg(a.aux + m * (long long)a.ldaux + a.n0 + n + j));
+              if (a.n0 + n + j < a.aux_cols) y[j] *= dsoftplus100_fast_from_h(__ldg(a.aux + m * (long long)a.ldaux + a.n0 + n + j));
           } else {
             const float2 bv = a.bias != nullptr ? __ldg(reinterpret_cast<const float2*>(a.bias + n)) : make_float2(0.f, 0.f);
             const float b2[2] = {bv.x, bv.y};
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
               y[j] += b2[j];
-              if (EPI == TCL_SOFTPLUS) y[j] = tcl_softplus100(y[j]);
+              if (EPI == TCL_SOFTPLUS) y[j] = softplus100_fast(y[j]);
               if (EPI == TCL_RELU) y[j] = fmaxf(y[j], 0.f);
             }
           }
@@ -186,6 +172,16 @@ int launch_linear(int epi, const LinArgs& a, size_t smem, unsigned grid, cudaStr
 }
 }  // namespace
 
+int tc_pack(const float* W, int ldw, int trans, int N, int K, int Np, int kblk, int nblocks, int planes, const TcIdxMap* rowmap,
+            const TcIdxMap* colmap, void* out, cudaStream_t st) {
+  const TcIdxMap none{};
+  const int tot = nblocks * Np * kblk;
+  k_tc_pack<<<(tot + 255) / 256, 256, 0, st>>>(W, ldw, trans, N, K, Np, kblk, nblocks, planes, rowmap != nullptr, rowmap ? *rowmap : none,
+                                               colmap != nullptr, colmap ? *colmap : none, (__nv_bfloat16*)out);
+  SDFB_LAUNCHED("k_tc_pack");
+  return 0;
+}
+
 int tc_gemm(int planes, int epi, const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy, int64_t M, int Np, int Kp,
             const float* aux, int ldaux, int aux_cols, void* scratch, cudaStream_t st) {
   return tc_gemm_ex(planes, epi, X, ldx, W, Kp, 0, Np, Kp, bias, Y, ldy, M, Np, Kp, aux, ldaux, aux_cols, scratch, st);
@@ -206,11 +202,9 @@ int tc_gemm_ex(int planes, int epi, const float* X, int ldx, const float* W, int
       const int Kc = Kp - k0 < 256 ? Kp - k0 : 256;
       const int Kc32 = (Kc + 31) / 32 * 32, nblocks = Kc32 / kKBL;
       const int Np64 = (Nc + 63) / 64 * 64;
-      const int tot = nblocks * Np64 * kKBL;
       const float* wsrc = trans_w ? W + (size_t)k0 * ldw + n0 : W + (size_t)n0 * ldw + k0;
       const int nv = Nw - n0 < Nc ? (Nw - n0 > 0 ? Nw - n0 : 0) : Nc, kv = Kw - k0 < Kc ? (Kw - k0 > 0 ? Kw - k0 : 0) : Kc;
-      k_tcl_pack<<<(tot + 255) / 256, 256, 0, st>>>(wsrc, ldw, nv, kv, Np64, nblocks, planes, trans_w, (__nv_bfloat16*)scratch);
-      SDFB_LAUNCHED("k_tcl_pack");
+      if (int r = tc_pack(wsrc, ldw, trans_w, nv, kv, Np64, kKBL, nblocks, planes, nullptr, nullptr, scratch, st)) return r;
       LinArgs a;
       a.X = X + k0; a.ldx = ldx; a.M = M; a.Kc32 = Kc32; a.Kvalid = kv; a.Wp = (const __nv_bfloat16*)scratch; a.Ncp = Nc; a.Np64 = Np64;
       a.bias = bias ? bias + n0 : nullptr; a.Y = Y; a.ldy = ldy; a.n0 = n0; a.accumulate = k0 > 0; a.final_chunk = k0 + 256 >= Kp;

@@ -3,30 +3,13 @@
 // (SS) or in registers (RS), weights streamed through a 2-stage ring by 1-D bulk copies, accumulator in registers (two warpgroups
 // of 64 rows).  Lets the descriptors / layouts be validated in isolation on the GPU.
 #include "tc_common.cuh"
+#include "tc_linear.h"
 #include "../../include/sdfb200_debug.h"
 
 namespace sdfb200 {
 using namespace tc;
 
 constexpr int kKB = 32;  // K elements per streamed weight block
-
-// fp32 W[N,K] (row-major) -> packed bf16 planes: for each K-block: for each plane: [k-chunk(4)][n][8] bf16
-__global__ void k_tc_pack_w(const float* __restrict__ W, int ldw, int N, int K, int Np, int nblocks, int planes, __nv_bfloat16* __restrict__ out) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // over nblocks * Np * 32
-  if (idx >= nblocks * Np * kKB) return;
-  const int kk = idx % kKB;
-  const int n = (idx / kKB) % Np;
-  const int b = idx / (kKB * Np);
-  const int k = b * kKB + kk;
-  const float w = (n < N && k < K) ? W[(size_t)n * ldw + k] : 0.f;
-  const __nv_bfloat16 hi = __float2bfloat16_rn(w);
-  const __nv_bfloat16 lo = __float2bfloat16_rn(w - __bfloat162float(hi));
-  const size_t plane_elems = (size_t)Np * kKB;
-  const size_t base = (size_t)b * planes * plane_elems;
-  const size_t off = (size_t)(kk / 8) * (Np * 8) + (size_t)n * 8 + (kk % 8);
-  out[base + off] = hi;
-  if (planes > 1) out[base + plane_elems + off] = lo;
-}
 
 template <int P, bool RS>
 __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict__ A, const __nv_bfloat16* __restrict__ Wp, int K, int Np, int Np64,
@@ -51,7 +34,7 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
       for (int j = 0; j < 8; ++j) split2(A[(size_t)r * K + k0 + 2 * j], A[(size_t)r * K + k0 + 2 * j + 1], hi[j], lo[j]);
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
-        const uint32_t off = (uint32_t)((k0 / 8 + c) * 2048 + r * 16);
+        const uint32_t off = (uint32_t)((k0 / 8 + c) * kAChunk + r * 16);
         *reinterpret_cast<uint4*>(a_smem + off) = make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
         if (P > 1) *reinterpret_cast<uint4*>(a_smem + (size_t)K * 256 + off) = make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
       }
@@ -63,17 +46,12 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
   if (warp == 8) {
     // ---- weight producer ----
     if (lane == 0) {
-      for (int b = 0; b < nblocks; ++b) {
-        const int s = b & 1;
-        mbar_wait(&empty[s], ((b >> 1) & 1) ^ 1);
-        mbar_arrive_expect_tx(&full[s], stage_bytes);
-        bulk_g2s(w_smem + (size_t)s * stage_bytes, reinterpret_cast<const uint8_t*>(Wp) + (size_t)b * stage_bytes, stage_bytes, &full[s]);
-      }
+      for (int b = 0; b < nblocks; ++b) ring_fill<2>(w_smem, full, empty, b, reinterpret_cast<const uint8_t*>(Wp), b, stage_bytes);
     }
   } else {
     // ---- two warpgroups, 64 rows each ----
     const int wg = warp >> 2, t = tid & 127;
-    const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c2 = (t & 3) * 2;
+    const int r0 = frag_row0(wg * 64, t), c2 = frag_cq(t);
     const int nch = Np64 / 64;
     float acc[4][32];
 #pragma unroll
@@ -83,8 +61,7 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
     const uint32_t lbo_b = (uint32_t)Np64 * 16, plane_b = (uint32_t)Np64 * kKB * 2;
     const uint32_t abase = smem_u32(a_smem) + wg * 64 * 16;
     for (int b = 0; b < nblocks; ++b) {
-      const int s = b & 1;
-      mbar_wait(&full[s], (b >> 1) & 1);
+      const int s = ring_wait<2>(full, b);
       const uint32_t wbase = smem_u32(w_smem + (size_t)s * stage_bytes);
       uint32_t afr[kKB / 16][2][4];
       if (RS) {
@@ -118,9 +95,7 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
             }
           }
         } else {
-          const uint64_t a0 = make_smem_desc(abase + kstep * 2 * 2048, 2048, 128);
-          const uint64_t a1 = make_smem_desc(abase + (uint32_t)K * 256 + kstep * 2 * 2048, 2048, 128);
-          wgmma_kstep_ss<P, 4>(acc, a0, a1, baddr, plane_b, lbo_b, nch);
+          wgmma_kstep_ss<P, 4>(acc, a_desc(abase, kstep), a_desc(abase + (uint32_t)K * 256, kstep), baddr, plane_b, lbo_b, nch);
         }
       }
       wg_commit();
@@ -132,7 +107,7 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
     for (int c = 0; c < 4; ++c) {
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
-        const int col = c * 64 + (i >> 2) * 8 + c2 + (i & 1), row = r0 + 8 * ((i >> 1) & 1);
+        const int col = frag_col(c2, c, i), row = frag_row(r0, i);
         if (c < nch && col < Np) D[(size_t)row * Np + col] = acc[c][i];
       }
     }
@@ -152,9 +127,7 @@ extern "C" int sdfb200_debug_tc_gemm(const float* A, const float* W, int32_t K, 
   const int Np = (N + 15) / 16 * 16, Np64 = (N + 63) / 64 * 64;
   const int nblocks = K / kKB;
   cudaStream_t st = (cudaStream_t)stream;
-  const int tot = nblocks * Np64 * kKB;
-  k_tc_pack_w<<<(tot + 255) / 256, 256, 0, st>>>(W, K, N, K, Np64, nblocks, planes, (__nv_bfloat16*)scratch);
-  SDFB_LAUNCHED("k_tc_pack_w");
+  if (int r = tc_pack(W, K, 0, N, K, Np64, kKB, nblocks, planes, nullptr, nullptr, scratch, st)) return r;
   const size_t smem = (mode_ts ? 0 : (size_t)planes * K * 256) + 2 * (size_t)planes * Np64 * kKB * 2 + 1024;
 #define LAUNCH(P_, TS_)                                                                                              \
   do {                                                                                                               \
@@ -171,10 +144,6 @@ extern "C" int sdfb200_debug_tc_gemm(const float* A, const float* W, int32_t K, 
 }
 
 // building-block test of the generic tensor-core Linear (tc_linear.cu) against a reference GEMM: same arguments as the internal sgemm()
-namespace sdfb200 {
-int tc_gemm(int planes, int epi, const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy, int64_t M, int Np, int Kp,
-            const float* aux, int ldaux, int aux_cols, void* scratch, cudaStream_t st);
-}
 extern "C" int sdfb200_debug_tc_linear(int32_t planes, int32_t epi, const float* X, int32_t ldx, const float* W, const float* bias, float* Y,
                                        int32_t ldy, int64_t M, int32_t Np, int32_t Kp, const float* aux, int32_t ldaux, int32_t aux_cols,
                                        void* scratch, void* stream) {

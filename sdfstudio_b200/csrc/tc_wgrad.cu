@@ -18,7 +18,7 @@ using namespace tc;
 namespace {
 constexpr int kWgThreads = 256;     // two warpgroups: staging + MMAs
 constexpr int kWgPts = 32;          // points per stage
-constexpr int kWgRowsA = 128;       // rows of the A operand tile (N chunk, zero padded)
+constexpr int kWgRowsA = 128;       // rows of the A operand tile (N chunk, zero padded): the 128-row A layout of tc_common.cuh
 constexpr int kWgRowsB = 256;       // rows of the B operand tile (K chunk, zero padded)
 constexpr uint32_t kWgPlaneA = (kWgPts / 8) * kWgRowsA * 16;          // 8 KB
 constexpr uint32_t kWgPlaneB = (kWgPts / 8) * kWgRowsB * 16;          // 16 KB
@@ -84,9 +84,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_tc_wgrad(const WgArgs a) {
       wg_arrive();
 #pragma unroll
       for (int j = 0; j < kWgPts / 16; ++j) {
-        const uint64_t a0 = make_smem_desc(abase + j * 2 * kWgRowsA * 16, kWgRowsA * 16, 128);
-        const uint64_t a1 = make_smem_desc(abase + kWgPlaneA + j * 2 * kWgRowsA * 16, kWgRowsA * 16, 128);
-        wgmma_kstep_ss<PL, 4>(acc, a0, a1, bbase + j * 2 * kWgRowsB * 16, kWgPlaneB, kWgRowsB * 16, nch);
+        wgmma_kstep_ss<PL, 4>(acc, a_desc(abase, j), a_desc(abase + kWgPlaneA, j), bbase + j * 2 * kWgRowsB * 16, kWgPlaneB, kWgRowsB * 16, nch);
       }
       wg_commit();
     }
@@ -99,12 +97,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_tc_wgrad(const WgArgs a) {
   }
   // ---------------- partial sums of this CTA -> workspace (zeros for a CTA without points) ----------------
   float* out = a.partial + (size_t)blockIdx.x * 256 * 256;
-  const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), c2 = (t & 3) * 2;
+  const int r0 = frag_row0(wg * 64, t), c2 = frag_cq(t);
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
-      const int n = r0 + 8 * ((i >> 1) & 1), k = c * 64 + (i >> 2) * 8 + c2;
+      const int n = frag_row(r0, i), k = frag_col(c2, c, i);
       if (c < nch) *reinterpret_cast<float2*>(out + (size_t)n * 256 + k) = make_float2(acc[c][i], acc[c][i + 1]);
     }
   }
