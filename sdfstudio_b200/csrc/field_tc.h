@@ -8,11 +8,12 @@ namespace sdfb200 {
 
 constexpr int kEpiWarps = 8;                                 // two consumer warpgroups: MMAs + epilogues, 64 tile rows each
 constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kTcThreads = kEpiThreads + 128;                // + one producer warpgroup (one thread streams the weights)
+constexpr int kTcThreads = kEpiThreads + 128;                // + one producer warpgroup: warp 8 streams the weights, warps 9..11 encode
+constexpr int kEncThreads = 96;                              // encoder warps: the geo input, Jacobians and colour-static columns of tile n + 1
 // register split after setmaxnreg.  The launch gets 168 per thread (65536 / 384, rounded down to a multiple of 8); the consumers can
-// only take what the producer warpgroup gives back: 256 x (240 - 168) = 128 x (168 - 24)
-constexpr int kConsumerRegs = 240;
-constexpr int kProducerRegs = 24;
+// only take what the producer warpgroup gives back: 256 x (216 - 168) = 128 x (168 - 72)
+constexpr int kConsumerRegs = 216;
+constexpr int kProducerRegs = 72;
 static_assert(2 * (kConsumerRegs - 168) <= 168 - kProducerRegs, "setmaxnreg.inc would wait for registers nobody frees");
 constexpr int kStages = 5;        // weight ring depth (16 KB per stage at two planes, next to the 128 KB A operand)
 constexpr int kKB = 16;           // K per streamed weight block of the 256-row layers (one 16 KB stage at two planes)
@@ -24,9 +25,13 @@ constexpr float kHalfPiF = 1.5707963267948966f;
 // kernel order of the geo input columns (K = 96): [grid features 0..31 | PE | x(3) | zero padding] -- every group of four hash
 // levels is one aligned 16-byte operand chunk.  W0 (columns) and W0^T (rows) are permuted accordingly at pack time.
 constexpr uint32_t kAPlane = 32 * 2048;   // one bf16 plane of the A operand: [K/8 = 32][128 rows][16 B]
-// per-CTA scratch: softplus'(z1) unorm16 [64 KB] | h2 planes [P x 64 KB] | input jacobian (PE [64][128] f32 | grid [96][128] f32)
+// per-CTA scratch: softplus'(z1) unorm16 [64 KB] | h2 planes [P x 64 KB] | two staging slots (tile parity), each
+//   geo input image [P][12 chunks][128 rows][16 B] | colour-static image, same layout (chunk 0 unused) | input jacobian
+//   (PE [64][128] f32 | grid [96][128] f32)
 constexpr size_t kJRBytes = (size_t)(kPeRows + kMaxGridDim * 3) * 128 * 4;
-__host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 + (size_t)planes * 65536 + kJRBytes; }
+constexpr uint32_t kImgPlane = (kInK / 8) * 128 * 16;      // one bf16 plane of a staged 96-column operand image (24 KB)
+__host__ __device__ constexpr size_t kSlotBytes(int planes) { return 2 * (size_t)planes * kImgPlane + kJRBytes; }
+__host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 + (size_t)planes * 65536 + 2 * kSlotBytes(planes); }
 
 // layers in the order the kernel runs them (and the producer streams them)
 enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };

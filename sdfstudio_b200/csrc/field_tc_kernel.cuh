@@ -65,16 +65,17 @@ __device__ __forceinline__ PointGeom point_geom(const TcArgs& a, long long p) {
   return g;
 }
 
-// accurate sin / sincos as real calls: one copy of the (long) range-reduction code instead of one per call site -- the roles of this
-// kernel share the SM's instruction cache, and `no instruction` stalls were 20 % of all samples with everything inlined
-static __device__ __noinline__ void sincos_call(float x, float* s, float* c) { sincosf(x, s, c); }
-static __device__ __noinline__ float sin_call(float x) { return sinf(x); }
+// accurate sin / sincos of the encoder warps.  Inlined: after setmaxnreg.dec a real call makes ptxas (CUDA 12.9) crash; both call
+// sites are in the encoder loop, so this is two copies of the range reduction, not one per consumer epilogue
+static __device__ __forceinline__ void sincos_call(float x, float* s, float* c) { sincosf(x, s, c); }
+static __device__ __forceinline__ float sin_call(float x) { return sinf(x); }
 
-// Hash-grid part of the geo input of one tile (gather warps, one thread per point).  Outputs: operand chunks 0..3 (bf16 planes,
-// kernel column order: four levels = one aligned 16-byte chunk) and, in the per-CTA global scratch, the grid jacobian
-// [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  One level at a time (smallest code).
+// Hash-grid part of the geo input of one tile, levels 4 grp .. 4 grp + 3 of one point (= operand chunk grp).  Outputs: bf16 planes
+// of the staged geo input image (`img`, planes `plane` bytes apart, kernel column order: four levels = one aligned 16-byte chunk)
+// and the grid jacobian [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  One level at a time (smallest code).
 template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int row, uint8_t* inA, uint8_t* enc, uint64_t pol_table) {
+__device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int row, int grp, uint8_t* img, uint32_t plane, uint8_t* enc,
+                                                 uint64_t pol_table) {
   float* Jg = reinterpret_cast<float*>(enc) + kPeRows * 128;
   const long long p_raw = (long long)tile * 128 + row;
   const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
@@ -82,7 +83,7 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
   const float x01 = (g.px + 2.0f) * 0.25f, y01 = (g.py + 2.0f) * 0.25f, z01 = (g.pz + 2.0f) * 0.25f;   // sdf_field.py:384
   // one level at a time, rolled (code size): 8 gathers in flight per thread, feature columns as 2-byte operand stores
 #pragma unroll 1
-  for (int l = 0; l < 16; ++l) {
+  for (int l = 4 * grp; l < 4 * grp + 4; ++l) {
     float o[2] = {0.f, 0.f};
     float dj[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
     if (a.use_grid && l < a.grid.n_levels && l < a.grid.active_levels) {
@@ -92,8 +93,8 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
       level_fetch_rt2(a.grid, a.table, c, tv, pol_table);
       level_finish<2, LAYOUT>(a.grid, c, tv, o, dj);
     }
-    store_a<P>(inA, kAPlane, row, 2 * l, o[0]);
-    store_a<P>(inA, kAPlane, row, 2 * l + 1, o[1]);
+    store_a<P>(img, plane, row, 2 * l, o[0]);
+    store_a<P>(img, plane, row, 2 * l + 1, o[1]);
     if (a.mode != 0 && l < a.grid.n_levels) {
 #pragma unroll
       for (int f = 0; f < 2; ++f) {
@@ -106,19 +107,24 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
   }
 }
 
-// PE | x | zero padding: chunks 4..11 of the geo input.  Kernel column 32 + i holds PE_i, 32 + pe_dim + j holds x_j
+// PE | x | zero padding: chunks 4..11 of the geo input.  Kernel column 32 + i holds PE_i, 32 + pe_dim + j holds x_j.  Also the
+// point outputs (contracted position and its norm) of a valid row.
 template <int P>
-__device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int row, uint8_t* inA, uint8_t* enc) {
+__device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int row, uint8_t* img, uint32_t plane, uint8_t* enc) {
   float* Jpe = reinterpret_cast<float*>(enc);
   const long long p_raw = (long long)tile * 128 + row;
   const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
   const PointGeom g = point_geom(a, p);
+  if (p_raw < a.n_points) {
+    if (a.out.points_norm) a.out.points_norm[p] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(g.px, g.px), __fmul_rn(g.py, g.py)), __fmul_rn(g.pz, g.pz)));
+    if (a.out.points) { a.out.points[p * 3] = g.px; a.out.points[p * 3 + 1] = g.py; a.out.points[p * 3 + 2] = g.pz; }
+  }
   const int deg = a.pe_degree, half = 3 * deg;
   const float pc[3] = {g.px, g.py, g.pz};
   // zero the chunks first (padding columns), then the live columns as 2-byte stores (same thread: program order)
   const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll 1
-  for (int ch = 4; ch < kInK / 8; ++ch) store_a_chunk<P>(inA, kAPlane, row, ch, z4, z4);
+  for (int ch = 4; ch < kInK / 8; ++ch) store_a_chunk<P>(img, plane, row, ch, z4, z4);
 #pragma unroll 1
   for (int i = 0; i < a.pe_dim; ++i) {                       // sin(x 2^k) | sin(x 2^k + pi/2)   (encodings.py:194-198)
     const int ia = i >= half ? i - half : i;
@@ -128,46 +134,60 @@ __device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int ro
     const float arg = i >= half ? xb * fr + kHalfPiF : xb * fr;
     float sv, cv;
     sincos_call(arg, &sv, &cv);
-    store_a<P>(inA, kAPlane, row, 32 + i, a.use_pe ? sv : 0.f);
+    store_a<P>(img, plane, row, 32 + i, a.use_pe ? sv : 0.f);
     // autograd of sin on the forward's own fp32 arguments: d/dx_b = 2^k cos(arg)
     if (a.mode != 0) Jpe[i * 128 + row] = a.use_pe ? fr * cv : 0.f;
   }
-  store_a<P>(inA, kAPlane, row, 32 + a.pe_dim + 0, pc[0]);
-  store_a<P>(inA, kAPlane, row, 32 + a.pe_dim + 1, pc[1]);
-  store_a<P>(inA, kAPlane, row, 32 + a.pe_dim + 2, pc[2]);
+  store_a<P>(img, plane, row, 32 + a.pe_dim + 0, pc[0]);
+  store_a<P>(img, plane, row, 32 + a.pe_dim + 1, pc[1]);
+  store_a<P>(img, plane, row, 32 + a.pe_dim + 2, pc[2]);
 }
 
-// static colour-operand columns of a tile (kernel columns 8..95 = chunks 1..11): x(3) | dir-enc(24) | dir(3) | appearance | 0,
-// written IN PLACE over the tile's geo input once G0 has consumed it (chunk 0 = [grad, n.v] comes from the epilogue warps)
+// static colour-operand columns of a tile (kernel columns 8..95 = chunks 1..11): x(3) | dir-enc(24) | dir(3) | appearance | 0, staged in
+// the same [plane][chunk][row][16 B] layout as the A operand; EB0 copies them over the A columns that B0 has consumed (chunk 0 =
+// [grad, n.v] comes from the epilogue)
 template <int P>
-__device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, int row, uint8_t* inA) {
+__device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, int row, uint8_t* img, uint32_t plane) {
   const long long p_raw = (long long)tile * 128 + row;
   const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
   const PointGeom g = point_geom(a, p);
   const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll 1
-  for (int ch = 1; ch < kInK / 8; ++ch) store_a_chunk<P>(inA, kAPlane, row, ch, z4, z4);
-  store_a<P>(inA, kAPlane, row, 8 + 0, g.px); store_a<P>(inA, kAPlane, row, 8 + 1, g.py); store_a<P>(inA, kAPlane, row, 8 + 2, g.pz);
+  for (int ch = 1; ch < kInK / 8; ++ch) store_a_chunk<P>(img, plane, row, ch, z4, z4);
+  store_a<P>(img, plane, row, 8 + 0, g.px); store_a<P>(img, plane, row, 8 + 1, g.py); store_a<P>(img, plane, row, 8 + 2, g.pz);
   // direction encoding: sin(d 2^k) | sin(d 2^k + pi/2), k = 0..3, then d itself (NeRFEncoding(4, include_input), encodings.py:167-208)
 #pragma unroll 1
   for (int i = 0; i < 12; ++i) {
     const int b = i >> 2;
     const float db = b == 0 ? g.dx : (b == 1 ? g.dy : g.dz);
     const float arg = db * (float)(1 << (i & 3));
-    store_a<P>(inA, kAPlane, row, 8 + 3 + i, sin_call(arg));
-    store_a<P>(inA, kAPlane, row, 8 + 15 + i, sin_call(arg + kHalfPiF));
+    store_a<P>(img, plane, row, 8 + 3 + i, sin_call(arg));
+    store_a<P>(img, plane, row, 8 + 15 + i, sin_call(arg + kHalfPiF));
   }
-  store_a<P>(inA, kAPlane, row, 8 + 27, g.dx); store_a<P>(inA, kAPlane, row, 8 + 28, g.dy); store_a<P>(inA, kAPlane, row, 8 + 29, g.dz);
+  store_a<P>(img, plane, row, 8 + 27, g.dx); store_a<P>(img, plane, row, 8 + 28, g.dy); store_a<P>(img, plane, row, 8 + 29, g.dz);
   if (a.appearance != nullptr) {
 #pragma unroll 1
-    for (int j = 0; j < a.app_dim; ++j) store_a<P>(inA, kAPlane, row, 8 + 30 + j, __ldg(a.appearance + g.ray * a.app_dim + j));
+    for (int j = 0; j < a.app_dim; ++j) store_a<P>(img, plane, row, 8 + 30 + j, __ldg(a.appearance + g.ray * a.app_dim + j));
   }
 }
 
+// Staging slot of a tile (per-CTA scratch, selected by the parity of the CTA's tile count): geo input image | colour-static image |
+// input jacobian (the layout next to kSlotBytes)
+template <int P>
+struct Slot {
+  uint8_t* base;
+  __device__ __forceinline__ uint8_t* geo() const { return base; }
+  __device__ __forceinline__ uint8_t* cs() const { return base + (size_t)P * kImgPlane; }
+  __device__ __forceinline__ uint8_t* jac() const { return base + 2 * (size_t)P * kImgPlane; }
+};
+template <int P>
+__device__ __forceinline__ Slot<P> slot_of(char* slots, int tile_no) { return Slot<P>{reinterpret_cast<uint8_t*>(slots) + (size_t)(tile_no & 1) * kSlotBytes(P)}; }
+
 #ifdef SDFB200_TC_TIMING
 // CTA 0, first 16 tiles, row = tile: clock64() of consumer thread 0 at [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring
-// order), [8] end of the encode, [15] tile end; cycle sums over the tile of [9] consumer thread 0 waiting for weights (full) and
-// [10] the producer waiting for a free ring slot (empty)
+// order), [8] the tile's geo input has landed (a_full; [8] - [0] is the consumers' wait for the encoder), [15] tile end; cycle sums
+// over the tile of [9] consumer thread 0 waiting for weights (full), [10] the producer waiting for a free ring slot (empty),
+// [12] encoder thread 0 busy on the tile and [13] encoder thread 0 waiting for its staging slot (enc_empty)
 __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
 #define TC_PUT(tno, k, v)                                                                                            \
   do {                                                                                                               \
@@ -178,22 +198,67 @@ __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE ins
 #endif
 #define TC_STAMP(k) do { if (tid == 0) TC_PUT(tile_no, k, TC_CLOCK()); } while (0)
 
-// Weight ring producer (one thread of the producer warpgroup): walks every K-block of every layer of every tile of this CTA in
-// consumption order and issues the bulk copy of block j once its slot has been released (all 8 consumer warps are through block
-// j - kStages).  Every block of every layer is one full stage (tc_blocks_fill_stages).
+// Barriers between the roles of the fused kernel.  Weight ring: full / empty (tc_common.cuh).  Staging slot s (tile parity):
+// enc_full[s] (count kEncThreads) once the encoder warps have written a tile's images, enc_empty[s] (count kEpiThreads) once the
+// consumers are done with them (after EB0; in sdf-only mode once the geo input has landed).  A operand: a_free (count 2, one per
+// consumer warpgroup) once a tile's last layer has read it, a_full (count 1 + the bulk copies' bytes) once the next tile's geo input
+// has landed in it.
+struct TcBars {
+  uint64_t full[kStages], empty[kStages];
+  uint64_t enc_full[2], enc_empty[2];
+  uint64_t a_full, a_free;
+};
+
+// Producer (one thread of the producer warpgroup).  Per tile: once the consumers have freed the A operand (a_free, from the second
+// tile on) and the encoder has staged the tile (enc_full), bulk-copies the staged geo input image into A columns 0..95 (a_full);
+// then walks every K-block of every layer in consumption order and issues the bulk copy of block j once its ring slot has been
+// released (all 8 consumer warps are through block j - kStages).  Every block of every layer is one full stage (tc_blocks_fill_stages).
 template <int P>
-__device__ __forceinline__ void produce_all(const TcArgs& a, int nlayers, uint8_t* ring, uint64_t* full, uint64_t* empty) {
+__device__ __forceinline__ void produce_all(const TcArgs& a, int nlayers, uint8_t* abuf, uint8_t* ring, char* slots, TcBars& b) {
   constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;
   uint32_t j = 0;
   int tile_no = 0;
   for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
     long long waited = 0;
+    if (tile_no > 0) mbar_wait(&b.a_free, (tile_no - 1) & 1);
+    mbar_wait(&b.enc_full[tile_no & 1], (tile_no >> 1) & 1);
+    const uint8_t* geo = slot_of<P>(slots, tile_no).geo();
+    mbar_arrive_expect_tx(&b.a_full, (uint32_t)P * kImgPlane);
+#pragma unroll
+    for (int pl = 0; pl < P; ++pl) bulk_g2s(abuf + pl * kAPlane, geo + pl * kImgPlane, kImgPlane, &b.a_full);
+    uint64_t* full = b.full;
+    uint64_t* empty = b.empty;
     for (int L = 0; L < nlayers; ++L) {
       const TcLayer& ly = a.layer[L];
       for (int kb = 0; kb < ly.nkb; ++kb, ++j)
         ring_fill<kStages>(ring, full, empty, j, reinterpret_cast<const uint8_t*>(a.blob) + ly.w_off, kb, kStageBytes, &waited);
     }
     TC_PUT(tile_no, 10, waited);
+  }
+}
+
+// Encoder warps (et = 0..95): walk the same tiles as the consumers and stage each one in its slot while the consumers run the tile
+// before it.  A tile is 768 items, 8 per thread: 512 (point, group of four hash levels), then 128 x (PE | x, point outputs) and, with
+// the colour MLP, 128 x colour-static columns.  Item i goes to thread i % 96, so each warp runs 32 consecutive items of one kind.
+template <int P, int LAYOUT>
+__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table) {
+  const int n_items = a.mode != 0 ? 768 : 640;
+  int tile_no = 0;
+  for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
+    const long long w0 = TC_CLOCK();
+    mbar_wait(&b.enc_empty[tile_no & 1], ((tile_no >> 1) & 1) ^ 1);
+    const long long w1 = TC_CLOCK();
+    const Slot<P> s = slot_of<P>(slots, tile_no);
+#pragma unroll 1
+    for (int i = et; i < n_items; i += kEncThreads) {
+      const int row = i & 127;
+      if (i < 512) encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jac(), pol_table);
+      else if (i < 640) encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jac());
+      else colour_static_tile<P>(a, tile, row, s.cs(), kImgPlane);
+    }
+    fence_async_global();                    // the geo image is read by the producer's bulk copy (async proxy)
+    mbar_arrive(&b.enc_full[tile_no & 1]);
+    if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - w1); TC_PUT(tile_no, 13, w1 - w0); }
   }
 }
 
@@ -245,27 +310,9 @@ struct TileCtx {
   float sdf_bias;
   uint32_t* sig_s;           // per-CTA scratch: softplus'(z1) as 2 x unorm16, [64 units][256 threads]
   uint32_t* gf_s;            //                  h2 as bf16x2 planes, [P][64 units][256 threads]
-  uint8_t* enc_s;            //                  input jacobian: PE [64][128] f32 | grid [96][128] f32
-  uint64_t pol_table, pol_keep;   // L2 policies of the hash-table gathers and of the jacobian reads
+  char* slots;               //                  the two staging slots written by the encoder warps (kSlotBytes each)
+  uint64_t pol_keep;         // L2 policy of the staged reads
 };
-
-// encode: thread t < 64 hash gathers of row wrow0 + t, thread t >= 64 PE / x of row wrow0 + t - 64
-template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_tile(const TileCtx& x, int tile) {
-  const TcArgs& a = x.a;
-  const int row = x.wrow0 + (x.t & 63);
-  if (x.t < 64) {
-    encode_tile_grid<P, LAYOUT>(a, tile, row, x.abuf, x.enc_s, x.pol_table);
-    const long long p = (long long)tile * 128 + row;
-    if (p < a.n_points) {
-      const PointGeom g = point_geom(a, p);
-      if (a.out.points_norm) a.out.points_norm[p] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(g.px, g.px), __fmul_rn(g.py, g.py)), __fmul_rn(g.pz, g.pz)));
-      if (a.out.points) { a.out.points[p * 3] = g.px; a.out.points[p * 3 + 1] = g.py; a.out.points[p * 3 + 2] = g.pz; }
-    }
-  } else {
-    encode_tile_pe<P>(a, tile, row, x.abuf, x.enc_s);
-  }
-}
 
 // E0 (after G0): h1 = softplus(z1) -> A ; softplus'(z1) -> scratch
 template <int P>
@@ -346,11 +393,11 @@ __device__ __forceinline__ void epi_eb1(const TileCtx& x, const float (&acc)[4][
 
 // EB0 (after B0): gin (96 cols, kernel order) . input jacobian -> d sdf / dx; then the colour misc operand over the (consumed) A columns
 // 0..95: chunk 0 = [grad(3), n.v, 0 x4] (sdf_field.py:572-584; columns re-ordered at pack time) from the thread pair that owns the row,
-// chunks 1..11 = [x, dir-enc, dir, appearance] one thread per row
+// chunks 1..11 = [x, dir-enc, dir, appearance] copied from the tile's staging slot (16-byte units, the warpgroup's 64 rows)
 template <int P>
-__device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const float (&acc)[4][32]) {
+__device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P>& s, const float (&acc)[4][32]) {
   const TcArgs& a = x.a;
-  const float* Jpe = reinterpret_cast<const float*>(x.enc_s);
+  const float* Jpe = reinterpret_cast<const float*>(s.jac());
   const float* Jg = Jpe + kPeRows * 128;
   const int deg = a.pe_degree, half = 3 * deg;
   float gr[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
@@ -397,7 +444,19 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const float 
     store_a_chunk<P>(x.abuf, kAPlane, row, 0, c0v);
     x.hs[128 + row] = grx; x.hs[256 + row] = gry; x.hs[384 + row] = grz;
   }
-  if (x.t < 64) colour_static_tile<P>(a, tile, x.wrow0 + x.t, x.abuf);
+  // unit k: plane k / (11 * 64), chunk 1 + (k / 64) % 11, row wrow0 + k % 64; all loads first, then the stores
+  constexpr int kUnits = 11 * 64 * P, kPer = (kUnits + 127) / 128;
+  uint4 v[kPer];
+#pragma unroll
+  for (int j = 0; j < kPer; ++j) {
+    const int k = x.t + 128 * j, pl = k / (11 * 64), ch = 1 + (k - pl * 11 * 64) / 64, row = x.wrow0 + (k & 63);
+    if (k < kUnits) v[j] = ld_stream_u4(s.cs() + pl * kImgPlane + ch * kAChunk + row * 16, x.pol_keep);
+  }
+#pragma unroll
+  for (int j = 0; j < kPer; ++j) {
+    const int k = x.t + 128 * j, pl = k / (11 * 64), ch = 1 + (k - pl * 11 * 64) / 64, row = x.wrow0 + (k & 63);
+    if (k < kUnits) *reinterpret_cast<uint4*>(x.abuf + pl * kAPlane + ch * kAChunk + row * 16) = v[j];
+  }
 }
 
 // C0 h2 operand: h2 (bf16 planes, saved by E1) back from the scratch over the misc columns that C0's first part has consumed
@@ -608,13 +667,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   float* hs = prm + 9 * 256;          // [7][128] per-row inputs of the heads: sdf, gradient (3), raw rgb (3)
   float* racc = hs + 7 * 128;         // [8][4] per-ray accumulators of the fused compositing (rays spanning several warps)
   float* lastrgb = racc + 32;         // [4][3]
-  __shared__ uint64_t full[kStages], empty[kStages];
+  __shared__ TcBars bars;
   __shared__ double wtot[4];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nlayers = a.mode == 0 ? 2 : L_COUNT;
+  char* slots = a.scratch + (size_t)blockIdx.x * a.scratch_per_cta + 65536 + (size_t)P * 65536;
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kEpiWarps); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], kEpiWarps); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&bars.enc_full[s], kEncThreads); mbar_init(&bars.enc_empty[s], kEpiThreads); }
+    mbar_init(&bars.a_full, 1);
+    mbar_init(&bars.a_free, 2);
     fence_barrier_init();
   }
   {
@@ -629,13 +692,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   }
   __syncthreads();
 
-  // ============================== producer warpgroup: one thread streams the weights ==============================
+  // ============ producer warpgroup: one thread streams the weights and the geo input, warps 9..11 encode the tile ahead ============
   if (tid >= kEpiThreads) {
     setmaxnreg_dec<kProducerRegs>();
-    if (tid == kEpiThreads) produce_all<P>(a, nlayers, ring, full, empty);
+    if (tid == kEpiThreads) produce_all<P>(a, nlayers, abuf, ring, slots, bars);
+    else if (tid >= kTcThreads - kEncThreads) encode_all<P, LAYOUT>(a, tid - (kTcThreads - kEncThreads), slots, bars, l2_policy_evict_last());
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();
+  uint64_t* full = bars.full;
+  uint64_t* empty = bars.empty;
 
   // ============================== two warpgroups, 64 rows of the tile each ==============================
   const int wg = warp >> 2, t = tid & 127;
@@ -645,8 +711,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   const float sdf_bias = __ldg(reinterpret_cast<const float*>(a.blob + a.b_g2));
   char* scr = a.scratch + (size_t)blockIdx.x * a.scratch_per_cta;
   const TileCtx x{a, tid, t, wg, wrow0, frag_row0(wrow0, t), frag_cq(t), abuf, prm, hs, racc, lastrgb, wtot, sdf_bias,
-                  reinterpret_cast<uint32_t*>(scr), reinterpret_cast<uint32_t*>(scr + 65536), reinterpret_cast<uint8_t*>(scr + 65536 + (size_t)P * 65536),
-                  l2_policy_evict_last(), l2_policy_evict_normal()};
+                  reinterpret_cast<uint32_t*>(scr), reinterpret_cast<uint32_t*>(scr + 65536), slots, l2_policy_evict_normal()};
   uint32_t it = 0;
   long long waited = 0;
   float acc[4][32];
@@ -667,21 +732,29 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     ++tile_no;
     TC_STAMP(0);
     waited = 0;
-    encode_tile<P, LAYOUT>(x, tile);
-    SYNC_A();
+    const int sl = tile_no & 1;
+    const Slot<P> s = slot_of<P>(slots, tile_no);
+    mbar_wait(&bars.a_full, tile_no & 1);      // the geo input staged by the encoder warps has landed in A columns 0..95
+    if (a.mode == 0) mbar_arrive(&bars.enc_empty[sl]);
     TC_STAMP(8);
     LAYER(L_G0, true);
     epi_e0<P>(x, acc);
     SYNC_A();
     LAYER(L_G1, true);
+    if (a.mode == 0) {                         // sdf only: A is free for the next tile's geo input
+      if (t == 0) mbar_arrive(&bars.a_free);
+      epi_e1<P>(x, tile, acc);
+      continue;
+    }
     epi_e1<P>(x, tile, acc);
-    if (a.mode == 0) continue;                 // sdf only
     SYNC_A();
     LAYER(L_B1, true);
     epi_eb1<P>(x, acc);
     SYNC_A();
     LAYER(L_B0, true);
-    epi_eb0<P>(x, tile, acc);
+    mbar_wait(&bars.enc_full[sl], (tile_no >> 1) & 1);   // (long complete: makes the encoder's jacobian / colour-static stores visible)
+    epi_eb0<P>(x, tile, s, acc);
+    mbar_arrive(&bars.enc_empty[sl]);
     SYNC_A();
     LAYER(L_C0MISC, true);
     reload_h2<P>(x);
@@ -690,6 +763,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     epi_ec0<P>(x, acc);
     SYNC_A();
     LAYER(L_C1, true);
+    if (t == 0) mbar_arrive(&bars.a_free);     // the last layer has read A: the next tile's geo input may land
     epi_ec1(x, acc);
     named_sync(3, kEpiThreads);                // both warpgroups' head inputs are in `hs`
     if (wg == 0) heads_and_composite(x, tile);

@@ -50,6 +50,8 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 }
 // make generic-proxy writes to shared memory visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// the same for generic-proxy writes to global memory that a later bulk copy reads
+__device__ __forceinline__ void fence_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 // ---- wgmma (warpgroup MMA, sm_90a) -------------------------------------------------------------------------------
 // All 128 threads of a warpgroup issue these together.  The accumulator lives in registers; for m64nN thread t of the warpgroup
@@ -154,6 +156,11 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 __device__ __forceinline__ float ld_stream_f1(const float* p, uint64_t pol) {
   float v;
   asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint4 ld_stream_u4(const void* p, uint64_t pol) {
+  uint4 v;
+  asm volatile("ld.global.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol) : "memory");
   return v;
 }
 
