@@ -155,7 +155,7 @@ int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* b
   // persistent CTAs, one per SM (the static tile loop needs no co-residency, but more CTAs than SMs would only add a tail wave)
   const int ctas = persistent_ctas();
   const int grid = a.n_tiles < ctas ? a.n_tiles : ctas;
-  const size_t smem = (size_t)t.planes * kAPlane + (size_t)kStages * t.planes * 256 * kKB * 2 + (9 * 256 + 7 * 128 + 32 + 12) * 4 + 1024;
+  const size_t smem = tc_smem_bytes(t.planes);
   const bool torch_layout = f.grid.layout == SDFB200_GRID_TORCH;
   if (t.planes == 2) return torch_layout ? launch_field_tc_p2_torch(a, grid, smem, st) : launch_field_tc_p2_tcnn(a, grid, smem, st);
   return torch_layout ? launch_field_tc_p1_torch(a, grid, smem, st) : launch_field_tc_p1_tcnn(a, grid, smem, st);

@@ -33,6 +33,16 @@ constexpr uint32_t kImgPlane = (kInK / 8) * 128 * 16;      // one bf16 plane of 
 __host__ __device__ constexpr size_t kSlotBytes(int planes) { return 2 * (size_t)planes * kImgPlane + kJRBytes; }
 __host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 + (size_t)planes * 65536 + 2 * kSlotBytes(planes); }
 
+constexpr int kHsFloats = 7 * 128;                         // head inputs of one tile: sdf, gradient (3), raw rgb (3) per row
+constexpr size_t kSmemPerBlock = 232448;                     // H100: 227 KB of shared memory per block (dynamic + static)
+constexpr size_t kStaticSmem = 1024;      // the kernel's static shared memory (barriers): one 1024-byte slot, the dynamic part is 1024-aligned
+// dynamic shared memory of the kernel: A operand | weight ring | epilogue parameters [9][256] f32 | head inputs by tile parity |
+// EB0 column table [96] float4
+__host__ __device__ constexpr size_t tc_smem_bytes(int planes) {
+  return (size_t)planes * kAPlane + (size_t)kStages * planes * 256 * kKB * 2 + (9 * 256 + 2 * kHsFloats) * 4 + 96 * 16;
+}
+static_assert(tc_smem_bytes(2) + kStaticSmem <= kSmemPerBlock, "shared memory of k_field_tc at two planes");
+
 // layers in the order the kernel runs them (and the producer streams them)
 enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
 

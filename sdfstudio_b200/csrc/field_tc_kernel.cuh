@@ -6,8 +6,9 @@
 // Persistent CTAs, one 128-point tile at a time.  Two consumer warpgroups own 64 rows of the tile each and run every layer as wgmma
 // m64n256k16 (m64n128k16 for B0; accumulator in registers, A operand in shared memory, weights streamed through a shared-memory
 // ring filled by 1-D bulk copies from a pre-packed image).  A warpgroup only reads and writes its own rows of the A operand, so the
-// two warpgroups meet only at the weight ring and at the per-point heads / compositing.  A third warpgroup gives its registers to
-// the consumers (setmaxnreg) and keeps one thread filling the ring, so no consumer warpgroup stalls while a slot is being freed.
+// two warpgroups meet only at the weight ring.  A third warpgroup gives its registers to the consumers (setmaxnreg), keeps one thread
+// filling the ring, so no consumer warpgroup stalls while a slot is being freed, and three encoder warps that stage the next tile and
+// run the heads of the previous one.
 // Per tile (everything stays on chip except three L2-resident spills):
 //   encode   one thread per point for position, contraction, hash gathers (+ jacobian), one for PE
 //            -> bf16 split planes of the geo input (A operand columns 0..95)
@@ -19,8 +20,8 @@
 //   grad     d sdf/dx = gin_x + PE jacobian + grid jacobian / 4      (what autograd computes at sdf_field.py:647-654)
 //   C0 C1    relu MLP on [x, dir-enc, grad, geo feature, appearance] (misc columns first, h2 accumulated onto them);
 //            last 256->3 layer as fp32 dots; sigmoid + padding
-//   heads    Laplace density, NeuS alpha, occupancy, normals; optional per-sample outputs
-//   render   (fused mode) segmented prefix product over the rays of the tile in double, weights, per-ray sums
+//   heads    (one encoder warp, a tile behind) Laplace density, NeuS alpha, occupancy, normals; optional per-sample outputs
+//   render   (fused mode, same warp) segmented prefix product over the rays of the tile in double, weights, per-ray sums
 // MMA = wgmma bf16 x bf16 -> fp32.  bf16x3: a0*w0 + a1*w0 + a0*w1 with a = a0+a1, w = w0+w1 (error ~2^-16 relative, fp32 accumulate).
 #pragma once
 #include "field_tc.h"
@@ -185,9 +186,11 @@ __device__ __forceinline__ Slot<P> slot_of(char* slots, int tile_no) { return Sl
 
 #ifdef SDFB200_TC_TIMING
 // CTA 0, first 16 tiles, row = tile: clock64() of consumer thread 0 at [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring
-// order), [8] the tile's geo input has landed (a_full; [8] - [0] is the consumers' wait for the encoder), [15] tile end; cycle sums
-// over the tile of [9] consumer thread 0 waiting for weights (full), [10] the producer waiting for a free ring slot (empty),
-// [12] encoder thread 0 busy on the tile and [13] encoder thread 0 waiting for its staging slot (enc_empty)
+// order), [8] the tile's geo input has landed (a_full; [8] - [0] is the consumers' wait for the encoder), [15] tile end = end of EC1
+// (head inputs handed over); cycle sums over the tile of [9] consumer thread 0 waiting for weights (full), [10] the producer waiting
+// for a free ring slot (empty), [12] encoder thread 0 busy staging the tile, [13] encoder thread 0 waiting for its staging slot
+// (enc_empty), [14] encoder thread 0 (heads warp) running the tile's heads / compositing, [16] consumer thread 0 waiting for the
+// tile's head-input buffer (hs_empty), [17] the heads warp waiting for the tile's head inputs (hs_full)
 __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
 #define TC_PUT(tno, k, v)                                                                                            \
   do {                                                                                                               \
@@ -202,12 +205,15 @@ __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE ins
 // enc_full[s] (count kEncThreads) once the encoder warps have written a tile's images, enc_empty[s] (count kEpiThreads) once the
 // consumers are done with them (after EB0; in sdf-only mode once the geo input has landed).  A operand: a_free (count 2, one per
 // consumer warpgroup) once a tile's last layer has read it, a_full (count 1 + the bulk copies' bytes) once the next tile's geo input
-// has landed in it.
+// has landed in it.  Head inputs `hs` (tile parity): hs_full[s] (count kEpiThreads) once the consumers have written a tile's (after
+// EC1), hs_empty[s] (count 32, the heads warp) once the heads warp has read them; not used in sdf-only mode.
 struct TcBars {
   uint64_t full[kStages], empty[kStages];
   uint64_t enc_full[2], enc_empty[2];
   uint64_t a_full, a_free;
+  uint64_t hs_full[2], hs_empty[2];
 };
+static_assert(sizeof(TcBars) + 4 * sizeof(double) <= kStaticSmem, "static shared memory of k_field_tc (kStaticSmem)");
 
 // Producer (one thread of the producer warpgroup).  Per tile: once the consumers have freed the A operand (a_free, from the second
 // tile on) and the encoder has staged the tile (enc_full), bulk-copies the staged geo input image into A columns 0..95 (a_full);
@@ -234,31 +240,6 @@ __device__ __forceinline__ void produce_all(const TcArgs& a, int nlayers, uint8_
         ring_fill<kStages>(ring, full, empty, j, reinterpret_cast<const uint8_t*>(a.blob) + ly.w_off, kb, kStageBytes, &waited);
     }
     TC_PUT(tile_no, 10, waited);
-  }
-}
-
-// Encoder warps (et = 0..95): walk the same tiles as the consumers and stage each one in its slot while the consumers run the tile
-// before it.  A tile is 768 items, 8 per thread: 512 (point, group of four hash levels), then 128 x (PE | x, point outputs) and, with
-// the colour MLP, 128 x colour-static columns.  Item i goes to thread i % 96, so each warp runs 32 consecutive items of one kind.
-template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table) {
-  const int n_items = a.mode != 0 ? 768 : 640;
-  int tile_no = 0;
-  for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
-    const long long w0 = TC_CLOCK();
-    mbar_wait(&b.enc_empty[tile_no & 1], ((tile_no >> 1) & 1) ^ 1);
-    const long long w1 = TC_CLOCK();
-    const Slot<P> s = slot_of<P>(slots, tile_no);
-#pragma unroll 1
-    for (int i = et; i < n_items; i += kEncThreads) {
-      const int row = i & 127;
-      if (i < 512) encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jac(), pol_table);
-      else if (i < 640) encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jac());
-      else colour_static_tile<P>(a, tile, row, s.cs(), kImgPlane);
-    }
-    fence_async_global();                    // the geo image is read by the producer's bulk copy (async proxy)
-    mbar_arrive(&b.enc_full[tile_no & 1]);
-    if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - w1); TC_PUT(tile_no, 13, w1 - w0); }
   }
 }
 
@@ -303,16 +284,23 @@ struct TileCtx {
   int r0, cq;                // accumulator rows r0, r0 + 8 of the tile and the column offset in every 8-column block
   uint8_t* abuf;             // A operand of every layer: [P][32 chunks][128 rows][16 B]
   const float* prm;          // [9][256] biases / fp32 weight rows used by the epilogues (smem: broadcast loads, not one LDG each)
-  float* hs;                 // [7][128] per-row inputs of the heads: sdf, gradient (3), raw rgb (3)
-  float* racc;               // [8][4] per-ray accumulators of the fused compositing (rays spanning several warps)
-  float* lastrgb;            // [4][3]
-  double* wtot;              // [4] per-warp scan totals of the fused compositing
+  float* hs;                 // [7][128] per-row inputs of the heads of the current tile: sdf, gradient (3), raw rgb (3)
+  const float4* coldesc;     // [96] EB0's view of the geo input columns 32..127 (ColDesc)
   float sdf_bias;
   uint32_t* sig_s;           // per-CTA scratch: softplus'(z1) as 2 x unorm16, [64 units][256 threads]
   uint32_t* gf_s;            //                  h2 as bf16x2 planes, [P][64 units][256 threads]
   char* slots;               //                  the two staging slots written by the encoder warps (kSlotBytes each)
-  uint64_t pol_keep;         // L2 policy of the staged reads
 };
+
+// softplus'(z1) in [0, 1] as unorm16 without F2I / I2F: s * 65535 (rounded, then kept apart from the add so that it is not contracted
+// into an FFMA) + 1.5 * 2^23 leaves round_to_nearest_even(s * 65535) in the low 16 bits, exactly what __float2uint_rn gives; the
+// decode puts u back into the mantissa of 2^23 and subtracts 2^23 (exact)
+__device__ __forceinline__ uint32_t unorm16x2_encode(float s0, float s1) {
+  const float f0 = __fadd_rn(__fmul_rn(s0, 65535.0f), 12582912.0f), f1 = __fadd_rn(__fmul_rn(s1, 65535.0f), 12582912.0f);
+  return __byte_perm(__float_as_uint(f0), __float_as_uint(f1), 0x5410);
+}
+__device__ __forceinline__ float unorm16_lo(uint32_t w) { return __fsub_rn(__uint_as_float(__byte_perm(w, 0x4B00u, 0x5410)), 8388608.0f) * (1.0f / 65535.0f); }
+__device__ __forceinline__ float unorm16_hi(uint32_t w) { return __fsub_rn(__uint_as_float(__byte_perm(w, 0x4B00u, 0x5432)), 8388608.0f) * (1.0f / 65535.0f); }
 
 // E0 (after G0): h1 = softplus(z1) -> A ; softplus'(z1) -> scratch
 template <int P>
@@ -328,7 +316,7 @@ __device__ __forceinline__ void epi_e0(const TileCtx& x, const float (&acc)[4][3
       softplus100_fast(acc[c][i] + b2.x, h0, s0);
       softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
       store_a_pair<P>(x.abuf, kAPlane, row, col, h0, h1);
-      if (x.a.mode != 0) x.sig_s[(c * 16 + (i >> 1)) * 256 + x.tid] = __float2uint_rn(s0 * 65535.0f) | (__float2uint_rn(s1 * 65535.0f) << 16);
+      if (x.a.mode != 0) x.sig_s[(c * 16 + (i >> 1)) * 256 + x.tid] = unorm16x2_encode(s0, s1);
     }
   }
 }
@@ -339,19 +327,22 @@ __device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, const float (
   const TcArgs& a = x.a;
   const float* p_bg1 = x.prm + 256;
   const float* p_wg2 = x.prm + 768;       // row 0 of the last geo layer
-  float sp[2] = {0.f, 0.f};
+  // one partial dot per accumulator row (r0, r0 + 8) as named scalars: an array indexed by the thread-dependent row below would live
+  // in local memory, written back after every FMA because the generic stores in between may alias it
+  float sp0 = 0.f, sp1 = 0.f;
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
-      const int col = frag_col(x.cq, c, i), h = (i >> 1) & 1, row = frag_row(x.r0, i);
+      const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
       const float2 b2 = *reinterpret_cast<const float2*>(p_bg1 + col);
       const float2 w2 = *reinterpret_cast<const float2*>(p_wg2 + col);
       float h0, h1, s0, s1;
       softplus100_fast(acc[c][i] + b2.x, h0, s0);
       softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
-      sp[h] = fmaf(w2.x, h0, sp[h]);
-      sp[h] = fmaf(w2.y, h1, sp[h]);
+      float& sp = (i >> 1) & 1 ? sp1 : sp0;
+      sp = fmaf(w2.x, h0, sp);
+      sp = fmaf(w2.y, h1, sp);
       if (a.mode != 0) {
         uint32_t hi, lo;
         split2(h0, h1, hi, lo);
@@ -362,17 +353,16 @@ __device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, const float (
       }
     }
   }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    sp[h] += __shfl_xor_sync(0xffffffffu, sp[h], 1);
-    sp[h] += __shfl_xor_sync(0xffffffffu, sp[h], 2);
-  }
+  sp0 += __shfl_xor_sync(0xffffffffu, sp0, 1);
+  sp0 += __shfl_xor_sync(0xffffffffu, sp0, 2);
+  sp1 += __shfl_xor_sync(0xffffffffu, sp1, 1);
+  sp1 += __shfl_xor_sync(0xffffffffu, sp1, 2);
   if ((x.t & 3) < 2) {
     const int h = x.t & 1, row = x.r0 + 8 * h;
-    const float sdf = sp[h] + x.sdf_bias;
+    const float sdf = (h ? sp1 : sp0) + x.sdf_bias;
     const long long p = (long long)tile * 128 + row;
     if (p < a.n_points && a.out.sdf) a.out.sdf[p] = sdf;
-    x.hs[row] = sdf;
+    if (a.mode != 0) x.hs[row] = sdf;
   }
 }
 
@@ -385,10 +375,25 @@ __device__ __forceinline__ void epi_eb1(const TileCtx& x, const float (&acc)[4][
     for (int i = 0; i < 32; i += 2) {
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
       const uint32_t sw = x.sig_s[(c * 16 + (i >> 1)) * 256 + x.tid];
-      const float s0 = (float)(sw & 0xFFFFu) * (1.0f / 65535.0f), s1 = (float)(sw >> 16) * (1.0f / 65535.0f);
-      store_a_pair<P>(x.abuf, kAPlane, row, col, acc[c][i] * s0, acc[c][i + 1] * s1);
+      store_a_pair<P>(x.abuf, kAPlane, row, col, acc[c][i] * unorm16_lo(sw), acc[c][i + 1] * unorm16_hi(sw));
     }
   }
+}
+
+// EB0's view of geo input column 32 + ip (ColDesc): float4 {row of the PE jacobian (int bits; -1: none, factor 1), then the weights of
+// the column on the x, y, z gradient}: PE column ip -> axis (ip mod 3 deg) / deg with factor 2^k cos(arg) from the jacobian, x column
+// -> its own axis with factor 1, padding -> all weights 0
+__device__ __forceinline__ float4 col_desc(const TcArgs& a, int ip) {
+  const int deg = a.pe_degree, half = 3 * deg;
+  int jrow = -1, ax = -1;
+  if (ip < a.pe_dim) {
+    const int ia = ip >= half ? ip - half : ip;
+    ax = ia < deg ? 0 : (ia < 2 * deg ? 1 : 2);
+    jrow = ip * 128;
+  } else if (ip - a.pe_dim < 3) {
+    ax = ip - a.pe_dim;
+  }
+  return make_float4(__int_as_float(jrow), ax == 0 ? 1.f : 0.f, ax == 1 ? 1.f : 0.f, ax == 2 ? 1.f : 0.f);
 }
 
 // EB0 (after B0): gin (96 cols, kernel order) . input jacobian -> d sdf / dx; then the colour misc operand over the (consumed) A columns
@@ -399,58 +404,57 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
   const TcArgs& a = x.a;
   const float* Jpe = reinterpret_cast<const float*>(s.jac());
   const float* Jg = Jpe + kPeRows * 128;
-  const int deg = a.pe_degree, half = 3 * deg;
-  float gr[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-#pragma unroll
-  for (int c = 0; c < 2; ++c) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int col = frag_col(x.cq, c, i), h = (i >> 1) & 1, row = frag_row(x.r0, i);
-      const float g = acc[c][i];
-      if (col < 32) {
-        if (col < a.grid_dim) {
-#pragma unroll
-          for (int d3 = 0; d3 < 3; ++d3) gr[h][d3] = fmaf(g, ld_stream_f1(Jg + (col * 3 + d3) * 128 + row, x.pol_keep), gr[h][d3]);
-        }
-      } else {
-        // PE column i -> axis (i mod 3 deg) / deg, factor 2^k cos(arg) ; x column -> its own axis, factor 1
-        const int ip = col - 32;
-        if (ip < a.pe_dim) {
-          const int ia = ip >= half ? ip - half : ip;
-          const int ax = ia < deg ? 0 : (ia < 2 * deg ? 1 : 2);
-          const float tv = g * ld_stream_f1(Jpe + ip * 128 + row, x.pol_keep);
-          gr[h][0] += ax == 0 ? tv : 0.f; gr[h][1] += ax == 1 ? tv : 0.f; gr[h][2] += ax == 2 ? tv : 0.f;
-        } else if (ip - a.pe_dim < 3) {
-          const int ax = ip - a.pe_dim;
-          gr[h][0] += ax == 0 ? g : 0.f; gr[h][1] += ax == 1 ? g : 0.f; gr[h][2] += ax == 2 ? g : 0.f;
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int d3 = 0; d3 < 3; ++d3) {
-      gr[h][d3] += __shfl_xor_sync(0xffffffffu, gr[h][d3], 1);
-      gr[h][d3] += __shfl_xor_sync(0xffffffffu, gr[h][d3], 2);
-    }
-  if ((x.t & 3) < 2) {
-    const int h = x.t & 1, row = x.r0 + 8 * h;
-    const long long p_raw = (long long)tile * 128 + row;
-    const PointGeom pg = point_geom(a, p_raw < a.n_points ? p_raw : a.n_points - 1);
-    const float grx = gr[h][0], gry = gr[h][1], grz = gr[h][2];
-    const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
-    const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? (grx / gn) * pg.dx + (gry / gn) * pg.dy + (grz / gn) * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
-    store_a_chunk<P>(x.abuf, kAPlane, row, 0, c0v);
-    x.hs[128 + row] = grx; x.hs[256 + row] = gry; x.hs[384 + row] = grz;
-  }
-  // unit k: plane k / (11 * 64), chunk 1 + (k / 64) % 11, row wrow0 + k % 64; all loads first, then the stores
+  // colour-static units (below) loaded first, so that they are in flight together with the jacobian loads
+  // unit k: plane k / (11 * 64), chunk 1 + (k / 64) % 11, row wrow0 + k % 64
   constexpr int kUnits = 11 * 64 * P, kPer = (kUnits + 127) / 128;
   uint4 v[kPer];
 #pragma unroll
   for (int j = 0; j < kPer; ++j) {
     const int k = x.t + 128 * j, pl = k / (11 * 64), ch = 1 + (k - pl * 11 * 64) / 64, row = x.wrow0 + (k & 63);
-    if (k < kUnits) v[j] = ld_stream_u4(s.cs() + pl * kImgPlane + ch * kAChunk + row * 16, x.pol_keep);
+    if (k < kUnits) v[j] = *reinterpret_cast<const uint4*>(s.cs() + pl * kImgPlane + ch * kAChunk + row * 16);
+  }
+  // d sdf / dx of rows r0 (g*0) and r0 + 8 (g*1), named scalars (see epi_e1).  Every column is accumulated the same way whatever its
+  // kind, the kind coming from the column table (ColDesc): a zero factor adds +-0, which leaves the sum as it is, so the result is
+  // the one of accumulating the live columns alone
+  float g0x = 0.f, g0y = 0.f, g0z = 0.f, g1x = 0.f, g1y = 0.f, g1z = 0.f;
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
+      const bool h = (i >> 1) & 1;
+      float& gx = h ? g1x : g0x;
+      float& gy = h ? g1y : g0y;
+      float& gz = h ? g1z : g0z;
+      const float g = acc[c][i];
+      if (c == 0 && i < 16) {                  // grid columns 0..31 (c, i are compile-time): g * grid jacobian row, or 0 past grid_dim
+        const bool live = col < a.grid_dim;
+        const float* j = Jg + col * 3 * 128 + row;
+        const float jx = live ? j[0] : 0.f, jy = live ? j[128] : 0.f, jz = live ? j[256] : 0.f;
+        gx = fmaf(g, jx, gx); gy = fmaf(g, jy, gy); gz = fmaf(g, jz, gz);
+      } else {                                 // PE | x | padding: (g * factor) onto the column's axis
+        const float4 d = x.coldesc[col - 32];
+        const int jrow = __float_as_int(d.x);
+        const float tv = __fmul_rn(g, jrow >= 0 ? Jpe[jrow + row] : 1.f);
+        gx = fmaf(tv, d.y, gx); gy = fmaf(tv, d.z, gy); gz = fmaf(tv, d.w, gz);
+      }
+    }
+  }
+  g0x += __shfl_xor_sync(0xffffffffu, g0x, 1); g0x += __shfl_xor_sync(0xffffffffu, g0x, 2);
+  g0y += __shfl_xor_sync(0xffffffffu, g0y, 1); g0y += __shfl_xor_sync(0xffffffffu, g0y, 2);
+  g0z += __shfl_xor_sync(0xffffffffu, g0z, 1); g0z += __shfl_xor_sync(0xffffffffu, g0z, 2);
+  g1x += __shfl_xor_sync(0xffffffffu, g1x, 1); g1x += __shfl_xor_sync(0xffffffffu, g1x, 2);
+  g1y += __shfl_xor_sync(0xffffffffu, g1y, 1); g1y += __shfl_xor_sync(0xffffffffu, g1y, 2);
+  g1z += __shfl_xor_sync(0xffffffffu, g1z, 1); g1z += __shfl_xor_sync(0xffffffffu, g1z, 2);
+  if ((x.t & 3) < 2) {
+    const int h = x.t & 1, row = x.r0 + 8 * h;
+    const long long p_raw = (long long)tile * 128 + row;
+    const PointGeom pg = point_geom(a, p_raw < a.n_points ? p_raw : a.n_points - 1);
+    const float grx = h ? g1x : g0x, gry = h ? g1y : g0y, grz = h ? g1z : g0z;
+    const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
+    const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? (grx / gn) * pg.dx + (gry / gn) * pg.dy + (grz / gn) * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
+    store_a_chunk<P>(x.abuf, kAPlane, row, 0, c0v);
+    x.hs[128 + row] = grx; x.hs[256 + row] = gry; x.hs[384 + row] = grz;
   }
 #pragma unroll
   for (int j = 0; j < kPer; ++j) {
@@ -492,40 +496,45 @@ __device__ __forceinline__ void epi_ec0(const TileCtx& x, const float (&acc)[4][
 __device__ __forceinline__ void epi_ec1(const TileCtx& x, const float (&acc)[4][32]) {
   const float* p_bc1 = x.prm + 1280;
   const float* p_wc2 = x.prm + 1536;      // [3][256]
-  float rr[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+  float r0r = 0.f, r0g = 0.f, r0b = 0.f, r1r = 0.f, r1g = 0.f, r1b = 0.f;   // rows r0, r0 + 8 (named scalars, see epi_e1)
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
-      const int col = frag_col(x.cq, c, i), h = (i >> 1) & 1;
+      const int col = frag_col(x.cq, c, i);
+      const bool h = (i >> 1) & 1;
+      float& rr = h ? r1r : r0r;
+      float& rg = h ? r1g : r0g;
+      float& rb = h ? r1b : r0b;
       const float v = fmaxf(acc[c][i] + p_bc1[col], 0.f);
-      rr[h][0] = fmaf(p_wc2[col], v, rr[h][0]);
-      rr[h][1] = fmaf(p_wc2[256 + col], v, rr[h][1]);
-      rr[h][2] = fmaf(p_wc2[512 + col], v, rr[h][2]);
+      rr = fmaf(p_wc2[col], v, rr);
+      rg = fmaf(p_wc2[256 + col], v, rg);
+      rb = fmaf(p_wc2[512 + col], v, rb);
     }
   }
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      rr[h][k] += __shfl_xor_sync(0xffffffffu, rr[h][k], 1);
-      rr[h][k] += __shfl_xor_sync(0xffffffffu, rr[h][k], 2);
-    }
+  r0r += __shfl_xor_sync(0xffffffffu, r0r, 1); r0r += __shfl_xor_sync(0xffffffffu, r0r, 2);
+  r0g += __shfl_xor_sync(0xffffffffu, r0g, 1); r0g += __shfl_xor_sync(0xffffffffu, r0g, 2);
+  r0b += __shfl_xor_sync(0xffffffffu, r0b, 1); r0b += __shfl_xor_sync(0xffffffffu, r0b, 2);
+  r1r += __shfl_xor_sync(0xffffffffu, r1r, 1); r1r += __shfl_xor_sync(0xffffffffu, r1r, 2);
+  r1g += __shfl_xor_sync(0xffffffffu, r1g, 1); r1g += __shfl_xor_sync(0xffffffffu, r1g, 2);
+  r1b += __shfl_xor_sync(0xffffffffu, r1b, 1); r1b += __shfl_xor_sync(0xffffffffu, r1b, 2);
   if ((x.t & 3) < 2) {
     const int h = x.t & 1, row = x.r0 + 8 * h;
-    x.hs[512 + row] = rr[h][0]; x.hs[640 + row] = rr[h][1]; x.hs[768 + row] = rr[h][2];
+    x.hs[512 + row] = h ? r1r : r0r; x.hs[640 + row] = h ? r1g : r0g; x.hs[768 + row] = h ? r1b : r0b;
   }
 }
 
-// per-point heads (warpgroup 0, thread = tile row) and, in fused mode, the per-ray compositing
-__device__ __forceinline__ void heads_and_composite(const TileCtx& x, int tile) {
-  const TcArgs& a = x.a;
-  const float* hs = x.hs;
-  float* racc = x.racc;
-  float* lastrgb = x.lastrgb;
-  double* wtot = x.wtot;
-  const int row = x.t, wq = x.tid >> 5, lane = x.tid & 31;
+// Per-point heads and, in fused mode, the per-ray compositing of one tile, run by one encoder warp on the head inputs `hs` that the
+// consumers left (sdf, gradient, raw rgb; the geometry is recomputed).  The warp walks the four 32-row chunks of the tile in order,
+// lane = row in the chunk.  A ray of S <= 32 samples lies in one chunk; a longer one spans S / 32 chunks: the chunk totals of its
+// transmittance scan go through `wtot` (chunk q -> wtot[q]) and its sums are carried from chunk to chunk in registers and written at
+// its last chunk, always in the same order.
+__device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float* hs, int tile, int lane, double* wtot) {
   const float* b_c2 = reinterpret_cast<const float*>(a.blob + a.b_c2);
+  float csum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};     // sums of the chunks so far of a ray longer than 32 samples
+#pragma unroll 1
+  for (int q = 0; q < 4; ++q) {
+  const int row = q * 32 + lane;
   const long long p_raw = (long long)tile * 128 + row;
   const bool valid = p_raw < a.n_points;
   const long long p = valid ? p_raw : a.n_points - 1;
@@ -565,8 +574,10 @@ __device__ __forceinline__ void heads_and_composite(const TileCtx& x, int tile) 
     // ---------------- fused compositing: the tile holds 128 / S whole rays; row -> (ray, sample) = (row / S, row % S) ----------------
     const int S = a.n_samples;
     const int s_idx = row % S;
-    const int rl = row / S;                                   // ray within the tile
     const bool dens = a.rnd.from_density != 0;
+    const bool multi = S > 32;                                // the ray spans chunks (warp-uniform)
+    const int first = multi ? (q * 32 / S) * (S / 32) : q;    // first chunk of the ray
+    const bool ray_end = !multi || q == first + S / 32 - 1;   // this chunk ends the ray (warp-uniform)
     // factor by which the transmittance drops across this sample: 1 - alpha + 1e-7 (rays.py:204-206), or as an exponent
     // delta * sigma for the density form (rays.py:160-170)
     const float dd = valid ? __fmul_rn(delta, density) : 0.f;
@@ -579,11 +590,11 @@ __device__ __forceinline__ void heads_and_composite(const TileCtx& x, int tile) 
     }
     double excl = __shfl_up_sync(0xffffffffu, incl, 1);
     if (lane == 0 || s_idx == 0) excl = dens ? 0.0 : 1.0;
-    if (lane == 31) wtot[wq] = incl;
-    named_sync(4, 128);
-    if (S > 32) {
-      const int first = (wq * 32 / S) * (S / 32);
-      for (int w2 = first; w2 < wq; ++w2) excl = dens ? excl + wtot[w2] : excl * wtot[w2];
+    if (multi) {
+      __syncwarp();                                           // every lane is through its reads of wtot from the chunk before
+      if (lane == 31) wtot[q] = incl;
+      __syncwarp();
+      for (int w2 = first; w2 < q; ++w2) excl = dens ? excl + wtot[w2] : excl * wtot[w2];
     }
     const float T = dens ? expf(-(float)excl) : (float)excl;
     const float al = dens ? __fsub_rn(1.0f, expf(-dd)) : alpha;
@@ -603,40 +614,27 @@ __device__ __forceinline__ void heads_and_composite(const TileCtx& x, int tile) 
       smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, d));
     }
     if (a.rnd.steps_minmax && lane == 0 && smin <= smax) { atomic_min_float(a.rnd.steps_minmax, smin); atomic_max_float(a.rnd.steps_minmax + 1, smax); }
-    if (S > 32) {
-      if (lane == 0) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) atomicAdd(&racc[k * 4 + rl], vs[k]);
-      }
-      if (s_idx == S - 1) { lastrgb[rl * 3] = rgbv[0]; lastrgb[rl * 3 + 1] = rgbv[1]; lastrgb[rl * 3 + 2] = rgbv[2]; }
-      named_sync(4, 128);
-      if (s_idx == 0) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) { vs[k] = racc[k * 4 + rl]; racc[k * 4 + rl] = 0.f; }
-      }
-    }
-    // transmittance after the last sample (alphas: transmittance[:, -1] = bg_transmittance, neus.py:101) / before it (densities: volsdf.py:67-68)
+    // transmittance after the last sample (alphas: transmittance[:, -1] = bg_transmittance, neus.py:101) / before it (densities:
+    // volsdf.py:67-68), and the colour of the last sample
     double tot;
     float lr, lg, lb;
-    if (S > 32) {
-      const int first = (wq * 32 / S) * (S / 32);
-      tot = dens ? 0.0 : 1.0;
-      const int nw = dens ? S / 32 - 1 : S / 32;
-      for (int w2 = first; w2 < first + nw; ++w2) tot = dens ? tot + wtot[w2] : tot * wtot[w2];
-      lr = lastrgb[rl * 3]; lg = lastrgb[rl * 3 + 1]; lb = lastrgb[rl * 3 + 2];
+    if (multi) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) { csum[k] += vs[k]; vs[k] = csum[k]; }   // lane 0: the chunk's sums, then the ray's so far
+      if (dens) {
+        tot = __shfl_sync(0xffffffffu, excl, 31);
+      } else {
+        tot = 1.0;
+        for (int w2 = first; w2 <= q; ++w2) tot *= wtot[w2];
+      }
+      lr = __shfl_sync(0xffffffffu, rgbv[0], 31); lg = __shfl_sync(0xffffffffu, rgbv[1], 31); lb = __shfl_sync(0xffffffffu, rgbv[2], 31);
     } else {
       const int last = (lane - s_idx) + S - 1;
       tot = __shfl_sync(0xffffffffu, dens ? excl : incl, last);
       lr = __shfl_sync(0xffffffffu, rgbv[0], last); lg = __shfl_sync(0xffffffffu, rgbv[1], last); lb = __shfl_sync(0xffffffffu, rgbv[2], last);
     }
-    if (S > 32 && dens) {
-      // exclusive sum at the last sample of the ray = transmittance exponent before the last sample; it lives in the last warp of the ray
-      if (s_idx == S - 1) wtot[wq] = excl;       // (wtot of the ray's last warp is no longer needed by anyone else)
-      named_sync(4, 128);
-      tot = wtot[(wq * 32 / S) * (S / 32) + S / 32 - 1];
-    }
-    const long long ray = (long long)tile * (128 / S) + rl;
-    if (s_idx == 0 && ray * S < a.n_points) {
+    const long long ray = (long long)tile * (128 / S) + row / S;
+    if (ray_end && s_idx == (multi ? S - 32 : 0) && ray * S < a.n_points) {
       const float acc = vs[0];
       if (a.rnd.rgb) {
         float bgc[3] = {0.f, 0.f, 0.f};
@@ -653,7 +651,53 @@ __device__ __forceinline__ void heads_and_composite(const TileCtx& x, int tile) 
       if (a.rnd.depth) a.rnd.depth[ray] = vs[7] / (acc + 1e-10f);
       if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)tot) : (float)tot;
     }
+    if (multi && ray_end) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) csum[k] = 0.f;
+    }
   }
+  }
+}
+
+// The heads warp's part of a tile: wait for its head inputs (hs_full), run the heads, hand the buffer back (hs_empty)
+__device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no, int lane, TcBars& b, float* hs, double* wtot) {
+  const long long w0 = TC_CLOCK();
+  mbar_wait(&b.hs_full[tile_no & 1], (tile_no >> 1) & 1);
+  const long long w1 = TC_CLOCK();
+  heads_and_composite(a, hs + (tile_no & 1) * kHsFloats, tile, lane, wtot);
+  mbar_arrive(&b.hs_empty[tile_no & 1]);
+  if (lane == 0) { TC_PUT(tile_no, 14, TC_CLOCK() - w1); TC_PUT(tile_no, 17, w1 - w0); }
+}
+
+// Encoder warps (et = 0..95): walk the same tiles as the consumers and stage each one in its slot while the consumers run the tile
+// before it.  A tile is 768 items, 8 per thread: 512 (point, group of four hash levels), then 128 x (PE | x, point outputs) and, with
+// the colour MLP, 128 x colour-static columns.  Item i goes to thread i % 96, so each warp runs 32 consecutive items of one kind.
+// Except in sdf-only mode, the first encoder warp then runs the heads of the tile before (the one the consumers are finishing), and
+// those of the last tile after the loop.  Staging tile n + 1 and the heads of tile n - 1 both fit in the consumers' tile n: slot
+// n + 1 was freed at EB0 of tile n - 1, and the head inputs of tile n - 1 are ready when tile n starts.
+template <int P, int LAYOUT>
+__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table, float* hs, double* wtot) {
+  const int n_items = a.mode != 0 ? 768 : 640;
+  const bool heads = a.mode != 0 && et < 32;     // the first encoder warp also runs the heads of the tile before
+  int tile_no = 0;
+  for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
+    const long long w0 = TC_CLOCK();
+    mbar_wait(&b.enc_empty[tile_no & 1], ((tile_no >> 1) & 1) ^ 1);
+    const long long w1 = TC_CLOCK();
+    const Slot<P> s = slot_of<P>(slots, tile_no);
+#pragma unroll 1
+    for (int i = et; i < n_items; i += kEncThreads) {
+      const int row = i & 127;
+      if (i < 512) encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jac(), pol_table);
+      else if (i < 640) encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jac());
+      else colour_static_tile<P>(a, tile, row, s.cs(), kImgPlane);
+    }
+    fence_async_global();                    // the geo image is read by the producer's bulk copy (async proxy)
+    mbar_arrive(&b.enc_full[tile_no & 1]);
+    if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - w1); TC_PUT(tile_no, 13, w1 - w0); }
+    if (heads && tile_no > 0) heads_of(a, tile - (int)gridDim.x, tile_no - 1, et, b, hs, wtot);
+  }
+  if (heads && tile_no > 0) heads_of(a, blockIdx.x + (tile_no - 1) * (int)gridDim.x, tile_no - 1, et, b, hs, wtot);   // the last tile
 }
 
 template <int P, int LAYOUT>
@@ -664,11 +708,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   uint8_t* ring = smem + P * kAPlane;
   float* fbuf = reinterpret_cast<float*>(ring + kStages * kStageBytes);
   float* prm = fbuf;                  // [9][256] biases / fp32 weight rows used by the epilogues
-  float* hs = prm + 9 * 256;          // [7][128] per-row inputs of the heads: sdf, gradient (3), raw rgb (3)
-  float* racc = hs + 7 * 128;         // [8][4] per-ray accumulators of the fused compositing (rays spanning several warps)
-  float* lastrgb = racc + 32;         // [4][3]
+  float* hs = prm + 9 * 256;          // [2][kHsFloats] per-row inputs of the heads, by tile parity: sdf, gradient (3), raw rgb (3)
+  float4* coldesc = reinterpret_cast<float4*>(hs + 2 * kHsFloats);    // [96] ColDesc of the geo input columns 32..127
   __shared__ TcBars bars;
-  __shared__ double wtot[4];
+  __shared__ double wtot[4];          // chunk totals of the compositing scan (heads warp)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nlayers = a.mode == 0 ? 2 : L_COUNT;
@@ -676,6 +719,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], kEpiWarps); }
     for (int s = 0; s < 2; ++s) { mbar_init(&bars.enc_full[s], kEncThreads); mbar_init(&bars.enc_empty[s], kEpiThreads); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&bars.hs_full[s], kEpiThreads); mbar_init(&bars.hs_empty[s], 32); }
     mbar_init(&bars.a_full, 1);
     mbar_init(&bars.a_free, 2);
     fence_barrier_init();
@@ -688,7 +732,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
                            reinterpret_cast<const float*>(blob + a.w_c2), reinterpret_cast<const float*>(blob + a.w_c2) + 256,
                            reinterpret_cast<const float*>(blob + a.w_c2) + 512};
     for (int i = tid; i < 9 * 256; i += kTcThreads) prm[i] = src[i >> 8][i & 255];
-    if (tid < 44) racc[tid] = 0.f;
+    if (tid < 96) coldesc[tid] = col_desc(a, tid);
   }
   __syncthreads();
 
@@ -696,7 +740,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   if (tid >= kEpiThreads) {
     setmaxnreg_dec<kProducerRegs>();
     if (tid == kEpiThreads) produce_all<P>(a, nlayers, abuf, ring, slots, bars);
-    else if (tid >= kTcThreads - kEncThreads) encode_all<P, LAYOUT>(a, tid - (kTcThreads - kEncThreads), slots, bars, l2_policy_evict_last());
+    else if (tid >= kTcThreads - kEncThreads) encode_all<P, LAYOUT>(a, tid - (kTcThreads - kEncThreads), slots, bars, l2_policy_evict_last(), hs, wtot);
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();
@@ -710,8 +754,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   const uint32_t a_base = smem_u32(abuf) + wrow0 * 16;
   const float sdf_bias = __ldg(reinterpret_cast<const float*>(a.blob + a.b_g2));
   char* scr = a.scratch + (size_t)blockIdx.x * a.scratch_per_cta;
-  const TileCtx x{a, tid, t, wg, wrow0, frag_row0(wrow0, t), frag_cq(t), abuf, prm, hs, racc, lastrgb, wtot, sdf_bias,
-                  reinterpret_cast<uint32_t*>(scr), reinterpret_cast<uint32_t*>(scr + 65536), slots, l2_policy_evict_normal()};
+  TileCtx x{a, tid, t, wg, wrow0, frag_row0(wrow0, t), frag_cq(t), abuf, prm, hs, coldesc, sdf_bias,
+            reinterpret_cast<uint32_t*>(scr), reinterpret_cast<uint32_t*>(scr + 65536), slots};
   uint32_t it = 0;
   long long waited = 0;
   float acc[4][32];
@@ -734,6 +778,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     waited = 0;
     const int sl = tile_no & 1;
     const Slot<P> s = slot_of<P>(slots, tile_no);
+    x.hs = hs + sl * kHsFloats;
     mbar_wait(&bars.a_full, tile_no & 1);      // the geo input staged by the encoder warps has landed in A columns 0..95
     if (a.mode == 0) mbar_arrive(&bars.enc_empty[sl]);
     TC_STAMP(8);
@@ -745,6 +790,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
       if (t == 0) mbar_arrive(&bars.a_free);
       epi_e1<P>(x, tile, acc);
       continue;
+    }
+    {
+      const long long w0 = TC_CLOCK();
+      mbar_wait(&bars.hs_empty[sl], ((tile_no >> 1) & 1) ^ 1);   // the heads warp is done with the tile two before
+      if (tid == 0) TC_PUT(tile_no, 16, TC_CLOCK() - w0);
     }
     epi_e1<P>(x, tile, acc);
     SYNC_A();
@@ -765,9 +815,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     LAYER(L_C1, true);
     if (t == 0) mbar_arrive(&bars.a_free);     // the last layer has read A: the next tile's geo input may land
     epi_ec1(x, acc);
-    named_sync(3, kEpiThreads);                // both warpgroups' head inputs are in `hs`
-    if (wg == 0) heads_and_composite(x, tile);
-    named_sync(3, kEpiThreads);                // `hs` / `racc` are rewritten by the next tile
+    mbar_arrive(&bars.hs_full[sl]);            // the heads warp takes the tile from here
     TC_STAMP(15);
     if (tid == 0) TC_PUT(tile_no, 9, waited);
   }

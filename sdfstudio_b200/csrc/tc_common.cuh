@@ -152,18 +152,6 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 template <uint32_t R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// ---- L2-hinted global load (per-CTA scratch of the fused kernel) -------------------------------------------------
-__device__ __forceinline__ float ld_stream_f1(const float* p, uint64_t pol) {
-  float v;
-  asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol) : "memory");
-  return v;
-}
-__device__ __forceinline__ uint4 ld_stream_u4(const void* p, uint64_t pol) {
-  uint4 v;
-  asm volatile("ld.global.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol) : "memory");
-  return v;
-}
-
 // ---- bf16 split helpers ------------------------------------------------------------------------------------------
 // x = hi + lo (+ O(2^-17 |x|)) with hi, lo bf16.  pack2 packs two bf16 (first element in the low half).
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
