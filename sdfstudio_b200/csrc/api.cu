@@ -19,7 +19,7 @@ bool field_tc_supported(const sdfb200_field_t& f, const FieldPlan& p);
 int field_tc_pack(const sdfb200_field_t& f, const FieldPlan& p, char* blob, cudaStream_t st);
 bool field_tc_render_supported(const sdfb200_field_t& f, const FieldPlan& p, int n_samples);
 int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* blob, const void* table, const sdfb200_field_in_t& in,
-                     const sdfb200_field_out_t& out, const TcRender* rnd, float* ws, size_t ws_floats, cudaStream_t st);
+                     const sdfb200_field_out_t& out, const sdfb200_field_render_t* rnd, float* ws, size_t ws_floats, cudaStream_t st);
 size_t field_tc_workspace_floats(const sdfb200_field_t& f, const FieldPlan& p, int64_t n_points);
 
 static int plan_or_fail(const sdfb200_field_t* f, FieldPlan& p) {
@@ -165,11 +165,7 @@ extern "C" int sdfb200_field_render(const sdfb200_field_t* f, const void* packed
   const bool fused = f->precision != SDFB200_PRECISION_FP32 && p.tc_bytes > 0 && so.geo_feature == nullptr &&
                      field_tc_render_supported(*f, p, in->n_samples);
   if (fused) {
-    TcRender t;
-    t.enabled = 1; t.from_density = rnd->from_density; t.bg_mode = rnd->bg_mode; t.clamp01 = rnd->clamp01; t.bg = rnd->bg;
-    t.rgb = rnd->out.rgb; t.depth = rnd->out.depth; t.normal = rnd->out.normal; t.accumulation = rnd->out.accumulation;
-    t.bg_transmittance = rnd->bg_transmittance; t.weights = rnd->weights; t.steps_minmax = rnd->out.steps_minmax;
-    r = field_tc_forward(*f, p, (const char*)packed, table, *in, so, &t, (float*)wsp, ws_floats, (cudaStream_t)stream);
+    r = field_tc_forward(*f, p, (const char*)packed, table, *in, so, rnd, (float*)wsp, ws_floats, (cudaStream_t)stream);
     if (r) return r;
   } else {
     const size_t stage = render_stage_floats(N);

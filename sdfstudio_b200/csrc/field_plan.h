@@ -136,11 +136,4 @@ inline void make_workspace_plan(const sdfb200_field_t& f, const FieldPlan& p, in
   w.floats_per_chunk = off;
 }
 
-// per-ray compositing inside the fused tensor-core kernel (field_tc.cu; requires 128 % n_samples == 0: every tile holds whole rays)
-struct TcRender {
-  int enabled, from_density, bg_mode, clamp01;
-  const float* bg;
-  float *rgb, *depth, *normal, *accumulation, *bg_transmittance, *weights, *steps_minmax;
-};
-
 }  // namespace sdfb200

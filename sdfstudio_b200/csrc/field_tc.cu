@@ -29,8 +29,6 @@ __global__ void k_fuse_c0(const float* __restrict__ Wc0, int ldc0, const float* 
 // -----------------------------------------------------------------------------------------------------------------
 // host side
 // -----------------------------------------------------------------------------------------------------------------
-static size_t tc_layer_bytes(int planes, int Np, int nkb, int kblk) { return (size_t)nkb * planes * Np * kblk * 2; }
-
 struct TcPlan {
   int planes;
   TcLayer layer[L_COUNT];
@@ -42,10 +40,7 @@ static void make_tc_plan(const sdfb200_field_t& f, const FieldPlan& p, TcPlan& t
   size_t off = p.tc_off;
   for (int l = 0; l < L_COUNT; ++l) {
     t.layer[l].w_off = off;
-    t.layer[l].Np = tc_layer_np(l);
-    t.layer[l].kblk = tc_layer_kblk(l);
-    t.layer[l].nkb = tc_layer_k(l) / t.layer[l].kblk;
-    off = align_up(off + tc_layer_bytes(t.planes, t.layer[l].Np, t.layer[l].nkb, t.layer[l].kblk), 256);
+    off = align_up(off + (size_t)tc_layer_nkb(l) * tc_stage_bytes(t.planes), 256);
   }
   t.wc_off = off;                       // fp32 [256][256]: Wgf * W2[1:,:]   (colour layer 0 applied to h2 directly)
   off = align_up(off + 256 * 256 * 4, 256);
@@ -86,8 +81,7 @@ int field_tc_pack(const sdfb200_field_t& f, const FieldPlan& p, char* blob, cuda
   TcPlan t;
   make_tc_plan(f, p, t);
   auto pack = [&](int L, const float* W, int ldw, int N, int K, const TcIdxMap* colmap, const TcIdxMap* rowmap) -> int {
-    const TcLayer& ly = t.layer[L];
-    return tc_pack(W, ldw, 0, N, K, ly.Np, ly.kblk, ly.nkb, t.planes, rowmap, colmap, blob + ly.w_off, st);
+    return tc_pack(W, ldw, 0, N, K, tc_layer_np(L), tc_layer_kblk(L), tc_layer_nkb(L), t.planes, rowmap, colmap, blob + t.layer[L].w_off, st);
   };
   const LayerPlan &g0 = p.geo[0], &g1 = p.geo[1], &g2 = p.geo[2], &c0 = p.col[0], &c1 = p.col[1];
   // geo input, kernel column order [grid(32) | PE | x | 0]  <-  reference order [x(3) | PE | grid]  (sdf_field.py:391-396)
@@ -120,7 +114,7 @@ int field_tc_pack(const sdfb200_field_t& f, const FieldPlan& p, char* blob, cuda
 }
 
 int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* blob, const void* table, const sdfb200_field_in_t& in,
-                     const sdfb200_field_out_t& out, const TcRender* rnd, float* ws, size_t ws_floats, cudaStream_t st) {
+                     const sdfb200_field_out_t& out, const sdfb200_field_render_t* rnd, float* ws, size_t ws_floats, cudaStream_t st) {
   const int64_t N = in.n_rays * (int64_t)in.n_samples;
   if (N == 0) return 0;
   TcPlan t;
@@ -128,7 +122,7 @@ int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* b
   const size_t per_cta = kScratchPerCta(t.planes);
   if (ws_floats * sizeof(float) < (size_t)kNumSMs * per_cta) return fail(SDFB200_EWORKSPACE, "workspace too small for the tensor-core path%s", "", 0);
   SDFB_REQUIRE(out.geo_feature == nullptr, "geo_feature is not produced by the tensor-core path (use precision fp32)");
-  const bool render = rnd != nullptr && rnd->enabled;
+  const bool render = rnd != nullptr;
   const bool sdf_only = !render && out.sdf && !out.gradients && !out.normals && !out.rgb && !out.density && !out.alpha && !out.occupancy;
   if (!sdf_only) {
     if (out.rgb || out.alpha || render) SDFB_REQUIRE(in.directions != nullptr, "directions required for rgb / alpha");
@@ -142,7 +136,7 @@ int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* b
   for (int l = 0; l < L_COUNT; ++l) a.layer[l] = t.layer[l];
   a.use_grid = f.use_grid_feature; a.pe_degree = f.pe_degree; a.use_pe = f.use_position_encoding;
   a.contraction = in.apply_contraction ? f.contraction : SDFB200_CONTRACT_NONE;
-  a.in_dim = p.in_dim; a.pe_dim = p.pe_dim; a.grid_dim = p.grid_dim; a.app_dim = f.appearance_dim; a.use_n_dot_v = f.use_n_dot_v;
+  a.pe_dim = p.pe_dim; a.grid_dim = p.grid_dim; a.app_dim = f.appearance_dim; a.use_n_dot_v = f.use_n_dot_v;
   a.mode = sdf_only ? 0 : 1;
   a.n_samples = in.n_samples; a.has_bins = in.bins != nullptr; a.n_points = N; a.n_tiles = (int)ceil_div(N, 128);
   a.rgb_padding = f.rgb_padding; a.cos_anneal = in.cos_anneal_ratio;
@@ -150,12 +144,13 @@ int field_tc_forward(const sdfb200_field_t& f, const FieldPlan& p, const char* b
   a.beta_min = in.beta_min; a.table = table; a.blob = blob;
   a.b_g0 = p.geo[0].b_off; a.b_g1 = p.geo[1].b_off; a.b_g2 = p.geo[2].b_off; a.w_g2 = p.geo[2].w_off;
   a.b_c0 = t.bc_off; a.b_c1 = p.col[1].b_off; a.w_c2 = p.col[2].w_off; a.b_c2 = p.col[2].b_off;
-  a.scratch = reinterpret_cast<char*>(ws); a.scratch_per_cta = per_cta; a.out = out;
-  if (render) a.rnd = *rnd; else { a.rnd = TcRender{}; a.rnd.enabled = 0; }
+  a.scratch = reinterpret_cast<char*>(ws); a.out = out;
+  a.render = render;
+  a.rnd = render ? *rnd : sdfb200_field_render_t{};
   // persistent CTAs, one per SM (the static tile loop needs no co-residency, but more CTAs than SMs would only add a tail wave)
   const int ctas = persistent_ctas();
   const int grid = a.n_tiles < ctas ? a.n_tiles : ctas;
-  const size_t smem = tc_smem_bytes(t.planes);
+  const size_t smem = tc_smem(t.planes).bytes;
   const bool torch_layout = f.grid.layout == SDFB200_GRID_TORCH;
   if (t.planes == 2) return torch_layout ? launch_field_tc_p2_torch(a, grid, smem, st) : launch_field_tc_p2_tcnn(a, grid, smem, st);
   return torch_layout ? launch_field_tc_p1_torch(a, grid, smem, st) : launch_field_tc_p1_tcnn(a, grid, smem, st);

@@ -25,23 +25,45 @@ constexpr float kHalfPiF = 1.5707963267948966f;
 // kernel order of the geo input columns (K = 96): [grid features 0..31 | PE | x(3) | zero padding] -- every group of four hash
 // levels is one aligned 16-byte operand chunk.  W0 (columns) and W0^T (rows) are permuted accordingly at pack time.
 constexpr uint32_t kAPlane = 32 * 2048;   // one bf16 plane of the A operand: [K/8 = 32][128 rows][16 B]
-// per-CTA scratch: softplus'(z1) unorm16 [64 KB] | h2 planes [P x 64 KB] | two staging slots (tile parity), each
-//   geo input image [P][12 chunks][128 rows][16 B] | colour-static image, same layout (chunk 0 unused) | input jacobian
-//   (PE [64][128] f32 | grid [96][128] f32)
-constexpr size_t kJRBytes = (size_t)(kPeRows + kMaxGridDim * 3) * 128 * 4;
 constexpr uint32_t kImgPlane = (kInK / 8) * 128 * 16;      // one bf16 plane of a staged 96-column operand image (24 KB)
-__host__ __device__ constexpr size_t kSlotBytes(int planes) { return 2 * (size_t)planes * kImgPlane + kJRBytes; }
-__host__ __device__ constexpr size_t kScratchPerCta(int planes) { return 65536 + (size_t)planes * 65536 + 2 * kSlotBytes(planes); }
+__host__ __device__ constexpr uint32_t tc_stage_bytes(int planes) { return (uint32_t)planes * 256 * kKB * 2; }   // one weight K-block
 
-constexpr int kHsFloats = 7 * 128;                         // head inputs of one tile: sdf, gradient (3), raw rgb (3) per row
-constexpr size_t kSmemPerBlock = 232448;                     // H100: 227 KB of shared memory per block (dynamic + static)
-constexpr size_t kStaticSmem = 1024;      // the kernel's static shared memory (barriers): one 1024-byte slot, the dynamic part is 1024-aligned
-// dynamic shared memory of the kernel: A operand | weight ring | epilogue parameters [9][256] f32 | head inputs by tile parity |
-// EB0 column table [96] float4
-__host__ __device__ constexpr size_t tc_smem_bytes(int planes) {
-  return (size_t)planes * kAPlane + (size_t)kStages * planes * 256 * kKB * 2 + (9 * 256 + 2 * kHsFloats) * 4 + 96 * 16;
+// rows of the epilogue parameters `prm` ([kPrmRows][256] f32): biases and the fp32 weight rows of the dot-product layers
+enum { PRM_B_G0 = 0, PRM_B_G1, PRM_W_G2 /* row 0 */, PRM_B_C0, PRM_B_C1, PRM_W_C2 /* rows 0..2 */, kPrmRows = PRM_W_C2 + 3 };
+// rows of the head inputs `hs` of one tile ([kHsRows][128] f32, one column per tile row)
+enum { HS_SDF = 0, HS_GRAD /* x, y, z */, HS_RGB = HS_GRAD + 3 /* raw r, g, b */, kHsRows = HS_RGB + 3 };
+
+// Dynamic shared memory of k_field_tc: byte offsets from its 1024-aligned base
+struct TcSmem { size_t a, ring, prm, hs, coldesc, bytes; };
+__host__ __device__ constexpr TcSmem tc_smem(int planes) {
+  TcSmem s{};                                                  // a: A operand of every layer [P][32 chunks][128 rows][16 B]
+  s.ring = s.a + (size_t)planes * kAPlane;                     // weight ring: kStages x one K-block
+  s.prm = s.ring + (size_t)kStages * tc_stage_bytes(planes);   // epilogue parameters [kPrmRows][256] f32
+  s.hs = s.prm + kPrmRows * 256 * 4;                           // head inputs by tile parity [2][kHsRows][128] f32
+  s.coldesc = s.hs + 2 * kHsRows * 128 * 4;                    // EB0's view of the geo input columns 32..127 [96] float4 (ColDesc)
+  s.bytes = s.coldesc + 96 * 16;
+  return s;
 }
-static_assert(tc_smem_bytes(2) + kStaticSmem <= kSmemPerBlock, "shared memory of k_field_tc at two planes");
+constexpr size_t kSmemPerBlock = 232448;  // H100: 227 KB of shared memory per block (dynamic + static)
+constexpr size_t kStaticSmem = 1024;      // the kernel's static shared memory (barriers): one 1024-byte slot, the dynamic part is 1024-aligned
+static_assert(tc_smem(2).bytes + kStaticSmem <= kSmemPerBlock, "shared memory of k_field_tc at two planes");
+
+// Per-CTA scratch of k_field_tc (caller workspace): byte offsets from the CTA's base.  sig and h2 are planes of [64 units][256 threads]
+// x 4 B (kFragWords) in the accumulator-fragment order of the thread that writes and later reads them.
+constexpr size_t kFragWords = 64 * 256;
+struct TcScratch { size_t sig, h2, slots, slot_bytes, geo, cs, jpe, jg, bytes; };
+__host__ __device__ constexpr TcScratch tc_scratch(int planes) {
+  TcScratch s{};                                               // sig: softplus'(z1) as 2 x unorm16
+  s.h2 = s.sig + kFragWords * 4;                               // h2 as bf16x2 planes [P]
+  s.slots = s.h2 + (size_t)planes * kFragWords * 4;            // two staging slots (tile parity), slot_bytes apart, each with:
+  s.cs = s.geo + (size_t)planes * kImgPlane;                   //   geo input image [P][12 chunks][128 rows][16 B] at geo = 0 and the
+  s.jpe = s.cs + (size_t)planes * kImgPlane;                   //   colour-static image (same layout, chunk 0 unused); PE jacobian
+  s.jg = s.jpe + (size_t)kPeRows * 128 * 4;                    //   [kPeRows][128] f32, grid jacobian [kMaxGridDim * 3][128] f32
+  s.slot_bytes = s.jg + (size_t)kMaxGridDim * 3 * 128 * 4;
+  s.bytes = s.slots + 2 * s.slot_bytes;                        // per CTA
+  return s;
+}
+__host__ __device__ constexpr size_t kScratchPerCta(int planes) { return tc_scratch(planes).bytes; }
 
 // layers in the order the kernel runs them (and the producer streams them)
 enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
@@ -52,6 +74,7 @@ enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
 __host__ __device__ constexpr int tc_layer_np(int L) { return L == L_B0 ? 128 : 256; }
 __host__ __device__ constexpr int tc_layer_k(int L) { return L == L_G0 || L == L_C0MISC ? kInK : 256; }
 __host__ __device__ constexpr int tc_layer_kblk(int L) { return kKB * 256 / tc_layer_np(L); }
+__host__ __device__ constexpr int tc_layer_nkb(int L) { return tc_layer_k(L) / tc_layer_kblk(L); }
 constexpr bool tc_blocks_fill_stages() {
   for (int L = 0; L < L_COUNT; ++L)
     if (tc_layer_np(L) * tc_layer_kblk(L) != 256 * kKB || tc_layer_kblk(L) % 16 != 0 || tc_layer_k(L) % tc_layer_kblk(L) != 0) return false;
@@ -61,15 +84,12 @@ static_assert(tc_blocks_fill_stages(), "every streamed weight block must be one 
 
 struct TcLayer {
   unsigned long long w_off;  // byte offset of the packed planes inside the blob
-  int Np;                    // rows of the weight tile (MMA N, a multiple of 64)
-  int nkb;                   // number of K blocks
-  int kblk;                  // K per block (tc_layer_kblk)
 };
 
 struct TcArgs {
   sdfb200_grid_t grid;
   TcLayer layer[L_COUNT];
-  int use_grid, pe_degree, use_pe, contraction, in_dim, pe_dim, grid_dim, app_dim, use_n_dot_v;
+  int use_grid, pe_degree, use_pe, contraction, pe_dim, grid_dim, app_dim, use_n_dot_v;
   int mode;  // 0: sdf only (G0, G1)   1: everything
   int n_samples, has_bins, n_tiles;
   long long n_points;
@@ -79,10 +99,10 @@ struct TcArgs {
   const char* blob;
   // fp32 section offsets (bytes)
   unsigned long long b_g0, b_g1, b_g2, w_g2, b_c0, b_c1, w_c2, b_c2;   // b_c0 = fused bias (bc0 + Wgf b2')
-  char* scratch;
-  unsigned long long scratch_per_cta;
+  char* scratch;               // tc_scratch(P).bytes per CTA
   sdfb200_field_out_t out;
-  TcRender rnd;
+  int render;                  // per-ray compositing in the same kernel (requires 128 % n_samples == 0: every tile holds whole rays)
+  sdfb200_field_render_t rnd;  // (clip_depth is applied after the kernel)
 };
 
 // one launcher per instantiation

@@ -73,11 +73,10 @@ static __device__ __forceinline__ float sin_call(float x) { return sinf(x); }
 
 // Hash-grid part of the geo input of one tile, levels 4 grp .. 4 grp + 3 of one point (= operand chunk grp).  Outputs: bf16 planes
 // of the staged geo input image (`img`, planes `plane` bytes apart, kernel column order: four levels = one aligned 16-byte chunk)
-// and the grid jacobian [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  One level at a time (smallest code).
+// and the grid jacobian Jg [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  One level at a time (smallest code).
 template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int row, int grp, uint8_t* img, uint32_t plane, uint8_t* enc,
+__device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int row, int grp, uint8_t* img, uint32_t plane, float* Jg,
                                                  uint64_t pol_table) {
-  float* Jg = reinterpret_cast<float*>(enc) + kPeRows * 128;
   const long long p_raw = (long long)tile * 128 + row;
   const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
   const PointGeom g = point_geom(a, p);
@@ -109,10 +108,9 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
 }
 
 // PE | x | zero padding: chunks 4..11 of the geo input.  Kernel column 32 + i holds PE_i, 32 + pe_dim + j holds x_j.  Also the
-// point outputs (contracted position and its norm) of a valid row.
+// point outputs (contracted position and its norm) of a valid row, and the PE jacobian Jpe [i][row].
 template <int P>
-__device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int row, uint8_t* img, uint32_t plane, uint8_t* enc) {
-  float* Jpe = reinterpret_cast<float*>(enc);
+__device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int row, uint8_t* img, uint32_t plane, float* Jpe) {
   const long long p_raw = (long long)tile * 128 + row;
   const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
   const PointGeom g = point_geom(a, p);
@@ -172,72 +170,62 @@ __device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, in
   }
 }
 
-// Staging slot of a tile (per-CTA scratch, selected by the parity of the CTA's tile count): geo input image | colour-static image |
-// input jacobian (the layout next to kSlotBytes)
+// Staging slot s of the per-CTA scratch (tc_scratch)
 template <int P>
 struct Slot {
   uint8_t* base;
-  __device__ __forceinline__ uint8_t* geo() const { return base; }
-  __device__ __forceinline__ uint8_t* cs() const { return base + (size_t)P * kImgPlane; }
-  __device__ __forceinline__ uint8_t* jac() const { return base + 2 * (size_t)P * kImgPlane; }
+  __device__ __forceinline__ Slot(char* slots, uint32_t s) : base(reinterpret_cast<uint8_t*>(slots) + s * tc_scratch(P).slot_bytes) {}
+  __device__ __forceinline__ uint8_t* geo() const { return base + tc_scratch(P).geo; }
+  __device__ __forceinline__ uint8_t* cs() const { return base + tc_scratch(P).cs; }
+  __device__ __forceinline__ float* jpe() const { return reinterpret_cast<float*>(base + tc_scratch(P).jpe); }
+  __device__ __forceinline__ float* jg() const { return reinterpret_cast<float*>(base + tc_scratch(P).jg); }
 };
-template <int P>
-__device__ __forceinline__ Slot<P> slot_of(char* slots, int tile_no) { return Slot<P>{reinterpret_cast<uint8_t*>(slots) + (size_t)(tile_no & 1) * kSlotBytes(P)}; }
 
 #ifdef SDFB200_TC_TIMING
 // CTA 0, first 16 tiles, row = tile: clock64() of consumer thread 0 at [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring
-// order), [8] the tile's geo input has landed (a_full; [8] - [0] is the consumers' wait for the encoder), [15] tile end = end of EC1
-// (head inputs handed over); cycle sums over the tile of [9] consumer thread 0 waiting for weights (full), [10] the producer waiting
-// for a free ring slot (empty), [12] encoder thread 0 busy staging the tile, [13] encoder thread 0 waiting for its staging slot
-// (enc_empty), [14] encoder thread 0 (heads warp) running the tile's heads / compositing, [16] consumer thread 0 waiting for the
-// tile's head-input buffer (hs_empty), [17] the heads warp waiting for the tile's head inputs (hs_full)
+// order), [8] the tile's geo input has landed (a full; [8] - [0] is the consumers' wait for the encoder), [15] tile end = end of EC1
+// (head inputs handed over); cycle sums over the tile of [9] consumer thread 0 waiting for weights (ring full), [10] the producer
+// waiting for a free ring slot (ring empty), [12] encoder thread 0 busy staging the tile, [13] encoder thread 0 waiting for its staging
+// slot (enc empty), [14] encoder thread 0 (heads warp) running the tile's heads / compositing, [16] consumer thread 0 waiting for the
+// tile's head-input buffer (hs empty), [17] the heads warp waiting for the tile's head inputs (hs full)
 __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
 #define TC_PUT(tno, k, v)                                                                                            \
   do {                                                                                                               \
     if (blockIdx.x == 0 && (tno) >= 0 && (tno) < 16) g_tc_timing[(tno) * 32 + (k)] = (v);                            \
   } while (0)
 #else
-#define TC_PUT(tno, k, v) do { } while (0)
+#define TC_PUT(tno, k, v) do { (void)(v); } while (0)
 #endif
 #define TC_STAMP(k) do { if (tid == 0) TC_PUT(tile_no, k, TC_CLOCK()); } while (0)
 
-// Barriers between the roles of the fused kernel.  Weight ring: full / empty (tc_common.cuh).  Staging slot s (tile parity):
-// enc_full[s] (count kEncThreads) once the encoder warps have written a tile's images, enc_empty[s] (count kEpiThreads) once the
-// consumers are done with them (after EB0; in sdf-only mode once the geo input has landed).  A operand: a_free (count 2, one per
-// consumer warpgroup) once a tile's last layer has read it, a_full (count 1 + the bulk copies' bytes) once the next tile's geo input
-// has landed in it.  Head inputs `hs` (tile parity): hs_full[s] (count kEpiThreads) once the consumers have written a tile's (after
-// EC1), hs_empty[s] (count 32, the heads warp) once the heads warp has read them; not used in sdf-only mode.
+// Hand-offs between the roles (tc_common.cuh), used once per tile (n = the CTA's tile count) except the ring.  Arrival counts:
 struct TcBars {
-  uint64_t full[kStages], empty[kStages];
-  uint64_t enc_full[2], enc_empty[2];
-  uint64_t a_full, a_free;
-  uint64_t hs_full[2], hs_empty[2];
+  Handoff<kStages> ring;  // weight ring, per K-block: full 1 + bytes, empty kEpiWarps
+  Handoff<2> enc;         // staging slots: full kEncThreads (images written), empty kEpiThreads (after EB0; sdf-only: after a full)
+  Handoff<1> a;           // A operand: full 1 + bytes (geo input landed), empty 2, one per consumer warpgroup (last layer has read A)
+  Handoff<2> hs;          // head inputs: full kEpiThreads (after EC1), empty 32 (the heads warp has read them); unused in sdf-only mode
 };
 static_assert(sizeof(TcBars) + 4 * sizeof(double) <= kStaticSmem, "static shared memory of k_field_tc (kStaticSmem)");
 
-// Producer (one thread of the producer warpgroup).  Per tile: once the consumers have freed the A operand (a_free, from the second
-// tile on) and the encoder has staged the tile (enc_full), bulk-copies the staged geo input image into A columns 0..95 (a_full);
-// then walks every K-block of every layer in consumption order and issues the bulk copy of block j once its ring slot has been
-// released (all 8 consumer warps are through block j - kStages).  Every block of every layer is one full stage (tc_blocks_fill_stages).
+// Producer (one thread of the producer warpgroup).  Per tile: once the consumers have freed the A operand and the encoder has staged
+// the tile, bulk-copies the staged geo input image into A columns 0..95; then walks every K-block of every layer in consumption order
+// and issues the bulk copy of block j once its ring slot has been released (all 8 consumer warps are through block j - kStages).
+// Every block of every layer is one full stage (tc_blocks_fill_stages).
 template <int P>
 __device__ __forceinline__ void produce_all(const TcArgs& a, int nlayers, uint8_t* abuf, uint8_t* ring, char* slots, TcBars& b) {
-  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;
   uint32_t j = 0;
   int tile_no = 0;
   for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
     long long waited = 0;
-    if (tile_no > 0) mbar_wait(&b.a_free, (tile_no - 1) & 1);
-    mbar_wait(&b.enc_full[tile_no & 1], (tile_no >> 1) & 1);
-    const uint8_t* geo = slot_of<P>(slots, tile_no).geo();
-    mbar_arrive_expect_tx(&b.a_full, (uint32_t)P * kImgPlane);
+    b.a.wait_empty(tile_no);
+    b.enc.wait_full(tile_no);
+    const uint8_t* geo = Slot<P>(slots, b.enc.slot(tile_no)).geo();
+    mbar_arrive_expect_tx(b.a.full_bar(tile_no), (uint32_t)P * kImgPlane);
 #pragma unroll
-    for (int pl = 0; pl < P; ++pl) bulk_g2s(abuf + pl * kAPlane, geo + pl * kImgPlane, kImgPlane, &b.a_full);
-    uint64_t* full = b.full;
-    uint64_t* empty = b.empty;
+    for (int pl = 0; pl < P; ++pl) bulk_g2s(abuf + pl * kAPlane, geo + pl * kImgPlane, kImgPlane, b.a.full_bar(tile_no));
     for (int L = 0; L < nlayers; ++L) {
-      const TcLayer& ly = a.layer[L];
-      for (int kb = 0; kb < ly.nkb; ++kb, ++j)
-        ring_fill<kStages>(ring, full, empty, j, reinterpret_cast<const uint8_t*>(a.blob) + ly.w_off, kb, kStageBytes, &waited);
+      for (int kb = 0; kb < tc_layer_nkb(L); ++kb, ++j)
+        ring_fill(b.ring, ring, j, reinterpret_cast<const uint8_t*>(a.blob) + a.layer[L].w_off, kb, tc_stage_bytes(P), &waited);
     }
     TC_PUT(tile_no, 10, waited);
   }
@@ -248,20 +236,20 @@ __device__ __forceinline__ void produce_all(const TcArgs& a, int nlayers, uint8_
 // complete (empty barrier count = 8 warps).  Each block is drained before the next is issued: with the producer in its own warpgroup and
 // 5 stages, keeping one block in flight (wait_group 1) measured no faster.
 template <int P, int L>
-__device__ __forceinline__ void layer_mma(float (&acc)[4][32], const TcLayer& ly, bool zero, uint32_t a_base, const uint8_t* ring, uint64_t* full,
-                                          uint64_t* empty, uint32_t& it, int lane, long long& waited) {
+__device__ __forceinline__ void layer_mma(float (&acc)[4][32], bool zero, uint32_t a_base, const uint8_t* ring, Handoff<kStages>& rb, uint32_t& it,
+                                          int lane, long long& waited) {
   constexpr int N = tc_layer_np(L);
   constexpr int KSTEPS = tc_layer_kblk(L) / 16;              // K steps per ring stage
-  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;
   constexpr uint32_t lbo_b = N * 16, plane_b = N * KSTEPS * 16 * 2;
   float (&d)[N / 2] = *reinterpret_cast<float (*)[N / 2]>(&acc[0][0]);
   if (zero) {
 #pragma unroll
     for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
   }
-  for (int kb = 0; kb < ly.nkb; ++kb, ++it) {
-    const int s = ring_wait<kStages>(full, it, &waited);
-    const uint32_t wbase = smem_u32(ring + (size_t)s * kStageBytes);
+#pragma unroll 1
+  for (int kb = 0; kb < tc_layer_nkb(L); ++kb, ++it) {
+    rb.wait_full(it, &waited);
+    const uint32_t wbase = smem_u32(ring + (size_t)rb.slot(it) * tc_stage_bytes(P));
     wg_fence_acc(d);
     wg_arrive();
 #pragma unroll
@@ -273,7 +261,7 @@ __device__ __forceinline__ void layer_mma(float (&acc)[4][32], const TcLayer& ly
     wg_wait<0>();
     wg_fence_acc(d);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
+    if (lane == 0) rb.arrive_empty(it);
   }
 }
 
@@ -282,14 +270,16 @@ struct TileCtx {
   const TcArgs& a;
   int tid, t, wg, wrow0;     // thread (0..255), thread in its warpgroup, warpgroup, first tile row of the warpgroup
   int r0, cq;                // accumulator rows r0, r0 + 8 of the tile and the column offset in every 8-column block
-  uint8_t* abuf;             // A operand of every layer: [P][32 chunks][128 rows][16 B]
-  const float* prm;          // [9][256] biases / fp32 weight rows used by the epilogues (smem: broadcast loads, not one LDG each)
-  float* hs;                 // [7][128] per-row inputs of the heads of the current tile: sdf, gradient (3), raw rgb (3)
-  const float4* coldesc;     // [96] EB0's view of the geo input columns 32..127 (ColDesc)
+  uint8_t* abuf;             // shared memory (tc_smem): A operand
+  const float (*prm)[256];   //   epilogue parameters (broadcast loads, not one LDG each)
+  float (*hs)[128];          //   head inputs of the current tile
+  const float4* coldesc;     //   EB0's column table
   float sdf_bias;
-  uint32_t* sig_s;           // per-CTA scratch: softplus'(z1) as 2 x unorm16, [64 units][256 threads]
-  uint32_t* gf_s;            //                  h2 as bf16x2 planes, [P][64 units][256 threads]
-  char* slots;               //                  the two staging slots written by the encoder warps (kSlotBytes each)
+  uint32_t* sig_s;           // per-CTA scratch (tc_scratch): softplus'(z1)
+  uint32_t* gf_s;            //   h2 planes
+  char* slots;               //   staging slots
+  // this thread's 4-byte unit for the accumulator pair (c, i) in a [64 units][256 threads] scratch plane (sig_s, gf_s)
+  __device__ __forceinline__ int unit(int c, int i) const { return (c * 16 + (i >> 1)) * kEpiThreads + tid; }
 };
 
 // softplus'(z1) in [0, 1] as unorm16 without F2I / I2F: s * 65535 (rounded, then kept apart from the add so that it is not contracted
@@ -305,7 +295,7 @@ __device__ __forceinline__ float unorm16_hi(uint32_t w) { return __fsub_rn(__uin
 // E0 (after G0): h1 = softplus(z1) -> A ; softplus'(z1) -> scratch
 template <int P>
 __device__ __forceinline__ void epi_e0(const TileCtx& x, const float (&acc)[4][32]) {
-  const float* p_bg0 = x.prm;
+  const float* p_bg0 = x.prm[PRM_B_G0];
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
@@ -316,7 +306,7 @@ __device__ __forceinline__ void epi_e0(const TileCtx& x, const float (&acc)[4][3
       softplus100_fast(acc[c][i] + b2.x, h0, s0);
       softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
       store_a_pair<P>(x.abuf, kAPlane, row, col, h0, h1);
-      if (x.a.mode != 0) x.sig_s[(c * 16 + (i >> 1)) * 256 + x.tid] = unorm16x2_encode(s0, s1);
+      if (x.a.mode != 0) x.sig_s[x.unit(c, i)] = unorm16x2_encode(s0, s1);
     }
   }
 }
@@ -325,8 +315,8 @@ __device__ __forceinline__ void epi_e0(const TileCtx& x, const float (&acc)[4][3
 template <int P>
 __device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, const float (&acc)[4][32]) {
   const TcArgs& a = x.a;
-  const float* p_bg1 = x.prm + 256;
-  const float* p_wg2 = x.prm + 768;       // row 0 of the last geo layer
+  const float* p_bg1 = x.prm[PRM_B_G1];
+  const float* p_wg2 = x.prm[PRM_W_G2];
   // one partial dot per accumulator row (r0, r0 + 8) as named scalars: an array indexed by the thread-dependent row below would live
   // in local memory, written back after every FMA because the generic stores in between may alias it
   float sp0 = 0.f, sp1 = 0.f;
@@ -340,29 +330,27 @@ __device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, const float (
       float h0, h1, s0, s1;
       softplus100_fast(acc[c][i] + b2.x, h0, s0);
       softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
-      float& sp = (i >> 1) & 1 ? sp1 : sp0;
+      float& sp = frag_half(i) ? sp1 : sp0;
       sp = fmaf(w2.x, h0, sp);
       sp = fmaf(w2.y, h1, sp);
       if (a.mode != 0) {
         uint32_t hi, lo;
         split2(h0, h1, hi, lo);
-        const int u = (c * 16 + (i >> 1)) * 256 + x.tid;
+        const int u = x.unit(c, i);
         x.gf_s[u] = hi;
-        if (P > 1) x.gf_s[64 * 256 + u] = lo;
+        if (P > 1) x.gf_s[kFragWords + u] = lo;
         store_a_pair<P>(x.abuf, kAPlane, row, col, w2.x * s0, w2.y * s1);
       }
     }
   }
-  sp0 += __shfl_xor_sync(0xffffffffu, sp0, 1);
-  sp0 += __shfl_xor_sync(0xffffffffu, sp0, 2);
-  sp1 += __shfl_xor_sync(0xffffffffu, sp1, 1);
-  sp1 += __shfl_xor_sync(0xffffffffu, sp1, 2);
+  sp0 = quad_sum(sp0);
+  sp1 = quad_sum(sp1);
   if ((x.t & 3) < 2) {
     const int h = x.t & 1, row = x.r0 + 8 * h;
     const float sdf = (h ? sp1 : sp0) + x.sdf_bias;
     const long long p = (long long)tile * 128 + row;
     if (p < a.n_points && a.out.sdf) a.out.sdf[p] = sdf;
-    if (a.mode != 0) x.hs[row] = sdf;
+    if (a.mode != 0) x.hs[HS_SDF][row] = sdf;
   }
 }
 
@@ -374,7 +362,7 @@ __device__ __forceinline__ void epi_eb1(const TileCtx& x, const float (&acc)[4][
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const uint32_t sw = x.sig_s[(c * 16 + (i >> 1)) * 256 + x.tid];
+      const uint32_t sw = x.sig_s[x.unit(c, i)];
       store_a_pair<P>(x.abuf, kAPlane, row, col, acc[c][i] * unorm16_lo(sw), acc[c][i + 1] * unorm16_hi(sw));
     }
   }
@@ -402,8 +390,8 @@ __device__ __forceinline__ float4 col_desc(const TcArgs& a, int ip) {
 template <int P>
 __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P>& s, const float (&acc)[4][32]) {
   const TcArgs& a = x.a;
-  const float* Jpe = reinterpret_cast<const float*>(s.jac());
-  const float* Jg = Jpe + kPeRows * 128;
+  const float* Jpe = s.jpe();
+  const float* Jg = s.jg();
   // colour-static units (below) loaded first, so that they are in flight together with the jacobian loads
   // unit k: plane k / (11 * 64), chunk 1 + (k / 64) % 11, row wrow0 + k % 64
   constexpr int kUnits = 11 * 64 * P, kPer = (kUnits + 127) / 128;
@@ -422,7 +410,7 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const bool h = (i >> 1) & 1;
+      const bool h = frag_half(i);
       float& gx = h ? g1x : g0x;
       float& gy = h ? g1y : g0y;
       float& gz = h ? g1z : g0z;
@@ -440,12 +428,8 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
       }
     }
   }
-  g0x += __shfl_xor_sync(0xffffffffu, g0x, 1); g0x += __shfl_xor_sync(0xffffffffu, g0x, 2);
-  g0y += __shfl_xor_sync(0xffffffffu, g0y, 1); g0y += __shfl_xor_sync(0xffffffffu, g0y, 2);
-  g0z += __shfl_xor_sync(0xffffffffu, g0z, 1); g0z += __shfl_xor_sync(0xffffffffu, g0z, 2);
-  g1x += __shfl_xor_sync(0xffffffffu, g1x, 1); g1x += __shfl_xor_sync(0xffffffffu, g1x, 2);
-  g1y += __shfl_xor_sync(0xffffffffu, g1y, 1); g1y += __shfl_xor_sync(0xffffffffu, g1y, 2);
-  g1z += __shfl_xor_sync(0xffffffffu, g1z, 1); g1z += __shfl_xor_sync(0xffffffffu, g1z, 2);
+  g0x = quad_sum(g0x); g0y = quad_sum(g0y); g0z = quad_sum(g0z);
+  g1x = quad_sum(g1x); g1y = quad_sum(g1y); g1z = quad_sum(g1z);
   if ((x.t & 3) < 2) {
     const int h = x.t & 1, row = x.r0 + 8 * h;
     const long long p_raw = (long long)tile * 128 + row;
@@ -454,7 +438,7 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
     const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
     const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? (grx / gn) * pg.dx + (gry / gn) * pg.dy + (grz / gn) * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
     store_a_chunk<P>(x.abuf, kAPlane, row, 0, c0v);
-    x.hs[128 + row] = grx; x.hs[256 + row] = gry; x.hs[384 + row] = grz;
+    x.hs[HS_GRAD][row] = grx; x.hs[HS_GRAD + 1][row] = gry; x.hs[HS_GRAD + 2][row] = grz;
   }
 #pragma unroll
   for (int j = 0; j < kPer; ++j) {
@@ -471,8 +455,8 @@ __device__ __forceinline__ void reload_h2(const TileCtx& x) {
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const int u = (c * 16 + (i >> 1)) * 256 + x.tid;
-      store_a_pair<P>(x.abuf, kAPlane, row, col, x.gf_s[u], x.gf_s[64 * 256 + u]);
+      const int u = x.unit(c, i);
+      store_a_pair<P>(x.abuf, kAPlane, row, col, x.gf_s[u], x.gf_s[kFragWords + u]);
     }
   }
 }
@@ -480,7 +464,7 @@ __device__ __forceinline__ void reload_h2(const TileCtx& x) {
 // EC0 (after C0): relu -> A
 template <int P>
 __device__ __forceinline__ void epi_ec0(const TileCtx& x, const float (&acc)[4][32]) {
-  const float* p_bc0 = x.prm + 1024;
+  const float* p_bc0 = x.prm[PRM_B_C0];
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
@@ -494,33 +478,29 @@ __device__ __forceinline__ void epi_ec0(const TileCtx& x, const float (&acc)[4][
 
 // EC1 (after C1): relu, last colour layer (256 -> 3) as fp32 dots -> heads
 __device__ __forceinline__ void epi_ec1(const TileCtx& x, const float (&acc)[4][32]) {
-  const float* p_bc1 = x.prm + 1280;
-  const float* p_wc2 = x.prm + 1536;      // [3][256]
+  const float* p_bc1 = x.prm[PRM_B_C1];
+  const float (*p_wc2)[256] = x.prm + PRM_W_C2;
   float r0r = 0.f, r0g = 0.f, r0b = 0.f, r1r = 0.f, r1g = 0.f, r1b = 0.f;   // rows r0, r0 + 8 (named scalars, see epi_e1)
 #pragma unroll
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int col = frag_col(x.cq, c, i);
-      const bool h = (i >> 1) & 1;
+      const bool h = frag_half(i);
       float& rr = h ? r1r : r0r;
       float& rg = h ? r1g : r0g;
       float& rb = h ? r1b : r0b;
       const float v = fmaxf(acc[c][i] + p_bc1[col], 0.f);
-      rr = fmaf(p_wc2[col], v, rr);
-      rg = fmaf(p_wc2[256 + col], v, rg);
-      rb = fmaf(p_wc2[512 + col], v, rb);
+      rr = fmaf(p_wc2[0][col], v, rr);
+      rg = fmaf(p_wc2[1][col], v, rg);
+      rb = fmaf(p_wc2[2][col], v, rb);
     }
   }
-  r0r += __shfl_xor_sync(0xffffffffu, r0r, 1); r0r += __shfl_xor_sync(0xffffffffu, r0r, 2);
-  r0g += __shfl_xor_sync(0xffffffffu, r0g, 1); r0g += __shfl_xor_sync(0xffffffffu, r0g, 2);
-  r0b += __shfl_xor_sync(0xffffffffu, r0b, 1); r0b += __shfl_xor_sync(0xffffffffu, r0b, 2);
-  r1r += __shfl_xor_sync(0xffffffffu, r1r, 1); r1r += __shfl_xor_sync(0xffffffffu, r1r, 2);
-  r1g += __shfl_xor_sync(0xffffffffu, r1g, 1); r1g += __shfl_xor_sync(0xffffffffu, r1g, 2);
-  r1b += __shfl_xor_sync(0xffffffffu, r1b, 1); r1b += __shfl_xor_sync(0xffffffffu, r1b, 2);
+  r0r = quad_sum(r0r); r0g = quad_sum(r0g); r0b = quad_sum(r0b);
+  r1r = quad_sum(r1r); r1g = quad_sum(r1g); r1b = quad_sum(r1b);
   if ((x.t & 3) < 2) {
     const int h = x.t & 1, row = x.r0 + 8 * h;
-    x.hs[512 + row] = h ? r1r : r0r; x.hs[640 + row] = h ? r1g : r0g; x.hs[768 + row] = h ? r1b : r0b;
+    x.hs[HS_RGB][row] = h ? r1r : r0r; x.hs[HS_RGB + 1][row] = h ? r1g : r0g; x.hs[HS_RGB + 2][row] = h ? r1b : r0b;
   }
 }
 
@@ -529,7 +509,7 @@ __device__ __forceinline__ void epi_ec1(const TileCtx& x, const float (&acc)[4][
 // lane = row in the chunk.  A ray of S <= 32 samples lies in one chunk; a longer one spans S / 32 chunks: the chunk totals of its
 // transmittance scan go through `wtot` (chunk q -> wtot[q]) and its sums are carried from chunk to chunk in registers and written at
 // its last chunk, always in the same order.
-__device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float* hs, int tile, int lane, double* wtot) {
+__device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float (*hs)[128], int tile, int lane, double* wtot) {
   const float* b_c2 = reinterpret_cast<const float*>(a.blob + a.b_c2);
   float csum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};     // sums of the chunks so far of a ray longer than 32 samples
 #pragma unroll 1
@@ -540,22 +520,22 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
   const long long p = valid ? p_raw : a.n_points - 1;
   const PointGeom pg = point_geom(a, p);
   const float dirx = pg.dx, diry = pg.dy, dirz = pg.dz, delta = pg.delta;
-  const float sdf = hs[row], grx = hs[128 + row], gry = hs[256 + row], grz = hs[384 + row];
+  const float sdf = hs[HS_SDF][row], grx = hs[HS_GRAD][row], gry = hs[HS_GRAD + 1][row], grz = hs[HS_GRAD + 2][row];
   const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
   const float nx = grx / gn, ny = gry / gn, nz = grz / gn;
   float rgbv[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float raw = hs[512 + c * 128 + row] + __ldg(b_c2 + c);
+    const float raw = hs[HS_RGB + c][row] + __ldg(b_c2 + c);
     rgbv[c] = sigmoidf_(raw) * (1.f + 2.f * a.rgb_padding) - a.rgb_padding;
   }
   float density = 0.f, alpha = 0.f;
-  if (a.out.density || (a.rnd.enabled && a.rnd.from_density)) {
+  if (a.out.density || (a.render && a.rnd.from_density)) {
     const float beta = fabsf(__ldg(a.beta)) + __ldg(a.beta_min);
     const float sg = sdf > 0.f ? 1.f : (sdf < 0.f ? -1.f : 0.f);
     density = (1.0f / beta) * (0.5f + 0.5f * sg * expm1f(-fabsf(sdf) / beta));
   }
-  if (a.out.alpha || (a.rnd.enabled && !a.rnd.from_density)) {
+  if (a.out.alpha || (a.render && !a.rnd.from_density)) {
     const float inv_s = fminf(fmaxf(expf(__ldg(a.variance) * 10.0f), 1e-6f), 1e6f);
     const float true_cos = dirx * grx + diry * gry + dirz * grz;
     const float iter_cos = -(fmaxf(-true_cos * 0.5f + 0.5f, 0.f) * (1.0f - a.cos_anneal) + fmaxf(-true_cos, 0.f) * a.cos_anneal);
@@ -570,7 +550,7 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
     if (a.out.occupancy) a.out.occupancy[p] = sigmoidf_(-10.0f * sdf);
     if (a.out.alpha) a.out.alpha[p] = alpha;
   }
-  if (a.rnd.enabled) {
+  if (a.render) {
     // ---------------- fused compositing: the tile holds 128 / S whole rays; row -> (ray, sample) = (row / S, row % S) ----------------
     const int S = a.n_samples;
     const int s_idx = row % S;
@@ -613,7 +593,7 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
       smin = fminf(smin, __shfl_xor_sync(0xffffffffu, smin, d));
       smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, d));
     }
-    if (a.rnd.steps_minmax && lane == 0 && smin <= smax) { atomic_min_float(a.rnd.steps_minmax, smin); atomic_max_float(a.rnd.steps_minmax + 1, smax); }
+    if (a.rnd.out.steps_minmax && lane == 0 && smin <= smax) { atomic_min_float(a.rnd.out.steps_minmax, smin); atomic_max_float(a.rnd.out.steps_minmax + 1, smax); }
     // transmittance after the last sample (alphas: transmittance[:, -1] = bg_transmittance, neus.py:101) / before it (densities:
     // volsdf.py:67-68), and the colour of the last sample
     double tot;
@@ -636,7 +616,7 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
     const long long ray = (long long)tile * (128 / S) + row / S;
     if (ray_end && s_idx == (multi ? S - 32 : 0) && ray * S < a.n_points) {
       const float acc = vs[0];
-      if (a.rnd.rgb) {
+      if (a.rnd.out.rgb) {
         float bgc[3] = {0.f, 0.f, 0.f};
         if (a.rnd.bg_mode == SDFB200_BG_COLOR) { bgc[0] = a.rnd.bg[0]; bgc[1] = a.rnd.bg[1]; bgc[2] = a.rnd.bg[2]; }
         else if (a.rnd.bg_mode == SDFB200_BG_PER_RAY) { bgc[0] = a.rnd.bg[ray * 3]; bgc[1] = a.rnd.bg[ray * 3 + 1]; bgc[2] = a.rnd.bg[ray * 3 + 2]; }
@@ -644,11 +624,11 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
         const float rem = 1.0f - acc;
         const float o[3] = {vs[1] + bgc[0] * rem, vs[2] + bgc[1] * rem, vs[3] + bgc[2] * rem};
 #pragma unroll
-        for (int c = 0; c < 3; ++c) a.rnd.rgb[ray * 3 + c] = a.rnd.clamp01 ? fminf(fmaxf(o[c], 0.f), 1.f) : o[c];
+        for (int c = 0; c < 3; ++c) a.rnd.out.rgb[ray * 3 + c] = a.rnd.clamp01 ? fminf(fmaxf(o[c], 0.f), 1.f) : o[c];
       }
-      if (a.rnd.accumulation) a.rnd.accumulation[ray] = acc;
-      if (a.rnd.normal) { a.rnd.normal[ray * 3] = vs[4]; a.rnd.normal[ray * 3 + 1] = vs[5]; a.rnd.normal[ray * 3 + 2] = vs[6]; }
-      if (a.rnd.depth) a.rnd.depth[ray] = vs[7] / (acc + 1e-10f);
+      if (a.rnd.out.accumulation) a.rnd.out.accumulation[ray] = acc;
+      if (a.rnd.out.normal) { a.rnd.out.normal[ray * 3] = vs[4]; a.rnd.out.normal[ray * 3 + 1] = vs[5]; a.rnd.out.normal[ray * 3 + 2] = vs[6]; }
+      if (a.rnd.out.depth) a.rnd.out.depth[ray] = vs[7] / (acc + 1e-10f);
       if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)tot) : (float)tot;
     }
     if (multi && ray_end) {
@@ -659,14 +639,14 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
   }
 }
 
-// The heads warp's part of a tile: wait for its head inputs (hs_full), run the heads, hand the buffer back (hs_empty)
-__device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no, int lane, TcBars& b, float* hs, double* wtot) {
-  const long long w0 = TC_CLOCK();
-  mbar_wait(&b.hs_full[tile_no & 1], (tile_no >> 1) & 1);
-  const long long w1 = TC_CLOCK();
-  heads_and_composite(a, hs + (tile_no & 1) * kHsFloats, tile, lane, wtot);
-  mbar_arrive(&b.hs_empty[tile_no & 1]);
-  if (lane == 0) { TC_PUT(tile_no, 14, TC_CLOCK() - w1); TC_PUT(tile_no, 17, w1 - w0); }
+// The heads warp's part of a tile: wait for its head inputs, run the heads, hand the buffer back
+__device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no, int lane, TcBars& b, float (*hs)[128], double* wtot) {
+  long long waited = 0;
+  b.hs.wait_full(tile_no, &waited);
+  const long long t0 = TC_CLOCK();
+  heads_and_composite(a, hs + b.hs.slot(tile_no) * kHsRows, tile, lane, wtot);
+  b.hs.arrive_empty(tile_no);
+  if (lane == 0) { TC_PUT(tile_no, 14, TC_CLOCK() - t0); TC_PUT(tile_no, 17, waited); }
 }
 
 // Encoder warps (et = 0..95): walk the same tiles as the consumers and stage each one in its slot while the consumers run the tile
@@ -676,25 +656,25 @@ __device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no,
 // those of the last tile after the loop.  Staging tile n + 1 and the heads of tile n - 1 both fit in the consumers' tile n: slot
 // n + 1 was freed at EB0 of tile n - 1, and the head inputs of tile n - 1 are ready when tile n starts.
 template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table, float* hs, double* wtot) {
+__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table, float (*hs)[128], double* wtot) {
   const int n_items = a.mode != 0 ? 768 : 640;
   const bool heads = a.mode != 0 && et < 32;     // the first encoder warp also runs the heads of the tile before
   int tile_no = 0;
   for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
-    const long long w0 = TC_CLOCK();
-    mbar_wait(&b.enc_empty[tile_no & 1], ((tile_no >> 1) & 1) ^ 1);
-    const long long w1 = TC_CLOCK();
-    const Slot<P> s = slot_of<P>(slots, tile_no);
+    long long waited = 0;
+    b.enc.wait_empty(tile_no, &waited);
+    const long long t0 = TC_CLOCK();
+    const Slot<P> s(slots, b.enc.slot(tile_no));
 #pragma unroll 1
     for (int i = et; i < n_items; i += kEncThreads) {
       const int row = i & 127;
-      if (i < 512) encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jac(), pol_table);
-      else if (i < 640) encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jac());
+      if (i < 512) encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jg(), pol_table);
+      else if (i < 640) encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jpe());
       else colour_static_tile<P>(a, tile, row, s.cs(), kImgPlane);
     }
     fence_async_global();                    // the geo image is read by the producer's bulk copy (async proxy)
-    mbar_arrive(&b.enc_full[tile_no & 1]);
-    if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - w1); TC_PUT(tile_no, 13, w1 - w0); }
+    b.enc.arrive_full(tile_no);
+    if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - t0); TC_PUT(tile_no, 13, waited); }
     if (heads && tile_no > 0) heads_of(a, tile - (int)gridDim.x, tile_no - 1, et, b, hs, wtot);
   }
   if (heads && tile_no > 0) heads_of(a, blockIdx.x + (tile_no - 1) * (int)gridDim.x, tile_no - 1, et, b, hs, wtot);   // the last tile
@@ -703,35 +683,34 @@ __device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots,
 template <int P, int LAYOUT>
 __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constant__ TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  constexpr uint32_t kStageBytes = (uint32_t)P * 256 * kKB * 2;        // one weight K-block, all planes (the 128-row layer: K blocks of 32)
-  uint8_t* abuf = smem;                                                // A operand of every layer: [P][32 chunks][128 rows][16 B]
-  uint8_t* ring = smem + P * kAPlane;
-  float* fbuf = reinterpret_cast<float*>(ring + kStages * kStageBytes);
-  float* prm = fbuf;                  // [9][256] biases / fp32 weight rows used by the epilogues
-  float* hs = prm + 9 * 256;          // [2][kHsFloats] per-row inputs of the heads, by tile parity: sdf, gradient (3), raw rgb (3)
-  float4* coldesc = reinterpret_cast<float4*>(hs + 2 * kHsFloats);    // [96] ColDesc of the geo input columns 32..127
+  constexpr TcSmem sm = tc_smem(P);
+  constexpr TcScratch scr = tc_scratch(P);
+  uint8_t* abuf = smem + sm.a;
+  uint8_t* ring = smem + sm.ring;
+  float (*prm)[256] = reinterpret_cast<float (*)[256]>(smem + sm.prm);
+  float (*hs)[128] = reinterpret_cast<float (*)[128]>(smem + sm.hs);
+  float4* coldesc = reinterpret_cast<float4*>(smem + sm.coldesc);
   __shared__ TcBars bars;
   __shared__ double wtot[4];          // chunk totals of the compositing scan (heads warp)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nlayers = a.mode == 0 ? 2 : L_COUNT;
-  char* slots = a.scratch + (size_t)blockIdx.x * a.scratch_per_cta + 65536 + (size_t)P * 65536;
+  char* cta_scr = a.scratch + (size_t)blockIdx.x * scr.bytes;
+  char* slots = cta_scr + scr.slots;
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], kEpiWarps); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&bars.enc_full[s], kEncThreads); mbar_init(&bars.enc_empty[s], kEpiThreads); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&bars.hs_full[s], kEpiThreads); mbar_init(&bars.hs_empty[s], 32); }
-    mbar_init(&bars.a_full, 1);
-    mbar_init(&bars.a_free, 2);
+    bars.ring.init(1, kEpiWarps);
+    bars.enc.init(kEncThreads, kEpiThreads);
+    bars.hs.init(kEpiThreads, 32);
+    bars.a.init(1, 2);
     fence_barrier_init();
   }
   {
     const char* blob = a.blob;
-    const float* src[9] = {reinterpret_cast<const float*>(blob + a.b_g0), reinterpret_cast<const float*>(blob + a.b_g1),
-                           reinterpret_cast<const float*>(blob + a.b_g1), reinterpret_cast<const float*>(blob + a.w_g2),
-                           reinterpret_cast<const float*>(blob + a.b_c0), reinterpret_cast<const float*>(blob + a.b_c1),
-                           reinterpret_cast<const float*>(blob + a.w_c2), reinterpret_cast<const float*>(blob + a.w_c2) + 256,
-                           reinterpret_cast<const float*>(blob + a.w_c2) + 512};
-    for (int i = tid; i < 9 * 256; i += kTcThreads) prm[i] = src[i >> 8][i & 255];
+    const float* src[kPrmRows] = {reinterpret_cast<const float*>(blob + a.b_g0), reinterpret_cast<const float*>(blob + a.b_g1),
+                                  reinterpret_cast<const float*>(blob + a.w_g2), reinterpret_cast<const float*>(blob + a.b_c0),
+                                  reinterpret_cast<const float*>(blob + a.b_c1), reinterpret_cast<const float*>(blob + a.w_c2),
+                                  reinterpret_cast<const float*>(blob + a.w_c2) + 256, reinterpret_cast<const float*>(blob + a.w_c2) + 512};
+    for (int i = tid; i < kPrmRows * 256; i += kTcThreads) prm[i >> 8][i & 255] = src[i >> 8][i & 255];
     if (tid < 96) coldesc[tid] = col_desc(a, tid);
   }
   __syncthreads();
@@ -744,8 +723,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();
-  uint64_t* full = bars.full;
-  uint64_t* empty = bars.empty;
 
   // ============================== two warpgroups, 64 rows of the tile each ==============================
   const int wg = warp >> 2, t = tid & 127;
@@ -753,9 +730,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   const int wg_bar = 1 + wg;                                 // named barrier of this warpgroup
   const uint32_t a_base = smem_u32(abuf) + wrow0 * 16;
   const float sdf_bias = __ldg(reinterpret_cast<const float*>(a.blob + a.b_g2));
-  char* scr = a.scratch + (size_t)blockIdx.x * a.scratch_per_cta;
   TileCtx x{a, tid, t, wg, wrow0, frag_row0(wrow0, t), frag_cq(t), abuf, prm, hs, coldesc, sdf_bias,
-            reinterpret_cast<uint32_t*>(scr), reinterpret_cast<uint32_t*>(scr + 65536), slots};
+            reinterpret_cast<uint32_t*>(cta_scr + scr.sig), reinterpret_cast<uint32_t*>(cta_scr + scr.h2), slots};
   uint32_t it = 0;
   long long waited = 0;
   float acc[4][32];
@@ -766,7 +742,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   } while (0)
 #define LAYER(L, zero)                                                                                 \
   do {                                                                                                 \
-    layer_mma<P, L>(acc, a.layer[L], zero, a_base, ring, full, empty, it, lane, waited);               \
+    layer_mma<P, L>(acc, zero, a_base, ring, bars.ring, it, lane, waited);                             \
     named_sync(wg_bar, 128); /* every warp of the warpgroup is done reading this layer's A operand */  \
     TC_STAMP(1 + (L));                                                                                 \
   } while (0)
@@ -776,25 +752,24 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     ++tile_no;
     TC_STAMP(0);
     waited = 0;
-    const int sl = tile_no & 1;
-    const Slot<P> s = slot_of<P>(slots, tile_no);
-    x.hs = hs + sl * kHsFloats;
-    mbar_wait(&bars.a_full, tile_no & 1);      // the geo input staged by the encoder warps has landed in A columns 0..95
-    if (a.mode == 0) mbar_arrive(&bars.enc_empty[sl]);
+    const Slot<P> s(slots, bars.enc.slot(tile_no));
+    x.hs = hs + bars.hs.slot(tile_no) * kHsRows;
+    bars.a.wait_full(tile_no);                 // the geo input staged by the encoder warps has landed in A columns 0..95
+    if (a.mode == 0) bars.enc.arrive_empty(tile_no);
     TC_STAMP(8);
     LAYER(L_G0, true);
     epi_e0<P>(x, acc);
     SYNC_A();
     LAYER(L_G1, true);
     if (a.mode == 0) {                         // sdf only: A is free for the next tile's geo input
-      if (t == 0) mbar_arrive(&bars.a_free);
+      if (t == 0) bars.a.arrive_empty(tile_no);
       epi_e1<P>(x, tile, acc);
       continue;
     }
     {
-      const long long w0 = TC_CLOCK();
-      mbar_wait(&bars.hs_empty[sl], ((tile_no >> 1) & 1) ^ 1);   // the heads warp is done with the tile two before
-      if (tid == 0) TC_PUT(tile_no, 16, TC_CLOCK() - w0);
+      long long hs_waited = 0;
+      bars.hs.wait_empty(tile_no, &hs_waited); // the heads warp is done with the tile two before
+      if (tid == 0) TC_PUT(tile_no, 16, hs_waited);
     }
     epi_e1<P>(x, tile, acc);
     SYNC_A();
@@ -802,9 +777,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     epi_eb1<P>(x, acc);
     SYNC_A();
     LAYER(L_B0, true);
-    mbar_wait(&bars.enc_full[sl], (tile_no >> 1) & 1);   // (long complete: makes the encoder's jacobian / colour-static stores visible)
+    bars.enc.wait_full(tile_no);               // (long complete: makes the encoder's jacobian / colour-static stores visible)
     epi_eb0<P>(x, tile, s, acc);
-    mbar_arrive(&bars.enc_empty[sl]);
+    bars.enc.arrive_empty(tile_no);
     SYNC_A();
     LAYER(L_C0MISC, true);
     reload_h2<P>(x);
@@ -813,9 +788,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     epi_ec0<P>(x, acc);
     SYNC_A();
     LAYER(L_C1, true);
-    if (t == 0) mbar_arrive(&bars.a_free);     // the last layer has read A: the next tile's geo input may land
+    if (t == 0) bars.a.arrive_empty(tile_no);  // the last layer has read A: the next tile's geo input may land
     epi_ec1(x, acc);
-    mbar_arrive(&bars.hs_full[sl]);            // the heads warp takes the tile from here
+    bars.hs.arrive_full(tile_no);              // the heads warp takes the tile from here
     TC_STAMP(15);
     if (tid == 0) TC_PUT(tile_no, 9, waited);
   }

@@ -37,9 +37,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+// adds the cycles it spent waiting to *waited in the timing build of the fused kernel (tools/tc_timing.py)
+#ifdef SDFB200_TC_TIMING
+#define TC_CLOCK() clock64()
+#else
+#define TC_CLOCK() 0ll
+#endif
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, long long* waited = nullptr) {
+  const long long w0 = TC_CLOCK();
   while (!mbar_try_wait(bar, parity)) {
   }
+  if (waited) *waited += TC_CLOCK() - w0;
 }
 
 // ---- 1-D bulk async copy global -> shared (completes on an mbarrier with complete_tx) -----------------------------
@@ -211,38 +219,47 @@ __device__ __forceinline__ uint64_t a_desc(uint32_t base, int kstep) { return ma
 // columns cq = frag_cq(t) and cq + 1.  Element i of n64 block c (the layout next to wgmma64_ss) sits at (frag_row(r0, i), frag_col(cq, c, i)).
 __device__ __forceinline__ int frag_row0(int row0, int t) { return row0 + (t >> 5) * 16 + ((t & 31) >> 2); }
 __device__ __forceinline__ int frag_cq(int t) { return (t & 3) * 2; }
+__device__ __forceinline__ int frag_half(int i) { return (i >> 1) & 1; }   // element i is in row r0 (0) or r0 + 8 (1)
 template <typename T>   // int, or long long for a global row index
-__device__ __forceinline__ T frag_row(T r0, int i) { return r0 + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ T frag_row(T r0, int i) { return r0 + 8 * frag_half(i); }
 __device__ __forceinline__ int frag_col(int cq, int c, int i) { return c * 64 + (i >> 2) * 8 + cq + (i & 1); }
 
+// sum over the four threads of a quad (the threads that share accumulator rows), in a fixed order: + lane ^ 1, then + lane ^ 2
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  return v;
+}
+
+// ---- hand-off between roles -------------------------------------------------------------------------------------
+// S slots with a full / empty mbarrier pair each (arrival counts set by the kernel); use n of the stream takes slot n % S.  The producing
+// role waits for empty, fills the slot and arrives on full (or hands full to bulk copies); the consuming role waits for full and arrives
+// on empty.  Both wait for phase (n / S) & 1, the producer with the other parity, so its first wait passes (a fresh barrier counts as
+// having completed the phase before its first).
+template <int S>
+struct Handoff {
+  uint64_t full[S], empty[S];
+  __device__ __forceinline__ void init(uint32_t full_count, uint32_t empty_count) {
+    for (int s = 0; s < S; ++s) { mbar_init(&full[s], full_count); mbar_init(&empty[s], empty_count); }
+  }
+  __device__ __forceinline__ static uint32_t slot(uint32_t n) { return n % S; }
+  __device__ __forceinline__ static uint32_t phase(uint32_t n) { return (n / S) & 1; }
+  __device__ __forceinline__ uint64_t* full_bar(uint32_t n) { return &full[slot(n)]; }
+  __device__ __forceinline__ void wait_empty(uint32_t n, long long* waited = nullptr) { mbar_wait(&empty[slot(n)], phase(n) ^ 1, waited); }
+  __device__ __forceinline__ void wait_full(uint32_t n, long long* waited = nullptr) { mbar_wait(&full[slot(n)], phase(n), waited); }
+  __device__ __forceinline__ void arrive_full(uint32_t n) { mbar_arrive(&full[slot(n)]); }
+  __device__ __forceinline__ void arrive_empty(uint32_t n) { mbar_arrive(&empty[slot(n)]); }
+};
+
 // ---- weight ring ------------------------------------------------------------------------------------------------
-// S stages of `bytes` each; block j of the stream goes to slot j % S.  full[s] (count 1) completes when a block has landed in slot s,
-// empty[s] (count = the consumers' arrivals, set by the kernel) when the consumers have released it.  Both functions add the cycles
-// they spent waiting to *waited in the timing build of the fused kernel (tools/tc_timing.py).
-#ifdef SDFB200_TC_TIMING
-#define TC_CLOCK() clock64()
-#else
-#define TC_CLOCK() 0ll
-#endif
+// S stages of `bytes` each at `ring`, handed off by h (full count 1); consumers take block j with wait_full(j), release it with arrive_empty(j).
 // producer (one thread): once the slot of stream block j has been released, copy block kb of the packed image `blocks` into it
 template <int S>
-__device__ __forceinline__ void ring_fill(uint8_t* ring, uint64_t* full, uint64_t* empty, uint32_t j, const uint8_t* blocks, int kb, uint32_t bytes,
+__device__ __forceinline__ void ring_fill(Handoff<S>& h, uint8_t* ring, uint32_t j, const uint8_t* blocks, int kb, uint32_t bytes,
                                           long long* waited = nullptr) {
-  const int s = j % S;
-  const long long w0 = TC_CLOCK();
-  mbar_wait(&empty[s], ((j / S) & 1) ^ 1);
-  if (waited) *waited += TC_CLOCK() - w0;
-  mbar_arrive_expect_tx(&full[s], bytes);
-  bulk_g2s(ring + (size_t)s * bytes, blocks + (size_t)kb * bytes, bytes, &full[s]);
-}
-// consumer: wait until block j is in its slot; returns the slot, which the caller releases (arrives on empty[slot]) when done with it
-template <int S>
-__device__ __forceinline__ int ring_wait(uint64_t* full, uint32_t j, long long* waited = nullptr) {
-  const int s = j % S;
-  const long long w0 = TC_CLOCK();
-  mbar_wait(&full[s], (j / S) & 1);
-  if (waited) *waited += TC_CLOCK() - w0;
-  return s;
+  h.wait_empty(j, waited);
+  mbar_arrive_expect_tx(h.full_bar(j), bytes);
+  bulk_g2s(ring + (size_t)h.slot(j) * bytes, blocks + (size_t)kb * bytes, bytes, h.full_bar(j));
 }
 
 // ---- fast softplus_100 ------------------------------------------------------------------------------------------

@@ -51,7 +51,7 @@ struct LinArgs {
 template <int P, int EPI>
 __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t full[kStagesL], empty[kStagesL];
+  __shared__ Handoff<kStagesL> bars;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nblocks = a.Kc32 / kKBL;
   const uint32_t stage_bytes = (uint32_t)P * a.Np64 * kKBL * 2;
@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
   uint8_t* ring = smem + P * kAPlaneL;
   const long long m0 = (long long)blockIdx.x * 128;
   if (tid == 0) {
-    for (int s = 0; s < kStagesL; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    bars.init(1, 2);
     fence_barrier_init();
   }
   if (tid < 256) {
@@ -91,7 +91,7 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
     // ---------------- weight producer ----------------
     if (lane == 0) {
       for (int b = 0; b < nblocks; ++b)
-        ring_fill<kStagesL>(ring, full, empty, b, reinterpret_cast<const uint8_t*>(a.Wp), b, stage_bytes);
+        ring_fill(bars, ring, b, reinterpret_cast<const uint8_t*>(a.Wp), b, stage_bytes);
     }
     return;
   }
@@ -107,8 +107,8 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
   const uint32_t lbo_b = (uint32_t)a.Np64 * 16, plane_b = (uint32_t)a.Np64 * kKBL * 2;
   const uint32_t abase = smem_u32(a_smem) + wg * 64 * 16;
   for (int b = 0; b < nblocks; ++b) {
-    const int s = ring_wait<kStagesL>(full, b);
-    const uint32_t wbase = smem_u32(ring + (size_t)s * stage_bytes);
+    bars.wait_full(b);
+    const uint32_t wbase = smem_u32(ring + (size_t)bars.slot(b) * stage_bytes);
     wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
     wg_arrive();
 #pragma unroll
@@ -119,7 +119,7 @@ __global__ void __launch_bounds__(kThreadsL, 1) k_tc_linear(const LinArgs a) {
     wg_commit();
     wg_wait<0>();
     wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
-    if (t == 0) mbar_arrive(&empty[s]);
+    if (t == 0) bars.arrive_empty(b);
   }
 #pragma unroll
   for (int c = 0; c < 4; ++c) {

@@ -15,14 +15,14 @@ template <int P, bool RS>
 __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict__ A, const __nv_bfloat16* __restrict__ Wp, int K, int Np, int Np64,
                                                          float* __restrict__ D) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint64_t full[2], empty[2];
+  __shared__ Handoff<2> bars;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nblocks = K / kKB;
   const uint32_t stage_bytes = (uint32_t)P * Np64 * kKB * 2;
   uint8_t* a_smem = smem;                                        // [P][K/8][128][16 B]   (SS mode only)
   uint8_t* w_smem = smem + (RS ? 0 : (size_t)P * K * 256);       // 2 stages
   if (tid == 0) {
-    mbar_init(&full[0], 1); mbar_init(&full[1], 1); mbar_init(&empty[0], 2); mbar_init(&empty[1], 2);
+    bars.init(1, 2);
     fence_barrier_init();
   }
   if (!RS && tid < 256) {
@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
   if (warp == 8) {
     // ---- weight producer ----
     if (lane == 0) {
-      for (int b = 0; b < nblocks; ++b) ring_fill<2>(w_smem, full, empty, b, reinterpret_cast<const uint8_t*>(Wp), b, stage_bytes);
+      for (int b = 0; b < nblocks; ++b) ring_fill(bars, w_smem, b, reinterpret_cast<const uint8_t*>(Wp), b, stage_bytes);
     }
   } else {
     // ---- two warpgroups, 64 rows each ----
@@ -61,8 +61,8 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
     const uint32_t lbo_b = (uint32_t)Np64 * 16, plane_b = (uint32_t)Np64 * kKB * 2;
     const uint32_t abase = smem_u32(a_smem) + wg * 64 * 16;
     for (int b = 0; b < nblocks; ++b) {
-      const int s = ring_wait<2>(full, b);
-      const uint32_t wbase = smem_u32(w_smem + (size_t)s * stage_bytes);
+      bars.wait_full(b);
+      const uint32_t wbase = smem_u32(w_smem + (size_t)bars.slot(b) * stage_bytes);
       uint32_t afr[kKB / 16][2][4];
       if (RS) {
         // A fragments straight from global memory: rows r0 / r0 + 8, columns 2c, 2c + 1 (+8) of each K step
@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(288, 1) k_tc_gemm_test(const float* __restrict
       wg_commit();
       wg_wait<0>();
       wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
-      if (t == 0) mbar_arrive(&empty[s]);
+      if (t == 0) bars.arrive_empty(b);
     }
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
