@@ -2,11 +2,10 @@
 // Replaces HashMLPDensityField.get_density / density_fn (nerfstudio/fields/density_fields.py:40-121, fields/base_field.py:48-65),
 // i.e. tcnn.NetworkWithInputEncoding + trunc_exp (field_components/activations.py:24-42).  One thread per point: the L2-gather-bound
 // grid lookup dominates (8 L corners), the <= 64-wide MLP runs in registers with the weights broadcast from shared memory.
+#include "field.h"
 #include "grid.cuh"
 
 namespace sdfb200 {
-
-int validate_grid(const sdfb200_grid_t* g);
 
 struct DensityArgs {
   sdfb200_grid_t grid;

@@ -14,6 +14,12 @@ constexpr int64_t kChunkPoints = 132 * 4 * 128;  // points per pass of the gener
 
 inline int pad16(int v) { return (v + kPad - 1) / kPad * kPad; }
 
+// bf16 split planes of the tensor-core engines: bf16x3 = 2 (w = w0 + w1), bf16 = 1
+inline int tc_planes(int32_t precision) { return precision == SDFB200_PRECISION_BF16 ? 1 : 2; }
+
+// layers of the fused kernel in the order it runs them (and the producer streams them); one packed tensor-core weight tile each
+enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
+
 struct LayerPlan {
   int K, N, Kp, Np;     // logical / padded dims
   size_t w_off;         // [Np, Kp] fp32   (folded weight; skip layer pre-scaled by 1/sqrt(2))
@@ -30,11 +36,18 @@ struct FieldPlan {
   int geo_feat;                          // geo_dims[n] - 1
   size_t head_off;                       // diffuse W[3,gf] b[3] tint W[3,gf] b[3] (fp32), (size_t)-1 if neither
   size_t fp32_bytes;                     // size of the fp32 section
-  size_t tc_off, tc_bytes;               // tensor-core (bf16 split-plane) section, 0 bytes for PRECISION_FP32
+  // tensor-core section: only when the fused kernel (k_field_tc) can run this descriptor, else fused = false and 0 bytes
+  bool fused;
+  size_t tc_off, tc_bytes;
+  size_t tc_w_off[L_COUNT];              // packed bf16 split planes of each L_* layer
+  size_t tc_wc_off, tc_bc_off;           // fp32 colour layer 0 pre-multiplied with the last geo layer: Wc [256][256], bc [256]
   size_t total_bytes;
 };
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// the fused kernel's part of the plan (field_tc.cu): sets fused, and the tensor-core section when it is set
+void plan_tc_section(const sdfb200_field_t& f, FieldPlan& p);
 
 // returns 0 on success, negative on an unsupported descriptor
 inline int make_field_plan(const sdfb200_field_t& f, FieldPlan& p) {
@@ -90,8 +103,8 @@ inline int make_field_plan(const sdfb200_field_t& f, FieldPlan& p) {
   if (f.use_diffuse_color || f.use_specular_tint) p.head_off = take((size_t)(2 * (3 * p.geo_feat + 4)) * 4);
   p.fp32_bytes = off;
   p.tc_off = off;
-  p.tc_bytes = 0;
-  p.total_bytes = off;
+  plan_tc_section(f, p);
+  p.total_bytes = p.tc_off + p.tc_bytes;
   return 0;
 }
 

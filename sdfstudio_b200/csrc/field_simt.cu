@@ -1,5 +1,6 @@
-// Generic fp32 (CUDA-core) evaluation of the SDF field: any layer count / skip connection / head combination of
-// SDFFieldConfig.  This is the exact-fp32 path (SDFB200_PRECISION_FP32) and the reference for the tensor-core path.
+// Generic evaluation of the SDF field: any layer count / skip connection / head combination of SDFFieldConfig.  With the exact-fp32
+// GEMM engine (k_sgemm) this is the SDFB200_PRECISION_FP32 path and the reference for the tensor-core paths; with the tensor-core
+// Linear (tc_linear.cu) as its GEMM engine it runs the shapes outside the fused kernel's family at bf16x3 / bf16.
 //
 // Stages (each a kernel; activations live in the caller's workspace, chunked so they stay L2-resident):
 //   k_field_inputs   positions (o + d*t), SceneContraction, NeRF PE           sdf_field.py:623-631, encodings.py:167-208
@@ -7,15 +8,11 @@
 //   k_sgemm<EPI>     weight-normed Linear + Softplus(beta=100) / ReLU         sdf_field.py:400-410, 586-592
 //   reverse sweep    d sdf / d x by explicit back-substitution (what torch.autograd.grad computes at :647-654)
 //   k_color_inputs / k_field_post   get_colors :532-612, LaplaceDensity :57-66, get_alpha :476-525
-#include "field_plan.h"
+#include "field.h"
 #include "grid.cuh"
 #include "tc_linear.h"
 
 namespace sdfb200 {
-
-int grid_encode(const sdfb200_grid_t& g, const void* table, const float* x01, int64_t n, float* out, int64_t out_ld,
-                float* dout_dx, cudaStream_t st);
-int validate_grid(const sdfb200_grid_t* g);
 
 __constant__ float c_offaxis[3][21] = {
     {0.8506508f, 0.809017f, 0.5257311f, 1.f, 0.809017f, 0.8506508f, 0.309017f, 0.f, 0.5f, 0.f, -0.5257311f, -0.309017f, 0.f, -0.309017f, 0.309017f, 0.5f, 0.5f, 0.f, -0.5f, -0.809017f, -0.809017f},
@@ -223,14 +220,13 @@ __global__ void __launch_bounds__(256) k_sgemm(const float* __restrict__ X, int 
   }
 }
 
-// GEMM engine of the current field call: 0 planes = the exact-fp32 CUDA-core kernel below; 1 / 2 = the generic tensor-core Linear
-// (bf16 / bf16x3, csrc/tc_linear.cu) with `scratch` for its packed weight chunk.  Set by field_forward_fp32 for the duration of a call.
+// GEMM engine of a field call: 0 planes = the exact-fp32 CUDA-core kernel above; 1 / 2 = the generic tensor-core Linear
+// (bf16 / bf16x3, csrc/tc_linear.cu) with `scratch` for its packed weight chunk
 struct GemmEngine { int planes; void* scratch; };
-static thread_local GemmEngine g_gemm = {0, nullptr};
 
-static int sgemm(int epi, const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy, int64_t M, int Np, int Kp,
-                 const float* aux, int ldaux, int aux_cols, cudaStream_t st) {
-  if (g_gemm.planes > 0) return tc_gemm(g_gemm.planes, epi, X, ldx, W, bias, Y, ldy, M, Np, Kp, aux, ldaux, aux_cols, g_gemm.scratch, st);
+static int sgemm(const GemmEngine& g, int epi, const float* X, int ldx, const float* W, const float* bias, float* Y, int ldy, int64_t M, int Np,
+                 int Kp, const float* aux, int ldaux, int aux_cols, cudaStream_t st) {
+  if (g.planes > 0) return tc_gemm(g.planes, epi, X, ldx, W, bias, Y, ldy, M, Np, Kp, aux, ldaux, aux_cols, g.scratch, st);
   dim3 grid((unsigned)ceil_div(M, 128), (unsigned)ceil_div(Np, 128));
   switch (epi) {
     case EPI_NONE: k_sgemm<EPI_NONE><<<grid, 256, 0, st>>>(X, ldx, W, bias, Y, ldy, M, Np, Kp, aux, ldaux, aux_cols); break;
@@ -503,7 +499,7 @@ int field_pack_fp32(const sdfb200_field_t& f, const FieldPlan& p, const sdfb200_
 
 // geo network forward on `n` points whose inputs are already in ws.in; keeps hidden activations in ws.h[].
 static int geo_forward(const sdfb200_field_t& f, const FieldPlan& p, const FieldWorkspace& w, float* ws, const char* blob, int64_t n,
-                       cudaStream_t st) {
+                       const GemmEngine& gemm, cudaStream_t st) {
   const float* X = ws + w.in;
   int ldx = p.in_pad;
   for (int l = 0; l < p.n_geo; ++l) {
@@ -511,7 +507,7 @@ static int geo_forward(const sdfb200_field_t& f, const FieldPlan& p, const Field
     const bool last = l == p.n_geo - 1;
     float* Y = last ? ws + w.outg : ws + w.h[l];
     const int ldy = last ? L.Np : ((l + 1 == f.geo_skip_layer) ? p.geo[l + 1].Kp : L.Np);
-    int r = sgemm(last ? EPI_NONE : EPI_SOFTPLUS, X, ldx, (const float*)(blob + L.w_off), (const float*)(blob + L.b_off), Y, ldy, n, L.Np, L.Kp,
+    int r = sgemm(gemm, last ? EPI_NONE : EPI_SOFTPLUS, X, ldx, (const float*)(blob + L.w_off), (const float*)(blob + L.b_off), Y, ldy, n, L.Np, L.Kp,
                   nullptr, 0, 0, st);
     if (r) return r;
     if (l + 1 == f.geo_skip_layer) {
@@ -527,7 +523,7 @@ static int geo_forward(const sdfb200_field_t& f, const FieldPlan& p, const Field
 
 // reverse sweep: d sdf / d inputs -> ws.gin
 static int geo_backward_inputs(const sdfb200_field_t& f, const FieldPlan& p, const FieldWorkspace& w, float* ws, const char* blob, int64_t n,
-                               cudaStream_t st) {
+                               const GemmEngine& gemm, cudaStream_t st) {
   const int nl = p.n_geo;
   float* G = ws + w.g0;
   float* G2 = ws + w.g1;
@@ -561,7 +557,7 @@ static int geo_backward_inputs(const sdfb200_field_t& f, const FieldPlan& p, con
     const bool skip = l == f.geo_skip_layer;
     const int hcols = p.geo[l - 1].N;
     const int ldh = skip ? L.Kp : p.geo[l - 1].Np;
-    int r = sgemm(EPI_MUL_DSOFTPLUS, G, ldg, (const float*)(blob + L.wt_off), nullptr, G2, L.Kp, n, L.Kp, L.Np, ws + w.h[l - 1], ldh, hcols, st);
+    int r = sgemm(gemm, EPI_MUL_DSOFTPLUS, G, ldg, (const float*)(blob + L.wt_off), nullptr, G2, L.Kp, n, L.Kp, L.Np, ws + w.h[l - 1], ldh, hcols, st);
     if (r) return r;
     if (skip) {
       k_copy_cols<<<(unsigned)n, 64, 0, st>>>(G2, L.Kp, hcols, skipgrad, p.in_pad, 0, p.in_dim, n, 1);
@@ -573,7 +569,7 @@ static int geo_backward_inputs(const sdfb200_field_t& f, const FieldPlan& p, con
   }
   {
     const LayerPlan& L = p.geo[0];
-    int r = sgemm(EPI_MUL_DSOFTPLUS, G, ldg, (const float*)(blob + L.wt_off), nullptr, ws + w.gin, p.in_pad, n, L.Kp, L.Np, nullptr, 0, 0, st);
+    int r = sgemm(gemm, EPI_MUL_DSOFTPLUS, G, ldg, (const float*)(blob + L.wt_off), nullptr, ws + w.gin, p.in_pad, n, L.Kp, L.Np, nullptr, 0, 0, st);
     if (r) return r;
   }
   if (have_skip) {
@@ -583,26 +579,23 @@ static int geo_backward_inputs(const sdfb200_field_t& f, const FieldPlan& p, con
   return 0;
 }
 
-int field_forward_fp32(const sdfb200_field_t& f, const FieldPlan& p, const char* blob, const void* table, const sdfb200_field_in_t& in,
-                       const sdfb200_field_out_t& out, float* ws, size_t ws_floats, cudaStream_t st, int gemm_planes) {
+size_t field_generic_workspace_floats(const sdfb200_field_t& f, const FieldPlan& p, int64_t n_points) {
+  FieldWorkspace w;
+  make_workspace_plan(f, p, n_points < kChunkPoints ? n_points : kChunkPoints, w);
+  return w.floats_per_chunk;
+}
+
+int field_forward_generic(const sdfb200_field_t& f, const FieldPlan& p, const char* blob, const void* table, const sdfb200_field_in_t& in,
+                          const sdfb200_field_out_t& out, float* ws, int gemm_planes, cudaStream_t st) {
   const int64_t N = in.n_rays * (int64_t)in.n_samples;
-  if (N == 0) return 0;
-  struct EngineScope {   // restores the exact-fp32 engine on every exit path
-    ~EngineScope() { g_gemm = {0, nullptr}; }
-  } engine_scope;
   const int64_t chunk = N < kChunkPoints ? N : kChunkPoints;
   FieldWorkspace w;
   make_workspace_plan(f, p, chunk, w);
-  if (ws_floats < w.floats_per_chunk) return fail(SDFB200_EWORKSPACE, "workspace too small%s (need %lld floats)", "", (long long)w.floats_per_chunk);
-  g_gemm = {gemm_planes, ws + w.tcw};
+  const GemmEngine gemm = {gemm_planes, ws + w.tcw};
 
   const bool want_color = out.rgb != nullptr;
   const bool want_grad = want_color || out.gradients || out.normals || out.alpha;
   const bool numerical = f.use_numerical_gradients != 0;
-  if (want_color || out.alpha) SDFB_REQUIRE(in.directions != nullptr, "directions required for rgb / alpha");
-  if (out.alpha) SDFB_REQUIRE(in.bins != nullptr && in.variance != nullptr, "alpha needs bins and the variance parameter");
-  if (out.density) SDFB_REQUIRE(in.beta != nullptr && in.beta_min != nullptr, "density needs beta and beta_min");
-  if (out.sampled_sdf) SDFB_REQUIRE(numerical, "sampled_sdf is only produced with use_numerical_gradients");
   const int use_grid = f.use_grid_feature;
 
   for (int64_t p0 = 0; p0 < N; p0 += chunk) {
@@ -630,7 +623,7 @@ int field_forward_fp32(const sdfb200_field_t& f, const FieldPlan& p, const char*
           int r = grid_encode(f.grid, table, ws + w.x01, n, ws + w.in + 3 + p.pe_dim, p.in_pad, nullptr, st);
           if (r) return r;
         }
-        int r = geo_forward(f, p, w, ws, blob, n, st);
+        int r = geo_forward(f, p, w, ws, blob, n, gemm, st);
         if (r) return r;
         k_store_col<<<pb, 256, 0, st>>>(ws + w.outg, p.geo[p.n_geo - 1].Np, n, ws + w.nsdf, 6, k);
         SDFB_LAUNCHED("k_store_col");
@@ -646,10 +639,10 @@ int field_forward_fp32(const sdfb200_field_t& f, const FieldPlan& p, const char*
       int r = grid_encode(f.grid, table, ws + w.x01, n, ws + w.in + 3 + p.pe_dim, p.in_pad, analytic ? ws + w.jac : nullptr, st);
       if (r) return r;
     }
-    int r = geo_forward(f, p, w, ws, blob, n, st);
+    int r = geo_forward(f, p, w, ws, blob, n, gemm, st);
     if (r) return r;
     if (analytic) {
-      r = geo_backward_inputs(f, p, w, ws, blob, n, st);
+      r = geo_backward_inputs(f, p, w, ws, blob, n, gemm, st);
       if (r) return r;
       GradArgs ga;
       ga.gin = ws + w.gin; ga.in = ws + w.in; ga.jac = ws + w.jac; ga.in_pad = p.in_pad; ga.pe_degree = f.pe_degree; ga.use_pe = f.use_position_encoding;
@@ -674,7 +667,7 @@ int field_forward_fp32(const sdfb200_field_t& f, const FieldPlan& p, const char*
         const LayerPlan& L = p.col[l];
         const bool last = l == p.n_col - 1;
         float* Y = bufs[l & 1];
-        r = sgemm(last ? EPI_NONE : EPI_RELU, X, ldx, (const float*)(blob + L.w_off), (const float*)(blob + L.b_off), Y, L.Np, n, L.Np, L.Kp, nullptr, 0, 0, st);
+        r = sgemm(gemm, last ? EPI_NONE : EPI_RELU, X, ldx, (const float*)(blob + L.w_off), (const float*)(blob + L.b_off), Y, L.Np, n, L.Np, L.Kp, nullptr, 0, 0, st);
         if (r) return r;
         X = Y; ldx = L.Np;
       }

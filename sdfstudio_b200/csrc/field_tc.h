@@ -1,5 +1,5 @@
-// Shared declarations of the fused tensor-core field kernel: constants, launch arguments, launchers (one translation unit per
-// (planes, table layout) instantiation: csrc/field_tc_p*_*.cu) and the host side (csrc/field_tc.cu).
+// Shared declarations of the fused tensor-core field kernel: constants, launch arguments and launchers (one translation unit per
+// (planes, table layout) instantiation: csrc/field_tc_p*_*.cu).  The host side (csrc/field_tc.cu) is declared in field.h.
 #pragma once
 #include "field_plan.h"
 
@@ -65,10 +65,7 @@ __host__ __device__ constexpr TcScratch tc_scratch(int planes) {
 }
 __host__ __device__ constexpr size_t kScratchPerCta(int planes) { return tc_scratch(planes).bytes; }
 
-// layers in the order the kernel runs them (and the producer streams them)
-enum { L_G0 = 0, L_G1, L_B1, L_B0, L_C0MISC, L_C0H, L_C1, L_COUNT };
-
-// Weight tile of layer L: N rows (the MMA's N; B0's 96 input rows padded to 128), K (the geo input and the colour misc operand are
+// Weight tile of layer L (L_* in field_plan.h): N rows (the MMA's N; B0's 96 input rows padded to 128), K (the geo input and the colour misc operand are
 // kInK wide) and the K per streamed block.  Every block is exactly one ring stage (256 x kKB elements per plane): the pack plan, the
 // producer and the MMAs all take the shapes from here.
 __host__ __device__ constexpr int tc_layer_np(int L) { return L == L_B0 ? 128 : 256; }

@@ -1,6 +1,7 @@
 // Stand-alone grid encode / backward kernels behind sdfb200_grid_encode{,_backward} (the tcnn.Encoding operator
 // boundary, nerfstudio/fields/sdf_field.py:230-241,386).  HBM/L2-gather bound: one thread per (point, level) so that
 // a warp covers 2 points x 16 levels and its F-wide outputs are written to consecutive addresses.
+#include "field.h"
 #include "grid.cuh"
 
 namespace sdfb200 {

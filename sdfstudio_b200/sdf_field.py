@@ -338,14 +338,26 @@ class SDFField(nn.Module):
         self._packed_key = key
         return self._packed
 
-    def _get_workspace(self, desc, n_points: int):
-        lib = _lib.load()
-        nbytes = lib.sdfb200_field_workspace_bytes(desc, n_points)
+    def _workspace_of(self, nbytes: int, query: str, dev):
+        """The shared workspace on `dev`, grown to at least `nbytes` (the result of the size query `query`; 0 = refused)."""
         if nbytes == 0:
-            _lib.check(-1, "sdfb200_field_workspace_bytes")
-        if self._workspace is None or self._workspace.numel() < nbytes or self._workspace.device != self.aabb.device:
-            self._workspace = torch.empty(nbytes, dtype=torch.uint8, device=self.aabb.device)
+            _lib.check(-1, query)
+        if self._workspace is None or self._workspace.numel() < nbytes or self._workspace.device != dev:
+            self._workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         return self._workspace
+
+    def _field_in(self, origins, directions, bins, n_samples: int, apply_contraction: bool, appearance):
+        """sdfb200_field_in_t of one call: pointers only, so the caller keeps the tensors alive until the call is made."""
+        fin = _lib.FieldIn()
+        fin.n_rays, fin.n_samples, fin.apply_contraction = origins.shape[0], n_samples, int(apply_contraction)
+        fin.origins, fin.directions, fin.bins = _lib.ptr(origins), _lib.ptr(directions), _lib.ptr(bins)
+        fin.appearance = _lib.ptr(appearance)
+        fin.variance = _lib.ptr(self.deviation_network.variance.detach())
+        fin.beta = _lib.ptr(self.laplace_density.beta.detach())
+        fin.beta_min = _lib.ptr(self.laplace_density.beta_min.detach())
+        fin.cos_anneal_ratio = float(self._cos_anneal_ratio)
+        fin.numerical_delta = float(self.numerical_gradients_delta)
+        return fin
 
     # ------------------------------------------------------------------ the kernel call
     def _run(self, origins, directions, bins, n_samples: int, wants, apply_contraction: bool, appearance=None) -> Dict[str, torch.Tensor]:
@@ -359,20 +371,12 @@ class SDFField(nn.Module):
         N = R * n_samples
         desc = self._field_desc()
         packed = self._packed_weights(desc)
-        ws = self._get_workspace(desc, N)
+        ws = self._workspace_of(lib.sdfb200_field_workspace_bytes(desc, N), "sdfb200_field_workspace_bytes", dev)
         gf = self.config.geo_feat_dim
         shapes = {"sdf": (N,), "geo_feature": (N, gf), "gradients": (N, 3), "normals": (N, 3), "rgb": (N, 3), "density": (N,), "alpha": (N,),
                   "occupancy": (N,), "points_norm": (N,), "sampled_sdf": (N, 6), "points": (N, 3)}
         outs = {k: torch.empty(shapes[k], device=dev, dtype=torch.float32) for k in wants}
-        fin = _lib.FieldIn()
-        fin.n_rays, fin.n_samples, fin.apply_contraction = R, n_samples, int(apply_contraction)
-        fin.origins, fin.directions, fin.bins = _lib.ptr(origins), _lib.ptr(directions), _lib.ptr(bins)
-        fin.appearance = _lib.ptr(appearance)
-        fin.variance = _lib.ptr(self.deviation_network.variance.detach())
-        fin.beta = _lib.ptr(self.laplace_density.beta.detach())
-        fin.beta_min = _lib.ptr(self.laplace_density.beta_min.detach())
-        fin.cos_anneal_ratio = float(self._cos_anneal_ratio)
-        fin.numerical_delta = float(self.numerical_gradients_delta)
+        fin = self._field_in(origins, directions, bins, n_samples, apply_contraction, appearance)
         fout = _lib.FieldOut()
         for k, t in outs.items():
             setattr(fout, k, t.data_ptr())
@@ -404,12 +408,7 @@ class SDFField(nn.Module):
             raise RuntimeError("sdfstudio_b200.SDFField runs on CUDA only (there is no CPU path)")
         desc = self._field_desc()
         packed = self._packed_weights(desc)
-        nbytes = lib.sdfb200_field_render_workspace_bytes(desc, R, S)
-        if nbytes == 0:
-            _lib.check(-1, "sdfb200_field_render_workspace_bytes")
-        if self._workspace is None or self._workspace.numel() < nbytes or self._workspace.device != dev:
-            self._workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        ws = self._workspace
+        ws = self._workspace_of(lib.sdfb200_field_render_workspace_bytes(desc, R, S), "sdfb200_field_render_workspace_bytes", dev)
         # one flat output allocation: per-ray block [R, 9] = rgb(3) depth normal(3) accumulation bg_transmittance | minmax(2) | per-sample blocks
         widths = [self._SAMPLE_SHAPES[k] for k in sample_outputs]
         flat = torch.empty(R * 9 + 2 + N * (sum(widths) + (1 if want_weights else 0)), device=dev, dtype=torch.float32)
@@ -450,16 +449,8 @@ class SDFField(nn.Module):
         rnd.bg_transmittance = bgT.data_ptr()
         rnd.out.rgb, rnd.out.normal, rnd.out.depth, rnd.out.accumulation, rnd.out.steps_minmax = (rgb.data_ptr(), nrm.data_ptr(), depth.data_ptr(),
                                                                                                    acc.data_ptr(), mm.data_ptr())
-        fin = _lib.FieldIn()
-        fin.n_rays, fin.n_samples, fin.apply_contraction = R, S, 1
-        fin.origins, fin.directions, fin.bins = _lib.ptr(origins), _lib.ptr(directions), _lib.ptr(bins)
         app = self._appearance(ray_samples.camera_indices, R, dev)
-        fin.appearance = _lib.ptr(app)
-        fin.variance = _lib.ptr(self.deviation_network.variance.detach())
-        fin.beta = _lib.ptr(self.laplace_density.beta.detach())
-        fin.beta_min = _lib.ptr(self.laplace_density.beta_min.detach())
-        fin.cos_anneal_ratio = float(self._cos_anneal_ratio)
-        fin.numerical_delta = float(self.numerical_gradients_delta)
+        fin = self._field_in(origins, directions, bins, S, True, app)
         table = self.encoding.compute_table() if self.use_grid_feature else None
         _lib.check(lib.sdfb200_field_render(desc, _lib.ptr(packed), _lib.ptr(table), fin, fout, rnd, _lib.ptr(ws), ws.numel(), _lib.stream_ptr()),
                    "sdfb200_field_render")

@@ -54,6 +54,16 @@ def test_invalid_arguments_return_error_codes_not_crashes():
     assert lib.sdfb200_field_packed_bytes(d) == 0
 
 
+FIELD_PRESETS = {
+    "neus-facto": dict(use_grid_feature=True, num_layers=2, num_layers_color=2, log2_hashmap_size=12),
+    "volsdf": dict(num_layers=8, num_layers_color=4),
+    "angelo": dict(use_grid_feature=True, num_layers=1, num_layers_color=4, use_numerical_gradients=True, hash_features_per_level=8,
+                   hash_smoothstep=False, use_position_encoding=False, log2_hashmap_size=12, base_res=64, max_res=4096),
+    "bakedsdf": dict(use_grid_feature=True, num_layers=2, num_layers_color=2, position_encoding_max_degree=8, use_diffuse_color=True,
+                     use_specular_tint=True, use_reflections=True, use_n_dot_v=True, off_axis=True, log2_hashmap_size=12),
+}
+
+
 def test_field_descriptor_roundtrip_all_presets():
     """packed / workspace size queries succeed for the five BASELINE config shapes (host logic only)."""
     import torch
@@ -63,14 +73,7 @@ def test_field_descriptor_roundtrip_all_presets():
 
     lib = _lib.load()
     aabb = torch.tensor([[-1.0, -1, -1], [1, 1, 1]])
-    presets = {
-        "neus-facto": dict(use_grid_feature=True, num_layers=2, num_layers_color=2, log2_hashmap_size=12),
-        "volsdf": dict(num_layers=8, num_layers_color=4),
-        "angelo": dict(use_grid_feature=True, num_layers=1, num_layers_color=4, use_numerical_gradients=True, hash_features_per_level=8,
-                       hash_smoothstep=False, use_position_encoding=False, log2_hashmap_size=12, base_res=64, max_res=4096),
-        "bakedsdf": dict(use_grid_feature=True, num_layers=2, num_layers_color=2, position_encoding_max_degree=8, use_diffuse_color=True,
-                         use_specular_tint=True, use_reflections=True, use_n_dot_v=True, off_axis=True, log2_hashmap_size=12),
-    }
+    presets = FIELD_PRESETS
     for name, kw in presets.items():
         f = sb.SDFField(sb.SDFFieldConfig(**kw), aabb, 4)
         d = f._field_desc()
@@ -81,6 +84,82 @@ def test_field_descriptor_roundtrip_all_presets():
     for n in ("glin0.weight_g", "glin0.weight_v", "glin2.bias", "clin0.weight_v", "laplace_density.beta", "deviation_network.variance",
               "embedding_appearance.embedding.weight", "encoding.params"):
         assert n in names, n
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason="the calls get sentinel device pointers, which a call that is not rejected would launch on")
+@pytest.mark.parametrize("precision", ["fp32", "bf16x3"])
+@pytest.mark.parametrize("preset", ["neus-facto", "volsdf"])
+def test_field_calls_reject_invalid_inputs(preset, precision):
+    """sdfb200_field_forward / sdfb200_field_render return these codes before any device work, on the fused (neus-facto at bf16x3) and the
+    generic engines: -1 for a missing pointer or a requested output whose inputs are missing, -2 for a too-small workspace.  The workspace
+    size is checked before the per-output requirements.  The pointers are sentinels that a rejected call never dereferences."""
+    import ctypes as C
+
+    import sdfstudio_b200 as sb
+    from sdfstudio_b200 import _lib
+
+    lib = _lib.load()
+    aabb = torch.tensor([[-1.0, -1, -1], [1, 1, 1]])
+    d = sb.SDFField(sb.SDFFieldConfig(**FIELD_PRESETS[preset], precision=precision), aabb, 4)._field_desc()
+    d_fp32 = sb.SDFField(sb.SDFFieldConfig(**FIELD_PRESETS[preset]), aabb, 4)._field_desc()
+    # only the fused kernel adds a packed section: the cases cover both engines
+    assert (lib.sdfb200_field_packed_bytes(d) > lib.sdfb200_field_packed_bytes(d_fp32)) == (preset == "neus-facto" and precision == "bf16x3")
+    R, S = 4, 32
+    big = 1 << 40
+    packed, table, ws = 0x10000, (0x20000 if d.use_grid_feature else None), 0x100000
+    stage_plus_one = (R * S * 9 + 64 + 1) * 4    # a composed render's staging plus one float: too small for any field call
+
+    def field_in(**kw):
+        fin = _lib.FieldIn()
+        fin.n_rays, fin.n_samples, fin.apply_contraction = R, S, 1
+        fin.origins, fin.directions, fin.bins, fin.variance, fin.beta, fin.beta_min = 0x30000, 0x40000, 0x50000, 0x60000, 0x70000, 0x80000
+        for k, v in kw.items():
+            setattr(fin, k, v)
+        return fin
+
+    def field_out(**kw):
+        out = _lib.FieldOut()
+        for k, v in kw.items():
+            setattr(out, k, v)
+        return out
+
+    def forward(fin=None, out=None, pk=packed, tb=table, nbytes=big):
+        return lib.sdfb200_field_forward(d, pk, tb, fin, out, ws, nbytes, None)
+
+    assert forward(None, field_out(sdf=0x90000)) == -1
+    assert forward(field_in(), None) == -1
+    assert forward(field_in(), field_out(sdf=0x90000), pk=None) == -1
+    assert forward(field_in(n_rays=0, origins=None), field_out(sdf=0x90000)) == 0            # an empty batch returns before the input checks
+    assert forward(field_in(origins=None), field_out(sdf=0x90000)) == -1
+    assert forward(field_in(directions=None), field_out(sdf=0x90000)) == -1                  # ray mode needs directions
+    if d.use_grid_feature:
+        assert forward(field_in(), field_out(sdf=0x90000), tb=None) == -1
+    assert forward(field_in(), field_out(sdf=0x90000), nbytes=0) == -1
+    assert forward(field_in(), field_out(sdf=0x90000), nbytes=4) == -2
+    assert forward(field_in(variance=None), field_out(alpha=0x90000), nbytes=4) == -2        # workspace before the per-output checks
+    assert forward(field_in(variance=None), field_out(alpha=0x90000)) == -1
+    assert forward(field_in(beta=None), field_out(density=0x90000)) == -1
+    assert forward(field_in(beta_min=None), field_out(density=0x90000)) == -1
+    assert forward(field_in(), field_out(sampled_sdf=0x90000)) == -1                           # numerical gradients only
+
+    def render(fin, out=None, nbytes=big, from_density=0, **kw):
+        rnd = _lib.FieldRender()
+        rnd.from_density, rnd.bg_mode, rnd.bg = from_density, _lib.BG_COLOR, 0xA0000
+        rnd.out.rgb, rnd.out.depth, rnd.out.steps_minmax = 0xB0000, 0xC0000, 0xD0000
+        for k, v in kw.items():
+            setattr(rnd.out if k in ("rgb", "depth", "steps_minmax") else rnd, k, v)
+        return lib.sdfb200_field_render(d, packed, table, fin, out, C.byref(rnd), ws, nbytes, None)
+
+    assert lib.sdfb200_field_render(d, packed, table, field_in(), None, None, ws, big, None) == -1
+    assert render(field_in(directions=None)) == -1
+    assert render(field_in(bins=None)) == -1
+    assert render(field_in(), bg=None) == -1                                                   # rgb without a background
+    assert render(field_in(), steps_minmax=None) == -1                                         # depth without steps_minmax
+    assert render(field_in(), nbytes=stage_plus_one) == -2
+    assert render(field_in(variance=None), nbytes=stage_plus_one) == -2
+    assert render(field_in(variance=None)) == -1                                               # NeuS alphas
+    assert render(field_in(beta=None), from_density=1) == -1                                   # Laplace density
+    assert render(field_in(), field_out(sampled_sdf=0x90000)) == -1
 
 
 def test_product_does_not_import_oracle():
