@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(128) k_density_field(const __grid_constant__ D
   for (int l = 0; l < a.grid.n_levels; ++l) {
     float f[F];
     float d[F][3];
-    if (l < a.grid.active_levels) encode_level<T, F, false>(a.grid, a.table, l, x01, y01, z01, f, d);
+    if (l < a.grid.active_levels) encode_level<T, F>(a.grid, a.table, l, x01, y01, z01, f, d);
     else
       for (int k = 0; k < F; ++k) f[k] = 0.f;
 #pragma unroll

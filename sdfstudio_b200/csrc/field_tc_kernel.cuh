@@ -90,7 +90,8 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
       LevelCtx c;
       float tv[8][2];
       level_prepare<LAYOUT>(a.grid, l, x01, y01, z01, c);
-      level_fetch_rt2(a.grid, a.table, c, tv, pol_table);
+      if (a.grid.table_dtype == SDFB200_DT_F16) level_fetch<__half, 2, true>(a.table, c, tv, pol_table);
+      else level_fetch<float, 2, true>(a.table, c, tv, pol_table);
       level_finish<2, LAYOUT>(a.grid, c, tv, o, dj);
     }
     store_a<P>(img, plane, row, 2 * l, o[0]);

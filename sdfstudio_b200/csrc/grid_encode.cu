@@ -19,7 +19,7 @@ __global__ void __launch_bounds__(256) k_grid_encode(const __grid_constant__ sdf
   float d[F][3];
   if (l < g.active_levels) {
     const float x = __ldg(x01 + p * 3), y = __ldg(x01 + p * 3 + 1), z = __ldg(x01 + p * 3 + 2);
-    encode_level<T, F, GRAD>(g, table, l, x, y, z, o, d);
+    encode_level<T, F>(g, table, l, x, y, z, o, d);
   } else {
 #pragma unroll
     for (int f = 0; f < F; ++f) {
@@ -68,56 +68,24 @@ __global__ void __launch_bounds__(256) k_grid_encode_bwd(const __grid_constant__
   float go[F];
 #pragma unroll
   for (int f = 0; f < F; ++f) go[f] = __ldg(dout + p * L * F + l * F + f);
-  const float s = g.scale[l];
-  const uint64_t base = g.offset[l];
-  if (dtable == nullptr) {
-    // input gradient only (autograd.grad(sdf, x) of the eikonal / normal path): no scatter
-  } else if (g.layout == SDFB200_GRID_TORCH) {
-    const float sx = x * s, sy = y * s, sz = z * s;
-    const float fxf = floorf(sx), fyf = floorf(sy), fzf = floorf(sz);
-    const uint32_t fc[3][2] = {{(uint32_t)(int)fxf, (uint32_t)(int)ceilf(sx)}, {(uint32_t)(int)fyf, (uint32_t)(int)ceilf(sy)}, {(uint32_t)(int)fzf, (uint32_t)(int)ceilf(sz)}};
-    float o[3] = {sx - fxf, sy - fyf, sz - fzf};
-    if (g.smoothstep)
-      for (int d = 0; d < 3; ++d) o[d] = o[d] * o[d] * (3.f - 2.f * o[d]);
-    const uint32_t mask = (1u << g.log2_hashmap_size) - 1u;
-    for (int c = 0; c < 8; ++c) {
-      const int bx = c & 1, by = (c >> 1) & 1, bz = (c >> 2) & 1;  // 1 = ceil corner (weight o), 0 = floor (1-o)
-      const float w = (bx ? o[0] : 1.f - o[0]) * (by ? o[1] : 1.f - o[1]) * (bz ? o[2] : 1.f - o[2]);
-      const uint32_t h = (fc[0][bx] ^ (fc[1][by] * kPrimeY) ^ (fc[2][bz] * kPrimeZ)) & mask;
-      float* dst = dtable + (base + h) * F;
+  LevelCtx c;
+  level_prepare(g, l, x, y, z, c);
+  // dtable == NULL: input gradient only (autograd.grad(sdf, x) of the eikonal / normal path), no scatter
+  if (dtable != nullptr) {
+    float w[8];
+    corner_weights(c, w);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
       float wv[F];
 #pragma unroll
-      for (int f = 0; f < F; ++f) wv[f] = w * go[f];
-      atomic_add_row<F>(dst, wv);
-    }
-  } else {
-    const uint32_t res = g.resolution[l], size = g.size[l];
-    const bool hashed = g.hashed[l];
-    float pz[3] = {fmaf(x, s, 0.5f), fmaf(y, s, 0.5f), fmaf(z, s, 0.5f)};
-    uint32_t cell[3];
-    float w[3];
-    for (int d = 0; d < 3; ++d) {
-      const float fl = floorf(pz[d]);
-      cell[d] = (uint32_t)(int)fl;
-      const float t = pz[d] - fl;
-      w[d] = g.smoothstep ? t * t * (3.f - 2.f * t) : t;
-    }
-    for (int c = 0; c < 8; ++c) {
-      const uint32_t ix = cell[0] + (c & 1), iy = cell[1] + ((c >> 1) & 1), iz = cell[2] + ((c >> 2) & 1);
-      const float wt = ((c & 1) ? w[0] : 1.f - w[0]) * ((c & 2) ? w[1] : 1.f - w[1]) * ((c & 4) ? w[2] : 1.f - w[2]);
-      uint32_t idx2 = hashed ? (ix ^ (iy * kPrimeY) ^ (iz * kPrimeZ)) : (ix + iy * res + iz * res * res);
-      idx2 %= size;
-      float* dst = dtable + (base + idx2) * F;
-      float wv[F];
-#pragma unroll
-      for (int f = 0; f < F; ++f) wv[f] = wt * go[f];
-      atomic_add_row<F>(dst, wv);
+      for (int f = 0; f < F; ++f) wv[f] = w[k] * go[f];
+      atomic_add_row<F>(dtable + (c.base + c.idx[k]) * F, wv);
     }
   }
   if (dx01 != nullptr) {
-    float o[F];
-    float d[F][3];
-    encode_level<T, F, true>(g, table, l, x, y, z, o, d);
+    float v[8][F], o[F], d[F][3];
+    level_fetch<T, F>(table, c, v);
+    level_finish<F>(g, c, v, o, d);
     float ax = 0.f, ay = 0.f, az = 0.f;
 #pragma unroll
     for (int f = 0; f < F; ++f) {
@@ -132,7 +100,7 @@ __global__ void __launch_bounds__(256) k_grid_encode_bwd(const __grid_constant__
 // its +-delta taps, point gi of sample n at row gi * n_samples + n -- that almost always fall into the SAME cell of a level (delta is the
 // finest level's cell size, the active levels are coarser).  One thread walks the taps of a (sample, level): while the 8 table rows
 // stay the same it gathers them once (forward) / accumulates the 8 row gradients in registers and issues ONE set of atomics
-// (backward) instead of `group` of them.  Arithmetic per point is the ungrouped kernels' (same prepare / finish expression trees).
+// (backward) instead of `group` of them.  Arithmetic per point is the ungrouped kernels'.
 // -----------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool same_rows(const LevelCtx& a, const LevelCtx& b) {
   bool same = true;
@@ -160,8 +128,7 @@ __global__ void __launch_bounds__(256) k_grid_encode_grouped(const __grid_consta
       LevelCtx c;
       level_prepare(g, l, __ldg(x01 + p * 3), __ldg(x01 + p * 3 + 1), __ldg(x01 + p * 3 + 2), c);
       if (!have || !same_rows(c, cur)) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) TableLoad<T, F>::load(table, c.base + c.idx[k], tv[k]);
+        level_fetch<T, F>(table, c, tv);
         have = true;
       }
       cur = c;
@@ -174,20 +141,6 @@ __global__ void __launch_bounds__(256) k_grid_encode_grouped(const __grid_consta
     float* op = out + p * out_ld + l * F;
 #pragma unroll
     for (int f = 0; f < F; ++f) op[f] = o[f];
-  }
-}
-
-// weight of table row k (LevelCtx order) in the blend of level_finish
-__device__ __forceinline__ void corner_weights(const sdfb200_grid_t& g, const LevelCtx& c, float (&w)[8]) {
-  if (g.layout == SDFB200_GRID_TORCH) {
-    const float ox = c.w[0], oy = c.w[1], oz = c.w[2], nx = 1.f - ox, ny = 1.f - oy, nz = 1.f - oz;
-    // (c,c,c)(c,f,c)(f,f,c)(f,c,c)(c,c,f)(c,f,f)(f,f,f)(f,c,f): the CEIL corner carries the offset
-    w[0] = ox * oy * oz; w[1] = ox * ny * oz; w[2] = nx * ny * oz; w[3] = nx * oy * oz;
-    w[4] = ox * oy * nz; w[5] = ox * ny * nz; w[6] = nx * ny * nz; w[7] = nx * oy * nz;
-  } else {
-#pragma unroll
-    for (int k = 0; k < 8; ++k)
-      w[k] = ((k & 1) ? c.w[0] : 1.f - c.w[0]) * ((k & 2) ? c.w[1] : 1.f - c.w[1]) * ((k & 4) ? c.w[2] : 1.f - c.w[2]);
   }
 }
 
@@ -225,7 +178,7 @@ __global__ void __launch_bounds__(256) k_grid_encode_bwd_grouped(const __grid_co
       have = true;
     }
     float w[8], go[F];
-    corner_weights(g, c, w);
+    corner_weights(c, w);
 #pragma unroll
     for (int f = 0; f < F; ++f) go[f] = __ldg(dout + p * L * F + l * F + f);
 #pragma unroll
@@ -258,13 +211,13 @@ __global__ void __launch_bounds__(256) k_grid_encode_bwd2(const __grid_constant_
       for (int f = 0; f < F; ++f) gdo[f] = 0.f;
     return;
   }
-  const float x[3] = {__ldg(x01 + p * 3), __ldg(x01 + p * 3 + 1), __ldg(x01 + p * 3 + 2)};
   const float gx[3] = {__ldg(g_dx + p * 3), __ldg(g_dx + p * 3 + 1), __ldg(g_dx + p * 3 + 2)};
   float go[F];
 #pragma unroll
   for (int f = 0; f < F; ++f) go[f] = __ldg(dout + p * L * F + l * F + f);
-  LevelGeom q;
-  level_geom(g, l, x, q);
+  LevelCtx q;
+  level_prepare(g, l, __ldg(x01 + p * 3), __ldg(x01 + p * 3 + 1), __ldg(x01 + p * 3 + 2), q);
+  const float dw[3] = {q.dw[0] * q.s, q.dw[1] * q.s, q.dw[2] * q.s};   // d w / d x01
   float acc_do[F];
 #pragma unroll
   for (int f = 0; f < F; ++f) acc_do[f] = 0.f;
@@ -278,11 +231,11 @@ __global__ void __launch_bounds__(256) k_grid_encode_bwd2(const __grid_constant_
       A[d] = b[d] ? q.w[d] : 1.f - q.w[d];
       sg[d] = b[d] ? 1.f : -1.f;
     }
-    const uint64_t row = corner_row(g, l, q.c[0][b[0]], q.c[1][b[1]], q.c[2][b[2]]);
+    const uint64_t row = q.base + q.idx[c];
     float v[F];
-    TableLoad<T, F>::load(table, row, v);
+    load_row<T, F>(table, row, v);
     // first derivatives of the corner weight
-    const float d0 = sg[0] * q.dw[0], d1 = sg[1] * q.dw[1], d2 = sg[2] * q.dw[2];
+    const float d0 = sg[0] * dw[0], d1 = sg[1] * dw[1], d2 = sg[2] * dw[2];
     const float gW = gx[0] * d0 * A[1] * A[2] + gx[1] * A[0] * d1 * A[2] + gx[2] * A[0] * A[1] * d2;
     float dot = 0.f;
 #pragma unroll
