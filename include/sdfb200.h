@@ -306,6 +306,41 @@ int sdfb200_render_packed(const float* weights, const float* rgb, const float* n
 /* torch.clip(depth, steps.min(), steps.max()) (:257) using the min/max accumulated by sdfb200_render. */
 int sdfb200_depth_clip(float* depth, const float* steps_minmax, int64_t n_rays, void* stream);
 
+/* Segmented packed samples (nerfacc 0.3.5 render_weight_from_alpha / accumulate_along_rays as models/neus_acc.py:102-120 calls them):
+ * the samples of ray r are [offsets[r], offsets[r+1]) of the flat list; offsets [n_rays+1] int64, offsets[0] = 0, non-decreasing.
+ * Deterministic (fixed-order double sums, no atomics).
+ * weights[i] = alphas[i] * prod_{j in segment, j < i} (1 - alphas[j])   (no +1e-7, unlike sdfb200_weights_from_alphas). */
+int sdfb200_packed_weights(const float* alphas, const int64_t* offsets, int64_t n_rays, float* weights, void* stream);
+/* out [n_rays, n_channels] = per-segment sum of weights * values ([N, n_channels]); values == NULL (n_channels = 1): sum of weights.
+ * An empty segment gives 0. */
+int sdfb200_packed_accumulate(const float* weights, const float* values, int32_t n_channels, const int64_t* offsets, int64_t n_rays,
+                              float* out, void* stream);
+/* g_weights [N] -> g_alphas [N]: T_k (g_k - S_k), S_k = g_{k+1} alpha_{k+1} + (1 - alpha_{k+1}) S_{k+1}; no division (finite at alpha = 1). */
+int sdfb200_packed_weights_backward(const float* alphas, const int64_t* offsets, int64_t n_rays, const float* g_weights, float* g_alphas,
+                                    void* stream);
+/* g_out [n_rays, n_channels] -> g_weights [N] = sum_c g_out[r_i, c] values[i, c] (or g_out[r_i]), g_values [N, n_channels] =
+ * weights[i] g_out[r_i, c]; either output may be NULL.  ray_indices [N] int64 in [0, n_rays). */
+int sdfb200_packed_accumulate_backward(const float* weights, const float* values, int32_t n_channels, const int64_t* ray_indices,
+                                       int64_t n_samples_total, const float* g_out, float* g_weights, float* g_values, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Occupancy grid of the neus-acc sampler (NeuSAccSampler, model_components/ray_samplers.py:1315-1503).  binary: the [res,res,res] bool
+ * grid (1 byte per voxel), voxel (x, y, z) at x*res^2 + y*res + z.
+ * ------------------------------------------------------------------------------------------------------------- */
+/* update_binary_grid's test (:1405-1424) on the n occupied voxels: sdf [n] at their centres, voxel_indices [n] int64 flat indices.
+ * alpha = ((p + 1e-5) / (c + 1e-5)).clip(0, 1) with c / p from sigmoid((max(|sdf| - bound, 0) +/- half_step) * inv_s[0]); voxels with
+ * !(alpha > alpha_thres) are cleared, no voxel is set. */
+int sdfb200_occupancy_prune(const float* sdf, const int64_t* voxel_indices, int64_t n, float bound, float half_step, const float* inv_s,
+                            float alpha_thres, uint8_t* binary, void* stream);
+/* nerfacc 0.3.5 ray_marching, AABB contraction, cone_angle = 0, dt = step_size: a sample (t0, t1) is kept where the midpoint lies in an
+ * occupied voxel of roi_aabb (HOST float[6] = min xyz, max xyz); empty voxels are skipped to the next voxel boundary in whole steps.
+ * Rays stop at t_mid >= far, when a step no longer advances t (fp32 absorption; nerfacc would not terminate), or after 2^26 loop
+ * iterations.  Two passes on the same inputs: offsets == NULL counts the samples of each ray into counts [n_rays] int32; otherwise
+ * offsets [n_rays] int64 (exclusive cumsum of the counts) places ray_indices [N] int64, t_starts / t_ends [N]. */
+int sdfb200_occupancy_march(const float* origins, const float* directions, const float* nears, const float* fars, int64_t n_rays,
+                            const float* roi_aabb, const uint8_t* binary, int32_t resolution, float step_size, const int64_t* offsets,
+                            int32_t* counts, int64_t* ray_indices, float* t_starts, float* t_ends, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * The step before the path (SURVEY.md section 8f rows 2-3): camera rays, colliders, meshing lattice.
  * ------------------------------------------------------------------------------------------------------------- */

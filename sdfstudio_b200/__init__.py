@@ -4,18 +4,19 @@ Host side mirrors the reference's plug points (SURVEY.md section 8b):
   encoding.Encoding            <- tinycudann.Encoding (HashGrid)        nerfstudio/fields/sdf_field.py:230-241
   sdf_field.SDFField           <- nerfstudio.fields.sdf_field.SDFField
   ray_samplers.*               <- nerfstudio.model_components.ray_samplers
+  packed.*                     <- nerfacc 0.3.5 render_weight_from_alpha / accumulate_along_rays (neus-acc)
   renderers.*                  <- nerfstudio.model_components.renderers
   rays.*                       <- nerfstudio.cameras.rays (containers + alpha/density -> weights)
 All arithmetic runs in libsdfb200.so (CUDA, sm_90a) behind the C ABI of include/sdfb200.h.  No CPU / PyTorch fallback.
 """
 from . import _lib  # noqa: F401
-from . import cameras, meshing  # noqa: F401
+from . import cameras, meshing, packed  # noqa: F401
 from .density_fields import HashMLPDensityField  # noqa: F401
 from .encoding import Encoding, HashEncoding  # noqa: F401
 from .field_heads import FieldHeadNames  # noqa: F401
 from .rays import Frustums, RayBundle, RaySamples  # noqa: F401
 from .ray_samplers import (  # noqa: F401
-    ErrorBoundedSampler, LinearDisparitySampler, LogSampler, NeuSSampler, PDFSampler, ProposalNetworkSampler, Sampler, SpacedSampler,
+    ErrorBoundedSampler, LinearDisparitySampler, LogSampler, NeuSAccSampler, NeuSSampler, PDFSampler, ProposalNetworkSampler, Sampler, SpacedSampler,
     SqrtSampler, UniformLinDispPiecewiseSampler, UniformSampler, UniSurfSampler,
 )
 from .renderers import AccumulationRenderer, DepthRenderer, RGBRenderer, SemanticRenderer, render_all, render_from_alphas  # noqa: F401

@@ -113,6 +113,12 @@ _PROTOS = {
     "sdfb200_render_alphas": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _i32, _vp, _vp, C.POINTER(RenderOut), _vp]),
     "sdfb200_depth_clip": (C.c_int, [_vp, _vp, _i64, _vp]),
     "sdfb200_render_packed": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _i32, _i32, C.POINTER(RenderOut), _vp, _sz, _vp]),
+    "sdfb200_packed_weights": (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
+    "sdfb200_packed_accumulate": (C.c_int, [_vp, _vp, _i32, _vp, _i64, _vp, _vp]),
+    "sdfb200_packed_weights_backward": (C.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
+    "sdfb200_packed_accumulate_backward": (C.c_int, [_vp, _vp, _i32, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "sdfb200_occupancy_prune": (C.c_int, [_vp, _vp, _i64, _f32, _f32, _vp, _f32, _vp, _vp]),
+    "sdfb200_occupancy_march": (C.c_int, [_vp, _vp, _vp, _vp, _i64, C.POINTER(C.c_float), _vp, _i32, _f32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "sdfb200_gemm_workspace_bytes": (_sz, []),
     "sdfb200_gemm_nt": (C.c_int, [_i32, _vp, _i64, _vp, _i64, _i32, _i32, _vp, _i32, _vp, _i64, _i64, _vp, _sz, _vp]),
     "sdfb200_gemm_nn": (C.c_int, [_i32, _vp, _i64, _vp, _i64, _i32, _i32, _vp, _i64, _i64, _vp, _sz, _vp]),

@@ -175,3 +175,58 @@ class RenderAlphasFn(torch.autograd.Function):
             _lib.check(lib.sdfb200_weights_backward(_lib.ptr(a), None, 0, R, S, _lib.ptr(g_w), _lib.ptr(g_last), 1, _lib.ptr(g_a), _lib.stream_ptr()),
                        "sdfb200_weights_backward")
         return g_a, g_rgb_s, g_nrm_s, None, None, None
+
+
+class PackedWeightsFn(torch.autograd.Function):
+    """alphas [N] of segmented packed samples (ray r = [offsets[r], offsets[r+1])) -> weights [N] = alpha * exclusive prod(1 - alpha)
+    (nerfacc 0.3.5 render_weight_from_alpha; sdfb200_packed_weights / sdfb200_packed_weights_backward)."""
+
+    @staticmethod
+    def forward(ctx, alphas, offsets):
+        lib = _lib.load()
+        a = _lib.f32c(alphas)
+        w = torch.empty_like(a)
+        R = offsets.numel() - 1
+        _lib.check(lib.sdfb200_packed_weights(_lib.ptr(a), _lib.ptr(offsets), R, _lib.ptr(w), _lib.stream_ptr()), "sdfb200_packed_weights")
+        ctx.save_for_backward(a, offsets)
+        return w
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_w):
+        lib = _lib.load()
+        a, offsets = ctx.saved_tensors
+        g_a = torch.zeros_like(a)
+        _lib.check(lib.sdfb200_packed_weights_backward(_lib.ptr(a), _lib.ptr(offsets), offsets.numel() - 1, _lib.ptr(_lib.f32c(g_w)), _lib.ptr(g_a),
+                                                       _lib.stream_ptr()), "sdfb200_packed_weights_backward")
+        return g_a, None
+
+
+class PackedAccumulateFn(torch.autograd.Function):
+    """weights [N], values [N,C] | None -> [R,C] per-segment sums of weights * values (nerfacc 0.3.5 accumulate_along_rays;
+    sdfb200_packed_accumulate / sdfb200_packed_accumulate_backward)."""
+
+    @staticmethod
+    def forward(ctx, weights, values, offsets, ray_indices):
+        lib = _lib.load()
+        w = _lib.f32c(weights)
+        v = _lib.f32c(values) if values is not None else None
+        C = v.shape[1] if v is not None else 1
+        R = offsets.numel() - 1
+        out = torch.empty(R, C, device=w.device, dtype=torch.float32)
+        _lib.check(lib.sdfb200_packed_accumulate(_lib.ptr(w), _lib.ptr(v), C, _lib.ptr(offsets), R, _lib.ptr(out), _lib.stream_ptr()),
+                   "sdfb200_packed_accumulate")
+        ctx.save_for_backward(w, v, ray_indices)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_out):
+        lib = _lib.load()
+        w, v, ray_indices = ctx.saved_tensors
+        C = v.shape[1] if v is not None else 1
+        g_w = torch.empty_like(w) if ctx.needs_input_grad[0] else None
+        g_v = torch.empty_like(v) if (v is not None and ctx.needs_input_grad[1]) else None
+        _lib.check(lib.sdfb200_packed_accumulate_backward(_lib.ptr(w), _lib.ptr(v), C, _lib.ptr(ray_indices), w.shape[0], _lib.ptr(_lib.f32c(g_out)),
+                                                          _lib.ptr(g_w), _lib.ptr(g_v), _lib.stream_ptr()), "sdfb200_packed_accumulate_backward")
+        return g_w, g_v, None, None

@@ -230,6 +230,60 @@ __global__ void k_render_packed_finish(const float* __restrict__ acc, int64_t R,
   if (o_normal) { o_normal[r * 3] = a[5]; o_normal[r * 3 + 1] = a[6]; o_normal[r * 3 + 2] = a[7]; }
 }
 
+// -----------------------------------------------------------------------------------------------------------------
+// segmented packed samples (nerfacc 0.3.5 render_weight_from_alpha / accumulate_along_rays, models/neus_acc.py:102-120): the samples of
+// ray r are the contiguous segment [offsets[r], offsets[r+1]).  ONE WARP PER RAY streams its segment (lane = sample % 32); every sum and
+// product runs in double in a fixed order, so the results are deterministic and need no atomics.
+// -----------------------------------------------------------------------------------------------------------------
+// w = alpha T, T = exclusive product of (1 - alpha) over the segment (no +1e-7, unlike the dense rays.py:204)
+__global__ void __launch_bounds__(256) k_packed_weights(const float* __restrict__ alphas, const int64_t* __restrict__ offsets, int64_t R,
+                                                        float* __restrict__ weights) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= R) return;  // whole warp
+  const int64_t b = offsets[r], e = offsets[r + 1];
+  double carry = 1.0;
+  for (int64_t s0 = b; s0 < e; s0 += 32) {
+    const int64_t s = s0 + lane;
+    const bool on = s < e;
+    const float al = on ? alphas[s] : 0.f;
+    double incl = 1.0 - (double)al;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const double o = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl *= o;
+    }
+    double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+    if (lane == 0) excl = 1.0;
+    if (on) weights[s] = (float)((double)al * (carry * excl));
+    carry *= __shfl_sync(0xffffffffu, incl, 31);
+  }
+}
+
+// out[r, c] = sum over the segment of w * values[:, c]  (values == NULL: sum of w, C = 1)
+__global__ void __launch_bounds__(256) k_packed_accumulate(const float* __restrict__ weights, const float* __restrict__ values,
+                                                           const int64_t* __restrict__ offsets, int64_t R, int C, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= R) return;  // whole warp
+  const int64_t b = offsets[r], e = offsets[r + 1];
+  for (int c0 = 0; c0 < C; c0 += 4) {
+    double acc[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int64_t s = b + lane; s < e; s += 32) {
+      const double w = (double)weights[s];
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (c0 + k < C) acc[k] += values ? w * (double)values[s * C + c0 + k] : w;
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], d);
+      if (lane == 0 && c0 + k < C) out[r * C + c0 + k] = (float)acc[k];
+    }
+  }
+}
+
 __global__ void k_depth_clip(float* __restrict__ depth, const float* __restrict__ mm, int64_t R) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r < R) depth[r] = fminf(fmaxf(depth[r], mm[0]), mm[1]);
@@ -326,5 +380,25 @@ extern "C" int sdfb200_render_packed(const float* weights, const float* rgb, con
   k_render_packed_finish<<<(unsigned)ceil_div(n_rays, 256), 256, 0, (cudaStream_t)stream>>>((const float*)workspace, n_rays, bg, bg_mode, clamp01, out->rgb,
                                                                                              out->depth, out->normal, out->accumulation);
   SDFB_LAUNCHED("k_render_packed_finish");
+  return 0;
+}
+
+extern "C" int sdfb200_packed_weights(const float* alphas, const int64_t* offsets, int64_t n_rays, float* weights, void* stream) {
+  SDFB_REQUIRE(n_rays >= 0, "bad sizes");
+  if (n_rays == 0) return 0;
+  SDFB_REQUIRE(alphas && offsets && weights, "NULL pointer");
+  k_packed_weights<<<(unsigned)ceil_div(n_rays, 8), 256, 0, (cudaStream_t)stream>>>(alphas, offsets, n_rays, weights);
+  SDFB_LAUNCHED("k_packed_weights");
+  return 0;
+}
+
+extern "C" int sdfb200_packed_accumulate(const float* weights, const float* values, int32_t n_channels, const int64_t* offsets, int64_t n_rays,
+                                         float* out, void* stream) {
+  SDFB_REQUIRE(n_rays >= 0 && n_channels >= 1, "bad sizes");
+  SDFB_REQUIRE(values != nullptr || n_channels == 1, "values == NULL accumulates the weights: n_channels must be 1");
+  if (n_rays == 0) return 0;
+  SDFB_REQUIRE(weights && offsets && out, "NULL pointer");
+  k_packed_accumulate<<<(unsigned)ceil_div(n_rays, 8), 256, 0, (cudaStream_t)stream>>>(weights, values, offsets, n_rays, n_channels, out);
+  SDFB_LAUNCHED("k_packed_accumulate");
   return 0;
 }

@@ -127,9 +127,97 @@ __global__ void __launch_bounds__(256) k_weights_bwd(const float* __restrict__ i
   }
 }
 
+// backward of k_packed_weights (w_k = alpha_k T_k over a segment), one warp per ray, without division (finite at alpha = 1):
+//   dL/dalpha_k = T_k (g_k - S_k),  S_k = g_{k+1} alpha_{k+1} + (1 - alpha_{k+1}) S_{k+1},  S_last = 0.
+// A forward pass stages T_k in g_alpha; a reverse pass scans R_k = g_k alpha_k + (1 - alpha_k) R_{k+1} (S_k = R_{k+1}) as a suffix
+// composition of affine maps in double and overwrites g_alpha.
+__global__ void __launch_bounds__(256) k_packed_weights_bwd(const float* __restrict__ alphas, const int64_t* __restrict__ offsets, int64_t R,
+                                                            const float* __restrict__ g_w, float* __restrict__ g_alpha) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (r >= R) return;  // whole warp
+  const int64_t b = offsets[r], e = offsets[r + 1];
+  if (e <= b) return;
+  double carry = 1.0;
+  for (int64_t s0 = b; s0 < e; s0 += 32) {
+    const int64_t s = s0 + lane;
+    const bool on = s < e;
+    double incl = on ? 1.0 - (double)alphas[s] : 1.0;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const double o = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl *= o;
+    }
+    double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+    if (lane == 0) excl = 1.0;
+    if (on) g_alpha[s] = (float)(carry * excl);
+    carry *= __shfl_sync(0xffffffffu, incl, 31);
+  }
+  double carry_r = 0.0;   // R of the first sample after this chunk
+  for (int64_t s0 = b + (e - 1 - b) / 32 * 32; s0 >= b; s0 -= 32) {
+    const int64_t s = s0 + lane;
+    const bool on = s < e;
+    const double al = on ? (double)alphas[s] : 0.0;
+    const double g = on ? (double)g_w[s] : 0.0;
+    double A = g * al, B = 1.0 - al;   // R_s = A + B R_{s+1}
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const double Ao = __shfl_down_sync(0xffffffffu, A, d);
+      const double Bo = __shfl_down_sync(0xffffffffu, B, d);
+      if (lane + d < 32) { A += B * Ao; B *= Bo; }
+    }
+    const double Rk = A + B * carry_r;
+    double S = __shfl_down_sync(0xffffffffu, Rk, 1);
+    if (lane == 31) S = carry_r;
+    if (on) g_alpha[s] = (float)((double)g_alpha[s] * (g - S));
+    carry_r = __shfl_sync(0xffffffffu, Rk, 0);
+  }
+}
+
+// backward of k_packed_accumulate, one thread per sample: dv[i, c] = w_i g[r_i, c],  dw_i = sum_c g[r_i, c] v[i, c]  (or g[r_i])
+__global__ void __launch_bounds__(256) k_packed_accumulate_bwd(const float* __restrict__ weights, const float* __restrict__ values,
+                                                               const int64_t* __restrict__ ray_indices, int64_t N, int C,
+                                                               const float* __restrict__ g_out, float* __restrict__ g_w, float* __restrict__ g_v) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const float* g = g_out + ray_indices[i] * C;
+  if (g_w) {
+    double s = 0.0;
+    for (int c = 0; c < C; ++c) s += (double)g[c] * (values ? (double)values[i * C + c] : 1.0);
+    g_w[i] = (float)s;
+  }
+  if (g_v) {
+    const float w = weights[i];
+    for (int c = 0; c < C; ++c) g_v[i * C + c] = __fmul_rn(w, g[c]);
+  }
+}
+
 }  // namespace sdfb200
 
 using namespace sdfb200;
+
+extern "C" int sdfb200_packed_weights_backward(const float* alphas, const int64_t* offsets, int64_t n_rays, const float* g_weights, float* g_alphas,
+                                               void* stream) {
+  SDFB_REQUIRE(n_rays >= 0, "bad sizes");
+  if (n_rays == 0) return 0;
+  SDFB_REQUIRE(alphas && offsets && g_weights && g_alphas, "NULL pointer");
+  k_packed_weights_bwd<<<(unsigned)ceil_div(n_rays, 8), 256, 0, (cudaStream_t)stream>>>(alphas, offsets, n_rays, g_weights, g_alphas);
+  SDFB_LAUNCHED("k_packed_weights_bwd");
+  return 0;
+}
+
+extern "C" int sdfb200_packed_accumulate_backward(const float* weights, const float* values, int32_t n_channels, const int64_t* ray_indices,
+                                                  int64_t n_samples_total, const float* g_out, float* g_weights, float* g_values, void* stream) {
+  SDFB_REQUIRE(n_samples_total >= 0 && n_channels >= 1, "bad sizes");
+  SDFB_REQUIRE(values != nullptr || n_channels == 1, "values == NULL accumulates the weights: n_channels must be 1");
+  if (n_samples_total == 0) return 0;
+  SDFB_REQUIRE(ray_indices && g_out, "NULL pointer");
+  if (g_values) SDFB_REQUIRE(values != nullptr && weights != nullptr, "g_values needs values and weights");
+  k_packed_accumulate_bwd<<<(unsigned)ceil_div(n_samples_total, 256), 256, 0, (cudaStream_t)stream>>>(weights, values, ray_indices, n_samples_total,
+                                                                                                     n_channels, g_out, g_weights, g_values);
+  SDFB_LAUNCHED("k_packed_accumulate_bwd");
+  return 0;
+}
 
 extern "C" int sdfb200_render_backward(const float* weights, const float* rgb, const float* normals, const float* euclid_bins, const float* bg,
                                        int32_t bg_mode, int64_t n_rays, int32_t n_samples, const float* accumulation, const float* depth,

@@ -2,6 +2,7 @@
 ``forward`` signatures and train/eval behaviour).  Every per-ray scan runs in libsdfb200.so (csrc/samplers.cu); the
 Python here only sequences kernels and draws the training-mode jitter with ``torch.rand`` in the reference's order.
 """
+import ctypes as C
 import math
 from typing import Callable, List, Optional, Tuple, Union
 
@@ -9,7 +10,8 @@ import torch
 from torch import nn
 
 from . import _lib
-from .rays import bins_of, make_ray_samples, spacing_bins_of, weights_from_alphas
+from .packed import OFFSETS_ATTR
+from .rays import Frustums, RaySamples, bins_of, make_ray_samples, spacing_bins_of, weights_from_alphas
 
 _SPACING_TORCH = {
     "uniform": (lambda x: x, lambda x: x),
@@ -463,3 +465,113 @@ class UniSurfSampler(Sampler):
         merged = torch.empty(R, sa + sb + 1, device=a.device, dtype=torch.float32)
         _lib.check(lib.sdfb200_merge_bins(_lib.ptr(a), _lib.ptr(b), R, sa, sb, _lib.ptr(merged), None, _lib.stream_ptr()), "sdfb200_merge_bins")
         return make_ray_samples(ray_bundle, merged, merged, ray_samples_1.spacing_to_euclidean_fn)
+
+
+class NeuSAccSampler(Sampler):
+    """neus-acc's occupancy-grid sampler, ray_samplers.py:1315-1503: same constructor, buffers (``_binary``, ``_update_counter``,
+    ``cube_coordinate``) and methods.  The prune (update_binary_grid) and the march (nerfacc.cuda.ray_marching, AABB contraction,
+    cone_angle 0) run in csrc/occupancy.cu.  nerfacc's OccupancyGrid module, which only supplies the ROI and the contraction type here,
+    is not reproduced, so its ``grid.*`` state-dict keys are absent.  The prune is deterministic given the field, so DDP ranks keep
+    identical grids without a collective."""
+
+    def __init__(self, aabb, neus_sampler: NeuSSampler = None, resolution: int = 128, num_samples: int = 8, num_samples_importance: int = 16,
+                 num_samples_boundary: int = 10, steps_warpup: int = 2000, steps_per_grid_update: int = 1000, importance_sampling: bool = False,
+                 local_rank: int = 0, single_jitter: bool = False) -> None:
+        super().__init__()
+        if importance_sampling:
+            raise NotImplementedError("NeuSAccSampler(importance_sampling=True) needs nerfacc.ray_resampling, which this package does not provide")
+        self.aabb = aabb
+        self.resolution = resolution
+        self.num_samples = num_samples
+        self.num_samples_importance = num_samples_importance
+        self.num_samples_boundary = num_samples_boundary
+        self.single_jitter = single_jitter
+        self.importance_sampling = importance_sampling
+        self.steps_warpup = steps_warpup
+        self.steps_per_grid_update = steps_per_grid_update
+        self.local_rank = local_rank
+        self.step_size = 0.01 / 5.0
+        self.alpha_thres = 0.001
+
+        # only supports cubic bbox for now
+        assert aabb[0, 0] == aabb[0, 1] and aabb[0, 0] == aabb[0, 2]
+        assert aabb[1, 0] == aabb[1, 1] and aabb[1, 0] == aabb[1, 2]
+        self.grid_size = self.resolution
+        self.voxel_size = (aabb[1, 0] - aabb[0, 0]) / self.grid_size
+        self.neus_sampler = neus_sampler
+        self._roi_aabb = [float(v) for v in torch.as_tensor(aabb, dtype=torch.float32).reshape(-1).tolist()]
+        self.register_buffer("_binary", torch.ones((self.grid_size, self.grid_size, self.grid_size), dtype=torch.bool))
+        self.register_buffer("_update_counter", torch.zeros(1, dtype=torch.int32))
+        self.init_grid_coordinate()
+
+    def init_grid_coordinate(self):
+        """The voxel centres [G^3, 3] in the reference's own torch.linspace / meshgrid order (:1361-1376)."""
+        aabb = self.aabb
+        offs = [torch.linspace(aabb[0, i] + self.voxel_size / 2.0, aabb[1, i] - self.voxel_size / 2.0, self.grid_size) for i in range(3)]
+        x, y, z = torch.meshgrid(*offs, indexing="ij")
+        self.register_buffer("cube_coordinate", torch.stack([x, y, z], dim=-1).reshape(-1, 3))
+
+    def update_step_size(self, step, inv_s=None):
+        assert inv_s is not None
+        inv_s = inv_s().item()
+        self.step_size = 14.0 / inv_s / 16
+
+    @torch.no_grad()
+    def update_binary_grid(self, step, sdf_fn=None, inv_s=None):
+        """After `steps_warpup`, every `steps_per_grid_update` steps: clears the occupied voxels whose centre's alpha bound is at most
+        `alpha_thres` (:1384-1433).  Voxels are never re-occupied."""
+        assert sdf_fn is not None
+        assert inv_s is not None
+        if not (step >= self.steps_warpup and step % self.steps_per_grid_update == 0):
+            return
+        lib = _lib.load()
+        binary = self._binary
+        voxels = torch.nonzero(binary.reshape(-1)).reshape(-1)
+        points = self.cube_coordinate[voxels]
+        sdf = torch.cat([sdf_fn(p).reshape(-1) for p in torch.split(points, 100000, dim=0)]) if voxels.numel() else points.new_zeros(0)
+        sdf = _lib.f32c(sdf)
+        bound = float(self.voxel_size * (3**0.5) / 2.0)   # the reference's fp32 tensor expression
+        inv = _lib.f32c(inv_s().detach().reshape(-1)[:1].to(binary.device))
+        _lib.check(lib.sdfb200_occupancy_prune(_lib.ptr(sdf), _lib.ptr(voxels), voxels.numel(), bound, self.step_size * 0.5, _lib.ptr(inv),
+                                               self.alpha_thres, binary.data_ptr(), _lib.stream_ptr()), "sdfb200_occupancy_prune")
+        self._update_counter += 1
+
+    def create_ray_samples_from_ray_indices(self, ray_bundle, ray_indices, t_starts, t_ends):
+        """Flat RaySamples [N] of packed samples (:1435-1454)."""
+        frustums = Frustums(origins=ray_bundle.origins[ray_indices], directions=ray_bundle.directions[ray_indices], starts=t_starts, ends=t_ends,
+                            pixel_area=torch.ones_like(t_starts))
+        return RaySamples(frustums=frustums, camera_indices=ray_bundle.camera_indices[ray_indices], deltas=t_ends - t_starts)
+
+    def march(self, ray_bundle):
+        """nerfacc.cuda.ray_marching on this grid: (ray_indices [N] int64 carrying the segment offsets, t_starts [N,1], t_ends [N,1])."""
+        lib = _lib.load()
+        o, d = _lib.f32c(ray_bundle.origins), _lib.f32c(ray_bundle.directions)
+        nears, fars = _lib.f32c(ray_bundle.nears[:, 0]), _lib.f32c(ray_bundle.fars[:, 0])
+        R, dev = o.shape[0], o.device
+        binary = self._binary
+        roi = (C.c_float * 6)(*self._roi_aabb)
+        args = (_lib.ptr(o), _lib.ptr(d), _lib.ptr(nears), _lib.ptr(fars), R, roi, binary.data_ptr(), self.grid_size, self.step_size)
+        counts = torch.empty(R, device=dev, dtype=torch.int32)
+        _lib.check(lib.sdfb200_occupancy_march(*args, None, _lib.ptr(counts), None, None, None, _lib.stream_ptr()), "sdfb200_occupancy_march")
+        offsets = torch.zeros(R + 1, device=dev, dtype=torch.int64)
+        torch.cumsum(counts, 0, out=offsets[1:])
+        n = int(offsets[-1])   # the one host read of the march (nerfacc makes the same)
+        ray_indices = torch.empty(n, device=dev, dtype=torch.int64)
+        t_starts = torch.empty(n, 1, device=dev, dtype=torch.float32)
+        t_ends = torch.empty(n, 1, device=dev, dtype=torch.float32)
+        if n > 0:
+            _lib.check(lib.sdfb200_occupancy_march(*args, _lib.ptr(offsets), None, _lib.ptr(ray_indices), _lib.ptr(t_starts), _lib.ptr(t_ends),
+                                                   _lib.stream_ptr()), "sdfb200_occupancy_march")
+        setattr(ray_indices, OFFSETS_ATTR, offsets)
+        return ray_indices, t_starts, t_ends
+
+    @torch.no_grad()
+    def generate_ray_samples(self, ray_bundle=None, sdf_fn: Optional[Callable] = None, alpha_fn: Optional[Callable] = None):
+        """The wrapped NeuSSampler until the first grid update; then (RaySamples [N], ray_indices [N] int64) of the march."""
+        assert ray_bundle is not None
+        assert sdf_fn is not None
+        if self._update_counter.item() <= 0:
+            return self.neus_sampler(ray_bundle, sdf_fn=sdf_fn)
+        assert alpha_fn is not None
+        ray_indices, t_starts, t_ends = self.march(ray_bundle)
+        return self.create_ray_samples_from_ray_indices(ray_bundle, ray_indices, t_starts, t_ends), ray_indices

@@ -61,6 +61,18 @@ def rays_of(ray_samples):
     return _lib.f32c(fr.origins[:, 0, :]), _lib.f32c(fr.directions[:, 0, :])
 
 
+def sample_geometry(ray_samples):
+    """What the field kernels take for a RaySamples: (origins, directions, bins, shape).  Dense samples [R,S]: per-ray origins /
+    directions [R,3] and euclidean bins [R,S+1].  Packed samples (flat frustums [N], NeuSAccSampler): per-sample origins / directions
+    [N,3] and bins [N,2] = (start, end), i.e. N rays of one sample each.  `shape` is the frustums' shape ((R,S) or (N,))."""
+    fr = ray_samples.frustums
+    if fr.starts.dim() == 2:
+        bins = torch.cat([fr.starts, fr.ends], dim=-1).float().contiguous()
+        return _lib.f32c(fr.origins), _lib.f32c(fr.directions), bins, tuple(fr.starts.shape[:1])
+    origins, directions = rays_of(ray_samples)
+    return origins, directions, bins_of(ray_samples), tuple(fr.starts.shape[:2])
+
+
 def weights_from_alphas(alphas: torch.Tensor, with_transmittance: bool = False):
     """rays.py:194-230.  alphas [R,S,1] -> weights [R,S,1] (, transmittance [R,S+1,1])."""
     if _ag.needs_grad(alphas):

@@ -18,7 +18,7 @@ from . import _lib
 from . import sdf_field_train as _train
 from .encoding import Encoding, growth_factor
 from .field_heads import FieldHeadNames
-from .rays import bins_of, rays_of
+from .rays import bins_of, rays_of, sample_geometry
 
 
 class LaplaceDensity(nn.Module):
@@ -478,11 +478,9 @@ class SDFField(nn.Module):
             pos = ray_samples.frustums.get_start_positions()
             h = _train.forward_geonetwork(self, pos.reshape(-1, 3)).view(*ray_samples.frustums.shape, -1)
             return h[..., :1]
-        origins, directions = rays_of(ray_samples)
-        bins = bins_of(ray_samples)
-        S = bins.shape[1] - 1
-        o = self._run(origins, directions, bins, S, ("sdf",), apply_contraction=False)
-        return o["sdf"].view(origins.shape[0], S, 1)
+        origins, directions, bins, shape = sample_geometry(ray_samples)
+        o = self._run(origins, directions, bins, bins.shape[1] - 1, ("sdf",), apply_contraction=False)
+        return o["sdf"].view(*shape, 1)
 
     def gradient(self, x, skip_spatial_distortion=False, return_sdf=False):
         """sdf_field.py:424-465."""
@@ -503,18 +501,12 @@ class SDFField(nn.Module):
             pos = ray_samples.frustums.get_start_positions()
             h = _train.forward_geonetwork(self, pos.reshape(-1, 3)).view(*ray_samples.frustums.shape, -1)
             return self.laplace_density(h[..., :1]), h[..., 1:]
-        origins, directions = rays_of(ray_samples)
-        bins = bins_of(ray_samples)
-        S = bins.shape[1] - 1
-        o = self._run(origins, directions, bins, S, ("density", "geo_feature"), apply_contraction=False)
-        R = origins.shape[0]
-        return o["density"].view(R, S, 1), o["geo_feature"].view(R, S, -1)
+        origins, directions, bins, shape = sample_geometry(ray_samples)
+        o = self._run(origins, directions, bins, bins.shape[1] - 1, ("density", "geo_feature"), apply_contraction=False)
+        return o["density"].view(*shape, 1), o["geo_feature"].view(*shape, -1)
 
     def get_alpha(self, ray_samples, sdf=None, gradients=None):
         """sdf_field.py:476-525."""
-        origins, directions = rays_of(ray_samples)
-        bins = bins_of(ray_samples)
-        R, S = origins.shape[0], bins.shape[1] - 1
         if self._differentiable():
             if sdf is None or gradients is None:
                 inputs = ray_samples.frustums.get_start_positions().reshape(-1, 3)
@@ -527,8 +519,9 @@ class SDFField(nn.Module):
                 gradients = gradients.view(*ray_samples.frustums.shape, -1)
             return _train.get_alpha(self, ray_samples, sdf, gradients)
         if sdf is None or gradients is None:
-            o = self._run(origins, directions, bins, S, ("alpha",), apply_contraction=False)
-            return o["alpha"].view(R, S, 1)
+            origins, directions, bins, shape = sample_geometry(ray_samples)
+            o = self._run(origins, directions, bins, bins.shape[1] - 1, ("alpha",), apply_contraction=False)
+            return o["alpha"].view(*shape, 1)
         inv_s = self.deviation_network.get_variance()
         d = ray_samples.frustums.directions
         true_cos = (d * gradients).sum(-1, keepdim=True)
@@ -556,8 +549,7 @@ class SDFField(nn.Module):
             raise AttributeError("Camera indices are not provided.")
         if self._differentiable():
             return _train.get_outputs(self, ray_samples, return_alphas=return_alphas, return_occupancy=return_occupancy)
-        origins, directions = rays_of(ray_samples)
-        bins = bins_of(ray_samples)
+        origins, directions, bins, shape = sample_geometry(ray_samples)
         R, S = origins.shape[0], bins.shape[1] - 1
         wants = ["rgb", "density", "sdf", "normals", "gradients", "points_norm"]
         if self.config.use_numerical_gradients:
@@ -569,18 +561,18 @@ class SDFField(nn.Module):
         app = self._appearance(ray_samples.camera_indices, R, origins.device)
         o = self._run(origins, directions, bins, S, wants, apply_contraction=True, appearance=app)
         outputs = {
-            FieldHeadNames.RGB: o["rgb"].view(R, S, 3),
-            FieldHeadNames.DENSITY: o["density"].view(R, S, 1),
-            FieldHeadNames.SDF: o["sdf"].view(R, S, 1),
-            FieldHeadNames.NORMAL: o["normals"].view(R, S, 3),
-            FieldHeadNames.GRADIENT: o["gradients"].view(R, S, 3),
-            "points_norm": o["points_norm"].view(R, S, 1),
-            "sampled_sdf": o["sampled_sdf"].view(R, S, 6) if "sampled_sdf" in o else None,
+            FieldHeadNames.RGB: o["rgb"].view(*shape, 3),
+            FieldHeadNames.DENSITY: o["density"].view(*shape, 1),
+            FieldHeadNames.SDF: o["sdf"].view(*shape, 1),
+            FieldHeadNames.NORMAL: o["normals"].view(*shape, 3),
+            FieldHeadNames.GRADIENT: o["gradients"].view(*shape, 3),
+            "points_norm": o["points_norm"].view(*shape, 1),
+            "sampled_sdf": o["sampled_sdf"].view(*shape, 6) if "sampled_sdf" in o else None,
         }
         if return_alphas:
-            outputs[FieldHeadNames.ALPHA] = o["alpha"].view(R, S, 1)
+            outputs[FieldHeadNames.ALPHA] = o["alpha"].view(*shape, 1)
         if return_occupancy:
-            outputs[FieldHeadNames.OCCUPANCY] = o["occupancy"].view(R, S, 1)
+            outputs[FieldHeadNames.OCCUPANCY] = o["occupancy"].view(*shape, 1)
         return outputs
 
     def forward(self, ray_samples, return_alphas=False, return_occupancy=False):
