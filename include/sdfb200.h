@@ -188,6 +188,40 @@ int sdfb200_density_field_forward(const sdfb200_grid_t* grid, const void* table,
                                   int64_t n, float* density, float* pre_activation, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Nerfacto background field (background_model="grid" of neus-facto-angelo / bakedangelo).  Replaces TCNNNerfactoField.forward
+ * (nerfstudio/fields/nerfacto_field.py:223-318 through fields/base_field.py:104-123) without normals, transients, semantics or
+ * predicted normals.  grid: tcnn layout, 2 features per level.  Normalisation as sdfb200_density_field_forward (aabb != NULL selects
+ * the SceneBox, else `contraction` then (x + 2) / 4).
+ * Geometry: ray mode (n_samples = S > 0): origins / directions [n_rays,3], bins [n_rays,S+1] euclidean edges, positions = midpoints
+ * origins + directions * (start + end) / 2 (rounded like the reference, no FMA), N = n_rays * S.  Point mode (n_samples = 0):
+ * origins = positions [n_rays,3], directions [n_rays,3], bins unused, N = n_rays.
+ * base_weights (fp32, row-major): [hidden_dim, in_pad] | (n_hidden_layers-1) x [hidden_dim, hidden_dim] | [16, hidden_dim], rows
+ * 0..geo_feat_dim live; in_pad = 2 L rounded up to 16.  head_weights: [hidden_dim_color, head_pad] | (n_hidden_layers_color-1) x
+ * [hidden_dim_color, hidden_dim_color] | [16, hidden_dim_color], rows 0..2 live; head input = cat(SH4 16, geo, appearance),
+ * head_pad = its width rounded up to 16.
+ * appearance: row r (the ray in ray mode, the point in point mode) at appearance + r * appearance_stride (stride 0 broadcasts one
+ * vector), or NULL for zeros.
+ * Outputs [N] / [N,3] / [N] / [N,geo_feat_dim]: density = exp(pre-activation), rgb = sigmoid(head) (NULL: the colour half is skipped and
+ * head_weights may be NULL; so may directions, in point mode only), pre_activation and geo_feature optional.  One launch, no workspace.
+ * Unsupported shapes return SDFB200_EUNSUPPORTED.
+ * ------------------------------------------------------------------------------------------------------------- */
+typedef struct sdfb200_nerfacto {
+  int32_t hidden_dim;             /* base MLP width: 16, 32 or 64 */
+  int32_t n_hidden_layers;        /* num_layers - 1: 1, 2 or 3 */
+  int32_t hidden_dim_color;       /* colour MLP width: 16, 32 or 64 */
+  int32_t n_hidden_layers_color;  /* num_layers_color - 1: 1, 2 or 3 */
+  int32_t geo_feat_dim;           /* <= 15 */
+  int32_t appearance_dim;         /* 16 + geo_feat_dim + appearance_dim <= 64 */
+  int32_t contraction;            /* SDFB200_CONTRACT_* (used when aabb == NULL) */
+  int32_t n_samples;              /* samples per ray (ray mode), 0 = point mode */
+} sdfb200_nerfacto_t;
+
+int sdfb200_nerfacto_field_forward(const sdfb200_grid_t* grid, const sdfb200_nerfacto_t* f, const void* table, const float* base_weights,
+                                   const float* head_weights, const float* aabb, const float* origins, const float* directions,
+                                   const float* bins, int64_t n_rays, const float* appearance, int64_t appearance_stride, float* density,
+                                   float* rgb, float* pre_activation, float* geo_feature, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Ray samplers.  Replace nerfstudio/model_components/ray_samplers.py.  A sample set is a pair of bin-edge buffers
  * [R, S+1]: `spacing` (normalised) and `euclid` (distance along the ray), cf. cameras/rays.py:295-339.
  * ------------------------------------------------------------------------------------------------------------- */
@@ -414,7 +448,8 @@ int sdfb200_version(void);
 const char* sdfb200_last_error_string(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches). */
 int64_t sdfb200_launch_count(void);
-/* sizeof() of the ABI structs (0 grid, 1 field, 2 field_params, 3 field_in, 4 field_out, 5 render_out, 6 field_render): lets a binding
+/* sizeof() of the ABI structs (0 grid, 1 field, 2 field_params, 3 field_in, 4 field_out, 5 render_out, 6 field_render,
+ * 7 nerfacto): lets a binding
  * verify its struct mirrors before the first call. */
 size_t sdfb200_struct_size(int32_t which);
 

@@ -74,6 +74,11 @@ class FieldRender(C.Structure):
                 ("weights", C.c_void_p), ("bg_transmittance", C.c_void_p), ("out", RenderOut)]
 
 
+class NerfactoDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("hidden_dim", "n_hidden_layers", "hidden_dim_color", "n_hidden_layers_color", "geo_feat_dim",
+                                         "appearance_dim", "contraction", "n_samples")]  # fmt: skip
+
+
 _lib = None
 _lock = threading.Lock()
 
@@ -98,6 +103,8 @@ _PROTOS = {
     "sdfb200_field_workspace_bytes": (_sz, [C.POINTER(FieldDesc), _i64]),
     "sdfb200_field_forward": (C.c_int, [C.POINTER(FieldDesc), _vp, _vp, C.POINTER(FieldIn), C.POINTER(FieldOut), _vp, _sz, _vp]),
     "sdfb200_density_field_forward": (C.c_int, [C.POINTER(GridDesc), _vp, _vp, _i32, _i32, _i32, _vp, _vp, _i64, _vp, _vp, _vp]),
+    "sdfb200_nerfacto_field_forward": (C.c_int, [C.POINTER(GridDesc), C.POINTER(NerfactoDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64,
+                                                 _vp, _vp, _vp, _vp, _vp]),
     "sdfb200_spaced_bins": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _vp, _vp]),
     "sdfb200_bins_to_euclid": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "sdfb200_pdf_sample": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _f32, _f32, _i32, _vp, _vp, _vp]),
@@ -175,7 +182,7 @@ def load():
             fn = getattr(lib, name)
             fn.restype = res
             fn.argtypes = args
-        for which, st in enumerate((GridDesc, FieldDesc, FieldParams, FieldIn, FieldOut, RenderOut, FieldRender)):
+        for which, st in enumerate((GridDesc, FieldDesc, FieldParams, FieldIn, FieldOut, RenderOut, FieldRender, NerfactoDesc)):
             if lib.sdfb200_struct_size(which) != C.sizeof(st):
                 raise Sdfb200Error(f"ABI mismatch: sizeof({st.__name__}) = {C.sizeof(st)} but the library says {lib.sdfb200_struct_size(which)}")
         _lib = lib

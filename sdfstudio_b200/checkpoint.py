@@ -1,4 +1,5 @@
-"""Loading existing sdfstudio checkpoints into the drop-in modules (SURVEY.md section 8f row 4).
+"""Loading existing sdfstudio checkpoints into the drop-in modules (SURVEY.md section 8f row 4): the SDF field, the proposal networks
+and the grid background field.
 
 A reference ``step-*.ckpt`` (engine/trainer.py:276-297) is ``{"step", "pipeline", "optimizers", "schedulers", "scalers"}`` where
 ``pipeline`` is ``Pipeline.state_dict()``: the field's tensors sit under ``_model.field.`` (``module.`` in front when the pipeline
@@ -71,3 +72,43 @@ def load_density_field_checkpoint(density_field, loaded_state, index: int = 0, s
     if strict and extra:
         raise RuntimeError(f"unexpected entries for the proposal network: {extra}")
     return [], extra
+
+
+BACKGROUND_PREFIX = "_model.field_background."
+_FLAT_KNOBS = {"mlp_base.params": "num_levels / log2_hashmap_size / max_res / hidden_dim / num_layers / geo_feat_dim",
+               "mlp_head.params": "hidden_dim_color / num_layers_color / geo_feat_dim / appearance_embedding_dim"}
+_EMPTY_PARAMS = ("direction_encoding.params", "position_encoding.params")
+
+
+def load_background_field_checkpoint(field, loaded_state, prefix: str = BACKGROUND_PREFIX, strict: bool = True) -> Tuple[list, list]:
+    """Load the ``background_model="grid"`` field of a reference neus-facto-angelo / bakedangelo checkpoint (``TCNNNerfactoField``,
+    nerfstudio/fields/nerfacto_field.py:86-221) into a ``sdfstudio_b200.TCNNNerfactoField``.  ``mlp_base.params`` / ``mlp_head.params``
+    are tiny-cuda-nn's flat vectors (fp16-stored ones are cast to fp32); their lengths are checked, the ordering inside them follows
+    tcnn's published layout (UNPINNED).  The zero-length ``params`` of the parameter-free encodings may be present or absent.
+    Returns (missing, unexpected); with ``strict`` any other mismatch raises."""
+    if isinstance(loaded_state, (str, bytes)) or hasattr(loaded_state, "__fspath__"):
+        loaded_state = torch.load(loaded_state, map_location="cpu")
+    sd = extract_state(loaded_state, prefix)
+    flats = {}
+    for key, knobs in _FLAT_KNOBS.items():
+        if key not in sd:
+            raise KeyError(f"{key} not found under {prefix}")
+        flat = sd.pop(key).reshape(-1).to(torch.float32)
+        need = field.get_parameter(key).numel()
+        if flat.numel() != need:
+            raise ValueError(f"{key} has {flat.numel()} entries, this background field needs {need} (check {knobs})")
+        flats[key] = flat
+    for key in _EMPTY_PARAMS:
+        v = sd.pop(key, None)
+        if v is not None and v.numel() != 0:
+            raise ValueError(f"{key} has {v.numel()} entries, the parameter-free encoding has none")
+    sd = {k: (v.to(torch.float32) if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in sd.items()}
+    with torch.no_grad():
+        for key, flat in flats.items():
+            p = field.get_parameter(key)
+            p.copy_(flat.to(p.device))
+    missing, unexpected = field.load_state_dict(sd, strict=False)
+    missing = [m for m in missing if m not in _FLAT_KNOBS and m not in _EMPTY_PARAMS and m != "aabb"]
+    if strict and (missing or unexpected):
+        raise RuntimeError(f"checkpoint does not match the background field: missing {missing}, unexpected {list(unexpected)}")
+    return missing, list(unexpected)

@@ -3,7 +3,7 @@
 // i.e. tcnn.NetworkWithInputEncoding + trunc_exp (field_components/activations.py:24-42).  One thread per point: the L2-gather-bound
 // grid lookup dominates (8 L corners), the <= 64-wide MLP runs in registers with the weights broadcast from shared memory.
 #include "field.h"
-#include "grid.cuh"
+#include "hash_mlp.cuh"
 
 namespace sdfb200 {
 
@@ -27,55 +27,10 @@ __global__ void __launch_bounds__(128) k_density_field(const __grid_constant__ D
   __syncthreads();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.n) return;
-  float px = __ldg(a.positions + i * 3), py = __ldg(a.positions + i * 3 + 1), pz = __ldg(a.positions + i * 3 + 2);
   float x01, y01, z01;
-  if (a.aabb != nullptr) {
-    // SceneBox.get_normalized_positions (data/scene_box.py:67-76)
-    const float lx = __ldg(a.aabb + 3) - __ldg(a.aabb), ly = __ldg(a.aabb + 4) - __ldg(a.aabb + 1), lz = __ldg(a.aabb + 5) - __ldg(a.aabb + 2);
-    x01 = (px - __ldg(a.aabb)) / lx; y01 = (py - __ldg(a.aabb + 1)) / ly; z01 = (pz - __ldg(a.aabb + 2)) / lz;
-  } else {
-    if (a.contraction != SDFB200_CONTRACT_NONE) {
-      const float mag = a.contraction == SDFB200_CONTRACT_LINF ? fmaxf(fabsf(px), fmaxf(fabsf(py), fabsf(pz))) : sqrtf(px * px + py * py + pz * pz);
-      if (mag >= 1.f) {
-        const float k = 2.f - 1.f / mag;
-        px = k * (px / mag); py = k * (py / mag); pz = k * (pz / mag);
-      }
-    }
-    x01 = (px + 2.0f) * 0.25f; y01 = (py + 2.0f) * 0.25f; z01 = (pz + 2.0f) * 0.25f;
-  }
-  // layer 0 accumulated level by level (the encoded vector is never materialised)
+  normalize_position(a.aabb, a.contraction, __ldg(a.positions + i * 3), __ldg(a.positions + i * 3 + 1), __ldg(a.positions + i * 3 + 2), x01, y01, z01);
   float h[H];
-#pragma unroll
-  for (int o = 0; o < H; ++o) h[o] = 0.f;
-  for (int l = 0; l < a.grid.n_levels; ++l) {
-    float f[F];
-    float d[F][3];
-    if (l < a.grid.active_levels) encode_level<T, F>(a.grid, a.table, l, x01, y01, z01, f, d);
-    else
-      for (int k = 0; k < F; ++k) f[k] = 0.f;
-#pragma unroll
-    for (int k = 0; k < F; ++k) {
-      const float v = f[k];
-      const float* wc = w_s + (l * F + k);
-#pragma unroll
-      for (int o = 0; o < H; ++o) h[o] = fmaf(wc[o * a.in_pad], v, h[o]);
-    }
-  }
-#pragma unroll
-  for (int o = 0; o < H; ++o) h[o] = fmaxf(h[o], 0.f);
-  const float* w = w_s + H * a.in_pad;
-  for (int layer = 1; layer < a.n_hidden; ++layer, w += H * H) {
-    float g[H];
-#pragma unroll
-    for (int o = 0; o < H; ++o) {
-      float acc = 0.f;
-#pragma unroll
-      for (int k = 0; k < H; ++k) acc = fmaf(w[o * H + k], h[k], acc);
-      g[o] = fmaxf(acc, 0.f);
-    }
-#pragma unroll
-    for (int o = 0; o < H; ++o) h[o] = g[o];
-  }
+  const float* w = hash_mlp_hidden<T, F, H>(a.grid, a.table, w_s, a.in_pad, a.n_hidden, x01, y01, z01, h);
   float out = 0.f;
 #pragma unroll
   for (int k = 0; k < H; ++k) out = fmaf(w[k], h[k], out);

@@ -17,7 +17,7 @@ import torch
 from torch import nn
 
 from . import _lib
-from .encoding import make_grid_desc
+from .encoding import _GridFn, make_grid_desc
 
 
 class _TruncExp(torch.autograd.Function):
@@ -34,43 +34,42 @@ class _TruncExp(torch.autograd.Function):
         return g * torch.exp(x.clamp(-15, 15))
 
 
-class _GridFn(torch.autograd.Function):
-    """hash-grid features of the flat tcnn-style parameter vector (grid table = its tail): forward / backward kernels of the
-    Encoding operator, gradient scattered into the tail of d(params)."""
+def fully_fused_weights(g: torch.Generator, in_dim: int, hidden_dim: int, n_hidden_layers: int, n_output_dims: int) -> torch.Tensor:
+    """Initial weights of a tcnn FullyFusedMLP (ReLU, no biases) as one flat vector: xavier-uniform [hidden, in_pad] (padded input
+    columns zero) | (n_hidden_layers - 1) x [hidden, hidden] | [16, hidden] (the output padded to 16 rows, rows >= n_output_dims zero)."""
+    in_pad = (in_dim + 15) // 16 * 16
+    w0 = (torch.rand(hidden_dim, in_pad, generator=g) * 2 - 1) * math.sqrt(6.0 / (in_pad + hidden_dim))
+    w0[:, in_dim:] = 0.0
+    ws = [w0.reshape(-1)]
+    for _ in range(n_hidden_layers - 1):
+        ws.append(((torch.rand(hidden_dim, hidden_dim, generator=g) * 2 - 1) * math.sqrt(6.0 / (2 * hidden_dim))).reshape(-1))
+    wo = torch.zeros(16, hidden_dim)
+    wo[:n_output_dims] = (torch.rand(n_output_dims, hidden_dim, generator=g) * 2 - 1) * math.sqrt(6.0 / (hidden_dim + 16))
+    ws.append(wo.reshape(-1))
+    return torch.cat(ws)
 
-    @staticmethod
-    def forward(ctx, x01, params, nb):
-        lib = _lib.load()
-        x = _lib.f32c(x01)
-        n = x.shape[0]
-        desc = nb.desc
-        desc.active_levels, desc.table_dtype = desc.n_levels, _lib.DT_F32
-        out = torch.empty(n, nb.in_dim, device=x.device, dtype=torch.float32)
-        table = params.detach()[nb.n_net:]
-        _lib.check(lib.sdfb200_grid_encode(desc, table.data_ptr(), _lib.ptr(x), n, _lib.ptr(out), nb.in_dim, None, _lib.stream_ptr()), "sdfb200_grid_encode")
-        ctx.save_for_backward(x, params)
-        ctx.nb = nb
-        return out
 
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, dout):
-        lib = _lib.load()
-        x, params = ctx.saved_tensors
-        nb = ctx.nb
-        dout = _lib.f32c(dout)
-        dparams = torch.zeros_like(params, dtype=torch.float32)
-        dx = torch.zeros_like(x) if ctx.needs_input_grad[0] else None
-        table = params.detach()[nb.n_net:]
-        _lib.check(lib.sdfb200_grid_encode_backward(nb.desc, table.data_ptr(), _lib.ptr(x), _lib.ptr(dout), x.shape[0], dparams[nb.n_net:].data_ptr(),
-                                                    _lib.ptr(dx), _lib.stream_ptr()), "sdfb200_grid_encode_backward")
-        return dx, dparams, None
+def relu_mlp(x: torch.Tensor, w: torch.Tensor, in_dim: int, in_pad: int, hidden_dim: int, n_hidden_layers: int):
+    """The hidden layers of a FullyFusedMLP over the flat weights `w` (layout of fully_fused_weights), through ATen on views of `w` so
+    that autograd reaches it: returns the last hidden activations [N, hidden] and the rest of `w` (the output matrix)."""
+    o = hidden_dim * in_pad
+    h = torch.relu(x @ w[:o].view(hidden_dim, in_pad)[:, :in_dim].t())
+    for _ in range(n_hidden_layers - 1):
+        h = torch.relu(h @ w[o: o + hidden_dim * hidden_dim].view(hidden_dim, hidden_dim).t())
+        o += hidden_dim * hidden_dim
+    return h, w[o:]
 
 
 class _NetworkWithInputEncoding(nn.Module):
-    def __init__(self, n_levels, n_features, log2_hashmap_size, base_res, per_level_scale, hidden_dim, n_hidden_layers, seed=1337):
+    """tcnn.NetworkWithInputEncoding(HashGrid, FullyFusedMLP with ReLU and no biases) as one flat parameter vector: network weights
+    ([hidden, in_pad] | (n_hidden - 1) x [hidden, hidden] | [16, hidden], rows 0..n_output_dims-1 of the output matrix live), then the
+    grid table.  The proposal networks use one output, the nerfacto field 1 + geo_feat_dim."""
+
+    def __init__(self, n_levels, n_features, log2_hashmap_size, base_res, per_level_scale, hidden_dim, n_hidden_layers, seed=1337, n_output_dims=1):
         super().__init__()
-        self.hidden_dim, self.n_hidden_layers = hidden_dim, n_hidden_layers
+        if not 1 <= n_output_dims <= 16:
+            raise NotImplementedError("n_output_dims must be 1..16 (one padded output block)")
+        self.hidden_dim, self.n_hidden_layers, self.n_output_dims = hidden_dim, n_hidden_layers, n_output_dims
         self.in_dim = n_levels * n_features
         self.in_pad = (self.in_dim + 15) // 16 * 16
         self.desc = make_grid_desc("tcnn", n_levels, n_features, log2_hashmap_size, base_res, per_level_scale, False)
@@ -78,17 +77,9 @@ class _NetworkWithInputEncoding(nn.Module):
         self.n_net = hidden_dim * self.in_pad + (n_hidden_layers - 1) * hidden_dim * hidden_dim + self.n_out_pad * hidden_dim
         self.n_grid = self.desc._total_entries * n_features
         g = torch.Generator().manual_seed(seed)
-        # tcnn: xavier-uniform weights, U(-1e-4, 1e-4) grid
-        w0 = (torch.rand(hidden_dim, self.in_pad, generator=g) * 2 - 1) * math.sqrt(6.0 / (self.in_pad + hidden_dim))
-        w0[:, self.in_dim:] = 0.0
-        ws = [w0.reshape(-1)]
-        for _ in range(n_hidden_layers - 1):
-            ws.append(((torch.rand(hidden_dim, hidden_dim, generator=g) * 2 - 1) * math.sqrt(6.0 / (2 * hidden_dim))).reshape(-1))
-        wo = torch.zeros(self.n_out_pad, hidden_dim)
-        wo[0] = (torch.rand(hidden_dim, generator=g) * 2 - 1) * math.sqrt(6.0 / (hidden_dim + 16))
-        ws.append(wo.reshape(-1))
-        grid = (torch.rand(self.n_grid, generator=g) * 2 - 1) * 1e-4
-        self.params = nn.Parameter(torch.cat(ws + [grid]))
+        w = fully_fused_weights(g, self.in_dim, hidden_dim, n_hidden_layers, n_output_dims)
+        grid = (torch.rand(self.n_grid, generator=g) * 2 - 1) * 1e-4   # tcnn: U(-1e-4, 1e-4) grid
+        self.params = nn.Parameter(torch.cat([w, grid]))
 
     @property
     def weights(self):
@@ -159,13 +150,8 @@ class HashMLPDensityField(nn.Module):
         else:
             x01 = (x - self.aabb[0]) / (self.aabb[1] - self.aabb[0])                  # SceneBox.get_normalized_positions
         feat = _GridFn.apply(x01, nb.params, nb)
-        w = nb.params[: nb.n_net]
-        o = nb.hidden_dim * nb.in_pad
-        h = torch.relu(feat @ w[:o].view(nb.hidden_dim, nb.in_pad)[:, : nb.in_dim].t())
-        for _ in range(nb.n_hidden_layers - 1):
-            h = torch.relu(h @ w[o: o + nb.hidden_dim * nb.hidden_dim].view(nb.hidden_dim, nb.hidden_dim).t())
-            o += nb.hidden_dim * nb.hidden_dim
-        pre = (h @ w[o: o + nb.hidden_dim]).view(*positions.shape[:-1], 1)
+        h, wo = relu_mlp(feat, nb.params[: nb.n_net], nb.in_dim, nb.in_pad, nb.hidden_dim, nb.n_hidden_layers)
+        pre = (h @ wo[: nb.hidden_dim]).view(*positions.shape[:-1], 1)
         dens = _TruncExp.apply(pre)
         return (dens, pre) if return_pre_activation else dens
 

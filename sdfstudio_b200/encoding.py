@@ -156,6 +156,40 @@ class _GridEncodeBwdFn(torch.autograd.Function):
         return g_dout, g_x, (g_table.to(table.dtype) if g_table is not None else None), None, None, None, None
 
 
+class _GridFn(torch.autograd.Function):
+    """hash-grid features of the flat parameter vector of a tiny-cuda-nn NetworkWithInputEncoding (grid table = its tail, `nb` the
+    module that owns it: density_fields._NetworkWithInputEncoding): forward / backward kernels of the Encoding operator, gradient
+    scattered into the tail of d(params).  The training path of the proposal and nerfacto fields."""
+
+    @staticmethod
+    def forward(ctx, x01, params, nb):
+        lib = _lib.load()
+        x = _lib.f32c(x01)
+        n = x.shape[0]
+        desc = nb.desc
+        desc.active_levels, desc.table_dtype = desc.n_levels, _lib.DT_F32
+        out = torch.empty(n, nb.in_dim, device=x.device, dtype=torch.float32)
+        table = params.detach()[nb.n_net:]
+        _lib.check(lib.sdfb200_grid_encode(desc, table.data_ptr(), _lib.ptr(x), n, _lib.ptr(out), nb.in_dim, None, _lib.stream_ptr()), "sdfb200_grid_encode")
+        ctx.save_for_backward(x, params)
+        ctx.nb = nb
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dout):
+        lib = _lib.load()
+        x, params = ctx.saved_tensors
+        nb = ctx.nb
+        dout = _lib.f32c(dout)
+        dparams = torch.zeros_like(params, dtype=torch.float32)
+        dx = torch.zeros_like(x) if ctx.needs_input_grad[0] else None
+        table = params.detach()[nb.n_net:]
+        _lib.check(lib.sdfb200_grid_encode_backward(nb.desc, table.data_ptr(), _lib.ptr(x), _lib.ptr(dout), x.shape[0], dparams[nb.n_net:].data_ptr(),
+                                                    _lib.ptr(dx), _lib.stream_ptr()), "sdfb200_grid_encode_backward")
+        return dx, dparams, None
+
+
 class Encoding(nn.Module):
     """``tinycudann.Encoding`` look-alike (HashGrid / DenseGrid otypes)."""
 

@@ -1,0 +1,264 @@
+"""H100-native drop-in for ``nerfstudio.fields.nerfacto_field.TCNNNerfactoField`` (nerfacto_field.py:67-318), the field behind
+``background_model="grid"`` of neus-facto-angelo and bakedangelo (models/base_surface_model.py:181-187), which the reference builds
+from four tiny-cuda-nn modules.  Same constructor, ``get_density``, ``get_outputs``, ``density_fn`` and ``forward``.
+
+* Evaluation (``torch.no_grad()`` or eval mode): ``forward`` is one kernel launch (sdfb200_nerfacto_field_forward): hash grid ->
+  ReLU MLP -> exp for the density, tcnn SphericalHarmonics(4) + geometry feature + appearance -> ReLU MLP -> sigmoid for the colour.
+* Training (autograd recording in train mode), and ``get_density`` / ``get_outputs`` / ``density_fn`` called on their own: the
+  differentiable composition of this package's grid operator, ATen matmuls on views of the flat parameters, SH-4 in torch,
+  ``trunc_exp`` and ``nn.Embedding``.
+
+Parameters keep the reference's names: ``mlp_base.params`` (network weights, then the grid table: the proposal networks' layout
+with an output of 1 + geo_feat_dim), ``mlp_head.params`` ([HC, pad16(16 + geo + app)] | (n - 1) x [HC, HC] | [16, HC]),
+``embedding_appearance.embedding.weight``, ``aabb`` and the empty ``direction_encoding.params`` / ``position_encoding.params``, so
+``checkpoint.load_background_field_checkpoint`` loads a reference checkpoint.
+
+tiny-cuda-nn is not vendored in the reference, so these points restate its published behaviour and are UNPINNED (DESIGN.md section 4):
+* SH signs: tcnn's SH uses the Condon-Shortley phase, i.e. nerfstudio's ``components_from_spherical_harmonics`` (utils/math.py:46-70)
+  with components 1, 3, 5, 7, 9, 11, 13 and 15 negated;
+* the padded input columns of ``mlp_head`` (64 for the default shape) contribute nothing, as for the proposal networks;
+* network weights come before the encoding's parameters inside ``NetworkWithInputEncoding.params``;
+* parameter-free encodings register a zero-length ``params`` (they appear in the state dict);
+* tcnn computes in fp16; this package computes in fp32.
+
+Not supported (``SurfaceModel`` uses none of them): ``compute_normals=True``, transient embeddings, semantics, predicted normals.
+"""
+import math
+from typing import Optional
+
+import numpy as np
+import torch
+from torch import nn
+
+from . import _lib
+from .density_fields import _NetworkWithInputEncoding, _TruncExp, fully_fused_weights, relu_mlp
+from .encoding import _GridFn
+from .field_heads import FieldHeadNames
+from .rays import rays_of
+from .sdf_field import _Embedding
+
+BASE_RES, FEATURES_PER_LEVEL = 16, 2   # fixed by the reference constructor (nerfacto_field.py:126-127)
+SH_DIM = 16                            # tcnn SphericalHarmonics, degree 4
+
+
+def sh4(x: torch.Tensor) -> torch.Tensor:
+    """tcnn SphericalHarmonics degree 4 of x in [-1,1]^3 ([..., 3] -> [..., 16])."""
+    x_, y, z = x[..., 0], x[..., 1], x[..., 2]
+    xx, yy, zz = x_ * x_, y * y, z * z
+    return torch.stack([
+        torch.full_like(x_, 0.28209479177387814), -0.4886025119029199 * y, 0.4886025119029199 * z, -0.4886025119029199 * x_,
+        1.0925484305920792 * x_ * y, -1.0925484305920792 * y * z, 0.9461746957575601 * zz - 0.31539156525251999, -1.0925484305920792 * x_ * z,
+        0.5462742152960396 * (xx - yy), -0.5900435899266435 * y * (3 * xx - yy), 2.890611442640554 * x_ * y * z, -0.4570457994644658 * y * (5 * zz - 1),
+        0.3731763325901154 * z * (5 * zz - 3), -0.4570457994644658 * x_ * (5 * zz - 1), 1.445305721320277 * z * (xx - yy), -0.5900435899266435 * x_ * (xx - 3 * yy),
+    ], dim=-1)  # fmt: skip
+
+
+class _ParamFreeEncoding(nn.Module):
+    """tcnn.Encoding without parameters (SphericalHarmonics, Frequency): tcnn registers a zero-length ``params`` even then.  The
+    encodings themselves are evaluated inside the kernel / by ``sh4``."""
+
+    def __init__(self, n_output_dims: int):
+        super().__init__()
+        self.n_output_dims = n_output_dims
+        self.params = nn.Parameter(torch.zeros(0))
+
+
+class _Network(nn.Module):
+    """tcnn.Network(FullyFusedMLP, ReLU, no biases) as one flat parameter vector: [hidden, in_pad] | (n_hidden - 1) x [hidden, hidden] |
+    [16, hidden], in_pad = n_input_dims rounded up to 16, rows 0..n_output_dims-1 of the output matrix live."""
+
+    def __init__(self, n_input_dims, n_output_dims, hidden_dim, n_hidden_layers, seed=1337):
+        super().__init__()
+        self.in_dim, self.in_pad = n_input_dims, (n_input_dims + 15) // 16 * 16
+        self.hidden_dim, self.n_hidden_layers, self.n_output_dims = hidden_dim, n_hidden_layers, n_output_dims
+        g = torch.Generator().manual_seed(seed)
+        self.params = nn.Parameter(fully_fused_weights(g, n_input_dims, hidden_dim, n_hidden_layers, n_output_dims))
+
+    def forward(self, x):
+        """[N, in_dim] -> [N, n_output_dims] (no output activation)."""
+        h, wo = relu_mlp(x, self.params, self.in_dim, self.in_pad, self.hidden_dim, self.n_hidden_layers)
+        return h @ wo.view(16, self.hidden_dim)[: self.n_output_dims].t()
+
+
+class TCNNNerfactoField(nn.Module):
+    """nerfacto_field.py:67-318."""
+
+    def __init__(self, aabb, num_images: int, num_layers: int = 2, hidden_dim: int = 64, geo_feat_dim: int = 15, num_levels: int = 16,
+                 max_res: int = 1024, log2_hashmap_size: int = 19, num_layers_color: int = 3, num_layers_transient: int = 2,
+                 hidden_dim_color: int = 64, hidden_dim_transient: int = 64, appearance_embedding_dim: int = 32, transient_embedding_dim: int = 16,
+                 use_transient_embedding: bool = False, use_semantics: bool = False, num_semantic_classes: int = 100, use_pred_normals: bool = False,
+                 use_average_appearance_embedding: bool = False, spatial_distortion=None) -> None:
+        super().__init__()
+        if use_transient_embedding or use_semantics or use_pred_normals:
+            raise NotImplementedError("transient embeddings, semantics and predicted normals are not supported (SurfaceModel uses none of them)")
+        if hidden_dim not in (16, 32, 64) or hidden_dim_color not in (16, 32, 64):
+            raise NotImplementedError("hidden_dim and hidden_dim_color must be 16, 32 or 64")
+        if num_layers not in (2, 3, 4) or num_layers_color not in (2, 3, 4):
+            raise NotImplementedError("num_layers and num_layers_color must be 2, 3 or 4")
+        if not 0 <= geo_feat_dim <= 15 or SH_DIM + geo_feat_dim + appearance_embedding_dim > 64:
+            raise NotImplementedError("needs geo_feat_dim <= 15 and 16 + geo_feat_dim + appearance_embedding_dim <= 64")
+        self.aabb = nn.Parameter(torch.as_tensor(aabb, dtype=torch.float32), requires_grad=False)
+        self.geo_feat_dim = geo_feat_dim
+        self.spatial_distortion = spatial_distortion
+        self.num_images = num_images
+        self.appearance_embedding_dim = appearance_embedding_dim
+        self.embedding_appearance = _Embedding(num_images, appearance_embedding_dim)
+        self.use_average_appearance_embedding = use_average_appearance_embedding
+        self.use_transient_embedding, self.use_semantics, self.use_pred_normals = use_transient_embedding, use_semantics, use_pred_normals
+        growth = float(np.exp((np.log(max_res) - np.log(BASE_RES)) / (num_levels - 1)))
+        self.direction_encoding = _ParamFreeEncoding(SH_DIM)
+        self.position_encoding = _ParamFreeEncoding(3 * 2 * 2)   # Frequency, n_frequencies = 2
+        self.mlp_base = _NetworkWithInputEncoding(num_levels, FEATURES_PER_LEVEL, log2_hashmap_size, BASE_RES, growth, hidden_dim, num_layers - 1,
+                                                  n_output_dims=1 + geo_feat_dim)
+        self.mlp_head = _Network(SH_DIM + geo_feat_dim + appearance_embedding_dim, 3, hidden_dim_color, num_layers_color - 1)
+        self._density_before_activation = None
+        self._locations = None
+        self._positions_of_last_call = None
+
+    # ------------------------------------------------------------------ reference attributes
+    @property
+    def _sample_locations(self):
+        """Normalised positions of the last evaluation (Field._sample_locations).  The kernel path does not materialise them: it keeps the
+        last call's ``frustums.get_positions`` (and through it that call's frustum tensors, until the next call) and normalises on first
+        access.  The composition path stores them like the reference."""
+        if self._locations is None and self._positions_of_last_call is not None:
+            with torch.no_grad():
+                self._locations = self._normalize(self._positions_of_last_call())
+        return self._locations
+
+    def _contraction_code(self) -> int:
+        sd = self.spatial_distortion
+        if sd is None:
+            return _lib.CONTRACT_NONE
+        order = getattr(sd, "order", None)
+        if order is None:
+            return _lib.CONTRACT_L2
+        if order == float("inf"):
+            return _lib.CONTRACT_LINF
+        raise NotImplementedError(f"SceneContraction order {order!r} is not supported")
+
+    def _differentiable(self) -> bool:
+        return torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters())
+
+    # ------------------------------------------------------------------ differentiable composition
+    def _normalize(self, positions):
+        if self.spatial_distortion is not None:
+            return (self.spatial_distortion(positions) + 2.0) / 4.0
+        return (positions - self.aabb[0]) / (self.aabb[1] - self.aabb[0])   # SceneBox.get_normalized_positions
+
+    def _base(self, x01):
+        """mlp_base: [N,3] in [0,1] -> [N, 1 + geo_feat_dim]."""
+        nb = self.mlp_base
+        feat = _GridFn.apply(x01, nb.params, nb)
+        h, wo = relu_mlp(feat, nb.params[: nb.n_net], nb.in_dim, nb.in_pad, nb.hidden_dim, nb.n_hidden_layers)
+        return h @ wo.view(16, nb.hidden_dim)[: nb.n_output_dims].t()
+
+    def _density_from_positions(self, positions):
+        x01 = self._normalize(positions)
+        self._locations, self._positions_of_last_call = x01, None
+        h = self._base(x01.reshape(-1, 3)).view(*positions.shape[:-1], -1)
+        density_before_activation, base_mlp_out = torch.split(h, [1, self.geo_feat_dim], dim=-1)
+        self._density_before_activation = density_before_activation
+        return _TruncExp.apply(density_before_activation), base_mlp_out
+
+    def get_density(self, ray_samples):
+        """nerfacto_field.py:223-243."""
+        return self._density_from_positions(ray_samples.frustums.get_positions())
+
+    def density_fn(self, positions: torch.Tensor) -> torch.Tensor:
+        """fields/base_field.py:48-65: the density at `positions` (a zero-length frustum there)."""
+        return self._density_from_positions(positions)[0]
+
+    def _appearance_mode(self):
+        if self.training:
+            return "camera"
+        return "mean" if self.use_average_appearance_embedding else "zeros"
+
+    def get_outputs(self, ray_samples, density_embedding: Optional[torch.Tensor] = None):
+        """nerfacto_field.py:245-318 without transients, semantics and predicted normals."""
+        assert density_embedding is not None
+        if ray_samples.camera_indices is None:
+            raise AttributeError("Camera indices are not provided.")
+        directions = (ray_samples.frustums.directions + 1.0) / 2.0          # get_normalized_directions
+        shape = directions.shape[:-1]
+        d = sh4(directions.reshape(-1, 3) * 2.0 - 1.0)                      # tcnn maps its [0,1] input back with 2x - 1
+        mode = self._appearance_mode()
+        A = self.appearance_embedding_dim
+        if mode == "camera":
+            app = self.embedding_appearance(ray_samples.camera_indices.squeeze())
+        elif mode == "mean":
+            app = torch.ones((*shape, A), device=directions.device) * self.embedding_appearance.mean(dim=0)
+        else:
+            app = torch.zeros((*shape, A), device=directions.device)
+        h = torch.cat([d, density_embedding.reshape(-1, self.geo_feat_dim), app.reshape(-1, A)], dim=-1)
+        rgb = torch.sigmoid(self.mlp_head(h)).view(*shape, -1)
+        return {FieldHeadNames.RGB: rgb}
+
+    # ------------------------------------------------------------------ forward
+    def forward(self, ray_samples, compute_normals: bool = False):
+        """fields/base_field.py:104-123."""
+        if compute_normals:
+            raise NotImplementedError("compute_normals=True is not supported by the nerfacto background field")
+        if self._differentiable():
+            density, density_embedding = self.get_density(ray_samples)
+            outputs = self.get_outputs(ray_samples, density_embedding=density_embedding)
+            outputs[FieldHeadNames.DENSITY] = density
+            return outputs
+        if ray_samples.camera_indices is None:
+            raise AttributeError("Camera indices are not provided.")
+        density, rgb = self._kernel_forward(ray_samples)
+        return {FieldHeadNames.RGB: rgb, FieldHeadNames.DENSITY: density}
+
+    def _kernel_forward(self, ray_samples):
+        """One sdfb200_nerfacto_field_forward launch.  Ray mode when the samples carry this package's contiguous [R, S+1] bin buffer
+        (rays.make_ray_samples), point mode (positions and directions per sample) for any other RaySamples."""
+        lib = _lib.load()
+        dev = self.aabb.device
+        if dev.type != "cuda":
+            raise RuntimeError("sdfstudio_b200.TCNNNerfactoField runs on CUDA only (there is no CPU path)")
+        fr = ray_samples.frustums
+        shape = tuple(fr.starts.shape[:-1])
+        bins = getattr(ray_samples, "_euclid_bins", None)
+        if bins is not None and len(shape) == 2 and getattr(fr, "offsets", None) is None:
+            origins, directions = rays_of(ray_samples)
+            n_rows, S = origins.shape[0], bins.shape[1] - 1
+            cam_rows = ray_samples.camera_indices.reshape(n_rows, -1)[:, 0]
+        else:
+            origins = _lib.f32c(fr.get_positions().reshape(-1, 3))
+            directions = _lib.f32c(fr.directions.reshape(-1, 3))
+            bins, n_rows, S = None, origins.shape[0], 0
+            cam_rows = ray_samples.camera_indices.reshape(-1)
+        N = math.prod(shape)
+        mode = self._appearance_mode()
+        stride = self.appearance_embedding_dim
+        if mode == "camera":
+            app = _lib.f32c(self.embedding_appearance(cam_rows.long()).detach())
+        elif mode == "mean":
+            app, stride = _lib.f32c(self.embedding_appearance.mean(dim=0).detach()), 0
+        else:
+            app = None
+        density = torch.empty(N, device=dev, dtype=torch.float32)
+        rgb = torch.empty(N, 3, device=dev, dtype=torch.float32)
+        pre = torch.empty(N, device=dev, dtype=torch.float32)
+        nb, nh = self.mlp_base, self.mlp_head
+        p = nb.params.detach()
+        desc = nb.desc
+        desc.active_levels, desc.table_dtype = desc.n_levels, _lib.DT_F32
+        code = self._contraction_code()
+        aabb = _lib.f32c(self.aabb.detach()) if code == _lib.CONTRACT_NONE else None
+        _lib.check(lib.sdfb200_nerfacto_field_forward(desc, self._desc(S), p[nb.n_net:].data_ptr(), p.data_ptr(), nh.params.detach().data_ptr(),
+                                                      _lib.ptr(aabb), _lib.ptr(origins), _lib.ptr(directions), _lib.ptr(bins), n_rows, _lib.ptr(app),
+                                                      stride, density.data_ptr(), rgb.data_ptr(), pre.data_ptr(), None, _lib.stream_ptr()),
+                   "sdfb200_nerfacto_field_forward")
+        self._density_before_activation = pre.view(*shape, 1)
+        self._locations, self._positions_of_last_call = None, fr.get_positions
+        return density.view(*shape, 1), rgb.view(*shape, 3)
+
+    def _desc(self, n_samples: int) -> "_lib.NerfactoDesc":
+        d = _lib.NerfactoDesc()
+        nb, nh = self.mlp_base, self.mlp_head
+        d.hidden_dim, d.n_hidden_layers = nb.hidden_dim, nb.n_hidden_layers
+        d.hidden_dim_color, d.n_hidden_layers_color = nh.hidden_dim, nh.n_hidden_layers
+        d.geo_feat_dim, d.appearance_dim = self.geo_feat_dim, self.appearance_embedding_dim
+        d.contraction, d.n_samples = self._contraction_code(), n_samples
+        return d

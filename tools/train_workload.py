@@ -39,6 +39,46 @@ def make_angelo_field(dev, precision, log2_t=22, seed=0):
     return field.to(dev).train()
 
 
+def make_proposal_sampler(dev):
+    """ProposalNetworkSampler (256, 96 -> 48 samples) over two seeded HashMLPDensityFields; returns (sampler, density_fns)."""
+    import sdfstudio_b200 as sb
+
+    aabb = torch.tensor([[-1.0, -1, -1], [1, 1, 1]])
+    g = torch.Generator().manual_seed(1)
+    nets = []
+    for max_res in (64, 256):
+        f = sb.HashMLPDensityField(aabb, num_layers=2, hidden_dim=16, num_levels=5, max_res=max_res, log2_hashmap_size=17).to(dev).eval()
+        with torch.no_grad():
+            nb = f.mlp_base
+            nb.params[nb.n_net:] = ((torch.rand(nb.n_grid, generator=g) * 2 - 1) * 2.0).to(dev)
+        nets.append(f)
+    fns = [n.density_fn for n in nets]
+    sampler = sb.ProposalNetworkSampler(num_proposal_samples_per_ray=(256, 96), num_nerf_samples_per_ray=S_TRAIN, num_proposal_network_iterations=2,
+                                        use_uniform_sampler=False).train()
+    return sampler, fns
+
+
+class Step(torch.nn.Module):
+    """field + compositing + loss as ONE module so that DDP sees every parameter of the step.  `merge` is where a model with a background
+    field blends it into the field's alpha and rgb (tools/nerfacto_bg_bench.py); this workload has none."""
+
+    def __init__(self, field):
+        super().__init__()
+        self.field = field
+
+    def merge(self, rs, alpha, rgb):
+        return alpha, rgb
+
+    def forward(self, rs, target, white):
+        import sdfstudio_b200 as sb
+
+        fo = self.field(rs, return_alphas=True)
+        alpha, rgb = self.merge(rs, fo[sb.FieldHeadNames.ALPHA], fo[sb.FieldHeadNames.RGB])
+        out = sb.render_from_alphas(alpha, rgb, fo[sb.FieldHeadNames.NORMAL], rs, white, training=True)
+        eik = ((fo[sb.FieldHeadNames.GRADIENT].norm(2, dim=-1) - 1) ** 2).mean()
+        return (out["rgb"] - target).abs().mean() + 0.1 * eik
+
+
 def main(args):
     import torch.distributed as dist
     from torch.nn.parallel import DistributedDataParallel as DDP
@@ -57,32 +97,7 @@ def main(args):
     precision = "bf16x3" if args.precision == "auto" else args.precision
     torch.backends.cuda.matmul.allow_tf32 = True           # scripts/train.py:59 (only the small ATen leftovers are affected)
     field = make_angelo_field(dev, precision)
-    aabb = torch.tensor([[-1.0, -1, -1], [1, 1, 1]])
-    g = torch.Generator().manual_seed(1)
-    nets = []
-    for max_res in (64, 256):
-        f = sb.HashMLPDensityField(aabb, num_layers=2, hidden_dim=16, num_levels=5, max_res=max_res, log2_hashmap_size=17).to(dev).eval()
-        with torch.no_grad():
-            nb = f.mlp_base
-            nb.params[nb.n_net:] = ((torch.rand(nb.n_grid, generator=g) * 2 - 1) * 2.0).to(dev)
-        nets.append(f)
-    fns = [n.density_fn for n in nets]
-    sampler = sb.ProposalNetworkSampler(num_proposal_samples_per_ray=(256, 96), num_nerf_samples_per_ray=S_TRAIN, num_proposal_network_iterations=2,
-                                        use_uniform_sampler=False).train()
-
-    class Step(torch.nn.Module):
-        """field + compositing + loss as ONE module so that DDP sees every parameter of the step"""
-
-        def __init__(self, field):
-            super().__init__()
-            self.field = field
-
-        def forward(self, rs, target, white):
-            fo = self.field(rs, return_alphas=True)
-            out = sb.render_from_alphas(fo[sb.FieldHeadNames.ALPHA], fo[sb.FieldHeadNames.RGB], fo[sb.FieldHeadNames.NORMAL], rs, white, training=True)
-            eik = ((fo[sb.FieldHeadNames.GRADIENT].norm(2, dim=-1) - 1) ** 2).mean()
-            return (out["rgb"] - target).abs().mean() + 0.1 * eik
-
+    sampler, fns = make_proposal_sampler(dev)
     model = Step(field)
     if world > 1:
         model = DDP(model, device_ids=[local_rank], find_unused_parameters=True, gradient_as_bucket_view=True)
