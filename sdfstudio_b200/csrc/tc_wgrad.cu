@@ -10,6 +10,9 @@
 // MMAs of the current ones.  Two warpgroups: D[n, k] += sum_m A[m, n] B[m, k] with warpgroup w owning the rows n in [64 w, 64 w + 64)
 // of a 128-row chunk, N = K columns in n64 blocks, K = 16 points per instruction; bf16x3 = a0 b0 + a1 b0 + a0 b1.  The per-CTA
 // partial sums go to a workspace and are reduced by a second kernel in a fixed order (deterministic, unlike atomics).
+// The wgmma accumulator is not rounded to nearest: over ~20 k points per CTA (the angelo workload's 2.75 M rows) its error on sums that
+// do not cancel (non-negative activations) grows to 1.5e-4 relative.  So a CTA adds its accumulator into its workspace slot every
+// kWgSlice stages (a fixed slice of its points, a fixed order) and restarts from zero; the slot sums those slices in ordinary fp32.
 #include "tc_common.cuh"
 
 namespace sdfb200 {
@@ -20,6 +23,7 @@ constexpr int kWgThreads = 256;     // two warpgroups: staging + MMAs
 constexpr int kWgPts = 32;          // points per stage
 constexpr int kWgRowsA = 128;       // rows of the A operand tile (N chunk, zero padded): the 128-row A layout of tc_common.cuh
 constexpr int kWgRowsB = 256;       // rows of the B operand tile (K chunk, zero padded)
+constexpr int kWgSlice = 32;        // stages (of kWgPts points) accumulated in the wgmma registers before they are added to the workspace
 constexpr uint32_t kWgPlaneA = (kWgPts / 8) * kWgRowsA * 16;          // 8 KB
 constexpr uint32_t kWgPlaneB = (kWgPts / 8) * kWgRowsB * 16;          // 16 KB
 constexpr uint32_t kWgStageBytes = 2 * (kWgPlaneA + kWgPlaneB);       // both operands, both planes
@@ -73,6 +77,32 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_tc_wgrad(const WgArgs a) {
   for (int c = 0; c < 4; ++c)
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+  // this thread's fragment of the CTA's workspace slot: the first spill stores, later ones add (zeros for a CTA without points)
+  float* out = a.partial + (size_t)blockIdx.x * 256 * 256;
+  const int r0 = frag_row0(wg * 64, t), c2 = frag_cq(t);
+  bool spilled = false;
+  auto spill = [&]() {
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int n = frag_row(r0, i), k = frag_col(c2, c, i);
+        if (c < nch) {
+          float2* dst = reinterpret_cast<float2*>(out + (size_t)n * 256 + k);
+          float2 v = make_float2(acc[c][i], acc[c][i + 1]);
+          if (spilled) {
+            const float2 prev = *dst;
+            v.x += prev.x;
+            v.y += prev.y;
+          }
+          *dst = v;
+        }
+        acc[c][i] = 0.f;
+        acc[c][i + 1] = 0.f;
+      }
+    }
+    spilled = true;
+  };
   int it = 0;
   if (blockIdx.x < nblk) stage(blockIdx.x, smem);
   __syncthreads();
@@ -93,19 +123,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) k_tc_wgrad(const WgArgs a) {
       wg_wait<0>();
       wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]); wg_fence_acc(acc[3]);
     }
+    if ((it + 1) % kWgSlice == 0 && blk + gridDim.x < nblk) spill();
     __syncthreads();
   }
-  // ---------------- partial sums of this CTA -> workspace (zeros for a CTA without points) ----------------
-  float* out = a.partial + (size_t)blockIdx.x * 256 * 256;
-  const int r0 = frag_row0(wg * 64, t), c2 = frag_cq(t);
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int n = frag_row(r0, i), k = frag_col(c2, c, i);
-      if (c < nch) *reinterpret_cast<float2*>(out + (size_t)n * 256 + k) = make_float2(acc[c][i], acc[c][i + 1]);
-    }
-  }
+  spill();
 }
 
 // C[n0 + n, k0 + k] (+)= sum_g partial[g][n][k]   in a fixed order
