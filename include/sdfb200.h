@@ -222,6 +222,45 @@ int sdfb200_nerfacto_field_forward(const sdfb200_grid_t* grid, const sdfb200_ner
                                    float* rgb, float* pre_activation, float* geo_feature, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Vanilla NeRF background field (background_model="mlp" of the surface presets, models/base_surface_model.py:188-201): the eval
+ * forward of NeRFField (nerfstudio/fields/vanilla_nerf_field.py:91-114 through fields/base_field.py:104-123) as ONE launch of the
+ * fused tensor-core kernel k_nerf_field_tc (precision bf16x3 or bf16).
+ * Family: base MLP 8 x 256 ReLU with the skip at layer 4, head MLP 2 x 128 ReLU, NeRFEncoding position / direction encodings with
+ * 0..10 frequencies (the host passes the frequencies 2**linspace(min, max, n) as torch computes them), with or without the input,
+ * positional encoding 1..63 columns wide.  sdfb200_nerf_field_in_family tells whether a descriptor is in it; the other entry points
+ * return SDFB200_EUNSUPPORTED (packed_bytes: 0) for one that is not.
+ * Geometry: ray mode (n_samples = S > 0): origins / directions [n_rows,3], bins [n_rows,S+1] euclidean edges, positions = midpoints
+ * origins + directions * (start + end) / 2, N = n_rows * S.  Point mode (n_samples = 0): origins = positions [n_rows,3], directions
+ * [n_rows,3], N = n_rows.  Then `contraction`.
+ * Pack: weights[12] / biases[12] = nn.Linear weight [out, in] / bias [out] of mlp_base.layers.0..7, mlp_head.layers.0..1,
+ * field_output_density.net, field_heads.0.net (fp32 device pointers), into `packed` (sdfb200_nerf_field_packed_bytes).
+ * Forward: density [N] = softplus(.), rgb [N,3] = sigmoid(.).  One launch, no workspace.
+ * ------------------------------------------------------------------------------------------------------------- */
+#define SDFB200_NERF_MAX_FREQS 10
+typedef struct sdfb200_nerf_field {
+  int32_t base_layers;            /* mlp_base: number of Linear layers (8) */
+  int32_t base_width;             /* 256 */
+  int32_t skip_layer;             /* the layer that takes cat([encoding, x]): 4 */
+  int32_t head_layers;            /* mlp_head: number of Linear layers (2) */
+  int32_t head_width;             /* 128 */
+  int32_t pe_frequencies;         /* position NeRFEncoding: num_frequencies (0..10) */
+  int32_t pe_include_input;
+  float pe_freqs[SDFB200_NERF_MAX_FREQS];
+  int32_t dir_frequencies;        /* direction NeRFEncoding */
+  int32_t dir_include_input;
+  float dir_freqs[SDFB200_NERF_MAX_FREQS];
+  int32_t contraction;            /* SDFB200_CONTRACT_* */
+  int32_t n_samples;              /* samples per ray (ray mode), 0 = point mode */
+  int32_t precision;              /* SDFB200_PRECISION_BF16X3 or _BF16 */
+} sdfb200_nerf_field_t;
+
+int sdfb200_nerf_field_in_family(const sdfb200_nerf_field_t* f);
+size_t sdfb200_nerf_field_packed_bytes(const sdfb200_nerf_field_t* f);
+int sdfb200_nerf_field_pack(const sdfb200_nerf_field_t* f, const float* const* weights, const float* const* biases, void* packed, void* stream);
+int sdfb200_nerf_field_forward(const sdfb200_nerf_field_t* f, const void* packed, const float* origins, const float* directions, const float* bins,
+                               int64_t n_rows, float* density, float* rgb, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Ray samplers.  Replace nerfstudio/model_components/ray_samplers.py.  A sample set is a pair of bin-edge buffers
  * [R, S+1]: `spacing` (normalised) and `euclid` (distance along the ray), cf. cameras/rays.py:295-339.
  * ------------------------------------------------------------------------------------------------------------- */
@@ -449,7 +488,7 @@ const char* sdfb200_last_error_string(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches). */
 int64_t sdfb200_launch_count(void);
 /* sizeof() of the ABI structs (0 grid, 1 field, 2 field_params, 3 field_in, 4 field_out, 5 render_out, 6 field_render,
- * 7 nerfacto): lets a binding
+ * 7 nerfacto, 8 nerf_field): lets a binding
  * verify its struct mirrors before the first call. */
 size_t sdfb200_struct_size(int32_t which);
 

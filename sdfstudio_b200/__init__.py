@@ -4,6 +4,7 @@ Host side mirrors the reference's plug points (SURVEY.md section 8b):
   encoding.Encoding            <- tinycudann.Encoding (HashGrid)        nerfstudio/fields/sdf_field.py:230-241
   sdf_field.SDFField           <- nerfstudio.fields.sdf_field.SDFField
   nerfacto_field.TCNNNerfactoField <- nerfstudio.fields.nerfacto_field.TCNNNerfactoField (background_model="grid")
+  nerf_field.NeRFField         <- nerfstudio.fields.vanilla_nerf_field.NeRFField (background_model="mlp")
   ray_samplers.*               <- nerfstudio.model_components.ray_samplers
   packed.*                     <- nerfacc 0.3.5 render_weight_from_alpha / accumulate_along_rays (neus-acc)
   renderers.*                  <- nerfstudio.model_components.renderers
@@ -16,6 +17,7 @@ from .density_fields import HashMLPDensityField  # noqa: F401
 from .encoding import Encoding, HashEncoding  # noqa: F401
 from .field_heads import FieldHeadNames  # noqa: F401
 from .nerfacto_field import TCNNNerfactoField  # noqa: F401
+from .nerf_field import NeRFEncoding, NeRFField  # noqa: F401
 from .rays import Frustums, RayBundle, RaySamples  # noqa: F401
 from .ray_samplers import (  # noqa: F401
     ErrorBoundedSampler, LinearDisparitySampler, LogSampler, NeuSAccSampler, NeuSSampler, PDFSampler, ProposalNetworkSampler, Sampler, SpacedSampler,

@@ -79,6 +79,18 @@ class NerfactoDesc(C.Structure):
                                          "appearance_dim", "contraction", "n_samples")]  # fmt: skip
 
 
+NERF_MAX_FREQS = 10
+
+
+class NerfFieldDesc(C.Structure):
+    _fields_ = [
+        ("base_layers", C.c_int32), ("base_width", C.c_int32), ("skip_layer", C.c_int32), ("head_layers", C.c_int32), ("head_width", C.c_int32),
+        ("pe_frequencies", C.c_int32), ("pe_include_input", C.c_int32), ("pe_freqs", C.c_float * NERF_MAX_FREQS),
+        ("dir_frequencies", C.c_int32), ("dir_include_input", C.c_int32), ("dir_freqs", C.c_float * NERF_MAX_FREQS),
+        ("contraction", C.c_int32), ("n_samples", C.c_int32), ("precision", C.c_int32),
+    ]  # fmt: skip
+
+
 _lib = None
 _lock = threading.Lock()
 
@@ -105,7 +117,11 @@ _PROTOS = {
     "sdfb200_density_field_forward": (C.c_int, [C.POINTER(GridDesc), _vp, _vp, _i32, _i32, _i32, _vp, _vp, _i64, _vp, _vp, _vp]),
     "sdfb200_nerfacto_field_forward": (C.c_int, [C.POINTER(GridDesc), C.POINTER(NerfactoDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64,
                                                  _vp, _vp, _vp, _vp, _vp]),
-    "sdfb200_spaced_bins": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "sdfb200_nerf_field_in_family": (C.c_int, [C.POINTER(NerfFieldDesc)]),
+    "sdfb200_nerf_field_packed_bytes": (_sz, [C.POINTER(NerfFieldDesc)]),
+    "sdfb200_nerf_field_pack": (C.c_int, [C.POINTER(NerfFieldDesc), C.POINTER(_vp), C.POINTER(_vp), _vp, _vp]),
+    "sdfb200_nerf_field_forward": (C.c_int, [C.POINTER(NerfFieldDesc), _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp]),
+    "sdfb200_spaced_bins":(C.c_int, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _vp, _vp]),
     "sdfb200_bins_to_euclid": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "sdfb200_pdf_sample": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _f32, _f32, _i32, _vp, _vp, _vp]),
     "sdfb200_merge_bins": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
@@ -182,7 +198,7 @@ def load():
             fn = getattr(lib, name)
             fn.restype = res
             fn.argtypes = args
-        for which, st in enumerate((GridDesc, FieldDesc, FieldParams, FieldIn, FieldOut, RenderOut, FieldRender, NerfactoDesc)):
+        for which, st in enumerate((GridDesc, FieldDesc, FieldParams, FieldIn, FieldOut, RenderOut, FieldRender, NerfactoDesc, NerfFieldDesc)):
             if lib.sdfb200_struct_size(which) != C.sizeof(st):
                 raise Sdfb200Error(f"ABI mismatch: sizeof({st.__name__}) = {C.sizeof(st)} but the library says {lib.sdfb200_struct_size(which)}")
         _lib = lib

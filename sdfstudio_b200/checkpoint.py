@@ -1,5 +1,5 @@
 """Loading existing sdfstudio checkpoints into the drop-in modules (SURVEY.md section 8f row 4): the SDF field, the proposal networks
-and the grid background field.
+and the grid and mlp background fields.
 
 A reference ``step-*.ckpt`` (engine/trainer.py:276-297) is ``{"step", "pipeline", "optimizers", "schedulers", "scalers"}`` where
 ``pipeline`` is ``Pipeline.state_dict()``: the field's tensors sit under ``_model.field.`` (``module.`` in front when the pipeline
@@ -13,6 +13,8 @@ was DDP-wrapped, pipelines/base_pipeline.py:426-439).  SDFField keeps the refere
 from typing import Dict, Tuple
 
 import torch
+
+from .nerf_field import NeRFField
 
 FIELD_PREFIX = "_model.field."
 
@@ -81,14 +83,22 @@ _EMPTY_PARAMS = ("direction_encoding.params", "position_encoding.params")
 
 
 def load_background_field_checkpoint(field, loaded_state, prefix: str = BACKGROUND_PREFIX, strict: bool = True) -> Tuple[list, list]:
-    """Load the ``background_model="grid"`` field of a reference neus-facto-angelo / bakedangelo checkpoint (``TCNNNerfactoField``,
-    nerfstudio/fields/nerfacto_field.py:86-221) into a ``sdfstudio_b200.TCNNNerfactoField``.  ``mlp_base.params`` / ``mlp_head.params``
+    """Load the background field of a reference checkpoint.  ``background_model="mlp"`` (``NeRFField``, vanilla_nerf_field.py:52-89):
+    the entries keep the reference's names and shapes, so this is ``load_state_dict`` after the prefix strip.
+    ``background_model="grid"`` (neus-facto-angelo / bakedangelo, ``TCNNNerfactoField``, nerfstudio/fields/nerfacto_field.py:86-221) into
+    a ``sdfstudio_b200.TCNNNerfactoField``: ``mlp_base.params`` / ``mlp_head.params``
     are tiny-cuda-nn's flat vectors (fp16-stored ones are cast to fp32); their lengths are checked, the ordering inside them follows
     tcnn's published layout (UNPINNED).  The zero-length ``params`` of the parameter-free encodings may be present or absent.
     Returns (missing, unexpected); with ``strict`` any other mismatch raises."""
     if isinstance(loaded_state, (str, bytes)) or hasattr(loaded_state, "__fspath__"):
         loaded_state = torch.load(loaded_state, map_location="cpu")
     sd = extract_state(loaded_state, prefix)
+    sd = {k: (v.to(torch.float32) if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in sd.items()}
+    if isinstance(field, NeRFField):
+        missing, unexpected = field.load_state_dict(sd, strict=False)
+        if strict and (missing or unexpected):
+            raise RuntimeError(f"checkpoint does not match the background field: missing {list(missing)}, unexpected {list(unexpected)}")
+        return list(missing), list(unexpected)
     flats = {}
     for key, knobs in _FLAT_KNOBS.items():
         if key not in sd:
@@ -102,7 +112,6 @@ def load_background_field_checkpoint(field, loaded_state, prefix: str = BACKGROU
         v = sd.pop(key, None)
         if v is not None and v.numel() != 0:
             raise ValueError(f"{key} has {v.numel()} entries, the parameter-free encoding has none")
-    sd = {k: (v.to(torch.float32) if torch.is_tensor(v) and v.is_floating_point() else v) for k, v in sd.items()}
     with torch.no_grad():
         for key, flat in flats.items():
             p = field.get_parameter(key)

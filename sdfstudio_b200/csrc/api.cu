@@ -138,6 +138,7 @@ extern "C" size_t sdfb200_struct_size(int32_t which) {
     case 5: return sizeof(sdfb200_render_out_t);
     case 6: return sizeof(sdfb200_field_render_t);
     case 7: return sizeof(sdfb200_nerfacto_t);
+    case 8: return sizeof(sdfb200_nerf_field_t);
     default: return 0;
   }
 }

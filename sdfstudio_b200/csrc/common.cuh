@@ -83,6 +83,18 @@ __device__ __forceinline__ float dsoftplus100_from_h(float h) { return -expm1f(-
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// SceneContraction (spatial_distortions.py:66-73): x <- (2 - 1/|x|) * (x/|x|) where |x| >= 1, |x| the L-inf or L2 norm.  Every
+// operation is rounded on its own (no FMA contraction), so the result is the reference's fp32 one.
+__device__ __forceinline__ void scene_contract(int contraction, float& px, float& py, float& pz) {
+  if (contraction == SDFB200_CONTRACT_NONE) return;
+  const float mag = contraction == SDFB200_CONTRACT_LINF ? fmaxf(fabsf(px), fmaxf(fabsf(py), fabsf(pz)))
+                                                         : sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
+  if (mag >= 1.f) {
+    const float k = __fsub_rn(2.f, __fdiv_rn(1.f, mag));
+    px = __fmul_rn(k, __fdiv_rn(px, mag)); py = __fmul_rn(k, __fdiv_rn(py, mag)); pz = __fmul_rn(k, __fdiv_rn(pz, mag));
+  }
+}
+
 // float atomic min / max by compare-and-swap (used for the batch-global steps.min()/max() of DepthRenderer, renderers.py:257)
 __device__ __forceinline__ void atomic_min_float(float* addr, float v) {
   int* ia = reinterpret_cast<int*>(addr);

@@ -111,15 +111,7 @@ __global__ void __launch_bounds__(256) k_field_inputs(const InputArgs a) {
   } else {
     px = __ldg(a.origins + gi * 3 + 0); py = __ldg(a.origins + gi * 3 + 1); pz = __ldg(a.origins + gi * 3 + 2);
   }
-  if (a.contraction != SDFB200_CONTRACT_NONE) {
-    // spatial_distortions.py:66-73: x <- (2 - 1/|x|) * (x/|x|) where |x| >= 1
-    float mag = a.contraction == SDFB200_CONTRACT_LINF ? fmaxf(fabsf(px), fmaxf(fabsf(py), fabsf(pz)))
-                                                        : sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
-    if (mag >= 1.f) {
-      const float k = __fsub_rn(2.f, __fdiv_rn(1.f, mag));
-      px = __fmul_rn(k, __fdiv_rn(px, mag)); py = __fmul_rn(k, __fdiv_rn(py, mag)); pz = __fmul_rn(k, __fdiv_rn(pz, mag));
-    }
-  }
+  scene_contract(a.contraction, px, py, pz);
   if (lane == 0) {
     if (a.points_norm) a.points_norm[gi] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
     if (a.points_out) { a.points_out[gi * 3] = px; a.points_out[gi * 3 + 1] = py; a.points_out[gi * 3 + 2] = pz; }

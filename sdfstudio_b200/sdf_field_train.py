@@ -29,11 +29,16 @@ _OFF_AXIS = [
 ]  # fmt: skip
 
 
-def nerf_encoding(x, num_frequencies: int, max_exp: float, include_input: bool, off_axis: bool = False):
-    """NeRFEncoding.forward (encodings.py:167-208), min_freq_exp = 0."""
-    freqs = 2 ** torch.linspace(0.0, max_exp, num_frequencies, device=x.device)
+def nerf_frequencies(min_exp: float, max_exp: float, num_frequencies: int) -> torch.Tensor:
+    """The encoding's frequencies 2**linspace(min, max, n), computed on the CPU as NeRFEncoding.forward does (encodings.py:183)."""
+    return 2 ** torch.linspace(min_exp, max_exp, num_frequencies)
+
+
+def nerf_encoding(x, num_frequencies: int, max_exp: float, include_input: bool, off_axis: bool = False, min_exp: float = 0.0):
+    """NeRFEncoding.forward (encodings.py:167-208)."""
+    freqs = nerf_frequencies(min_exp, max_exp, num_frequencies).to(x.device)
     base = x @ torch.tensor(_OFF_AXIS, device=x.device, dtype=x.dtype).T if off_axis else x
-    scaled = (base[..., None] * freqs).reshape(*base.shape[:-1], -1)
+    scaled = (base[..., None] * freqs).reshape(*base.shape[:-1], base.shape[-1] * num_frequencies)
     enc = torch.sin(torch.cat([scaled, scaled + torch.pi / 2.0], dim=-1))
     return torch.cat([enc, x], dim=-1) if include_input else enc
 

@@ -4,8 +4,10 @@
 1024-ray Python chunk loop ``Model.get_outputs_for_camera_ray_bundle`` (models/base_model.py:165-189) by large chunks
 (default 65 536 rays per launch sequence) and per-rank contiguous ray slices (parallel.py).
 
-This is host orchestration only; the background model, the losses and the training loop stay with sdfstudio.
+With ``field_background`` (NeRFField, TCNNNerfactoField or any field with the ``Field.forward`` contract) the renderer also runs the
+background branch of base_surface_model.py:313-328.  This is host orchestration only; the losses and the training loop stay with sdfstudio.
 """
+import copy
 from typing import Dict, Optional
 
 import torch
@@ -13,14 +15,17 @@ from torch import nn
 
 from . import parallel
 from .field_heads import FieldHeadNames
-from .ray_samplers import ErrorBoundedSampler, NeuSSampler
-from .renderers import render_all, render_from_alphas
+from .ray_samplers import ErrorBoundedSampler, LinearDisparitySampler, NeuSSampler
+from .renderers import RGBRenderer, render_all, render_from_alphas
 
 
 class SurfaceRenderer(nn.Module):
-    """``kind="neus"``: NeuSSampler + alpha compositing; ``kind="volsdf"``: ErrorBoundedSampler + Laplace-density weights."""
+    """``kind="neus"``: NeuSSampler + alpha compositing; ``kind="volsdf"``: ErrorBoundedSampler + Laplace-density weights.
+    ``field_background``: the background model, evaluated on ``num_samples_outside`` samples per ray between the far plane and
+    ``far_plane_bg`` (SurfaceModelConfig.num_samples_outside / far_plane_bg) and merged as ``rgb += bg_transmittance * rgb_bg``."""
 
-    def __init__(self, field, sampler, collider=None, kind: str = "neus", background_color="white", eval_num_rays_per_chunk: int = 65536):
+    def __init__(self, field, sampler, collider=None, kind: str = "neus", background_color="white", eval_num_rays_per_chunk: int = 65536,
+                 field_background=None, num_samples_outside: int = 32, far_plane_bg: float = 1000.0):
         super().__init__()
         if kind not in ("neus", "volsdf"):
             raise ValueError("kind must be 'neus' or 'volsdf'")
@@ -29,6 +34,9 @@ class SurfaceRenderer(nn.Module):
         self.field, self.sampler, self.collider, self.kind = field, sampler, collider, kind
         self.background_color = background_color
         self.eval_num_rays_per_chunk = eval_num_rays_per_chunk
+        self.field_background = field_background
+        self.far_plane_bg = far_plane_bg
+        self.sampler_bg = LinearDisparitySampler(num_samples=num_samples_outside) if field_background is not None else None
 
     def _background(self, device):
         if isinstance(self.background_color, str) and self.background_color in ("white", "black"):
@@ -44,8 +52,19 @@ class SurfaceRenderer(nn.Module):
         field_outputs = self.field(ray_samples)
         return {"ray_samples": ray_samples, "field_outputs": field_outputs, "eik_points": eik_points}
 
+    def background_rgb(self, ray_bundle, background) -> torch.Tensor:
+        """base_surface_model.py:317-326: the background field's colour of each ray, sampled from the far plane to far_plane_bg.  The
+        caller's bundle is left as it is."""
+        bundle = copy.copy(ray_bundle)
+        bundle.nears = ray_bundle.fars
+        bundle.fars = torch.ones_like(ray_bundle.fars) * self.far_plane_bg
+        ray_samples_bg = self.sampler_bg(bundle)
+        field_outputs_bg = self.field_background(ray_samples_bg)
+        weights_bg = ray_samples_bg.get_weights(field_outputs_bg[FieldHeadNames.DENSITY])
+        return RGBRenderer(background_color=background).train(self.training)(field_outputs_bg[FieldHeadNames.RGB], weights_bg)
+
     def get_outputs(self, ray_bundle) -> Dict[str, torch.Tensor]:
-        """base_surface_model.py:292-365 without the background model / patch warping branches."""
+        """base_surface_model.py:292-365 without the patch warping branch."""
         if self.collider is not None:
             ray_bundle = self.collider(ray_bundle)
         s = self.sample_and_forward_field(ray_bundle)
@@ -53,10 +72,17 @@ class SurfaceRenderer(nn.Module):
         bg = self._background(ray_bundle.origins.device)
         if self.kind == "neus":
             out = render_from_alphas(fo[FieldHeadNames.ALPHA], fo[FieldHeadNames.RGB], fo[FieldHeadNames.NORMAL], rs, bg, training=self.training)
-        else:
+        elif self.field_background is None:
             weights = rs.get_weights(fo[FieldHeadNames.DENSITY])
             out = render_all(weights, fo[FieldHeadNames.RGB], fo[FieldHeadNames.NORMAL], rs, bg, training=self.training)
             out["weights"] = weights
+        else:                                                                        # volsdf.py:67-68
+            weights, transmittance = rs.get_weights_and_transmittance(fo[FieldHeadNames.DENSITY])
+            out = render_all(weights, fo[FieldHeadNames.RGB], fo[FieldHeadNames.NORMAL], rs, bg, training=self.training)
+            out["weights"] = weights
+            out["bg_transmittance"] = transmittance[:, -1, :]
+        if self.field_background is not None:
+            out["rgb"] = out["rgb"] + out["bg_transmittance"] * self.background_rgb(ray_bundle, bg)
         dn = getattr(ray_bundle, "directions_norm", None)
         if dn is not None:
             out["depth"] = out["depth"] / dn                                        # base_surface_model.py:303-304
