@@ -185,7 +185,8 @@ struct Slot {
 #ifdef SDFB200_TC_TIMING
 // CTA 0, first 16 tiles, row = tile: clock64() of consumer thread 0 at [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring
 // order), [8] the tile's geo input has landed (a full; [8] - [0] is the consumers' wait for the encoder), [15] tile end = end of EC1
-// (head inputs handed over); cycle sums over the tile of [9] consumer thread 0 waiting for weights (ring full), [10] the producer
+// (head inputs handed over), [18..23] end of the epilogues E0, E1, EB1, EB0, h2 reload, EC0 (before the SYNC_A that hands their A
+// operand to the next layer's MMAs); cycle sums over the tile of [9] consumer thread 0 waiting for weights (ring full), [10] the producer
 // waiting for a free ring slot (ring empty), [12] encoder thread 0 busy staging the tile, [13] encoder thread 0 waiting for its staging
 // slot (enc empty), [14] encoder thread 0 (heads warp) running the tile's heads / compositing, [16] consumer thread 0 waiting for the
 // tile's head-input buffer (hs empty), [17] the heads warp waiting for the tile's head inputs (hs full)
@@ -293,19 +294,43 @@ __device__ __forceinline__ uint32_t unorm16x2_encode(float s0, float s1) {
 __device__ __forceinline__ float unorm16_lo(uint32_t w) { return __fsub_rn(__uint_as_float(__byte_perm(w, 0x4B00u, 0x5410)), 8388608.0f) * (1.0f / 65535.0f); }
 __device__ __forceinline__ float unorm16_hi(uint32_t w) { return __fsub_rn(__uint_as_float(__byte_perm(w, 0x4B00u, 0x5432)), 8388608.0f) * (1.0f / 65535.0f); }
 
+// The epilogue parameters of the thread's columns in n64 block c, one float2 (columns cq, cq + 1) per 8-column block: element pairs
+// i, i + 2 of the accumulator use v[i >> 2].  The epilogues load a block's parameters into registers before they store any of its
+// results: `prm` and the A operand are both shared memory, so a parameter load placed after an A store cannot be moved above it, and
+// loading per pair would make every pair wait for the one before (load -> softplus -> split -> store -> next load).
+// The epilogues walk the four n64 blocks of the accumulator in a rolled loop: every pass works on acc[0], then moves blocks 1..3 down
+// by one (96 register moves).  Unrolled, the seven epilogues were ~9 k instructions of straight-line code per tile that every consumer
+// warp fetched once, next to the encoder warps' code; rolled, each is one block's worth, run four times.  The accumulator is consumed:
+// the layer after an epilogue starts from zero.
+__device__ __forceinline__ void acc_shift(float (&acc)[4][32]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[c][i] = acc[c + 1][i];
+  }
+}
+
+template <int N>
+__device__ __forceinline__ void load_prm_block(const float* prow, int cq, int c, int j0, float2 (&v)[N]) {
+#pragma unroll
+  for (int j = 0; j < N; ++j) v[j] = *reinterpret_cast<const float2*>(prow + frag_col(cq, c, 4 * (j0 + j)));
+}
+
 // E0 (after G0): h1 = softplus(z1) -> A ; softplus'(z1) -> scratch
 template <int P>
-__device__ __forceinline__ void epi_e0(const TileCtx& x, const float (&acc)[4][32]) {
+__device__ __forceinline__ void epi_e0(const TileCtx& x, float (&acc)[4][32]) {
   const float* p_bg0 = x.prm[PRM_B_G0];
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
+#pragma unroll 1
+  for (int c = 0; c < 4; ++c, acc_shift(acc)) {
+    float2 bias[8];
+    load_prm_block(p_bg0, x.cq, c, 0, bias);
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const float2 b2 = *reinterpret_cast<const float2*>(p_bg0 + col);
+      const float2 b2 = bias[i >> 2];
       float h0, h1, s0, s1;
-      softplus100_fast(acc[c][i] + b2.x, h0, s0);
-      softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
+      softplus100_fast(acc[0][i] + b2.x, h0, s0);
+      softplus100_fast(acc[0][i + 1] + b2.y, h1, s1);
       store_a_pair<P>(x.abuf, kAPlane, row, col, h0, h1);
       if (x.a.mode != 0) x.sig_s[x.unit(c, i)] = unorm16x2_encode(s0, s1);
     }
@@ -314,23 +339,25 @@ __device__ __forceinline__ void epi_e0(const TileCtx& x, const float (&acc)[4][3
 
 // E1 (after G1): sdf = W2[0,:] . h2 + b (fp32) -> output / heads ; h2 -> scratch planes ; g2 = W2[0,:] * softplus'(z2) -> A
 template <int P>
-__device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, const float (&acc)[4][32]) {
+__device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, float (&acc)[4][32]) {
   const TcArgs& a = x.a;
   const float* p_bg1 = x.prm[PRM_B_G1];
   const float* p_wg2 = x.prm[PRM_W_G2];
   // one partial dot per accumulator row (r0, r0 + 8) as named scalars: an array indexed by the thread-dependent row below would live
   // in local memory, written back after every FMA because the generic stores in between may alias it
   float sp0 = 0.f, sp1 = 0.f;
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
+#pragma unroll 1
+  for (int c = 0; c < 4; ++c, acc_shift(acc)) {
+    float2 bias[2], wrow[2];   // parameters of two 8-column blocks (4 pairs) at a time: whole n64 blocks spill at P = 1
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
+      if (i % 8 == 0) { load_prm_block(p_bg1, x.cq, c, i >> 2, bias); load_prm_block(p_wg2, x.cq, c, i >> 2, wrow); }
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const float2 b2 = *reinterpret_cast<const float2*>(p_bg1 + col);
-      const float2 w2 = *reinterpret_cast<const float2*>(p_wg2 + col);
+      const float2 b2 = bias[(i >> 2) & 1];
+      const float2 w2 = wrow[(i >> 2) & 1];
       float h0, h1, s0, s1;
-      softplus100_fast(acc[c][i] + b2.x, h0, s0);
-      softplus100_fast(acc[c][i + 1] + b2.y, h1, s1);
+      softplus100_fast(acc[0][i] + b2.x, h0, s0);
+      softplus100_fast(acc[0][i + 1] + b2.y, h1, s1);
       float& sp = frag_half(i) ? sp1 : sp0;
       sp = fmaf(w2.x, h0, sp);
       sp = fmaf(w2.y, h1, sp);
@@ -355,16 +382,28 @@ __device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, const float (
   }
 }
 
-// EB1 (after B1): g1 = (W1^T g2) * softplus'(z1) -> A
+// EB1 (after B1): g1 = (W1^T g2) * softplus'(z1) -> A.  The 16 softplus' words of n64 block c + 1 are loaded (from L2) while block c is
+// multiplied and stored, so their latency is paid once per tile rather than once per word.
 template <int P>
-__device__ __forceinline__ void epi_eb1(const TileCtx& x, const float (&acc)[4][32]) {
+__device__ __forceinline__ void epi_eb1(const TileCtx& x, float (&acc)[4][32]) {
+  uint32_t sw[16], sw_next[16];
 #pragma unroll
-  for (int c = 0; c < 4; ++c) {
+  for (int k = 0; k < 16; ++k) sw[k] = x.sig_s[x.unit(0, 2 * k)];
+#pragma unroll 1
+  for (int c = 0; c < 4; ++c, acc_shift(acc)) {
+    if (c < 3) {
+#pragma unroll
+      for (int k = 0; k < 16; ++k) sw_next[k] = x.sig_s[x.unit(c + 1, 2 * k)];
+    }
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const uint32_t sw = x.sig_s[x.unit(c, i)];
-      store_a_pair<P>(x.abuf, kAPlane, row, col, acc[c][i] * unorm16_lo(sw), acc[c][i + 1] * unorm16_hi(sw));
+      const uint32_t w = sw[i >> 1];
+      store_a_pair<P>(x.abuf, kAPlane, row, col, acc[0][i] * unorm16_lo(w), acc[0][i + 1] * unorm16_hi(w));
+    }
+    if (c < 3) {
+#pragma unroll
+      for (int k = 0; k < 16; ++k) sw[k] = sw_next[k];
     }
   }
 }
@@ -451,7 +490,7 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
 // C0 h2 operand: h2 (bf16 planes, saved by E1) back from the scratch over the misc columns that C0's first part has consumed
 template <int P>
 __device__ __forceinline__ void reload_h2(const TileCtx& x) {
-#pragma unroll
+#pragma unroll 1
   for (int c = 0; c < 4; ++c) {
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
@@ -464,26 +503,28 @@ __device__ __forceinline__ void reload_h2(const TileCtx& x) {
 
 // EC0 (after C0): relu -> A
 template <int P>
-__device__ __forceinline__ void epi_ec0(const TileCtx& x, const float (&acc)[4][32]) {
+__device__ __forceinline__ void epi_ec0(const TileCtx& x, float (&acc)[4][32]) {
   const float* p_bc0 = x.prm[PRM_B_C0];
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
+#pragma unroll 1
+  for (int c = 0; c < 4; ++c, acc_shift(acc)) {
+    float2 bias[8];
+    load_prm_block(p_bc0, x.cq, c, 0, bias);
 #pragma unroll
     for (int i = 0; i < 32; i += 2) {
       const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const float2 b2 = *reinterpret_cast<const float2*>(p_bc0 + col);
-      store_a_pair<P>(x.abuf, kAPlane, row, col, fmaxf(acc[c][i] + b2.x, 0.f), fmaxf(acc[c][i + 1] + b2.y, 0.f));
+      const float2 b2 = bias[i >> 2];
+      store_a_pair<P>(x.abuf, kAPlane, row, col, fmaxf(acc[0][i] + b2.x, 0.f), fmaxf(acc[0][i + 1] + b2.y, 0.f));
     }
   }
 }
 
 // EC1 (after C1): relu, last colour layer (256 -> 3) as fp32 dots -> heads
-__device__ __forceinline__ void epi_ec1(const TileCtx& x, const float (&acc)[4][32]) {
+__device__ __forceinline__ void epi_ec1(const TileCtx& x, float (&acc)[4][32]) {
   const float* p_bc1 = x.prm[PRM_B_C1];
   const float (*p_wc2)[256] = x.prm + PRM_W_C2;
   float r0r = 0.f, r0g = 0.f, r0b = 0.f, r1r = 0.f, r1g = 0.f, r1b = 0.f;   // rows r0, r0 + 8 (named scalars, see epi_e1)
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
+#pragma unroll 1
+  for (int c = 0; c < 4; ++c, acc_shift(acc)) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int col = frag_col(x.cq, c, i);
@@ -491,7 +532,7 @@ __device__ __forceinline__ void epi_ec1(const TileCtx& x, const float (&acc)[4][
       float& rr = h ? r1r : r0r;
       float& rg = h ? r1g : r0g;
       float& rb = h ? r1b : r0b;
-      const float v = fmaxf(acc[c][i] + p_bc1[col], 0.f);
+      const float v = fmaxf(acc[0][i] + p_bc1[col], 0.f);
       rr = fmaf(p_wc2[0][col], v, rr);
       rg = fmaf(p_wc2[1][col], v, rg);
       rb = fmaf(p_wc2[2][col], v, rb);
@@ -760,6 +801,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     TC_STAMP(8);
     LAYER(L_G0, true);
     epi_e0<P>(x, acc);
+    TC_STAMP(18);
     SYNC_A();
     LAYER(L_G1, true);
     if (a.mode == 0) {                         // sdf only: A is free for the next tile's geo input
@@ -773,20 +815,25 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
       if (tid == 0) TC_PUT(tile_no, 16, hs_waited);
     }
     epi_e1<P>(x, tile, acc);
+    TC_STAMP(19);
     SYNC_A();
     LAYER(L_B1, true);
     epi_eb1<P>(x, acc);
+    TC_STAMP(20);
     SYNC_A();
     LAYER(L_B0, true);
     bars.enc.wait_full(tile_no);               // (long complete: makes the encoder's jacobian / colour-static stores visible)
     epi_eb0<P>(x, tile, s, acc);
     bars.enc.arrive_empty(tile_no);
+    TC_STAMP(21);
     SYNC_A();
     LAYER(L_C0MISC, true);
     reload_h2<P>(x);
+    TC_STAMP(22);
     SYNC_A();
     LAYER(L_C0H, false);                       // accumulates onto the misc columns' result
     epi_ec0<P>(x, acc);
+    TC_STAMP(23);
     SYNC_A();
     LAYER(L_C1, true);
     if (t == 0) bars.a.arrive_empty(tile_no);  // the last layer has read A: the next tile's geo input may land

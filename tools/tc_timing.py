@@ -1,5 +1,5 @@
 """Per-phase cycle breakdown of the fused tensor-core field kernel (CTA 0, consumer thread 0, first tiles): the wait for the staged geo
-input, every layer (its MMAs plus the epilogue before them), EC1, the cycles the consumers waited for weights and the producer for a
+input, every epilogue and every layer's MMAs apart, EC1, the cycles the consumers waited for weights and the producer for a
 free ring slot, the encoder warps' busy and slot-wait cycles per tile, and the heads warp's cycles on the tile's heads.  Uses the timing build of the kernel
 inside libsdfb200_dbg.so (sdfstudio_b200/build.py).   usage: tools/tc_timing.py [precision] [log2T] [table dtype] [fused|unfused]"""
 import ctypes
@@ -53,16 +53,22 @@ lib.sdfb200_debug_tc_timing.argtypes = [ctypes.c_void_p]
 buf = (ctypes.c_longlong * 512)()
 assert lib.sdfb200_debug_tc_timing(buf) == 0
 # stamps written by the kernel (field_tc_kernel.cuh, TC_STAMP / TC_PUT), consumer thread 0: [0] tile start, [8] the tile's geo input
-# has landed (a_full), [1 + L] end of layer L in the order the kernel runs them, [15] end of the tile (EC1 done, head inputs handed to
-# the heads warp); stamp 1 + L minus the previous one = the layer's MMAs + the epilogue before them.  Cycle sums over the tile: [9]
-# consumer thread 0 waiting for weights, [10] producer waiting for a free ring slot, [12] encoder thread 0 busy staging the tile, [13]
-# encoder thread 0 waiting for the tile's staging slot (enc_empty), [14] encoder thread 0 (the heads warp) running the tile's heads and
-# compositing, [16] consumer thread 0 waiting for the tile's head-input buffer (hs_empty), [17] the heads warp waiting for the tile's
-# head inputs (hs_full).
-layers = ["G0", "E0+G1", "E1+B1", "EB1+B0", "EB0+C0 misc", "h2 reload+C0 h2", "EC0+C1"]
+# has landed (a_full), [1 + L] end of layer L's MMAs in the order the kernel runs them, [18..23] end of the epilogues E0, E1, EB1, EB0,
+# h2 reload, EC0 (the epilogue in front of layers 1..6), [15] end of the tile (EC1 done, head inputs handed to the heads warp).  An
+# epilogue's cycles run from the end of the layer before it to its own stamp; a layer's MMA cycles from the end of the epilogue in front
+# of it (or the a_full stamp for G0) to the layer's stamp, so they include the warpgroup barrier and any wait for weights.  Cycle sums
+# over the tile: [9] consumer thread 0 waiting for weights, [10] producer waiting for a free ring slot, [12] encoder thread 0 busy
+# staging the tile, [13] encoder thread 0 waiting for the tile's staging slot (enc_empty), [14] encoder thread 0 (the heads warp)
+# running the tile's heads and compositing, [16] consumer thread 0 waiting for the tile's head-input buffer (hs_empty), [17] the heads
+# warp waiting for the tile's head inputs (hs_full).
+layers = ["G0", "G1", "B1", "B0", "C0 misc", "C0 h2", "C1"]
+epis = ["E0", "E1", "EB1", "EB0", "h2 reload", "EC0"]      # epis[L - 1] runs in front of layer L
 for t in (5, 10):
     st = [buf[t * 32 + k] for k in range(32)]
-    prev = [st[8]] + st[1:7]
-    print(f"tile {t}: total {st[15] - st[0]} cycles  a_full wait {st[8] - st[0]}  " + "  ".join(f"{n} {st[L + 1] - prev[L]}" for L, n in enumerate(layers))
-          + f"  EC1 {st[15] - st[7]}  |  consumer weight wait {st[9]}  hs_empty wait {st[16]}  producer slot wait {st[10]}"
+    epi = [st[18 + L] - st[1 + L] for L in range(6)] + [st[15] - st[7]]
+    mma = [st[1] - st[8]] + [st[2 + L] - st[18 + L] for L in range(6)]
+    print(f"tile {t}: total {st[15] - st[0]} cycles  a_full wait {st[8] - st[0]}  |  epilogues {sum(epi)}: "
+          + "  ".join(f"{n} {v}" for n, v in zip(epis + ["EC1"], epi))
+          + f"  |  MMAs {sum(mma)}: " + "  ".join(f"{n} {v}" for n, v in zip(layers, mma))
+          + f"  |  consumer weight wait {st[9]}  hs_empty wait {st[16]}  producer slot wait {st[10]}"
           + f"  |  encoder busy {st[12]}  encoder slot wait {st[13]}  heads {st[14]}  heads wait {st[17]}")
