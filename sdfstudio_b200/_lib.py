@@ -231,5 +231,32 @@ def f32c(t):
     return t.contiguous()
 
 
+def require_cuda(dev, what: str):
+    if dev.type != "cuda":
+        raise RuntimeError(f"sdfstudio_b200.{what} runs on CUDA only (there is no CPU path)")
+
+
+def render_out(rgb=None, depth=None, normal=None, accumulation=None, steps_minmax=None) -> RenderOut:
+    """sdfb200_render_out_t over the given tensors (None -> NULL: that output is not written)."""
+    return RenderOut(ptr(rgb), ptr(depth), ptr(normal), ptr(accumulation), ptr(steps_minmax))
+
+
+_MINMAX_SEED = {}
+
+
+def steps_minmax_seed(dev):
+    """{+inf, -inf}, the start value of steps_minmax, cached on `dev` so that a call makes no host->device copy.  Shared: clone it or
+    copy it into the output, never write into it."""
+    t = _MINMAX_SEED.get(str(dev))
+    if t is None:
+        t = _MINMAX_SEED[str(dev)] = torch.tensor([float("inf"), float("-inf")], device=dev, dtype=torch.float32)
+    return t
+
+
+def packed_key(params, precision):
+    """Cache key of a blob packed from `params`: it changes when a parameter is reallocated or modified in place."""
+    return tuple((p.data_ptr(), p._version) for p in params), precision
+
+
 def launch_count() -> int:
     return int(load().sdfb200_launch_count())

@@ -13,6 +13,11 @@ def needs_grad(*ts) -> bool:
     return torch.is_grad_enabled() and any(t is not None and torch.is_tensor(t) and t.requires_grad for t in ts)
 
 
+def training_step(module, params) -> bool:
+    """True when autograd is recording a training step of `module` through `params`: the fields then take their differentiable path."""
+    return torch.is_grad_enabled() and module.training and any(p.requires_grad for p in params)
+
+
 class WeightsFromAlphasFn(torch.autograd.Function):
     """alphas [R,S] -> weights [R,S], transmittance [R,S+1] (rays.py:194-230).  Gradients flow back through the weights and
     through every transmittance column (bg_transmittance = transmittance[:, -1], models/neus.py:101)."""
@@ -109,15 +114,10 @@ class RenderFn(torch.autograd.Function):
         o_depth = torch.zeros(R, device=dev)
         o_nrm = torch.zeros(R, 3, device=dev)
         o_acc = torch.empty(R, device=dev)
-        mm = torch.tensor([float("inf"), float("-inf")], device=dev)
-        out = _lib.RenderOut()
-        out.accumulation = o_acc.data_ptr()
-        if rgb is not None:
-            out.rgb = o_rgb.data_ptr()
-        if normals is not None:
-            out.normal = o_nrm.data_ptr()
-        if bins is not None:
-            out.depth, out.steps_minmax = o_depth.data_ptr(), mm.data_ptr()
+        mm = _lib.steps_minmax_seed(dev).clone()
+        has_depth = bins is not None
+        out = _lib.render_out(o_rgb if rgb is not None else None, o_depth if has_depth else None, o_nrm if normals is not None else None, o_acc,
+                              mm if has_depth else None)
         _lib.check(lib.sdfb200_render(_lib.ptr(w), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(bins), _lib.ptr(bg), bg_mode, 0, 0, R, S, out,
                                       _lib.stream_ptr()), "sdfb200_render")
         ctx.tensors = (w, rgb, normals, bins, bg, o_acc, o_depth)
@@ -147,10 +147,8 @@ class RenderAlphasFn(torch.autograd.Function):
         w = torch.empty(R, S, device=dev)
         o_rgb, o_depth, o_nrm = torch.empty(R, 3, device=dev), torch.empty(R, device=dev), torch.empty(R, 3, device=dev)
         o_acc, o_bgT = torch.empty(R, device=dev), torch.empty(R, device=dev)
-        mm = torch.tensor([float("inf"), float("-inf")], device=dev)
-        out = _lib.RenderOut()
-        out.rgb, out.depth, out.normal, out.accumulation, out.steps_minmax = (o_rgb.data_ptr(), o_depth.data_ptr(), o_nrm.data_ptr(), o_acc.data_ptr(),
-                                                                               mm.data_ptr())
+        mm = _lib.steps_minmax_seed(dev).clone()
+        out = _lib.render_out(o_rgb, o_depth, o_nrm, o_acc, mm)
         _lib.check(lib.sdfb200_render_alphas(_lib.ptr(a), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(bins), _lib.ptr(bg), bg_mode, 0, R, S, _lib.ptr(w),
                                              o_bgT.data_ptr(), out, _lib.stream_ptr()), "sdfb200_render_alphas")
         ctx.tensors = (w, rgb, normals, bins, bg, o_acc, o_depth)

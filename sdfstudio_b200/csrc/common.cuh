@@ -95,6 +95,16 @@ __device__ __forceinline__ void scene_contract(int contraction, float& px, float
   }
 }
 
+// Frustums.get_positions (cameras/rays.py) of sample s of ray r, bins [R, S+1]: origins + directions * (starts + ends) / 2 in the
+// reference's operation order, each operation rounded on its own (no FMA), so the positions are the reference's fp32 ones
+__device__ __forceinline__ void ray_midpoint(const float* origins, const float* directions, const float* bins, long long r, int S, long long s,
+                                             float (&x)[3]) {
+  const float* b = bins + r * (S + 1) + s;
+  const float se = __fadd_rn(__ldg(b), __ldg(b + 1));
+#pragma unroll
+  for (int c = 0; c < 3; ++c) x[c] = __fadd_rn(__ldg(origins + r * 3 + c), __fmul_rn(__fmul_rn(__ldg(directions + r * 3 + c), se), 0.5f));
+}
+
 // float atomic min / max by compare-and-swap (used for the batch-global steps.min()/max() of DepthRenderer, renderers.py:257)
 __device__ __forceinline__ void atomic_min_float(float* addr, float v) {
   int* ia = reinterpret_cast<int*>(addr);

@@ -54,6 +54,8 @@ __device__ __forceinline__ PointGeom point_geom(const TcArgs& a, long long p) {
     g.px = __ldg(a.origins + p * 3); g.py = __ldg(a.origins + p * 3 + 1); g.pz = __ldg(a.origins + p * 3 + 2);
     if (a.directions) { g.dx = __ldg(a.directions + p * 3); g.dy = __ldg(a.directions + p * 3 + 1); g.dz = __ldg(a.directions + p * 3 + 2); }
   }
+  // scene_contract's operations, written out: calling it moves the hoisted argument loads of the tcnn-layout instantiations and costs
+  // them 16 more bytes of stack and 4 of spill (CUDA 12.9)
   if (a.contraction != SDFB200_CONTRACT_NONE) {
     const float mag = a.contraction == SDFB200_CONTRACT_LINF
                           ? fmaxf(fabsf(g.px), fmaxf(fabsf(g.py), fabsf(g.pz)))

@@ -96,18 +96,13 @@ struct NfArgs {
 
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
-// position (contracted) and direction of sample p.  Ray mode: Frustums.get_positions, origins + directions * (starts + ends) / 2 in the
-// reference's operation order, each operation rounded on its own
+// position (contracted) and direction of sample p (ray mode: the midpoint of its bin)
 __device__ __forceinline__ void sample_geom(const NfArgs& a, long long p, float (&x)[3], float (&d)[3]) {
   if (a.S) {
     const long long r = p / a.S;
-    const float* b = a.bins + r * (a.S + 1) + (p - r * a.S);
-    const float se = __fadd_rn(__ldg(b), __ldg(b + 1));
+    ray_midpoint(a.origins, a.directions, a.bins, r, a.S, p - r * a.S, x);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      d[c] = __ldg(a.directions + r * 3 + c);
-      x[c] = __fadd_rn(__ldg(a.origins + r * 3 + c), __fmul_rn(__fmul_rn(d[c], se), 0.5f));
-    }
+    for (int c = 0; c < 3; ++c) d[c] = __ldg(a.directions + r * 3 + c);
   } else {
 #pragma unroll
     for (int c = 0; c < 3; ++c) { x[c] = __ldg(a.origins + p * 3 + c); d[c] = __ldg(a.directions + p * 3 + c); }

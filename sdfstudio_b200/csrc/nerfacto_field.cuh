@@ -74,12 +74,7 @@ __global__ void __launch_bounds__(kNerfactoThreads) k_nerfacto_field(const __gri
     const long long row = a.S ? i / a.S : i;   // ray (ray mode) or point: the row of origins, directions and appearance
     float p[3];
     if (a.S) {
-      // Frustums.get_positions (cameras/rays.py): origins + directions * (starts + ends) / 2, rounded step by step (no FMA), so that
-      // the grid cells are those of the reference's fp32 positions
-      const float* b = a.bins + row * (a.S + 1) + (i - row * a.S);
-      const float se = __fadd_rn(__ldg(b), __ldg(b + 1));
-#pragma unroll
-      for (int c = 0; c < 3; ++c) p[c] = __fadd_rn(__ldg(a.origins + row * 3 + c), __fmul_rn(__fmul_rn(__ldg(a.directions + row * 3 + c), se), 0.5f));
+      ray_midpoint(a.origins, a.directions, a.bins, row, a.S, i - row * a.S, p);
     } else {
 #pragma unroll
       for (int c = 0; c < 3; ++c) p[c] = __ldg(a.origins + i * 3 + c);

@@ -17,7 +17,9 @@ import torch
 from torch import nn
 
 from . import _lib
+from .autograd_ops import training_step
 from .encoding import _GridFn, make_grid_desc
+from .spatial_distortions import contraction_code
 
 
 class _TruncExp(torch.autograd.Function):
@@ -106,35 +108,24 @@ class HashMLPDensityField(nn.Module):
         growth = float(np.exp((np.log(max_res) - np.log(base_res)) / (num_levels - 1)))
         self.mlp_base = _NetworkWithInputEncoding(num_levels, features_per_level, log2_hashmap_size, base_res, growth, hidden_dim, num_layers - 1)
 
-    def _contraction_code(self):
-        sd = self.spatial_distortion
-        if sd is None:
-            return None
-        order = getattr(sd, "order", None)
-        if order is None:
-            return _lib.CONTRACT_L2
-        if order == float("inf"):
-            return _lib.CONTRACT_LINF
-        raise NotImplementedError(f"SceneContraction order {order!r}")
-
     def density_from_positions(self, positions: torch.Tensor, return_pre_activation: bool = False):
         """positions [..., 3] -> density [..., 1] (fields/base_field.py:48-65 + density_fields.py:98-118)."""
-        if torch.is_grad_enabled() and self.training and self.mlp_base.params.requires_grad:
+        if training_step(self, (self.mlp_base.params,)):
             return self._density_differentiable(positions, return_pre_activation)
         lib = _lib.load()
         pos = _lib.f32c(positions.reshape(-1, 3))
         n = pos.shape[0]
         dens = torch.empty(n, device=pos.device, dtype=torch.float32)
         pre = torch.empty_like(dens) if return_pre_activation else None
-        code = self._contraction_code()
-        aabb = None if code is not None else _lib.f32c(self.aabb.detach())
+        code = contraction_code(self.spatial_distortion)
+        aabb = _lib.f32c(self.aabb.detach()) if code == _lib.CONTRACT_NONE else None
         nb = self.mlp_base
         p = nb.params.detach()
         w, table = p[: nb.n_net], p[nb.n_net:]
         desc = nb.desc
         desc.active_levels = desc.n_levels
         desc.table_dtype = _lib.DT_F32
-        _lib.check(lib.sdfb200_density_field_forward(desc, table.data_ptr(), w.data_ptr(), nb.hidden_dim, nb.n_hidden_layers, code or 0, _lib.ptr(aabb),
+        _lib.check(lib.sdfb200_density_field_forward(desc, table.data_ptr(), w.data_ptr(), nb.hidden_dim, nb.n_hidden_layers, code, _lib.ptr(aabb),
                                                      _lib.ptr(pos), n, _lib.ptr(dens), _lib.ptr(pre), _lib.stream_ptr()), "sdfb200_density_field_forward")
         dens = dens.view(*positions.shape[:-1], 1)
         return (dens, pre.view(*positions.shape[:-1], 1)) if return_pre_activation else dens

@@ -25,11 +25,11 @@ from torch import nn
 
 from . import _lib
 from . import linear_ops as _lo
+from .autograd_ops import training_step
 from .field_heads import FieldHeadNames
-from .rays import rays_of
+from .rays import point_or_ray_inputs
 from .sdf_field_train import nerf_encoding, nerf_frequencies
-
-_ORDER_CODE = {float("inf"): _lib.CONTRACT_LINF, None: _lib.CONTRACT_L2}
+from .spatial_distortions import contraction_code
 
 
 class Identity(nn.Module):
@@ -160,15 +160,6 @@ class NeRFField(nn.Module):
         self._packed_key = None
 
     # ------------------------------------------------------------------ engine choice
-    def _contraction_code(self) -> int:
-        sd = self.spatial_distortion
-        if sd is None:
-            return _lib.CONTRACT_NONE
-        order = getattr(sd, "order", None)
-        if order not in _ORDER_CODE:
-            raise NotImplementedError(f"SceneContraction order {order!r} is not supported")
-        return _ORDER_CODE[order]
-
     def _desc(self, n_samples: int = 0) -> "_lib.NerfFieldDesc":
         d = _lib.NerfFieldDesc()
         b, h = self.mlp_base, self.mlp_head
@@ -183,7 +174,7 @@ class NeRFField(nn.Module):
             setattr(d, pre + "_include_input", int(inc))
             if ok:
                 getattr(d, pre + "_freqs")[:n] = nerf_frequencies(lo, hi, n).tolist()
-        d.contraction = self._contraction_code()
+        d.contraction = contraction_code(self.spatial_distortion)
         d.n_samples = n_samples
         d.precision = _lib.PRECISION[self.precision]
         return d
@@ -192,8 +183,7 @@ class NeRFField(nn.Module):
         """'aten' (fp32), 'compose' (linear_ops GEMMs, differentiable) or 'kernel' (one fused launch) for a forward call."""
         if self.precision == "fp32":
             return "aten"
-        recording = torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters())
-        if recording or not _lib.load().sdfb200_nerf_field_in_family(self._desc()):
+        if training_step(self, self.parameters()) or not _lib.load().sdfb200_nerf_field_in_family(self._desc()):
             return "compose"
         return "kernel"
 
@@ -213,12 +203,8 @@ class NeRFField(nn.Module):
             x = self._dense(layer, x, True)
         return x
 
-    def _check_device(self, t):
-        if t.device.type != "cuda":
-            raise RuntimeError("sdfstudio_b200.NeRFField runs on CUDA only (there is no CPU path)")
-
     def _density_from_positions(self, positions):
-        self._check_device(positions)
+        _lib.require_cuda(positions.device, "NeRFField")
         if self.spatial_distortion is not None:
             positions = self.spatial_distortion(positions)
         shape = positions.shape[:-1]
@@ -238,7 +224,7 @@ class NeRFField(nn.Module):
     def get_outputs(self, ray_samples, density_embedding: Optional[torch.Tensor] = None):
         """vanilla_nerf_field.py:106-114."""
         directions = ray_samples.frustums.directions
-        self._check_device(directions)
+        _lib.require_cuda(directions.device, "NeRFField")
         shape = directions.shape[:-1]
         encoded_dir = self.direction_encoding(directions.reshape(-1, 3))
         mlp_out = self._mlp(self.mlp_head, torch.cat([encoded_dir, density_embedding.reshape(encoded_dir.shape[0], density_embedding.shape[-1])], dim=-1))
@@ -265,7 +251,7 @@ class NeRFField(nn.Module):
         """The weights in the fused kernel's layout (tc_pack); rebuilt only when a parameter changed."""
         lib = _lib.load()
         params = [p for lin in self._linears() for p in (lin.weight, lin.bias)]
-        key = (tuple((p.data_ptr(), p._version) for p in params), desc.precision)
+        key = _lib.packed_key(params, desc.precision)
         if self._packed is not None and key == self._packed_key:
             return self._packed
         packed = torch.empty(lib.sdfb200_nerf_field_packed_bytes(desc), dtype=torch.uint8, device=params[0].device)
@@ -278,20 +264,10 @@ class NeRFField(nn.Module):
         return packed
 
     def _kernel_forward(self, ray_samples):
-        """One sdfb200_nerf_field_forward launch.  Ray mode when the samples carry this package's contiguous [R, S+1] bin buffer
-        (rays.make_ray_samples), point mode (positions and directions per sample) for any other RaySamples."""
+        """One sdfb200_nerf_field_forward launch, in ray or point mode (rays.point_or_ray_inputs)."""
         lib = _lib.load()
-        fr = ray_samples.frustums
-        self._check_device(fr.directions)
-        shape = tuple(fr.starts.shape[:-1])
-        bins = getattr(ray_samples, "_euclid_bins", None)
-        if bins is not None and len(shape) == 2 and getattr(fr, "offsets", None) is None:
-            origins, directions = rays_of(ray_samples)
-            n_rows, S = origins.shape[0], bins.shape[1] - 1
-        else:
-            origins = _lib.f32c(fr.get_positions().reshape(-1, 3))
-            directions = _lib.f32c(fr.directions.expand(*shape, 3).reshape(-1, 3))
-            bins, n_rows, S = None, origins.shape[0], 0
+        _lib.require_cuda(ray_samples.frustums.directions.device, "NeRFField")
+        origins, directions, bins, n_rows, S, shape = point_or_ray_inputs(ray_samples)
         desc = self._desc(S)
         packed = self._packed_weights(desc)
         N = math.prod(shape)

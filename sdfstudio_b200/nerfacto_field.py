@@ -31,11 +31,13 @@ import torch
 from torch import nn
 
 from . import _lib
+from .autograd_ops import training_step
 from .density_fields import _NetworkWithInputEncoding, _TruncExp, fully_fused_weights, relu_mlp
 from .encoding import _GridFn
 from .field_heads import FieldHeadNames
-from .rays import rays_of
+from .rays import point_or_ray_inputs
 from .sdf_field import _Embedding
+from .spatial_distortions import contraction_code
 
 BASE_RES, FEATURES_PER_LEVEL = 16, 2   # fixed by the reference constructor (nerfacto_field.py:126-127)
 SH_DIM = 16                            # tcnn SphericalHarmonics, degree 4
@@ -127,18 +129,7 @@ class TCNNNerfactoField(nn.Module):
         return self._locations
 
     def _contraction_code(self) -> int:
-        sd = self.spatial_distortion
-        if sd is None:
-            return _lib.CONTRACT_NONE
-        order = getattr(sd, "order", None)
-        if order is None:
-            return _lib.CONTRACT_L2
-        if order == float("inf"):
-            return _lib.CONTRACT_LINF
-        raise NotImplementedError(f"SceneContraction order {order!r} is not supported")
-
-    def _differentiable(self) -> bool:
-        return torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters())
+        return contraction_code(self.spatial_distortion)
 
     # ------------------------------------------------------------------ differentiable composition
     def _normalize(self, positions):
@@ -199,7 +190,7 @@ class TCNNNerfactoField(nn.Module):
         """fields/base_field.py:104-123."""
         if compute_normals:
             raise NotImplementedError("compute_normals=True is not supported by the nerfacto background field")
-        if self._differentiable():
+        if training_step(self, self.parameters()):
             density, density_embedding = self.get_density(ray_samples)
             outputs = self.get_outputs(ray_samples, density_embedding=density_embedding)
             outputs[FieldHeadNames.DENSITY] = density
@@ -210,24 +201,13 @@ class TCNNNerfactoField(nn.Module):
         return {FieldHeadNames.RGB: rgb, FieldHeadNames.DENSITY: density}
 
     def _kernel_forward(self, ray_samples):
-        """One sdfb200_nerfacto_field_forward launch.  Ray mode when the samples carry this package's contiguous [R, S+1] bin buffer
-        (rays.make_ray_samples), point mode (positions and directions per sample) for any other RaySamples."""
+        """One sdfb200_nerfacto_field_forward launch, in ray or point mode (rays.point_or_ray_inputs)."""
         lib = _lib.load()
         dev = self.aabb.device
-        if dev.type != "cuda":
-            raise RuntimeError("sdfstudio_b200.TCNNNerfactoField runs on CUDA only (there is no CPU path)")
-        fr = ray_samples.frustums
-        shape = tuple(fr.starts.shape[:-1])
-        bins = getattr(ray_samples, "_euclid_bins", None)
-        if bins is not None and len(shape) == 2 and getattr(fr, "offsets", None) is None:
-            origins, directions = rays_of(ray_samples)
-            n_rows, S = origins.shape[0], bins.shape[1] - 1
-            cam_rows = ray_samples.camera_indices.reshape(n_rows, -1)[:, 0]
-        else:
-            origins = _lib.f32c(fr.get_positions().reshape(-1, 3))
-            directions = _lib.f32c(fr.directions.reshape(-1, 3))
-            bins, n_rows, S = None, origins.shape[0], 0
-            cam_rows = ray_samples.camera_indices.reshape(-1)
+        _lib.require_cuda(dev, "TCNNNerfactoField")
+        origins, directions, bins, n_rows, S, shape = point_or_ray_inputs(ray_samples)
+        cams = ray_samples.camera_indices
+        cam_rows = cams.reshape(n_rows, -1)[:, 0] if bins is not None else cams.reshape(-1)
         N = math.prod(shape)
         mode = self._appearance_mode()
         stride = self.appearance_embedding_dim
@@ -251,7 +231,7 @@ class TCNNNerfactoField(nn.Module):
                                                       stride, density.data_ptr(), rgb.data_ptr(), pre.data_ptr(), None, _lib.stream_ptr()),
                    "sdfb200_nerfacto_field_forward")
         self._density_before_activation = pre.view(*shape, 1)
-        self._locations, self._positions_of_last_call = None, fr.get_positions
+        self._locations, self._positions_of_last_call = None, ray_samples.frustums.get_positions
         return density.view(*shape, 1), rgb.view(*shape, 3)
 
     def _desc(self, n_samples: int) -> "_lib.NerfactoDesc":

@@ -73,6 +73,22 @@ def sample_geometry(ray_samples):
     return origins, directions, bins_of(ray_samples), tuple(fr.starts.shape[:2])
 
 
+def point_or_ray_inputs(ray_samples):
+    """What the background field kernels take for a RaySamples: (origins, directions, bins | None, n_rows, S, shape).  Ray mode when
+    the samples carry this package's contiguous [R, S+1] bin buffer (make_ray_samples): per-ray origins / directions [R,3] and the
+    bins, S samples per row.  Point mode for any other RaySamples: positions and directions [N,3] per sample, bins None and S = 0.
+    `shape` is the frustums' shape."""
+    fr = ray_samples.frustums
+    shape = tuple(fr.starts.shape[:-1])
+    bins = getattr(ray_samples, "_euclid_bins", None)
+    if bins is not None and len(shape) == 2 and getattr(fr, "offsets", None) is None:
+        origins, directions = rays_of(ray_samples)
+        return origins, directions, bins, origins.shape[0], bins.shape[1] - 1, shape
+    origins = _lib.f32c(fr.get_positions().reshape(-1, 3))
+    directions = _lib.f32c(fr.directions.expand(*shape, 3).reshape(-1, 3))
+    return origins, directions, None, origins.shape[0], 0, shape
+
+
 def weights_from_alphas(alphas: torch.Tensor, with_transmittance: bool = False):
     """rays.py:194-230.  alphas [R,S,1] -> weights [R,S,1] (, transmittance [R,S+1,1])."""
     if _ag.needs_grad(alphas):

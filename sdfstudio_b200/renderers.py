@@ -13,18 +13,6 @@ from . import autograd_ops as _ag
 from .rays import bins_of
 
 
-_MM_INIT = {}
-
-
-def _minmax_init(dev):
-    """device-resident {+inf, -inf} (cloned on the device: no host->device copy / sync per call)."""
-    t = _MM_INIT.get(str(dev))
-    if t is None:
-        t = torch.tensor([float("inf"), float("-inf")], device=dev, dtype=torch.float32)
-        _MM_INIT[str(dev)] = t
-    return t.clone()
-
-
 def _background(background, R, dev):
     """-> (bg_mode, bg tensor | None)"""
     if isinstance(background, str):
@@ -70,41 +58,24 @@ def _render(weights, rgb=None, normals=None, bins=None, background=None, clamp01
     w = _lib.f32c(weights[..., 0])
     R, S = w.shape
     dev = w.device
-    out = _lib.RenderOut()
     res = {}
     bg_mode, bg_t = _lib.BG_COLOR, None
-    rgb_c = None
+    rgb_c = nrm_c = mm = None
     if rgb is not None:
         rgb_c = _lib.f32c(rgb)
         res["rgb"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
-        out.rgb = res["rgb"].data_ptr()
-        if isinstance(background, str):
-            if background == "last_sample":
-                bg_mode = _lib.BG_LAST_SAMPLE
-            elif background == "random":
-                bg_mode, bg_t = _lib.BG_PER_RAY, torch.rand(R, 3, device=dev)
-            else:
-                raise ValueError(f"unknown background {background!r}")
-        else:
-            bg_t = _lib.f32c(torch.as_tensor(background, dtype=torch.float32).to(dev))
-            if bg_t.dim() == 2:
-                bg_mode = _lib.BG_PER_RAY
-    nrm_c = None
+        bg_mode, bg_t = _background(background, R, dev)
     if want_normal:
         nrm_c = _lib.f32c(normals)
-        res["normal"] = torch.empty(R, nrm_c.shape[-1], device=dev, dtype=torch.float32)
         if nrm_c.shape[-1] != 3:
             raise NotImplementedError("SemanticRenderer: only 3 channels (normals) are composited by the kernel")
-        out.normal = res["normal"].data_ptr()
+        res["normal"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
     if want_acc:
         res["accumulation"] = torch.empty(R, device=dev, dtype=torch.float32)
-        out.accumulation = res["accumulation"].data_ptr()
-    mm = None
     if depth_method is not None:
         res["depth"] = torch.empty(R, device=dev, dtype=torch.float32)
-        out.depth = res["depth"].data_ptr()
-        mm = _minmax_init(dev)
-        out.steps_minmax = mm.data_ptr()
+        mm = _lib.steps_minmax_seed(dev).clone()
+    out = _lib.render_out(res.get("rgb"), res.get("depth"), res.get("normal"), res.get("accumulation"), mm)
     _lib.check(lib.sdfb200_render(_lib.ptr(w), _lib.ptr(rgb_c), _lib.ptr(nrm_c), _lib.ptr(bins), _lib.ptr(bg_t), bg_mode, int(clamp01),
                                   int(depth_method == "median"), R, S, out, _lib.stream_ptr()), "sdfb200_render")
     if depth_method == "expected" and clip_depth:
@@ -125,9 +96,8 @@ def _render_packed(weights, ray_indices, num_rays, rgb=None, normals=None, ray_s
     N, R = w.shape[0], int(num_rays)
     dev = w.device
     idx = ray_indices.reshape(-1).to(torch.int64).contiguous()
-    out = _lib.RenderOut()
     res = {}
-    rgb_c = nrm_c = st = en = bg_t = None
+    rgb_c = nrm_c = st = en = bg_t = mm = None
     bg_mode = _lib.BG_COLOR
     if rgb is not None:
         if isinstance(background, str) and background == "last_sample":
@@ -135,19 +105,16 @@ def _render_packed(weights, ray_indices, num_rays, rgb=None, normals=None, ray_s
         bg_mode, bg_t = _background(background, R, dev)
         rgb_c = _lib.f32c(rgb.reshape(-1, 3))
         res["rgb"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
-        out.rgb = res["rgb"].data_ptr()
     if want_normal:
         nrm_c = _lib.f32c(normals.reshape(-1, 3))
         res["normal"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
-        out.normal = res["normal"].data_ptr()
     if want_acc:
         res["accumulation"] = torch.empty(R, device=dev, dtype=torch.float32)
-        out.accumulation = res["accumulation"].data_ptr()
     if want_depth:
         st, en = _lib.f32c(ray_samples.frustums.starts.reshape(-1)), _lib.f32c(ray_samples.frustums.ends.reshape(-1))
         res["depth"] = torch.empty(R, device=dev, dtype=torch.float32)
-        mm = _minmax_init(dev)
-        out.depth, out.steps_minmax = res["depth"].data_ptr(), mm.data_ptr()
+        mm = _lib.steps_minmax_seed(dev).clone()
+    out = _lib.render_out(res.get("rgb"), res.get("depth"), res.get("normal"), res.get("accumulation"), mm)
     ws = torch.empty(max(R, 1) * 8, device=dev, dtype=torch.float32)
     _lib.check(lib.sdfb200_render_packed(_lib.ptr(w), _lib.ptr(rgb_c), _lib.ptr(nrm_c), _lib.ptr(st), _lib.ptr(en), _lib.ptr(idx), N, R, _lib.ptr(bg_t), bg_mode,
                                          int(clamp01), out, _lib.ptr(ws), ws.numel() * 4, _lib.stream_ptr()), "sdfb200_render_packed")
@@ -236,25 +203,12 @@ def render_from_alphas(alphas, rgb, normals, ray_samples, background, training: 
     R, S = a.shape
     dev = a.device
     rgb_c, nrm_c, bins = _lib.f32c(rgb), _lib.f32c(normals), bins_of(ray_samples)
-    bg_mode, bg_t = _lib.BG_COLOR, None
-    if isinstance(background, str):
-        if background == "last_sample":
-            bg_mode = _lib.BG_LAST_SAMPLE
-        elif background == "random":
-            bg_mode, bg_t = _lib.BG_PER_RAY, torch.rand(R, 3, device=dev)
-        else:
-            raise ValueError(f"unknown background {background!r}")
-    else:
-        bg_t = _lib.f32c(torch.as_tensor(background, dtype=torch.float32).to(dev))
-        if bg_t.dim() == 2:
-            bg_mode = _lib.BG_PER_RAY
+    bg_mode, bg_t = _background(background, R, dev)
     res = {"rgb": torch.empty(R, 3, device=dev), "depth": torch.empty(R, device=dev), "normal": torch.empty(R, 3, device=dev),
            "accumulation": torch.empty(R, device=dev), "bg_transmittance": torch.empty(R, device=dev)}
     w = torch.empty(R, S, device=dev) if want_weights else None
-    mm = _minmax_init(dev)
-    out = _lib.RenderOut()
-    out.rgb, out.depth, out.normal, out.accumulation, out.steps_minmax = (res["rgb"].data_ptr(), res["depth"].data_ptr(), res["normal"].data_ptr(),
-                                                                           res["accumulation"].data_ptr(), mm.data_ptr())
+    mm = _lib.steps_minmax_seed(dev).clone()
+    out = _lib.render_out(res["rgb"], res["depth"], res["normal"], res["accumulation"], mm)
     _lib.check(lib.sdfb200_render_alphas(_lib.ptr(a), _lib.ptr(rgb_c), _lib.ptr(nrm_c), _lib.ptr(bins), _lib.ptr(bg_t), bg_mode, int(not training), R, S,
                                          _lib.ptr(w), res["bg_transmittance"].data_ptr(), out, _lib.stream_ptr()), "sdfb200_render_alphas")
     _lib.check(lib.sdfb200_depth_clip(out.depth, out.steps_minmax, R, _lib.stream_ptr()), "sdfb200_depth_clip")

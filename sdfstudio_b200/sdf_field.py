@@ -5,6 +5,7 @@ reference state_dict loads directly; the arithmetic runs in libsdfb200.so throug
 
 Swap-in under ns-train: ``SDFFieldConfig._target`` of this module (see INTEGRATION.md).
 """
+import itertools
 import math
 import warnings
 from dataclasses import dataclass, field
@@ -16,9 +17,12 @@ from torch import nn
 
 from . import _lib
 from . import sdf_field_train as _train
+from .autograd_ops import training_step
 from .encoding import Encoding, growth_factor
 from .field_heads import FieldHeadNames
 from .rays import bins_of, rays_of, sample_geometry
+from .renderers import _background
+from .spatial_distortions import contraction_code
 
 
 class LaplaceDensity(nn.Module):
@@ -248,17 +252,6 @@ class SDFField(nn.Module):
         return torch.sigmoid(-10.0 * sdf)
 
     # ------------------------------------------------------------------ descriptor / packed weights
-    def _contraction_code(self) -> int:
-        sd = self.spatial_distortion
-        if sd is None:
-            return _lib.CONTRACT_NONE
-        order = getattr(sd, "order", None)
-        if order is None:
-            return _lib.CONTRACT_L2
-        if order == float("inf"):
-            return _lib.CONTRACT_LINF
-        raise NotImplementedError(f"SceneContraction order {order!r} is not supported")
-
     def _field_desc(self) -> "_lib.FieldDesc":
         c = self.config
         d = _lib.FieldDesc()
@@ -269,7 +262,7 @@ class SDFField(nn.Module):
         d.pe_degree = c.position_encoding_max_degree
         d.use_position_encoding = int(c.use_position_encoding)
         d.off_axis = int(c.off_axis)
-        d.contraction = self._contraction_code()
+        d.contraction = contraction_code(self.spatial_distortion)
         n_geo = self.num_layers - 1
         if n_geo > _lib.MAX_LAYERS or self.num_layers_color - 1 > _lib.MAX_LAYERS:
             raise NotImplementedError("too many layers")
@@ -289,21 +282,20 @@ class SDFField(nn.Module):
         return d
 
     def _mlp_params(self):
-        ps = []
+        """The MLPs' parameters, lazily (so that the engine choice touches none of them outside a training step)."""
         for l in range(self.num_layers - 1):
-            ps += list(getattr(self, f"glin{l}").parameters())
+            yield from getattr(self, f"glin{l}").parameters()
         for l in range(self.num_layers_color - 1):
-            ps += list(getattr(self, f"clin{l}").parameters())
+            yield from getattr(self, f"clin{l}").parameters()
         for n in ("diffuse_color_pred", "specular_tint_pred"):
             if hasattr(self, n):
-                ps += list(getattr(self, n).parameters())
-        return ps
+                yield from getattr(self, n).parameters()
 
     def _packed_weights(self, desc):
         """Fold weight-norm and lay the weights out for the kernels; redone only when a parameter changed."""
         lib = _lib.load()
-        params = self._mlp_params()
-        key = (tuple((p.data_ptr(), p._version) for p in params), desc.precision)
+        params = list(self._mlp_params())
+        key = _lib.packed_key(params, desc.precision)
         if self._packed is not None and key == self._packed_key:
             return self._packed
         nbytes = lib.sdfb200_field_packed_bytes(desc)
@@ -365,8 +357,7 @@ class SDFField(nn.Module):
         `wants`: iterable of output names of sdfb200_field_out_t.  Returns flat tensors ([N] / [N,k])."""
         lib = _lib.load()
         dev = self.aabb.device
-        if dev.type != "cuda":
-            raise RuntimeError("sdfstudio_b200.SDFField runs on CUDA only (there is no CPU path)")
+        _lib.require_cuda(dev, "SDFField")
         R = origins.shape[0]
         N = R * n_samples
         desc = self._field_desc()
@@ -404,8 +395,7 @@ class SDFField(nn.Module):
         R, S = origins.shape[0], bins.shape[1] - 1
         N = R * S
         dev = origins.device
-        if dev.type != "cuda":
-            raise RuntimeError("sdfstudio_b200.SDFField runs on CUDA only (there is no CPU path)")
+        _lib.require_cuda(dev, "SDFField")
         desc = self._field_desc()
         packed = self._packed_weights(desc)
         ws = self._workspace_of(lib.sdfb200_field_render_workspace_bytes(desc, R, S), "sdfb200_field_render_workspace_bytes", dev)
@@ -413,9 +403,7 @@ class SDFField(nn.Module):
         widths = [self._SAMPLE_SHAPES[k] for k in sample_outputs]
         flat = torch.empty(R * 9 + 2 + N * (sum(widths) + (1 if want_weights else 0)), device=dev, dtype=torch.float32)
         mm = flat[R * 9: R * 9 + 2]
-        if getattr(self, "_mm_init", None) is None or self._mm_init.device != dev:
-            self._mm_init = torch.tensor([float("inf"), float("-inf")], device=dev)
-        mm.copy_(self._mm_init)
+        mm.copy_(_lib.steps_minmax_seed(dev))
         off = R * 9 + 2
         fout = _lib.FieldOut()
         res = {}
@@ -426,17 +414,7 @@ class SDFField(nn.Module):
             res[k] = t.view(R, S, w_)
         rnd = _lib.FieldRender()
         rnd.from_density, rnd.clamp01, rnd.clip_depth = int(from_density), int(not training), int(clip_depth)
-        bg_t = None
-        if isinstance(background, str):
-            if background == "last_sample":
-                rnd.bg_mode = _lib.BG_LAST_SAMPLE
-            elif background == "random":
-                rnd.bg_mode, bg_t = _lib.BG_PER_RAY, torch.rand(R, 3, device=dev)
-            else:
-                raise ValueError(f"unknown background {background!r}")
-        else:
-            bg_t = _lib.f32c(torch.as_tensor(background, dtype=torch.float32).to(dev))
-            rnd.bg_mode = _lib.BG_PER_RAY if bg_t.dim() == 2 else _lib.BG_COLOR
+        rnd.bg_mode, bg_t = _background(background, R, dev)
         rnd.bg = _lib.ptr(bg_t)
         if want_weights:
             wt = flat[off: off + N]
@@ -447,8 +425,7 @@ class SDFField(nn.Module):
         nrm = flat[R * 3: R * 6].view(R, 3)
         depth, acc, bgT = flat[R * 6: R * 7], flat[R * 7: R * 8], flat[R * 8: R * 9]
         rnd.bg_transmittance = bgT.data_ptr()
-        rnd.out.rgb, rnd.out.normal, rnd.out.depth, rnd.out.accumulation, rnd.out.steps_minmax = (rgb.data_ptr(), nrm.data_ptr(), depth.data_ptr(),
-                                                                                                   acc.data_ptr(), mm.data_ptr())
+        rnd.out = _lib.render_out(rgb, depth, nrm, acc, mm)
         app = self._appearance(ray_samples.camera_indices, R, dev)
         fin = self._field_in(origins, directions, bins, S, True, app)
         table = self.encoding.compute_table() if self.use_grid_feature else None
@@ -461,7 +438,7 @@ class SDFField(nn.Module):
         """True when autograd is recording a training step: the methods below then return graph-carrying tensors from the
         autograd composition in sdf_field_train.py (grid operator = this package's kernels incl. double backward).  Everything
         under torch.no_grad() -- samplers, evaluation, meshing -- and eval mode runs the fused kernels."""
-        return torch.is_grad_enabled() and self.training and (self.encoding.table.requires_grad or any(p.requires_grad for p in self._mlp_params()))
+        return training_step(self, itertools.chain((self.encoding.table,), self._mlp_params()))
 
     # ------------------------------------------------------------------ reference methods
     def forward_geonetwork(self, inputs):

@@ -8,6 +8,8 @@ from typing import Optional, Union
 import torch
 from torch import nn
 
+from . import _lib
+
 
 class SpatialDistortion(nn.Module):
     def forward(self, positions):  # pragma: no cover - interface
@@ -24,3 +26,15 @@ class SceneContraction(SpatialDistortion):
         outside = mag >= 1
         safe = torch.where(outside, mag, torch.ones_like(mag))  # keeps the unused branch finite for autograd
         return torch.where(outside, (2 - 1 / safe) * (positions / safe), positions)
+
+
+def contraction_code(sd) -> int:
+    """The kernels' contraction code of a spatial distortion (None = no contraction): CONTRACT_NONE / _LINF / _L2."""
+    if sd is None:
+        return _lib.CONTRACT_NONE
+    order = getattr(sd, "order", None)
+    if order is None:
+        return _lib.CONTRACT_L2
+    if order == float("inf"):
+        return _lib.CONTRACT_LINF
+    raise NotImplementedError(f"SceneContraction order {order!r} is not supported")
