@@ -62,6 +62,23 @@ CPU_CASES: Dict[str, Tuple[FieldSpec, dict]] = {
     ),
 }
 
+# the training-mode sampler golden (make_golden_samplers_train.py): the first TRAIN_SAMPLER_RAYS rays of this case (its
+# sdf crosses zero on most of them, so UniSurf finds surfaces).  The ErrorBoundedSampler runs at beta0 = TRAIN_SAMPLER_BETA0
+# in place of the field's beta: small enough that it does not converge and runs all of max_total_iters = 5 iterations.
+TRAIN_SAMPLER_CASE = "neusfacto_c1_init"
+TRAIN_SAMPLER_RAYS = 32
+TRAIN_SAMPLER_BETA0 = 0.005
+
+
+def proposal_density(positions, level: int):
+    """Analytic density [..., 1] for the proposal levels of the training-mode sampler golden: a shell of radius 0.5 (the
+    case's sphere), sharper at the second level.  Plain torch ops, so the reference, the oracle and the GPU tests (on CPU
+    copies of the positions) evaluate it to the same bits."""
+    r = positions.norm(dim=-1, keepdim=True)
+    width = 0.05 if level == 0 else 0.02
+    return 50.0 * torch.exp(-(((r - 0.5) / width) ** 2)) + 0.1
+
+
 def synthetic_rays(R: int, seed: int, radius: float = 2.7, dtype=torch.float32):
     """DTU-shaped synthetic rays (SURVEY.md section 8d config 2): cameras on a sphere of radius ~2.7 looking at the origin
     through a 384x384 pinhole (fx~925), uniformly random pixels.  Returns origins, unit directions, camera_indices."""

@@ -231,10 +231,24 @@ def volsdf_updated_beta(beta0, beta, sdf, d_star, deltas, eps: float, beta_iters
     return beta_max
 
 
+def frustum_centres(origins, directions, bins: Bins):
+    """Frustums.get_positions (rays.py:47-57): [R, S, 3] sample positions at the bin centres."""
+    return origins[:, None, :] + directions[:, None, :] * ((bins.starts + bins.ends) / 2)[..., None]
+
+
+def _next(rands: Optional[List], i: int):
+    return None if rands is None else rands[i]
+
+
 def error_bounded_sampler(nears, fars, sdf_fn: Callable, beta0, num_samples=64, num_samples_eval=128, num_samples_extra=32,
-                          eps=0.1, beta_iters=10, max_total_iters=5, trace: Optional[list] = None) -> Bins:
-    """ray_samplers.py:613-702, eval mode (no jitter), without the eikonal-point draw (:688-692, torch.randint)."""
-    cur = spaced_sampler(nears, fars, num_samples_eval, "uniform")
+                          eps=0.1, beta_iters=10, max_total_iters=5, trace: Optional[list] = None, t_rand=None,
+                          u_rands: Optional[List] = None, t_rand_extra=None, eikonal_idx=None, origins=None, directions=None):
+    """ray_samplers.py:613-702.  Training mode takes the reference's draws in its order: ``t_rand`` of the first uniform
+    draw, ``u_rands[k]`` of the k-th PDF draw (one per loop iteration) and ``t_rand_extra`` of the extra uniform draw.
+    With ``eikonal_idx`` (the reference's torch.randint draw, :688-692) the frustum centres of the final pre-extra samples at
+    those flat indices are returned as well: ``(bins, points)``."""
+    cur = spaced_sampler(nears, fars, num_samples_eval, "uniform", t_rand)
+    n_pdf = 0
     deltas = cur.deltas
     bound = (1.0 / (4.0 * torch.log(torch.tensor(eps + 1.0)))) * (deltas**2.0).sum(-1)
     beta = torch.sqrt(bound)
@@ -261,29 +275,45 @@ def error_bounded_sampler(nears, fars, sdf_fn: Callable, beta0, num_samples=64, 
             err_sec = torch.exp(-d_star / beta.unsqueeze(-1)) * (deltas**2.0) / (4 * beta.unsqueeze(-1) ** 2)
             err_int = torch.cumsum(err_sec, dim=-1)
             w = (torch.clamp(torch.exp(err_int), max=1.0e6) - 1.0) * transmittance
-            new = pdf_sampler(cur, w, num_samples_eval, histogram_padding=1e-5)
+            new = pdf_sampler(cur, w, num_samples_eval, histogram_padding=1e-5, u_rand=_next(u_rands, n_pdf))
             cur, sorted_index = merge_bins(cur, new)
         else:
-            cur = pdf_sampler(cur, weights, num_samples, histogram_padding=1e-5)
+            cur = pdf_sampler(cur, weights, num_samples, histogram_padding=1e-5, u_rand=_next(u_rands, n_pdf))
+        n_pdf += 1
+    points = None
+    if eikonal_idx is not None:
+        points = frustum_centres(origins, directions, cur).reshape(-1, 3)[eikonal_idx]
     if num_samples_extra > 0:
-        uni = spaced_sampler(nears, fars, num_samples_extra, "uniform")
+        uni = spaced_sampler(nears, fars, num_samples_extra, "uniform", t_rand_extra)
         cur, _ = merge_bins(cur, uni)
-    return cur
+    return cur if eikonal_idx is None else (cur, points)
 
 
 # ---- UniSurf ------------------------------------------------------------------------------------------------------
 def unisurf_sampler(origins, directions, nears, fars, sdf_fn: Callable, delta: float = 0.25, num_samples_interval=64,
-                    num_samples_outside=32, num_samples_importance=32, num_marching_steps=256):
-    """ray_samplers.py:993-1093, eval mode.  Returns (Bins, surface_points, mask)."""
-    march = spaced_sampler(nears, fars, num_marching_steps, "uniform")
+                    num_samples_outside=32, num_samples_importance=32, num_marching_steps=256, t_rand_march=None, u_rand_importance=None,
+                    t_rand_outside=None, t_rand_interval=None):
+    """ray_samplers.py:993-1093.  Returns (Bins, surface_points, mask).  Training mode takes the reference's draws: the
+    marching, importance (PDF), outside and interval draws, in that order.  (The reference also draws 1024 random surface
+    points, between the outside and the interval draws, when no ray has a surface crossing; those are not sample positions.)"""
+    march = spaced_sampler(nears, fars, num_marching_steps, "uniform", t_rand_march)
     sdf = sdf_fn(march.starts)  # [R, M]
     occ = torch.sigmoid(-10.0 * sdf)
     w, _ = weights_from_alphas(occ)
-    imp = pdf_sampler(march, w, num_samples_importance, histogram_padding=1e-5)
-    outside = spaced_sampler(nears, fars, num_samples_outside, "uniform")
+    imp = pdf_sampler(march, w, num_samples_importance, histogram_padding=1e-5, u_rand=u_rand_importance)
+    outside = spaced_sampler(nears, fars, num_samples_outside, "uniform", t_rand_outside)
     uni_imp, _ = merge_bins(imp, outside)
+    z, mask, n2, f2 = unisurf_interval(march.starts, sdf, nears, fars, delta)
+    surface_points = origins[mask] + directions[mask] * z[..., None]
+    interval = spaced_sampler(n2, f2, num_samples_interval, "uniform", t_rand_interval)
+    merged = merge_bins_euclidean(interval, uni_imp)
+    return merged, surface_points, mask
+
+
+def unisurf_interval(starts, sdf, nears, fars, delta: float):
+    """ray_samplers.py:1031-1076: the first positive-to-negative sign change of the marching sdf [R, M] at the euclidean
+    ``starts`` [R, M] -> (z of the hit rays [H], hit mask [R], new nears [R,1], new fars [R,1])."""
     R, M = sdf.shape
-    starts = march.starts
     sign_matrix = torch.cat([torch.sign(sdf[:, :-1] * sdf[:, 1:]), torch.ones(R, 1, dtype=sdf.dtype)], dim=-1)
     cost = sign_matrix * torch.arange(M, 0, -1).to(sdf.dtype)
     values, indices = torch.min(cost, -1)
@@ -293,23 +323,19 @@ def unisurf_sampler(origins, directions, nears, fars, sdf_fn: Callable, delta: f
     ind2 = torch.clamp(indices + 1, max=M - 1)
     d_high, v_high = starts[ar, ind2][mask], sdf[ar, ind2][mask]
     z = (v_low * d_high - v_high * d_low) / (v_low - v_high)
-    surface_points = origins[mask] + directions[mask] * z[..., None]
     dists = fars - nears
     n2, f2 = nears.clone(), fars.clone()
     n2[mask] = z[:, None] - dists[mask] * delta
     f2[mask] = z[:, None] + dists[mask] * delta
-    n2 = torch.maximum(n2, nears)
-    f2 = torch.minimum(f2, fars)
-    interval = spaced_sampler(n2, f2, num_samples_interval, "uniform")
-    merged = merge_bins_euclidean(interval, uni_imp)
-    return merged, surface_points, mask
+    return z, mask, torch.maximum(n2, nears), torch.minimum(f2, fars)
 
 
 # ---- proposal-network sampler (neus-facto / bakedsdf) ---------------------------------------------------------------
 def proposal_sampler(origins, directions, nears, fars, density_fns: List[Callable], num_proposal_samples=(256, 96),
-                     num_nerf_samples=48, anneal: float = 1.0, use_uniform: bool = False):
-    """ray_samplers.py:537-578, eval mode.  density_fns[i](positions [R,S,3]) -> [R,S] (positions = frustum *centres*,
-    rays.py:47-57).  Returns (final Bins, weights_list, bins_list)."""
+                     num_nerf_samples=48, anneal: float = 1.0, use_uniform: bool = False, t_rand=None, u_rands: Optional[List] = None):
+    """ray_samplers.py:537-578.  density_fns[i](positions [R,S,3]) -> [R,S] (positions = frustum *centres*,
+    rays.py:47-57).  Training mode takes the reference's draws: ``t_rand`` of the initial spaced draw and ``u_rands[i-1]`` of
+    the PDF draw of level i.  Returns (final Bins, weights_list, bins_list)."""
     weights_list, bins_list = [], []
     n = len(num_proposal_samples)
     cur, weights = None, None
@@ -317,12 +343,11 @@ def proposal_sampler(origins, directions, nears, fars, density_fns: List[Callabl
         is_prop = i < n
         ns = num_proposal_samples[i] if is_prop else num_nerf_samples
         if i == 0:
-            cur = spaced_sampler(nears, fars, ns, "uniform" if use_uniform else "piecewise")
+            cur = spaced_sampler(nears, fars, ns, "uniform" if use_uniform else "piecewise", t_rand)
         else:
-            cur = pdf_sampler(cur, torch.pow(weights, anneal), ns, histogram_padding=0.01)
+            cur = pdf_sampler(cur, torch.pow(weights, anneal), ns, histogram_padding=0.01, u_rand=_next(u_rands, i - 1))
         if is_prop:
-            pos = origins[:, None, :] + directions[:, None, :] * ((cur.starts + cur.ends) / 2)[..., None]
-            dens = density_fns[i](pos)
+            dens = density_fns[i](frustum_centres(origins, directions, cur))
             weights, _ = weights_from_density(cur.deltas, dens)
             weights_list.append(weights)
             bins_list.append(cur)

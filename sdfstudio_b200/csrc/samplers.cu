@@ -227,8 +227,12 @@ __device__ __forceinline__ float volsdf_dstar(const float* e, const float* sd, i
 // sum E_i of the section errors and the exclusive prefix sum I_i of delta * sigma -- both as warp scans in double carried across
 // 32-sample rows (not the sequential order of torch.cumsum: agreement at the 1e-7 level, like the compositing kernels).  Per-sample
 // quantities that do not depend on beta (delta, d*, sdf) are cached in shared memory once per ray.
-// torch.clamp and .max(-1) propagate NaN (a slightly negative Heron area gives sqrt(<0) = NaN d_star in the reference): fminf / fmaxf
-// would drop it, so it is carried explicitly -- a NaN bound leaves beta untouched, as in the reference.
+// torch.clamp and .max(-1) propagate NaN: fminf / fmaxf would drop it, so it is carried explicitly -- a NaN bound leaves beta untouched,
+// as in the reference.  The NaN comes through I: a NaN sdf sample (or bin) makes delta * sigma NaN from that sample on.  d* itself is
+// not NaN for finite inputs: the Heron branch runs only when neither squared test fires and b + c - a > 0, and there the rounded area is
+// not negative (tests/test_oracle_samplers_train.py searches near-degenerate triangles of every orientation and magnitude for one).  So E
+// is NaN only where I is NaN too, and the NaN-keeping clamp of exp(E) below and the plain fminf of the err weights in k_volsdf_step give
+// the same results.
 constexpr int kVolsdfMaxS = 1000;   // 4 rays x 3 x S floats of dynamic shared memory stay under the 48 KB default
 __device__ __forceinline__ double warp_scan_incl(double v, int lane) {
 #pragma unroll

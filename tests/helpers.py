@@ -14,6 +14,28 @@ def load_golden(name, device="cpu"):
     return {k: torch.from_numpy(v).to(device) for k, v in np.load(os.path.join(GOLDEN_DIR, name + ".npz")).items()}
 
 
+def load_train_golden():
+    """tests/golden/samplers_train.{npz,json} (oracle/make_golden_samplers_train.py): (arrays, meta).  meta["draws"][run] lists the
+    reference's random draws of that run in order; ``train_draws`` returns the drawn tensors."""
+    import json
+
+    with open(os.path.join(GOLDEN_DIR, "samplers_train.json")) as f:
+        meta = json.load(f)
+    return load_golden("samplers_train"), meta
+
+
+def train_draws(G, meta, run):
+    return [G[f"{run}.draw{k}"] for k in range(len(meta["draws"][run]))]
+
+
+def train_case_inputs():
+    """The golden's rays (the first TRAIN_SAMPLER_RAYS of cases.TRAIN_SAMPLER_CASE) and the fp32 oracle field of that case."""
+    spec, kw, o, d, cam, nears, fars = cases.case_inputs(cases.TRAIN_SAMPLER_CASE)
+    n = cases.TRAIN_SAMPLER_RAYS
+    oracle = OracleField(spec, init_params(spec, **cases.init_kwargs(kw)))
+    return spec, kw, o[:n], d[:n], cam[:n], nears[:n], fars[:n], oracle
+
+
 def product_field(spec: FieldSpec, params, kw, device="cuda", precision="fp32", table_dtype="fp32"):
     """sdfstudio_b200.SDFField with the oracle's seeded parameters loaded (names match the reference state_dict)."""
     import sdfstudio_b200 as sb
