@@ -442,6 +442,22 @@ int sdfb200_collide(const float* origins, const float* directions, int64_t n_ray
 int sdfb200_lattice_points(const double* bbox_min, const double* bbox_max, const int32_t* resolution, int64_t start, int64_t n,
                            float* points, void* stream);
 
+/* Marching cubes on volume [nx, ny, nz] fp32 ('ij' order, z fastest), in place of skimage.measure.marching_cubes
+ * (utils/marching_cubes.py:133-142, :201-209, :305-314).  dims (int64[3]), origin and spacing (float[3]) are HOST arrays.  A corner is
+ * inside when v < level; an ambiguous face is resolved by the asymptotic decider on its four values, so a closed surface comes out
+ * closed; no interior vertex.  mask [nx, ny, nz] uint8 or NULL: cube (i, j, k) is processed when mask[i, j, k] != 0.  One vertex per
+ * cut edge used by a processed cube, at origin + spacing * (idx + t) with t = (level - v0) / (v1 - v0) along the edge; vertices ordered
+ * by the linear index of the point that owns the edge (its +x, +y, +z edges), then by axis; faces by cube, then table order; triangles
+ * wind so that their normal and the vertex normals (central-difference gradients, negated, normalised) point down the values.
+ * Two passes over the same inputs, one warp per (i, j) row: offsets == NULL counts into counts (workspace of
+ * sdfb200_marching_cubes_workspace_bytes(dims): int32 [2, nx*ny], each row's vertices then its faces); otherwise, with the same counts
+ * and offsets [2, nx*ny] int64 = their exclusive cumsum, verts / normals [V,3] fp32 and faces [F,3] int32 are written.
+ * Deterministic (no atomics). */
+size_t sdfb200_marching_cubes_workspace_bytes(const int64_t* dims);
+int sdfb200_marching_cubes(const float* volume, const int64_t* dims, float level, const uint8_t* mask, const float* origin,
+                           const float* spacing, const int64_t* offsets, int32_t* counts, float* verts, float* normals, int32_t* faces,
+                           void* stream);
+
 /* Training path: backward of sdfb200_render (expected depth) / sdfb200_render_alphas' compositing w.r.t. the per-sample
  * inputs (autograd over renderers.py:42-295 in the reference).  `accumulation`, `depth` = forward outputs (depth BEFORE the
  * global clip).  g_rgb [R,3], g_depth [R], g_normal [R,3], g_accumulation [R], g_weights_in [R,S]: incoming gradients, each
