@@ -467,6 +467,17 @@ int sdfb200_render_backward(const float* weights, const float* rgb, const float*
                             const float* g_rgb, const float* g_depth, const float* g_normal, const float* g_accumulation,
                             const float* g_weights_in, float* g_weights, float* g_rgb_samples, float* g_normal_samples, void* stream);
 
+/* backward of sdfb200_render_packed (before its depth clip) w.r.t. the per-sample inputs, in any sample order; nerfacc's
+ * accumulate_along_rays is differentiable in the reference (renderers.py:78-79, 194, 251-252).  `accumulation`, `depth` [n_rays] = forward
+ * outputs; g_rgb [R,3], g_depth [R], g_normal [R,3], g_accumulation [R] may each be NULL.  Outputs: g_weights [N] (required),
+ * g_rgb_samples / g_normal_samples [N,3] and g_steps [N] (d/d (starts + ends) / 2) may be NULL; each is zero where its incoming gradient
+ * is NULL or the sample's ray index lies outside [0, n_rays).  bg_mode: SDFB200_BG_COLOR or SDFB200_BG_PER_RAY. */
+int sdfb200_render_packed_backward(const float* weights, const float* rgb, const float* normals, const float* starts, const float* ends,
+                                   const int64_t* ray_indices, int64_t n_samples_total, int64_t n_rays, const float* bg, int32_t bg_mode,
+                                   const float* accumulation, const float* depth, const float* g_rgb, const float* g_depth,
+                                   const float* g_normal, const float* g_accumulation, float* g_weights, float* g_rgb_samples,
+                                   float* g_normal_samples, float* g_steps, void* stream);
+
 /* backward of sdfb200_weights_from_alphas (from_density = 0) or sdfb200_weights_from_density (from_density = 1):
  * g_weights [R,S] (+ the gradient of the returned transmittance) -> g_in [R,S].  g_transmittance may be NULL; otherwise
  * g_transmittance_cols = 1 (alphas only: [R], gradient of transmittance[:, -1] = bg_transmittance, models/neus.py:101) or the

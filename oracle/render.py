@@ -1,8 +1,9 @@
 """TEST INFRASTRUCTURE -- CPU restatement of the renderers (SURVEY.md section 8a rows a18-a20).
 
 Follows nerfstudio/model_components/renderers.py: RGBRenderer :53-118, AccumulationRenderer :171-197,
-DepthRenderer :215-261, SemanticRenderer :284-295 (dense branch only; the packed nerfacc branch is out of scope).
-Inputs are plain tensors: rgb [R,S,3], weights [R,S,1], starts/ends [R,S,1].
+DepthRenderer :215-261, SemanticRenderer :284-295.  Dense branch: rgb [R,S,3], weights [R,S,1], starts/ends [R,S,1].  Packed branch
+(``ray_indices`` + ``num_rays``, :74-79, :192-194, :249-257): rgb [N,3], weights / starts / ends [N,1], nerfacc.accumulate_along_rays
+restated as a per-ray ``index_add`` (differentiable like nerfacc's).
 """
 from typing import Optional, Union
 
@@ -52,3 +53,25 @@ def render_depth(weights, starts, ends, method: str = "expected"):
 def render_semantics(semantics, weights):
     """renderers.py:284-295 (used as the normal renderer, base_surface_model.py:216)."""
     return torch.sum(weights * semantics, dim=-2)
+
+
+def accumulate_along_rays(weights, ray_indices, values, num_rays):
+    """nerfacc.accumulate_along_rays as the packed branch calls it: [num_rays, C] per-ray sums of weights [N,1] * values [N,C]
+    (values None: of the weights).  Rays without a sample get 0."""
+    src = weights if values is None else weights * values
+    return torch.zeros(num_rays, src.shape[-1], dtype=src.dtype).index_add(0, ray_indices, src)
+
+
+def render_rgb_packed(rgb, weights, ray_indices, num_rays, background: torch.Tensor, training: bool = False):
+    """renderers.py:74-79 + :84-90 (background tensor [3] or [R,3]; 'last_sample' raises NotImplementedError there)."""
+    comp = accumulate_along_rays(weights, ray_indices, rgb, num_rays)
+    acc = accumulate_along_rays(weights, ray_indices, None, num_rays)
+    comp = comp + background * (1.0 - acc)
+    return comp if training else torch.clamp(comp, min=0.0, max=1.0)
+
+
+def render_depth_packed(weights, starts, ends, ray_indices, num_rays):
+    """renderers.py:246-257: expected depth of packed samples, clipped to the batch's [steps.min(), steps.max()]."""
+    steps = (starts + ends) / 2
+    depth = accumulate_along_rays(weights, ray_indices, steps, num_rays) / (accumulate_along_rays(weights, ray_indices, None, num_rays) + 1e-10)
+    return torch.clip(depth, steps.min(), steps.max())

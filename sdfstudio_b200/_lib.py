@@ -106,6 +106,8 @@ _PROTOS = {
     "sdfb200_grid_encode_backward_grouped": (C.c_int, [C.POINTER(GridDesc), _vp, _vp, _i64, _i32, _vp, _vp]),
     "sdfb200_grid_encode_backward_backward": (C.c_int, [C.POINTER(GridDesc), _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "sdfb200_render_backward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "sdfb200_render_packed_backward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                 _vp]),
     "sdfb200_weights_backward": (C.c_int, [_vp, _vp, _i32, _i64, _i32, _vp, _vp, _i32, _vp, _vp]),
     "sdfb200_generate_rays": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "sdfb200_collide": (C.c_int, [_vp, _vp, _i64, _i32, C.POINTER(C.c_float), _f32, _vp, _vp, _vp]),

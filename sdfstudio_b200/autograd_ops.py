@@ -175,6 +175,57 @@ class RenderAlphasFn(torch.autograd.Function):
         return g_a, g_rgb_s, g_nrm_s, None, None, None
 
 
+class PackedRenderFn(torch.autograd.Function):
+    """packed samples: weights [N] (+ rgb, normals [N,3], starts, ends [N]), ray_indices [N] in any order -> rgb [R,3], UNCLIPPED expected
+    depth [R], normal [R,3], accumulation [R], steps_minmax [2] (sdfb200_render_packed; backward sdfb200_render_packed_backward).  What
+    nerfacc.accumulate_along_rays gives the reference's renderers (renderers.py:78-79, 194, 251-252), differentiable like it.  Absent inputs
+    are passed as None and yield zero-filled outputs."""
+
+    @staticmethod
+    def forward(ctx, weights, rgb, normals, starts, ends, ray_indices, num_rays, bg, bg_mode):
+        lib = _lib.load()
+        w = _lib.f32c(weights)
+        N, R, dev = w.shape[0], int(num_rays), w.device
+        rgb = _lib.f32c(rgb) if rgb is not None else None
+        normals = _lib.f32c(normals) if normals is not None else None
+        has_depth = starts is not None
+        st, en = (_lib.f32c(starts), _lib.f32c(ends)) if has_depth else (None, None)
+        o_rgb, o_depth, o_nrm = torch.zeros(R, 3, device=dev), torch.zeros(R, device=dev), torch.zeros(R, 3, device=dev)
+        o_acc = torch.empty(R, device=dev)
+        mm = _lib.steps_minmax_seed(dev).clone()
+        out = _lib.render_out(o_rgb if rgb is not None else None, o_depth if has_depth else None, o_nrm if normals is not None else None, o_acc,
+                              mm if has_depth else None)
+        ws = torch.empty(max(R, 1) * 8, device=dev, dtype=torch.float32)
+        _lib.check(lib.sdfb200_render_packed(_lib.ptr(w), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(st), _lib.ptr(en), _lib.ptr(ray_indices), N, R,
+                                             _lib.ptr(bg), bg_mode, 0, out, _lib.ptr(ws), ws.numel() * 4, _lib.stream_ptr()), "sdfb200_render_packed")
+        ctx.tensors = (w, rgb, normals, st, en, ray_indices, bg, o_acc, o_depth)
+        ctx.bg_mode = bg_mode
+        ctx.mark_non_differentiable(mm)
+        return o_rgb, o_depth, o_nrm, o_acc, mm
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_rgb, g_depth, g_nrm, g_acc, _g_mm):
+        lib = _lib.load()
+        w, rgb, nrm, st, en, ri, bg, acc, depth = ctx.tensors
+        N, R = w.shape[0], acc.shape[0]
+        g_rgb = _lib.f32c(g_rgb) if (g_rgb is not None and rgb is not None) else None
+        g_depth = _lib.f32c(g_depth) if (g_depth is not None and st is not None) else None
+        g_nrm = _lib.f32c(g_nrm) if (g_nrm is not None and nrm is not None) else None
+        g_acc = _lib.f32c(g_acc) if g_acc is not None else None
+        g_w = torch.empty_like(w)
+        g_rgb_s = torch.empty(N, 3, device=w.device) if (ctx.needs_input_grad[1] and rgb is not None) else None
+        g_nrm_s = torch.empty(N, 3, device=w.device) if (ctx.needs_input_grad[2] and nrm is not None) else None
+        want_steps = st is not None and (ctx.needs_input_grad[3] or ctx.needs_input_grad[4])
+        g_steps = torch.empty(N, device=w.device) if want_steps else None
+        _lib.check(lib.sdfb200_render_packed_backward(_lib.ptr(w), _lib.ptr(rgb), _lib.ptr(nrm), _lib.ptr(st), _lib.ptr(en), _lib.ptr(ri), N, R,
+                                                      _lib.ptr(bg), ctx.bg_mode, _lib.ptr(acc), _lib.ptr(depth), _lib.ptr(g_rgb), _lib.ptr(g_depth),
+                                                      _lib.ptr(g_nrm), _lib.ptr(g_acc), _lib.ptr(g_w), _lib.ptr(g_rgb_s), _lib.ptr(g_nrm_s),
+                                                      _lib.ptr(g_steps), _lib.stream_ptr()), "sdfb200_render_packed_backward")
+        g_half = g_steps * 0.5 if want_steps else None          # step = (starts + ends) / 2
+        return g_w, g_rgb_s, g_nrm_s, g_half, g_half, None, None, None, None
+
+
 class PackedWeightsFn(torch.autograd.Function):
     """alphas [N] of segmented packed samples (ray r = [offsets[r], offsets[r+1])) -> weights [N] = alpha * exclusive prod(1 - alpha)
     (nerfacc 0.3.5 render_weight_from_alpha; sdfb200_packed_weights / sdfb200_packed_weights_backward)."""

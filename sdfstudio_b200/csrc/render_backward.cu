@@ -174,6 +174,54 @@ __global__ void __launch_bounds__(256) k_packed_weights_bwd(const float* __restr
   }
 }
 
+// backward of sdfb200_render_packed (the ray_indices branch of the renderers), one thread per sample; any sample order, like the
+// forward's atomics.  Same per-sample terms as k_render_bwd with r = ray_indices[i] and step = (starts + ends) / 2; a sample whose ray
+// index lies outside [0, R) does not reach the forward and gets zero gradients.  g_steps [N]: d/d step_i = g_depth[r] w_i / (acc_r + 1e-10).
+struct PackedRenderBwdArgs {
+  const float *weights, *rgb, *normals, *starts, *ends, *bg;
+  const int64_t* ray_indices;
+  int bg_mode; int64_t N, R;
+  const float *acc, *depth;
+  const float *g_rgb, *g_depth, *g_normal, *g_acc;
+  float *g_weights, *g_rgb_s, *g_normal_s, *g_steps;
+};
+
+__global__ void __launch_bounds__(256) k_render_packed_bwd(const PackedRenderBwdArgs a) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.N) return;
+  const int64_t r = a.ray_indices[i];
+  const bool in = r >= 0 && r < a.R;
+  const float w = a.weights[i];
+  float gw = 0.f, e[3] = {0.f, 0.f, 0.f}, m[3] = {0.f, 0.f, 0.f}, gs = 0.f;
+  if (in && a.g_rgb) {
+    const float* b = a.bg_mode == SDFB200_BG_PER_RAY ? a.bg + r * 3 : a.bg;
+    for (int c = 0; c < 3; ++c) {
+      const float g = a.g_rgb[r * 3 + c];
+      gw += g * (a.rgb[i * 3 + c] - b[c]);   // out = sum w c + bg (1 - sum w)
+      e[c] = g * w;
+    }
+  }
+  if (in && a.g_normal) {
+    for (int c = 0; c < 3; ++c) {
+      const float g = a.g_normal[r * 3 + c];
+      gw += g * a.normals[i * 3 + c];
+      m[c] = g * w;
+    }
+  }
+  if (in && a.g_acc) gw += a.g_acc[r];
+  if (in && a.g_depth) {
+    // depth = sum(w step) / (acc + 1e-10)   (renderers.py:249-252, before the global clip)
+    const float step = (a.starts[i] + a.ends[i]) * 0.5f;
+    const float q = a.g_depth[r] / (a.acc[r] + 1e-10f);
+    gw += q * (step - a.depth[r]);
+    gs = q * w;
+  }
+  a.g_weights[i] = gw;
+  if (a.g_rgb_s) for (int c = 0; c < 3; ++c) a.g_rgb_s[i * 3 + c] = e[c];
+  if (a.g_normal_s) for (int c = 0; c < 3; ++c) a.g_normal_s[i * 3 + c] = m[c];
+  if (a.g_steps) a.g_steps[i] = gs;
+}
+
 // backward of k_packed_accumulate, one thread per sample: dv[i, c] = w_i g[r_i, c],  dw_i = sum_c g[r_i, c] v[i, c]  (or g[r_i])
 __global__ void __launch_bounds__(256) k_packed_accumulate_bwd(const float* __restrict__ weights, const float* __restrict__ values,
                                                                const int64_t* __restrict__ ray_indices, int64_t N, int C,
@@ -235,6 +283,27 @@ extern "C" int sdfb200_render_backward(const float* weights, const float* rgb, c
   a.g_weights_in = g_weights_in; a.g_weights = g_weights; a.g_rgb_s = g_rgb_samples; a.g_normal_s = g_normal_samples;
   k_render_bwd<<<(unsigned)ceil_div(n_rays * n_samples, 256), 256, 0, (cudaStream_t)stream>>>(a);
   SDFB_LAUNCHED("k_render_bwd");
+  return 0;
+}
+
+extern "C" int sdfb200_render_packed_backward(const float* weights, const float* rgb, const float* normals, const float* starts, const float* ends,
+                                              const int64_t* ray_indices, int64_t n_samples_total, int64_t n_rays, const float* bg, int32_t bg_mode,
+                                              const float* accumulation, const float* depth, const float* g_rgb, const float* g_depth,
+                                              const float* g_normal, const float* g_accumulation, float* g_weights, float* g_rgb_samples,
+                                              float* g_normal_samples, float* g_steps, void* stream) {
+  SDFB_REQUIRE(n_samples_total >= 0 && n_rays >= 0, "bad sizes");
+  if (n_samples_total == 0) return 0;
+  SDFB_REQUIRE(weights && ray_indices && g_weights, "NULL pointer");
+  SDFB_REQUIRE(bg_mode != SDFB200_BG_LAST_SAMPLE, "background 'last_sample' is not defined for packed samples (renderers.py:76-77)");
+  if (g_rgb) SDFB_REQUIRE(rgb != nullptr && bg != nullptr, "g_rgb needs rgb and background");
+  if (g_normal) SDFB_REQUIRE(normals != nullptr, "g_normal needs normals");
+  if (g_depth) SDFB_REQUIRE(starts != nullptr && ends != nullptr && depth != nullptr && accumulation != nullptr, "g_depth needs starts, ends, depth, accumulation");
+  PackedRenderBwdArgs a;
+  a.weights = weights; a.rgb = rgb; a.normals = normals; a.starts = starts; a.ends = ends; a.bg = bg; a.ray_indices = ray_indices; a.bg_mode = bg_mode;
+  a.N = n_samples_total; a.R = n_rays; a.acc = accumulation; a.depth = depth; a.g_rgb = g_rgb; a.g_depth = g_depth; a.g_normal = g_normal;
+  a.g_acc = g_accumulation; a.g_weights = g_weights; a.g_rgb_s = g_rgb_samples; a.g_normal_s = g_normal_samples; a.g_steps = g_steps;
+  k_render_packed_bwd<<<(unsigned)ceil_div(n_samples_total, 256), 256, 0, (cudaStream_t)stream>>>(a);
+  SDFB_LAUNCHED("k_render_packed_bwd");
   return 0;
 }
 

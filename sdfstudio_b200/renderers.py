@@ -87,15 +87,47 @@ def _render(weights, rgb=None, normals=None, bins=None, background=None, clamp01
     return res
 
 
+def _render_packed_grad(weights, idx, R, rgb, normals, starts, ends, background, clamp01, want_acc):
+    """training path of _render_packed: same outputs through PackedRenderFn, the depth clip as a torch.clamp like the dense path."""
+    bg_mode, bg_t = _lib.BG_COLOR, None
+    if rgb is not None:
+        if isinstance(background, str) and background == "last_sample":
+            raise NotImplementedError("Background color 'last_sample' not implemented for packed samples.")
+        bg_mode, bg_t = _background(background, R, weights.device)
+    rs = lambda t, *shape: t.reshape(*shape) if t is not None else None  # noqa: E731
+    o_rgb, o_depth, o_nrm, o_acc, mm = _ag.PackedRenderFn.apply(weights.reshape(-1), rs(rgb, -1, 3), rs(normals, -1, 3), rs(starts, -1), rs(ends, -1),
+                                                                idx, R, bg_t, bg_mode)
+    res = {}
+    if rgb is not None:
+        res["rgb"] = torch.clamp(o_rgb, 0.0, 1.0) if clamp01 else o_rgb
+    if normals is not None:
+        res["normal"] = o_nrm
+    if want_acc:
+        res["accumulation"] = o_acc[:, None]
+    if starts is not None:
+        lo, hi = mm[0], mm[1]
+        if _ag.needs_grad(starts, ends):   # the clip bounds steps.min() / steps.max() (renderers.py:257) pass gradient to their samples
+            steps = (starts + ends) / 2
+            lo, hi = steps.min(), steps.max()
+        res["depth"] = torch.clamp(o_depth, min=lo, max=hi)[:, None]
+    return res
+
+
 def _render_packed(weights, ray_indices, num_rays, rgb=None, normals=None, ray_samples=None, background=None, clamp01=False, want_acc=False,
                    want_normal=False, want_depth=False):
     """packed-sample branch (samples of all rays in one flat list + ``ray_indices``; what nerfacc.accumulate_along_rays does in the
-    reference, renderers.py:74-79,192-194,249-253): one scatter-add launch + one per-ray finishing launch (sdfb200_render_packed)."""
+    reference, renderers.py:74-79,192-194,249-253): one scatter-add launch + one per-ray finishing launch (sdfb200_render_packed).
+    nerfacc.accumulate_along_rays is differentiable, so under autograd this goes through PackedRenderFn."""
+    idx = ray_indices.reshape(-1).to(torch.int64).contiguous()
+    starts = ray_samples.frustums.starts if want_depth else None
+    ends = ray_samples.frustums.ends if want_depth else None
+    if _ag.needs_grad(weights, rgb, normals if want_normal else None, starts, ends):
+        return _render_packed_grad(weights, idx, int(num_rays), rgb, normals if want_normal else None, starts, ends, background, clamp01,
+                                   want_acc)
     lib = _lib.load()
     w = _lib.f32c(weights.reshape(-1))
     N, R = w.shape[0], int(num_rays)
     dev = w.device
-    idx = ray_indices.reshape(-1).to(torch.int64).contiguous()
     res = {}
     rgb_c = nrm_c = st = en = bg_t = mm = None
     bg_mode = _lib.BG_COLOR
