@@ -487,6 +487,23 @@ int sdfb200_weights_backward(const float* alphas_or_density, const float* euclid
                              int32_t n_samples, const float* g_weights, const float* g_transmittance, int32_t g_transmittance_cols,
                              float* g_in, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Training path: the interlevel loss that trains the proposal networks.  Replaces interlevel_loss (mip-NeRF 360,
+ * model_components/losses.py:38-112) and interlevel_loss_zip (Zip-NeRF, :116-172) for one proposal level.
+ * fine_bins [R,Sf+1], fine_weights [R,Sf]: the final level's spacing bin edges and weights (constants);
+ * proposal_bins [R,Sp+1], proposal_weights [R,Sp]: the proposal level's.  1 <= Sf, Sp <= 1024.
+ * form OUTER: elements max(w - w_outer, 0)^2 / (w + 1e-7) over the R*Sf fine samples; form ZIP: the fine histogram blurred
+ * with radius blur_radius (> 0) and resampled on the proposal edges, elements max(w_gt - wp, 0)^2 / (wp + 1e-5) over the R*Sp
+ * proposal samples.  Outputs: loss_per_ray [R] (required; the sum of a ray's elements), loss [1] (the mean over all elements,
+ * the per-ray sums added in a fixed order; NULL: not computed) and grad_proposal_weights [R,Sp] =
+ * d loss_per_ray[r] / d proposal_weights[r, :] (NULL: not computed).  No atomics: the same inputs give the same bits.
+ * One launch, two with `loss`.  n_rays = 0 launches nothing and writes nothing.
+ * ------------------------------------------------------------------------------------------------------------- */
+enum { SDFB200_INTERLEVEL_OUTER = 0, SDFB200_INTERLEVEL_ZIP = 1 };
+int sdfb200_interlevel_loss(const float* fine_bins, const float* fine_weights, int32_t n_fine, const float* proposal_bins,
+                            const float* proposal_weights, int32_t n_proposal, int64_t n_rays, int32_t form, float blur_radius,
+                            float* loss_per_ray, float* loss, float* grad_proposal_weights, void* stream);
+
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Training path: dense-layer GEMMs on wgmma (bf16x3 = parity grade, bf16 = fast), fp32 row-major in / out.  They replace the ATen /

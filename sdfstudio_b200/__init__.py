@@ -8,14 +8,16 @@ Host side mirrors the reference's plug points (SURVEY.md section 8b):
   ray_samplers.*               <- nerfstudio.model_components.ray_samplers
   packed.*                     <- nerfacc 0.3.5 render_weight_from_alpha / accumulate_along_rays (neus-acc)
   renderers.*                  <- nerfstudio.model_components.renderers
+  losses.*                     <- nerfstudio.model_components.losses (the interlevel losses of the proposal networks)
   rays.*                       <- nerfstudio.cameras.rays (containers + alpha/density -> weights)
 All arithmetic runs in libsdfb200.so (CUDA, sm_90a) behind the C ABI of include/sdfb200.h.  No CPU / PyTorch fallback.
 """
 from . import _lib  # noqa: F401
-from . import cameras, meshing, packed  # noqa: F401
+from . import cameras, losses, meshing, packed  # noqa: F401
 from .density_fields import HashMLPDensityField  # noqa: F401
 from .encoding import Encoding, HashEncoding  # noqa: F401
 from .field_heads import FieldHeadNames  # noqa: F401
+from .losses import interlevel_loss, interlevel_loss_zip, ray_samples_to_sdist  # noqa: F401
 from .nerfacto_field import TCNNNerfactoField  # noqa: F401
 from .nerf_field import NeRFEncoding, NeRFField  # noqa: F401
 from .rays import Frustums, RayBundle, RaySamples  # noqa: F401

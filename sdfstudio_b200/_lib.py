@@ -22,6 +22,7 @@ BG_COLOR, BG_LAST_SAMPLE, BG_PER_RAY = 0, 1, 2
 CAMERA_PERSPECTIVE, CAMERA_FISHEYE = 1, 2
 COLLIDER_AABB, COLLIDER_NEAR_FAR, COLLIDER_SPHERE = 0, 1, 2
 PRECISION = {"fp32": 0, "bf16x3": 1, "bf16": 2}
+INTERLEVEL_OUTER, INTERLEVEL_ZIP = 0, 1
 
 
 class GridDesc(C.Structure):
@@ -109,6 +110,7 @@ _PROTOS = {
     "sdfb200_render_packed_backward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                                  _vp]),
     "sdfb200_weights_backward": (C.c_int, [_vp, _vp, _i32, _i64, _i32, _vp, _vp, _i32, _vp, _vp]),
+    "sdfb200_interlevel_loss": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _i32, _i64, _i32, _f32, _vp, _vp, _vp, _vp]),
     "sdfb200_generate_rays": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp]),
     "sdfb200_collide": (C.c_int, [_vp, _vp, _i64, _i32, C.POINTER(C.c_float), _f32, _vp, _vp, _vp]),
     "sdfb200_lattice_points": (C.c_int, [C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int32), _i64, _i64, _vp, _vp]),

@@ -279,3 +279,32 @@ class PackedAccumulateFn(torch.autograd.Function):
         _lib.check(lib.sdfb200_packed_accumulate_backward(_lib.ptr(w), _lib.ptr(v), C, _lib.ptr(ray_indices), w.shape[0], _lib.ptr(_lib.f32c(g_out)),
                                                           _lib.ptr(g_w), _lib.ptr(g_v), _lib.stream_ptr()), "sdfb200_packed_accumulate_backward")
         return g_w, g_v, None, None
+
+
+class InterlevelLossFn(torch.autograd.Function):
+    """One proposal level of the interlevel loss (losses.py:38-172): proposal weights [R,Sp] -> the mean over all elements (0-dim).
+    form = _lib.INTERLEVEL_OUTER or _lib.INTERLEVEL_ZIP (blur_radius is read by the latter only).  The forward kernel writes
+    d (a ray's sum) / d proposal weights next to the loss, so the backward is one scale by grad / count.  Only the proposal weights
+    are differentiable: the bin edges and the fine weights are constants here, as they are in the reference."""
+
+    @staticmethod
+    def forward(ctx, proposal_weights, proposal_bins, fine_bins, fine_weights, form, blur_radius):
+        lib = _lib.load()
+        wp = _lib.f32c(proposal_weights)
+        R, sp = wp.shape
+        sf = fine_weights.shape[1]
+        per_ray = torch.empty(R, device=wp.device, dtype=torch.float32)
+        loss = torch.empty((), device=wp.device, dtype=torch.float32)
+        grad = torch.empty_like(wp) if ctx.needs_input_grad[0] else None
+        _lib.check(lib.sdfb200_interlevel_loss(_lib.ptr(fine_bins), _lib.ptr(fine_weights), sf, _lib.ptr(proposal_bins), _lib.ptr(wp), sp, R, form,
+                                               float(blur_radius), _lib.ptr(per_ray), _lib.ptr(loss), _lib.ptr(grad), _lib.stream_ptr()),
+                   "sdfb200_interlevel_loss")
+        ctx.save_for_backward(grad)
+        ctx.count = R * (sp if form == _lib.INTERLEVEL_ZIP else sf)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_loss):
+        (grad,) = ctx.saved_tensors
+        return grad * (g_loss / ctx.count), None, None, None, None, None
