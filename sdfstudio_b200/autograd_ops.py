@@ -2,7 +2,9 @@
 
 The reference trains through ATen autograd over rays.py:131-230 and renderers.py:42-295; here every op keeps its forward
 kernel and gets an explicit backward kernel (csrc/render_backward.cu: sdfb200_render_backward, sdfb200_weights_backward).
-Used automatically by rays.py / renderers.py when an input requires grad; the no-grad (rendering) path does not go through here.
+Used automatically by rays.py / renderers.py when an input requires grad.  Each dense compositing op has one launch function here
+(launch_*): it allocates the outputs, builds the RenderOut and launches the kernel.  The no-grad (rendering) path calls it directly, with
+its in-kernel clamp / median and only the outputs it asks for; the Function's forward calls it and keeps what its backward needs.
 """
 import torch
 
@@ -18,18 +20,89 @@ def training_step(module, params) -> bool:
     return torch.is_grad_enabled() and module.training and any(p.requires_grad for p in params)
 
 
+def launch_weights_from_alphas(a, with_transmittance: bool):
+    """alphas [R,S] (fp32, contiguous) -> weights [R,S], transmittance [R,S+1] | None (sdfb200_weights_from_alphas)."""
+    R, S = a.shape
+    w = torch.empty_like(a)
+    T = a.new_empty(R, S + 1) if with_transmittance else None
+    _lib.check(_lib.load().sdfb200_weights_from_alphas(_lib.ptr(a), R, S, _lib.ptr(w), _lib.ptr(T), _lib.stream_ptr()), "sdfb200_weights_from_alphas")
+    return w, T
+
+
+def launch_weights_from_density(d, bins, with_transmittance: bool):
+    """densities [R,S] (fp32, contiguous), euclidean bins [R,S+1] -> weights [R,S], transmittance [R,S] | None
+    (sdfb200_weights_from_density)."""
+    R, S = d.shape
+    w = torch.empty_like(d)
+    T = torch.empty_like(d) if with_transmittance else None
+    _lib.check(_lib.load().sdfb200_weights_from_density(_lib.ptr(d), _lib.ptr(bins), R, S, _lib.ptr(w), _lib.ptr(T), _lib.stream_ptr()),
+               "sdfb200_weights_from_density")
+    return w, T
+
+
+def launch_render(w, rgb, normals, bins, bg, bg_mode, clamp01=False, median=False, want_acc=True):
+    """weights [R,S] (+ rgb, normals [R,S,3], bins [R,S+1], all fp32 contiguous or None) -> rgb [R,3], depth [R], normal [R,3],
+    accumulation [R], steps_minmax [2] (sdfb200_render).  An output whose input is None (accumulation: want_acc False) is not computed
+    and comes back as None; the depth is the unclipped one."""
+    R, S = w.shape
+    dev = w.device
+    o_rgb = w.new_empty(R, 3) if rgb is not None else None
+    o_nrm = w.new_empty(R, 3) if normals is not None else None
+    o_depth = w.new_empty(R) if bins is not None else None
+    o_acc = w.new_empty(R) if want_acc else None
+    mm = _lib.steps_minmax_seed(dev).clone() if bins is not None else None
+    out = _lib.render_out(o_rgb, o_depth, o_nrm, o_acc, mm)
+    _lib.check(_lib.load().sdfb200_render(_lib.ptr(w), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(bins), _lib.ptr(bg), bg_mode, int(clamp01),
+                                          int(median), R, S, out, _lib.stream_ptr()), "sdfb200_render")
+    return o_rgb, o_depth, o_nrm, o_acc, mm
+
+
+def launch_render_alphas(a, rgb, normals, bins, bg, bg_mode, clamp01=False, want_weights=True):
+    """alphas [R,S] (+ rgb, normals [R,S,3], bins [R,S+1], fp32 contiguous) -> weights [R,S] | None, rgb [R,3], unclipped depth [R],
+    normal [R,3], accumulation [R], bg_transmittance [R], steps_minmax [2] in one launch (sdfb200_render_alphas)."""
+    R, S = a.shape
+    dev = a.device
+    w = a.new_empty(R, S) if want_weights else None
+    o_rgb, o_depth, o_nrm = a.new_empty(R, 3), a.new_empty(R), a.new_empty(R, 3)
+    o_acc, o_bgT = a.new_empty(R), a.new_empty(R)
+    mm = _lib.steps_minmax_seed(dev).clone()
+    out = _lib.render_out(o_rgb, o_depth, o_nrm, o_acc, mm)
+    _lib.check(_lib.load().sdfb200_render_alphas(_lib.ptr(a), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(bins), _lib.ptr(bg), bg_mode, int(clamp01), R, S,
+                                                 _lib.ptr(w), _lib.ptr(o_bgT), out, _lib.stream_ptr()), "sdfb200_render_alphas")
+    return w, o_rgb, o_depth, o_nrm, o_acc, o_bgT, mm
+
+
+def launch_render_packed(w, rgb, normals, starts, ends, ray_indices, R, bg, bg_mode, clamp01=False, want_acc=True):
+    """packed samples: weights [N] (+ rgb, normals [N,3], starts, ends [N], fp32 contiguous or None), int64 ray_indices [N] in any order ->
+    rgb [R,3], unclipped depth [R], normal [R,3], accumulation [R], steps_minmax [2] (sdfb200_render_packed).  An output whose input is
+    None (accumulation: want_acc False) is not computed and comes back as None."""
+    N, dev = w.shape[0], w.device
+    o_rgb = w.new_empty(R, 3) if rgb is not None else None
+    o_nrm = w.new_empty(R, 3) if normals is not None else None
+    o_depth = w.new_empty(R) if starts is not None else None
+    o_acc = w.new_empty(R) if want_acc else None
+    mm = _lib.steps_minmax_seed(dev).clone() if starts is not None else None
+    out = _lib.render_out(o_rgb, o_depth, o_nrm, o_acc, mm)
+    ws = w.new_empty(max(R, 1) * 8)
+    _lib.check(_lib.load().sdfb200_render_packed(_lib.ptr(w), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(starts), _lib.ptr(ends), _lib.ptr(ray_indices),
+                                                 N, R, _lib.ptr(bg), bg_mode, int(clamp01), out, _lib.ptr(ws), ws.numel() * 4, _lib.stream_ptr()),
+               "sdfb200_render_packed")
+    return o_rgb, o_depth, o_nrm, o_acc, mm
+
+
+def _or_zeros(t, like, *shape):
+    """an output the launch did not compute (its input was None): zeros, so that the Function returns a tensor in every place"""
+    return t if t is not None else like.new_zeros(shape)
+
+
 class WeightsFromAlphasFn(torch.autograd.Function):
     """alphas [R,S] -> weights [R,S], transmittance [R,S+1] (rays.py:194-230).  Gradients flow back through the weights and
     through every transmittance column (bg_transmittance = transmittance[:, -1], models/neus.py:101)."""
 
     @staticmethod
     def forward(ctx, alphas):
-        lib = _lib.load()
         a = _lib.f32c(alphas)
-        R, S = a.shape
-        w = torch.empty_like(a)
-        T = torch.empty(R, S + 1, device=a.device, dtype=torch.float32)
-        _lib.check(lib.sdfb200_weights_from_alphas(_lib.ptr(a), R, S, _lib.ptr(w), _lib.ptr(T), _lib.stream_ptr()), "sdfb200_weights_from_alphas")
+        w, T = launch_weights_from_alphas(a, True)
         ctx.save_for_backward(a)
         return w, T
 
@@ -54,13 +127,8 @@ class WeightsFromDensityFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, density, bins):
-        lib = _lib.load()
         d = _lib.f32c(density)
-        R, S = d.shape
-        w = torch.empty_like(d)
-        T = torch.empty_like(d)
-        _lib.check(lib.sdfb200_weights_from_density(_lib.ptr(d), _lib.ptr(bins), R, S, _lib.ptr(w), _lib.ptr(T), _lib.stream_ptr()),
-                   "sdfb200_weights_from_density")
+        w, T = launch_weights_from_density(d, bins, True)
         ctx.save_for_backward(d, bins)
         return w, T
 
@@ -104,22 +172,13 @@ class RenderFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, weights, rgb, normals, bins, bg, bg_mode):
-        lib = _lib.load()
         w = _lib.f32c(weights)
-        R, S = w.shape
-        dev = w.device
+        R = w.shape[0]
         rgb = _lib.f32c(rgb) if rgb is not None else None
         normals = _lib.f32c(normals) if normals is not None else None
-        o_rgb = torch.zeros(R, 3, device=dev)
-        o_depth = torch.zeros(R, device=dev)
-        o_nrm = torch.zeros(R, 3, device=dev)
-        o_acc = torch.empty(R, device=dev)
-        mm = _lib.steps_minmax_seed(dev).clone()
-        has_depth = bins is not None
-        out = _lib.render_out(o_rgb if rgb is not None else None, o_depth if has_depth else None, o_nrm if normals is not None else None, o_acc,
-                              mm if has_depth else None)
-        _lib.check(lib.sdfb200_render(_lib.ptr(w), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(bins), _lib.ptr(bg), bg_mode, 0, 0, R, S, out,
-                                      _lib.stream_ptr()), "sdfb200_render")
+        o_rgb, o_depth, o_nrm, o_acc, mm = launch_render(w, rgb, normals, bins, bg, bg_mode)
+        o_rgb, o_depth, o_nrm = _or_zeros(o_rgb, w, R, 3), _or_zeros(o_depth, w, R), _or_zeros(o_nrm, w, R, 3)
+        mm = mm if mm is not None else _lib.steps_minmax_seed(w.device).clone()
         ctx.tensors = (w, rgb, normals, bins, bg, o_acc, o_depth)
         ctx.bg_mode = bg_mode
         ctx.mark_non_differentiable(mm)
@@ -139,18 +198,9 @@ class RenderAlphasFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, alphas, rgb, normals, bins, bg, bg_mode):
-        lib = _lib.load()
         a = _lib.f32c(alphas)
-        R, S = a.shape
-        dev = a.device
         rgb, normals = _lib.f32c(rgb), _lib.f32c(normals)
-        w = torch.empty(R, S, device=dev)
-        o_rgb, o_depth, o_nrm = torch.empty(R, 3, device=dev), torch.empty(R, device=dev), torch.empty(R, 3, device=dev)
-        o_acc, o_bgT = torch.empty(R, device=dev), torch.empty(R, device=dev)
-        mm = _lib.steps_minmax_seed(dev).clone()
-        out = _lib.render_out(o_rgb, o_depth, o_nrm, o_acc, mm)
-        _lib.check(lib.sdfb200_render_alphas(_lib.ptr(a), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(bins), _lib.ptr(bg), bg_mode, 0, R, S, _lib.ptr(w),
-                                             o_bgT.data_ptr(), out, _lib.stream_ptr()), "sdfb200_render_alphas")
+        w, o_rgb, o_depth, o_nrm, o_acc, o_bgT, mm = launch_render_alphas(a, rgb, normals, bins, bg, bg_mode)
         ctx.tensors = (w, rgb, normals, bins, bg, o_acc, o_depth)
         ctx.alphas = a
         ctx.bg_mode = bg_mode
@@ -183,21 +233,14 @@ class PackedRenderFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, weights, rgb, normals, starts, ends, ray_indices, num_rays, bg, bg_mode):
-        lib = _lib.load()
         w = _lib.f32c(weights)
-        N, R, dev = w.shape[0], int(num_rays), w.device
+        R = int(num_rays)
         rgb = _lib.f32c(rgb) if rgb is not None else None
         normals = _lib.f32c(normals) if normals is not None else None
-        has_depth = starts is not None
-        st, en = (_lib.f32c(starts), _lib.f32c(ends)) if has_depth else (None, None)
-        o_rgb, o_depth, o_nrm = torch.zeros(R, 3, device=dev), torch.zeros(R, device=dev), torch.zeros(R, 3, device=dev)
-        o_acc = torch.empty(R, device=dev)
-        mm = _lib.steps_minmax_seed(dev).clone()
-        out = _lib.render_out(o_rgb if rgb is not None else None, o_depth if has_depth else None, o_nrm if normals is not None else None, o_acc,
-                              mm if has_depth else None)
-        ws = torch.empty(max(R, 1) * 8, device=dev, dtype=torch.float32)
-        _lib.check(lib.sdfb200_render_packed(_lib.ptr(w), _lib.ptr(rgb), _lib.ptr(normals), _lib.ptr(st), _lib.ptr(en), _lib.ptr(ray_indices), N, R,
-                                             _lib.ptr(bg), bg_mode, 0, out, _lib.ptr(ws), ws.numel() * 4, _lib.stream_ptr()), "sdfb200_render_packed")
+        st, en = (_lib.f32c(starts), _lib.f32c(ends)) if starts is not None else (None, None)
+        o_rgb, o_depth, o_nrm, o_acc, mm = launch_render_packed(w, rgb, normals, st, en, ray_indices, R, bg, bg_mode)
+        o_rgb, o_depth, o_nrm = _or_zeros(o_rgb, w, R, 3), _or_zeros(o_depth, w, R), _or_zeros(o_nrm, w, R, 3)
+        mm = mm if mm is not None else _lib.steps_minmax_seed(w.device).clone()
         ctx.tensors = (w, rgb, normals, st, en, ray_indices, bg, o_acc, o_depth)
         ctx.bg_mode = bg_mode
         ctx.mark_non_differentiable(mm)

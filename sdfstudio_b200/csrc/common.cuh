@@ -83,6 +83,92 @@ __device__ __forceinline__ float dsoftplus100_from_h(float h) { return -expm1f(-
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// ---- SDFField heads (sdf_field.py), shared by the generic engine (field_simt.cu) and the fused kernel (field_tc_kernel.cuh).  The
+// expressions are contractible, so both engines get the same fused multiply-adds.
+
+// LaplaceDensity.forward (sdf_field.py:57-71) with beta = |beta| + beta_min
+__device__ __forceinline__ float sdf_density(float sdf, float beta_param, float beta_min) {
+  const float beta = fabsf(beta_param) + beta_min;
+  const float sg = sdf > 0.f ? 1.f : (sdf < 0.f ? -1.f : 0.f);
+  return (1.0f / beta) * (0.5f + 0.5f * sg * expm1f(-fabsf(sdf) / beta));
+}
+
+// get_alpha (sdf_field.py:494-517): true_cos = direction . gradient, delta the sample's length, inv_s = exp(10 variance) clamped
+__device__ __forceinline__ float neus_alpha(float sdf, float true_cos, float delta, float variance, float cos_anneal) {
+  const float inv_s = fminf(fmaxf(expf(variance * 10.0f), 1e-6f), 1e6f);
+  const float iter_cos = -(fmaxf(-true_cos * 0.5f + 0.5f, 0.f) * (1.0f - cos_anneal) + fmaxf(-true_cos, 0.f) * cos_anneal);
+  const float prev_cdf = sigmoidf_((sdf - iter_cos * delta * 0.5f) * inv_s), next_cdf = sigmoidf_((sdf + iter_cos * delta * 0.5f) * inv_s);
+  return fminf(fmaxf((prev_cdf - next_cdf + 1e-5f) / (prev_cdf + 1e-5f), 0.f), 1.f);
+}
+
+// F.normalize(g, p=2, eps=1e-12)
+__device__ __forceinline__ float3 normalize_eps(float x, float y, float z) {
+  const float n = fmaxf(sqrtf(x * x + y * y + z * z), 1e-12f);
+  return make_float3(x / n, y / n, z / n);
+}
+
+// rgb * (1 + 2 padding) - padding (sdf_field.py:610)
+__device__ __forceinline__ float padded_rgb(float rgb, float padding) { return rgb * (1.f + 2.f * padding) - padding; }
+
+// sigmoid(-10 sdf) (sdf_field.py:529)
+__device__ __forceinline__ float occupancy(float sdf) { return sigmoidf_(-10.0f * sdf); }
+
+// ---- transmittance and compositing (cameras/rays.py:131-230, model_components/renderers.py:42-261)
+
+struct ScanAdd {
+  template <class T> __device__ __forceinline__ T operator()(T a, T b) const { return a + b; }
+};
+struct ScanMul {
+  template <class T> __device__ __forceinline__ T operator()(T a, T b) const { return a * b; }
+};
+
+// inclusive scan of v over the 32 lanes of a full warp (Hillis-Steele: log2(32) shuffle steps, every lane in the same order)
+template <class T, class Op = ScanAdd>
+__device__ __forceinline__ T warp_scan_incl(T v, int lane, Op op = Op()) {
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const T o = __shfl_up_sync(0xffffffffu, v, d);
+    if (lane >= d) v = op(v, o);
+  }
+  return v;
+}
+// the exclusive scan from the inclusive one: shifted up by one lane, the identity on lane 0
+template <class T>
+__device__ __forceinline__ T warp_scan_excl(T incl, int lane, T identity) {
+  const T e = __shfl_up_sync(0xffffffffu, incl, 1);
+  return lane == 0 ? identity : e;
+}
+
+// the factor by which a NeuS alpha lowers the transmittance: 1 - alpha + 1e-7 (rays.py:204-206)
+__device__ __forceinline__ float neus_trans_factor(float alpha) { return __fadd_rn(__fsub_rn(1.0f, alpha), 1e-7f); }
+
+// background colour of ray r (renderers.py:97-118): one colour, one per ray, or the ray's last sample colour `last`
+__device__ __forceinline__ void ray_background(int bg_mode, const float* bg, int64_t r, const float* last, float (&c)[3]) {
+  if (bg_mode == SDFB200_BG_COLOR) { c[0] = bg[0]; c[1] = bg[1]; c[2] = bg[2]; }
+  else if (bg_mode == SDFB200_BG_PER_RAY) { c[0] = bg[r * 3]; c[1] = bg[r * 3 + 1]; c[2] = bg[r * 3 + 2]; }
+  else { c[0] = last[0]; c[1] = last[1]; c[2] = last[2]; }
+}
+
+// The end of the compositing of ray r from its sums of w, w rgb, w normal and w step: rgb over the background (clamped to [0, 1] when
+// clamp01), accumulation, normal and expected depth (renderers.py:97-118, 190-197, 249-252).  Contractible: `sum + bg * (1 - acc)` becomes
+// one fma per channel.  A NULL output is not written; the background is read only for the rgb.
+__device__ __forceinline__ void finish_ray(int64_t r, float acc, const float (&wrgb)[3], const float (&wn)[3], float wstep, int bg_mode, const float* bg,
+                                           const float* last, int clamp01, float* o_rgb, float* o_acc, float* o_normal, float* o_depth) {
+  if (o_rgb) {
+    float bgc[3];
+    ray_background(bg_mode, bg, r, last, bgc);
+    const float rem = 1.0f - acc;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float v = wrgb[c] + bgc[c] * rem;
+      o_rgb[r * 3 + c] = clamp01 ? fminf(fmaxf(v, 0.f), 1.f) : v;
+    }
+  }
+  if (o_acc) o_acc[r] = acc;
+  if (o_normal) { o_normal[r * 3] = wn[0]; o_normal[r * 3 + 1] = wn[1]; o_normal[r * 3 + 2] = wn[2]; }
+  if (o_depth) o_depth[r] = wstep / (acc + 1e-10f);
+}
+
 // SceneContraction (spatial_distortions.py:66-73): x <- (2 - 1/|x|) * (x/|x|) where |x| >= 1, |x| the L-inf or L2 norm.  Every
 // operation is rounded on its own (no FMA contraction), so the result is the reference's fp32 one.
 __device__ __forceinline__ void scene_contract(int contraction, float& px, float& py, float& pz) {

@@ -339,9 +339,8 @@ __global__ void __launch_bounds__(256) k_color_inputs(const ColorInArgs a) {
   const int64_t r = a.has_bins ? gi / a.n_samples : gi;
   const float dx = __ldg(a.directions + r * 3), dy = __ldg(a.directions + r * 3 + 1), dz = __ldg(a.directions + r * 3 + 2);
   const float gx = a.grad[i * 3], gy = a.grad[i * 3 + 1], gz = a.grad[i * 3 + 2];
-  // F.normalize(p=2, eps=1e-12)
-  const float nrm = fmaxf(sqrtf(gx * gx + gy * gy + gz * gz), 1e-12f);
-  const float nx = gx / nrm, ny = gy / nrm, nz = gz / nrm;
+  const float3 nv = normalize_eps(gx, gy, gz);
+  const float nx = nv.x, ny = nv.y, nz = nv.z;
   float ex = dx, ey = dy, ez = dz;
   if (a.use_reflections) {
     const float dot = 2.0f * (nx * -dx + ny * -dy + nz * -dz);
@@ -415,8 +414,8 @@ __global__ void __launch_bounds__(256) k_field_post(const PostArgs a) {
   if (a.grad) { gx = a.grad[i * 3]; gy = a.grad[i * 3 + 1]; gz = a.grad[i * 3 + 2]; }
   if (a.gradients) { a.gradients[gi * 3] = gx; a.gradients[gi * 3 + 1] = gy; a.gradients[gi * 3 + 2] = gz; }
   if (a.normals) {
-    const float nrm = fmaxf(sqrtf(gx * gx + gy * gy + gz * gz), 1e-12f);
-    a.normals[gi * 3] = gx / nrm; a.normals[gi * 3 + 1] = gy / nrm; a.normals[gi * 3 + 2] = gz / nrm;
+    const float3 nv = normalize_eps(gx, gy, gz);
+    a.normals[gi * 3] = nv.x; a.normals[gi * 3 + 1] = nv.y; a.normals[gi * 3 + 2] = nv.z;
   }
   if (a.rgb) {
     float rgb[3];
@@ -431,31 +430,16 @@ __global__ void __launch_bounds__(256) k_field_post(const PostArgs a) {
         rgb[c] = fminf(fmaxf(spec + diffuse, 0.f), 1.f);
       }
     }
-    for (int c = 0; c < 3; ++c) a.rgb[gi * 3 + c] = rgb[c] * (1.f + 2.f * a.rgb_padding) - a.rgb_padding;
+    for (int c = 0; c < 3; ++c) a.rgb[gi * 3 + c] = padded_rgb(rgb[c], a.rgb_padding);
   }
-  if (a.density) {
-    // LaplaceDensity.forward, sdf_field.py:57-71
-    const float beta = fabsf(__ldg(a.beta)) + __ldg(a.beta_min);
-    const float al = 1.0f / beta;
-    const float sg = sdf > 0.f ? 1.f : (sdf < 0.f ? -1.f : 0.f);
-    a.density[gi] = al * (0.5f + 0.5f * sg * expm1f(-fabsf(sdf) / beta));
-  }
-  if (a.occupancy) a.occupancy[gi] = sigmoidf_(-10.0f * sdf);
+  if (a.density) a.density[gi] = sdf_density(sdf, __ldg(a.beta), __ldg(a.beta_min));
+  if (a.occupancy) a.occupancy[gi] = occupancy(sdf);
   if (a.alpha) {
-    // get_alpha, sdf_field.py:494-517
     const int64_t r = gi / a.n_samples;
     const int s = (int)(gi - r * a.n_samples);
     const float dxr = __ldg(a.directions + r * 3), dyr = __ldg(a.directions + r * 3 + 1), dzr = __ldg(a.directions + r * 3 + 2);
     const float delta = __fsub_rn(__ldg(a.bins + r * (a.n_samples + 1) + s + 1), __ldg(a.bins + r * (a.n_samples + 1) + s));
-    const float inv_s = fminf(fmaxf(expf(__ldg(a.variance) * 10.0f), 1e-6f), 1e6f);
-    const float true_cos = dxr * gx + dyr * gy + dzr * gz;
-    const float ratio = a.cos_anneal;
-    const float iter_cos = -(fmaxf(-true_cos * 0.5f + 0.5f, 0.f) * (1.0f - ratio) + fmaxf(-true_cos, 0.f) * ratio);
-    const float est_next = sdf + iter_cos * delta * 0.5f;
-    const float est_prev = sdf - iter_cos * delta * 0.5f;
-    const float prev_cdf = sigmoidf_(est_prev * inv_s), next_cdf = sigmoidf_(est_next * inv_s);
-    const float p = prev_cdf - next_cdf, c = prev_cdf;
-    a.alpha[gi] = fminf(fmaxf((p + 1e-5f) / (c + 1e-5f), 0.f), 1.f);
+    a.alpha[gi] = neus_alpha(sdf, dxr * gx + dyr * gy + dzr * gz, delta, __ldg(a.variance), a.cos_anneal);
   }
 }
 

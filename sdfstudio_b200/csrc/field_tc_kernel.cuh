@@ -477,8 +477,8 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
     const long long p_raw = (long long)tile * 128 + row;
     const PointGeom pg = point_geom(a, p_raw < a.n_points ? p_raw : a.n_points - 1);
     const float grx = h ? g1x : g0x, gry = h ? g1y : g0y, grz = h ? g1z : g0z;
-    const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
-    const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? (grx / gn) * pg.dx + (gry / gn) * pg.dy + (grz / gn) * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
+    const float3 n = normalize_eps(grx, gry, grz);
+    const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? n.x * pg.dx + n.y * pg.dy + n.z * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
     store_a_chunk<P>(x.abuf, kAPlane, row, 0, c0v);
     x.hs[HS_GRAD][row] = grx; x.hs[HS_GRAD + 1][row] = gry; x.hs[HS_GRAD + 2][row] = grz;
   }
@@ -565,33 +565,21 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
   const PointGeom pg = point_geom(a, p);
   const float dirx = pg.dx, diry = pg.dy, dirz = pg.dz, delta = pg.delta;
   const float sdf = hs[HS_SDF][row], grx = hs[HS_GRAD][row], gry = hs[HS_GRAD + 1][row], grz = hs[HS_GRAD + 2][row];
-  const float gn = fmaxf(sqrtf(grx * grx + gry * gry + grz * grz), 1e-12f);      // F.normalize eps
-  const float nx = grx / gn, ny = gry / gn, nz = grz / gn;
+  const float3 nv = normalize_eps(grx, gry, grz);
+  const float nx = nv.x, ny = nv.y, nz = nv.z;
   float rgbv[3];
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const float raw = hs[HS_RGB + c][row] + __ldg(b_c2 + c);
-    rgbv[c] = sigmoidf_(raw) * (1.f + 2.f * a.rgb_padding) - a.rgb_padding;
-  }
+  for (int c = 0; c < 3; ++c) rgbv[c] = padded_rgb(sigmoidf_(hs[HS_RGB + c][row] + __ldg(b_c2 + c)), a.rgb_padding);
   float density = 0.f, alpha = 0.f;
-  if (a.out.density || (a.render && a.rnd.from_density)) {
-    const float beta = fabsf(__ldg(a.beta)) + __ldg(a.beta_min);
-    const float sg = sdf > 0.f ? 1.f : (sdf < 0.f ? -1.f : 0.f);
-    density = (1.0f / beta) * (0.5f + 0.5f * sg * expm1f(-fabsf(sdf) / beta));
-  }
-  if (a.out.alpha || (a.render && !a.rnd.from_density)) {
-    const float inv_s = fminf(fmaxf(expf(__ldg(a.variance) * 10.0f), 1e-6f), 1e6f);
-    const float true_cos = dirx * grx + diry * gry + dirz * grz;
-    const float iter_cos = -(fmaxf(-true_cos * 0.5f + 0.5f, 0.f) * (1.0f - a.cos_anneal) + fmaxf(-true_cos, 0.f) * a.cos_anneal);
-    const float prev_cdf = sigmoidf_((sdf - iter_cos * delta * 0.5f) * inv_s), next_cdf = sigmoidf_((sdf + iter_cos * delta * 0.5f) * inv_s);
-    alpha = fminf(fmaxf((prev_cdf - next_cdf + 1e-5f) / (prev_cdf + 1e-5f), 0.f), 1.f);
-  }
+  if (a.out.density || (a.render && a.rnd.from_density)) density = sdf_density(sdf, __ldg(a.beta), __ldg(a.beta_min));
+  if (a.out.alpha || (a.render && !a.rnd.from_density))
+    alpha = neus_alpha(sdf, dirx * grx + diry * gry + dirz * grz, delta, __ldg(a.variance), a.cos_anneal);
   if (valid) {
     if (a.out.rgb) { a.out.rgb[p * 3] = rgbv[0]; a.out.rgb[p * 3 + 1] = rgbv[1]; a.out.rgb[p * 3 + 2] = rgbv[2]; }
     if (a.out.gradients) { a.out.gradients[p * 3] = grx; a.out.gradients[p * 3 + 1] = gry; a.out.gradients[p * 3 + 2] = grz; }
     if (a.out.normals) { a.out.normals[p * 3] = nx; a.out.normals[p * 3 + 1] = ny; a.out.normals[p * 3 + 2] = nz; }
     if (a.out.density) a.out.density[p] = density;
-    if (a.out.occupancy) a.out.occupancy[p] = sigmoidf_(-10.0f * sdf);
+    if (a.out.occupancy) a.out.occupancy[p] = occupancy(sdf);
     if (a.out.alpha) a.out.alpha[p] = alpha;
   }
   if (a.render) {
@@ -605,8 +593,9 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
     // factor by which the transmittance drops across this sample: 1 - alpha + 1e-7 (rays.py:204-206), or as an exponent
     // delta * sigma for the density form (rays.py:160-170)
     const float dd = valid ? __fmul_rn(delta, density) : 0.f;
-    double f = dens ? (double)dd : (valid ? (double)__fadd_rn(__fsub_rn(1.0f, alpha), 1e-7f) : 1.0);
+    double f = dens ? (double)dd : (valid ? (double)neus_trans_factor(alpha) : 1.0);
     double incl = f;
+    // segmented by ray (s_idx >= d), so not the plain warp_scan_incl of common.cuh
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
       const double o = __shfl_up_sync(0xffffffffu, incl, d);
@@ -659,20 +648,9 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
     }
     const long long ray = (long long)tile * (128 / S) + row / S;
     if (ray_end && s_idx == (multi ? S - 32 : 0) && ray * S < a.n_points) {
-      const float acc = vs[0];
-      if (a.rnd.out.rgb) {
-        float bgc[3] = {0.f, 0.f, 0.f};
-        if (a.rnd.bg_mode == SDFB200_BG_COLOR) { bgc[0] = a.rnd.bg[0]; bgc[1] = a.rnd.bg[1]; bgc[2] = a.rnd.bg[2]; }
-        else if (a.rnd.bg_mode == SDFB200_BG_PER_RAY) { bgc[0] = a.rnd.bg[ray * 3]; bgc[1] = a.rnd.bg[ray * 3 + 1]; bgc[2] = a.rnd.bg[ray * 3 + 2]; }
-        else { bgc[0] = lr; bgc[1] = lg; bgc[2] = lb; }
-        const float rem = 1.0f - acc;
-        const float o[3] = {vs[1] + bgc[0] * rem, vs[2] + bgc[1] * rem, vs[3] + bgc[2] * rem};
-#pragma unroll
-        for (int c = 0; c < 3; ++c) a.rnd.out.rgb[ray * 3 + c] = a.rnd.clamp01 ? fminf(fmaxf(o[c], 0.f), 1.f) : o[c];
-      }
-      if (a.rnd.out.accumulation) a.rnd.out.accumulation[ray] = acc;
-      if (a.rnd.out.normal) { a.rnd.out.normal[ray * 3] = vs[4]; a.rnd.out.normal[ray * 3 + 1] = vs[5]; a.rnd.out.normal[ray * 3 + 2] = vs[6]; }
-      if (a.rnd.out.depth) a.rnd.out.depth[ray] = vs[7] / (acc + 1e-10f);
+      const float last[3] = {lr, lg, lb};
+      finish_ray(ray, vs[0], {vs[1], vs[2], vs[3]}, {vs[4], vs[5], vs[6]}, vs[7], a.rnd.bg_mode, a.rnd.bg, last, a.rnd.clamp01, a.rnd.out.rgb,
+                 a.rnd.out.accumulation, a.rnd.out.normal, a.rnd.out.depth);
       if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)tot) : (float)tot;
     }
     if (multi && ray_end) {

@@ -15,16 +15,6 @@ constexpr size_t kInterlevelSmemBudget = 48 * 1024;
 
 constexpr unsigned kFullWarp = 0xffffffffu;
 
-// inclusive prefix sum over the warp's 32 values
-__device__ __forceinline__ double warp_scan(double v, int lane) {
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const double u = __shfl_up_sync(kFullWarp, v, d);
-    if (lane >= d) v += u;
-  }
-  return v;
-}
-
 // butterfly sum: every lane ends with the same value, added in the same order on every call
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
@@ -117,14 +107,14 @@ k_interlevel_zip(const float* __restrict__ c_all, const float* __restrict__ w_al
     const int k = base + lane;
     const bool live = k < nk - 1;
     const float dx = live ? __fsub_rn(x[k + 1], x[k]) : 0.f;
-    const double inner_d = carry_inner + warp_scan(live ? (double)slope[k] : 0.0, lane);
+    const double inner_d = carry_inner + warp_scan_incl(live ? (double)slope[k] : 0.0, lane);
     const float inner = (float)inner_d;
-    const double yr_d = carry_yr + warp_scan(live ? (double)__fmul_rn(dx, inner) : 0.0, lane);
+    const double yr_d = carry_yr + warp_scan_incl(live ? (double)__fmul_rn(dx, inner) : 0.0, lane);
     const float yr_hi = clip0((float)yr_d);   // y_r[k+1]
     float yr_lo = __shfl_up_sync(kFullWarp, yr_hi, 1);
     if (lane == 0) yr_lo = prev_yr;
     const float area = __fmul_rn(__fmul_rn(__fadd_rn(yr_hi, yr_lo), 0.5f), dx);
-    const double cum_d = carry_cum + warp_scan(live ? (double)area : 0.0, lane);
+    const double cum_d = carry_cum + warp_scan_incl(live ? (double)area : 0.0, lane);
     if (live) ycum[k + 1] = (float)cum_d;
     // the running sums stay in double across tiles: only what is stored or multiplied is rounded to fp32, as in one long cumsum
     carry_inner = __shfl_sync(kFullWarp, inner_d, 31);
@@ -189,7 +179,7 @@ k_interlevel_outer(const float* __restrict__ c_all, const float* __restrict__ w_
   double carry = 0.0;
   for (int base = 0; base < sp; base += 32) {
     const int j = base + lane;
-    const double s = carry + warp_scan(j < sp ? (double)wp[j] : 0.0, lane);
+    const double s = carry + warp_scan_incl(j < sp ? (double)wp[j] : 0.0, lane);
     if (j < sp) cy[j + 1] = (float)s;
     carry = __shfl_sync(kFullWarp, s, 31);
   }
@@ -211,7 +201,7 @@ k_interlevel_outer(const float* __restrict__ c_all, const float* __restrict__ w_
       sum += (double)__fmul_rn(m, q);              // m^2 / (w + eps)
       g = -2.0 * (double)q;
     }
-    const double s = carry + warp_scan(g, lane);
+    const double s = carry + warp_scan_incl(g, lane);
     if (i < sf) gsum[i + 1] = s;
     carry = __shfl_sync(kFullWarp, s, 31);
   }

@@ -118,12 +118,7 @@ __device__ void emit_vertex(const McArgs& a, int64_t i, int64_t j, int64_t k, in
 }
 
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int& total) {
-  int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
+  const int x = warp_scan_incl(v, lane);
   total = __shfl_sync(0xffffffffu, x, 31);
   return x - v;
 }

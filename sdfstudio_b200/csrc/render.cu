@@ -15,7 +15,7 @@ __global__ void __launch_bounds__(128) k_weights_from_alphas(const float* __rest
     const float Tf = (float)T;
     if (trans) trans[r * (S + 1) + i] = Tf;
     weights[r * S + i] = __fmul_rn(a, Tf);
-    T *= (double)__fadd_rn(__fsub_rn(1.0f, a), 1e-7f);
+    T *= (double)neus_trans_factor(a);
   }
   if (trans) trans[r * (S + 1) + S] = (float)T;
 }
@@ -72,10 +72,8 @@ __global__ void __launch_bounds__(128) k_render(const RenderArgs a) {
       }
     }
     if (a.o_rgb && a.rgb) {
-      float bgc[3] = {0.f, 0.f, 0.f};
-      if (a.bg_mode == SDFB200_BG_COLOR) { bgc[0] = a.bg[0]; bgc[1] = a.bg[1]; bgc[2] = a.bg[2]; }
-      else if (a.bg_mode == SDFB200_BG_PER_RAY) { bgc[0] = a.bg[r * 3]; bgc[1] = a.bg[r * 3 + 1]; bgc[2] = a.bg[r * 3 + 2]; }
-      else { const float* c = a.rgb + (r * S + S - 1) * 3; bgc[0] = c[0]; bgc[1] = c[1]; bgc[2] = c[2]; }
+      float bgc[3];
+      ray_background(a.bg_mode, a.bg, r, a.rgb + (r * S + S - 1) * 3, bgc);
       const float rem = __fsub_rn(1.0f, acc);
       float o[3] = {__fadd_rn(cr, __fmul_rn(bgc[0], rem)), __fadd_rn(cg, __fmul_rn(bgc[1], rem)), __fadd_rn(cb, __fmul_rn(bgc[2], rem))};
       for (int c = 0; c < 3; ++c) a.o_rgb[r * 3 + c] = a.clamp01 ? fminf(fmaxf(o[c], 0.f), 1.f) : o[c];
@@ -126,15 +124,8 @@ __global__ void __launch_bounds__(256) k_render_alphas(const RenderAlphaArgs a) 
     const int s = s0 + lane;
     const bool on = s < S;
     const float al = on ? a.alphas[r * S + s] : 0.f;
-    double f = on ? (double)__fadd_rn(__fsub_rn(1.0f, al), 1e-7f) : 1.0;   // rays.py:204-206
-    double incl = f;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const double o = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl *= o;
-    }
-    double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl = 1.0;
+    const double incl = warp_scan_incl(on ? (double)neus_trans_factor(al) : 1.0, lane, ScanMul());
+    const double excl = warp_scan_excl(incl, lane, 1.0);
     const float T = (float)(carry * excl);
     carry *= __shfl_sync(0xffffffffu, incl, 31);
     const float w = __fmul_rn(al, T);
@@ -158,19 +149,9 @@ __global__ void __launch_bounds__(256) k_render_alphas(const RenderAlphaArgs a) 
     smin = fminf(smin, __shfl_xor_sync(0xffffffffu, smin, d)); smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, d));
   }
   if (lane == 0) {
-    if (a.o_rgb && a.rgb) {
-      float bgc[3] = {0.f, 0.f, 0.f};
-      if (a.bg_mode == SDFB200_BG_COLOR) { bgc[0] = a.bg[0]; bgc[1] = a.bg[1]; bgc[2] = a.bg[2]; }
-      else if (a.bg_mode == SDFB200_BG_PER_RAY) { bgc[0] = a.bg[r * 3]; bgc[1] = a.bg[r * 3 + 1]; bgc[2] = a.bg[r * 3 + 2]; }
-      else { const float* c = a.rgb + (r * S + S - 1) * 3; bgc[0] = c[0]; bgc[1] = c[1]; bgc[2] = c[2]; }
-      const float rem = 1.0f - acc;
-      const float o[3] = {cr + bgc[0] * rem, cg + bgc[1] * rem, cb + bgc[2] * rem};
-      for (int c = 0; c < 3; ++c) a.o_rgb[r * 3 + c] = a.clamp01 ? fminf(fmaxf(o[c], 0.f), 1.f) : o[c];
-    }
-    if (a.o_acc) a.o_acc[r] = acc;
+    finish_ray(r, acc, {cr, cg, cb}, {nx, ny, nz}, dsum, a.bg_mode, a.bg, a.rgb + (r * S + S - 1) * 3, a.clamp01, a.rgb ? a.o_rgb : nullptr, a.o_acc,
+               a.normals ? a.o_normal : nullptr, a.eu ? a.o_depth : nullptr);
     if (a.o_bgT) a.o_bgT[r] = (float)carry;                               // transmittance[:, -1] (bg_transmittance)
-    if (a.o_normal && a.normals) { a.o_normal[r * 3] = nx; a.o_normal[r * 3 + 1] = ny; a.o_normal[r * 3 + 2] = nz; }
-    if (a.o_depth && a.eu) a.o_depth[r] = dsum / (acc + 1e-10f);
     if (a.o_minmax && a.eu && smin <= smax) { atomic_min_float(a.o_minmax, smin); atomic_max_float(a.o_minmax + 1, smax); }
   }
 }
@@ -217,6 +198,7 @@ __global__ void k_render_packed_finish(const float* __restrict__ acc, int64_t R,
   if (r >= R) return;
   const float* a = acc + r * 8;
   const float w = a[0];
+  // not finish_ray: packed samples have no last-sample background, and its three-way background select costs 20 % more instructions here
   if (o_rgb) {
     const float* b = bg_mode == SDFB200_BG_PER_RAY ? bg + r * 3 : bg;
     const float rem = 1.0f - w;
@@ -247,14 +229,8 @@ __global__ void __launch_bounds__(256) k_packed_weights(const float* __restrict_
     const int64_t s = s0 + lane;
     const bool on = s < e;
     const float al = on ? alphas[s] : 0.f;
-    double incl = 1.0 - (double)al;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const double o = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl *= o;
-    }
-    double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl = 1.0;
+    const double incl = warp_scan_incl(1.0 - (double)al, lane, ScanMul());
+    const double excl = warp_scan_excl(incl, lane, 1.0);
     if (on) weights[s] = (float)((double)al * (carry * excl));
     carry *= __shfl_sync(0xffffffffu, incl, 31);
   }

@@ -25,11 +25,9 @@ __global__ void __launch_bounds__(256) k_render_bwd(const RenderBwdArgs a) {
   if (a.g_rgb) {
     const float g0 = a.g_rgb[r * 3], g1 = a.g_rgb[r * 3 + 1], g2 = a.g_rgb[r * 3 + 2];
     const float* c = a.rgb + i * 3;
-    float b0 = 0.f, b1 = 0.f, b2 = 0.f;
-    if (a.bg_mode == SDFB200_BG_COLOR) { b0 = a.bg[0]; b1 = a.bg[1]; b2 = a.bg[2]; }
-    else if (a.bg_mode == SDFB200_BG_PER_RAY) { b0 = a.bg[r * 3]; b1 = a.bg[r * 3 + 1]; b2 = a.bg[r * 3 + 2]; }
-    else { const float* cl = a.rgb + (r * S + S - 1) * 3; b0 = cl[0]; b1 = cl[1]; b2 = cl[2]; }
-    gw += g0 * (c[0] - b0) + g1 * (c[1] - b1) + g2 * (c[2] - b2);   // out = sum w c + bg (1 - sum w)
+    float b[3];
+    ray_background(a.bg_mode, a.bg, r, a.rgb + (r * S + S - 1) * 3, b);
+    gw += g0 * (c[0] - b[0]) + g1 * (c[1] - b[1]) + g2 * (c[2] - b[2]);   // out = sum w c + bg (1 - sum w)
     if (a.g_rgb_s) {
       float e0 = g0 * w, e1 = g1 * w, e2 = g2 * w;
       if (a.bg_mode == SDFB200_BG_LAST_SAMPLE && s == S - 1) {
@@ -79,29 +77,15 @@ __global__ void __launch_bounds__(256) k_weights_bwd(const float* __restrict__ i
       float f = 1.f, al = 0.f, delta = 0.f, T;
       if (!from_density) {
         al = on ? in[r * S + s] : 0.f;
-        f = on ? __fadd_rn(__fsub_rn(1.0f, al), 1e-7f) : 1.f;
-        double incl = (double)f;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const double o = __shfl_up_sync(0xffffffffu, incl, d);
-          if (lane >= d) incl *= o;
-        }
-        double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-        if (lane == 0) excl = 1.0;
-        T = (float)(carryT * excl);
+        f = on ? neus_trans_factor(al) : 1.f;
+        const double incl = warp_scan_incl((double)f, lane, ScanMul());
+        T = (float)(carryT * warp_scan_excl(incl, lane, 1.0));
         carryT *= __shfl_sync(0xffffffffu, incl, 31);
       } else {
         delta = on ? __fsub_rn(eu[r * (S + 1) + s + 1], eu[r * (S + 1) + s]) : 0.f;
         const float dd = on ? __fmul_rn(delta, in[r * S + s]) : 0.f;
-        double incl = (double)dd;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const double o = __shfl_up_sync(0xffffffffu, incl, d);
-          if (lane >= d) incl += o;
-        }
-        double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-        if (lane == 0) excl = 0.0;
-        T = expf(-(float)(carryI + excl));
+        const double incl = warp_scan_incl((double)dd, lane);
+        T = expf(-(float)(carryI + warp_scan_excl(incl, lane, 0.0)));
         carryI += __shfl_sync(0xffffffffu, incl, 31);
         f = expf(-dd);
         al = 1.0f - f;
@@ -109,12 +93,7 @@ __global__ void __launch_bounds__(256) k_weights_bwd(const float* __restrict__ i
       const float gw = on ? g_weights[r * S + s] : 0.f;
       const float gt = (on && (from_density ? gt_cols >= 1 : gt_cols > 1)) ? g_T[r * gt_cols + s] : 0.f;
       const double u = (double)gw * (double)(al * T) + (double)gt * (double)T;
-      double uincl = u;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const double o = __shfl_up_sync(0xffffffffu, uincl, d);
-        if (lane >= d) uincl += o;
-      }
+      const double uincl = warp_scan_incl(u, lane);
       if (pass == 1 && on) {
         const double suffix = U - (carryU + uincl);                       // sum_{k>s} gw_k w_k
         const double tail = suffix + ((!from_density && gt_cols >= 1) ? (double)g_T[r * gt_cols + (gt_cols - 1)] * TS : 0.0);
@@ -142,14 +121,8 @@ __global__ void __launch_bounds__(256) k_packed_weights_bwd(const float* __restr
   for (int64_t s0 = b; s0 < e; s0 += 32) {
     const int64_t s = s0 + lane;
     const bool on = s < e;
-    double incl = on ? 1.0 - (double)alphas[s] : 1.0;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const double o = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl *= o;
-    }
-    double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl = 1.0;
+    const double incl = warp_scan_incl(on ? 1.0 - (double)alphas[s] : 1.0, lane, ScanMul());
+    const double excl = warp_scan_excl(incl, lane, 1.0);
     if (on) g_alpha[s] = (float)(carry * excl);
     carry *= __shfl_sync(0xffffffffu, incl, 31);
   }
@@ -194,6 +167,7 @@ __global__ void __launch_bounds__(256) k_render_packed_bwd(const PackedRenderBwd
   const float w = a.weights[i];
   float gw = 0.f, e[3] = {0.f, 0.f, 0.f}, m[3] = {0.f, 0.f, 0.f}, gs = 0.f;
   if (in && a.g_rgb) {
+    // not ray_background: packed samples have no last-sample background, and the pointer select here takes 2 registers fewer
     const float* b = a.bg_mode == SDFB200_BG_PER_RAY ? a.bg + r * 3 : a.bg;
     for (int c = 0; c < 3; ++c) {
       const float g = a.g_rgb[r * 3 + c];

@@ -177,7 +177,7 @@ __global__ void __launch_bounds__(128) k_neus_weights(const float* __restrict__ 
     const float next_cdf = sigmoidf_(__fmul_rn(__fadd_rn(mid, half), inv_s));
     const float alpha = __fdiv_rn(__fadd_rn(__fsub_rn(prev_cdf, next_cdf), 1e-5f), __fadd_rn(prev_cdf, 1e-5f));
     w[i] = __fmul_rn(alpha, (float)T);
-    T *= (double)__fadd_rn(__fsub_rn(1.0f, alpha), 1e-7f);
+    T *= (double)neus_trans_factor(alpha);
   }
   w[S - 1] = 0.f;
 }
@@ -234,14 +234,6 @@ __device__ __forceinline__ float volsdf_dstar(const float* e, const float* sd, i
 // is NaN only where I is NaN too, and the NaN-keeping clamp of exp(E) below and the plain fminf of the err weights in k_volsdf_step give
 // the same results.
 constexpr int kVolsdfMaxS = 1000;   // 4 rays x 3 x S floats of dynamic shared memory stay under the 48 KB default
-__device__ __forceinline__ double warp_scan_incl(double v, int lane) {
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const double o = __shfl_up_sync(0xffffffffu, v, d);
-    if (lane >= d) v += o;
-  }
-  return v;
-}
 __device__ float volsdf_error_bound_warp(const float* delta_s, const float* dstar_s, const float* sdf_s, int S, float beta, int lane) {
   double carryE = 0.0, carryI = 0.0;
   float best = -INFINITY;

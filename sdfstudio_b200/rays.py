@@ -93,13 +93,8 @@ def weights_from_alphas(alphas: torch.Tensor, with_transmittance: bool = False):
     """rays.py:194-230.  alphas [R,S,1] -> weights [R,S,1] (, transmittance [R,S+1,1])."""
     if _ag.needs_grad(alphas):
         w, T = _ag.WeightsFromAlphasFn.apply(alphas[..., 0])
-        return (w[..., None], T[..., None]) if with_transmittance else w[..., None]
-    lib = _lib.load()
-    a = _lib.f32c(alphas[..., 0])
-    R, S = a.shape
-    w = torch.empty_like(a)
-    T = torch.empty(R, S + 1, device=a.device, dtype=torch.float32) if with_transmittance else None
-    _lib.check(lib.sdfb200_weights_from_alphas(_lib.ptr(a), R, S, _lib.ptr(w), _lib.ptr(T), _lib.stream_ptr()), "sdfb200_weights_from_alphas")
+    else:
+        w, T = _ag.launch_weights_from_alphas(_lib.f32c(alphas[..., 0]), with_transmittance)
     return (w[..., None], T[..., None]) if with_transmittance else w[..., None]
 
 
@@ -107,14 +102,8 @@ def weights_from_density(bins: torch.Tensor, densities: torch.Tensor, with_trans
     """rays.py:146-192.  bins [R,S+1] euclidean, densities [R,S,1]."""
     if _ag.needs_grad(densities):
         w, T = _ag.WeightsFromDensityFn.apply(densities[..., 0], bins)
-        return (w[..., None], T[..., None]) if with_transmittance else w[..., None]
-    lib = _lib.load()
-    d = _lib.f32c(densities[..., 0])
-    R, S = d.shape
-    w = torch.empty_like(d)
-    T = torch.empty_like(d) if with_transmittance else None
-    _lib.check(lib.sdfb200_weights_from_density(_lib.ptr(d), _lib.ptr(bins), R, S, _lib.ptr(w), _lib.ptr(T), _lib.stream_ptr()),
-               "sdfb200_weights_from_density")
+    else:
+        w, T = _ag.launch_weights_from_density(_lib.f32c(densities[..., 0]), bins, with_transmittance)
     return (w[..., None], T[..., None]) if with_transmittance else w[..., None]
 
 

@@ -54,36 +54,26 @@ def _render(weights, rgb=None, normals=None, bins=None, background=None, clamp01
             want_acc=False, want_normal=False, clip_depth=True):
     if _ag.needs_grad(weights, rgb, normals if want_normal else None):
         return _render_grad(weights, rgb, normals, bins, background, clamp01, depth_method, want_acc, want_normal, clip_depth)
-    lib = _lib.load()
     w = _lib.f32c(weights[..., 0])
-    R, S = w.shape
-    dev = w.device
-    res = {}
-    bg_mode, bg_t = _lib.BG_COLOR, None
-    rgb_c = nrm_c = mm = None
-    if rgb is not None:
-        rgb_c = _lib.f32c(rgb)
-        res["rgb"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
-        bg_mode, bg_t = _background(background, R, dev)
-    if want_normal:
-        nrm_c = _lib.f32c(normals)
-        if nrm_c.shape[-1] != 3:
-            raise NotImplementedError("SemanticRenderer: only 3 channels (normals) are composited by the kernel")
-        res["normal"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
-    if want_acc:
-        res["accumulation"] = torch.empty(R, device=dev, dtype=torch.float32)
-    if depth_method is not None:
-        res["depth"] = torch.empty(R, device=dev, dtype=torch.float32)
-        mm = _lib.steps_minmax_seed(dev).clone()
-    out = _lib.render_out(res.get("rgb"), res.get("depth"), res.get("normal"), res.get("accumulation"), mm)
-    _lib.check(lib.sdfb200_render(_lib.ptr(w), _lib.ptr(rgb_c), _lib.ptr(nrm_c), _lib.ptr(bins), _lib.ptr(bg_t), bg_mode, int(clamp01),
-                                  int(depth_method == "median"), R, S, out, _lib.stream_ptr()), "sdfb200_render")
+    R = w.shape[0]
+    bg_mode, bg_t = _background(background, R, w.device) if rgb is not None else (_lib.BG_COLOR, None)
+    nrm_c = _lib.f32c(normals) if want_normal else None
+    if nrm_c is not None and nrm_c.shape[-1] != 3:
+        raise NotImplementedError("SemanticRenderer: only 3 channels (normals) are composited by the kernel")
+    o_rgb, o_depth, o_nrm, o_acc, mm = _ag.launch_render(w, _lib.f32c(rgb) if rgb is not None else None, nrm_c,
+                                                         bins if depth_method is not None else None, bg_t, bg_mode, clamp01,
+                                                         depth_method == "median", want_acc)
     if depth_method == "expected" and clip_depth:
-        _lib.check(lib.sdfb200_depth_clip(out.depth, out.steps_minmax, R, _lib.stream_ptr()), "sdfb200_depth_clip")
-    if "depth" in res:
-        res["depth"] = res["depth"][:, None]
-    if "accumulation" in res:
-        res["accumulation"] = res["accumulation"][:, None]
+        _lib.check(_lib.load().sdfb200_depth_clip(_lib.ptr(o_depth), _lib.ptr(mm), R, _lib.stream_ptr()), "sdfb200_depth_clip")
+    res = {}
+    if o_rgb is not None:
+        res["rgb"] = o_rgb
+    if o_nrm is not None:
+        res["normal"] = o_nrm
+    if o_acc is not None:
+        res["accumulation"] = o_acc[:, None]
+    if o_depth is not None:
+        res["depth"] = o_depth[:, None]
     return res
 
 
@@ -124,37 +114,26 @@ def _render_packed(weights, ray_indices, num_rays, rgb=None, normals=None, ray_s
     if _ag.needs_grad(weights, rgb, normals if want_normal else None, starts, ends):
         return _render_packed_grad(weights, idx, int(num_rays), rgb, normals if want_normal else None, starts, ends, background, clamp01,
                                    want_acc)
-    lib = _lib.load()
     w = _lib.f32c(weights.reshape(-1))
-    N, R = w.shape[0], int(num_rays)
-    dev = w.device
-    res = {}
-    rgb_c = nrm_c = st = en = bg_t = mm = None
-    bg_mode = _lib.BG_COLOR
+    R = int(num_rays)
+    bg_mode, bg_t = _lib.BG_COLOR, None
     if rgb is not None:
         if isinstance(background, str) and background == "last_sample":
             raise NotImplementedError("Background color 'last_sample' not implemented for packed samples.")
-        bg_mode, bg_t = _background(background, R, dev)
-        rgb_c = _lib.f32c(rgb.reshape(-1, 3))
-        res["rgb"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
-    if want_normal:
-        nrm_c = _lib.f32c(normals.reshape(-1, 3))
-        res["normal"] = torch.empty(R, 3, device=dev, dtype=torch.float32)
-    if want_acc:
-        res["accumulation"] = torch.empty(R, device=dev, dtype=torch.float32)
-    if want_depth:
-        st, en = _lib.f32c(ray_samples.frustums.starts.reshape(-1)), _lib.f32c(ray_samples.frustums.ends.reshape(-1))
-        res["depth"] = torch.empty(R, device=dev, dtype=torch.float32)
-        mm = _lib.steps_minmax_seed(dev).clone()
-    out = _lib.render_out(res.get("rgb"), res.get("depth"), res.get("normal"), res.get("accumulation"), mm)
-    ws = torch.empty(max(R, 1) * 8, device=dev, dtype=torch.float32)
-    _lib.check(lib.sdfb200_render_packed(_lib.ptr(w), _lib.ptr(rgb_c), _lib.ptr(nrm_c), _lib.ptr(st), _lib.ptr(en), _lib.ptr(idx), N, R, _lib.ptr(bg_t), bg_mode,
-                                         int(clamp01), out, _lib.ptr(ws), ws.numel() * 4, _lib.stream_ptr()), "sdfb200_render_packed")
-    if want_depth:
-        _lib.check(lib.sdfb200_depth_clip(out.depth, out.steps_minmax, R, _lib.stream_ptr()), "sdfb200_depth_clip")
-        res["depth"] = res["depth"][:, None]
-    if want_acc:
-        res["accumulation"] = res["accumulation"][:, None]
+        bg_mode, bg_t = _background(background, R, w.device)
+    rs = lambda t, *shape: _lib.f32c(t.reshape(*shape)) if t is not None else None  # noqa: E731
+    o_rgb, o_depth, o_nrm, o_acc, mm = _ag.launch_render_packed(w, rs(rgb, -1, 3), rs(normals if want_normal else None, -1, 3), rs(starts, -1),
+                                                                rs(ends, -1), idx, R, bg_t, bg_mode, clamp01, want_acc)
+    res = {}
+    if o_rgb is not None:
+        res["rgb"] = o_rgb
+    if o_nrm is not None:
+        res["normal"] = o_nrm
+    if o_acc is not None:
+        res["accumulation"] = o_acc[:, None]
+    if o_depth is not None:
+        _lib.check(_lib.load().sdfb200_depth_clip(_lib.ptr(o_depth), _lib.ptr(mm), R, _lib.stream_ptr()), "sdfb200_depth_clip")
+        res["depth"] = o_depth[:, None]
     return res
 
 
@@ -230,21 +209,13 @@ def render_from_alphas(alphas, rgb, normals, ray_samples, background, training: 
         if want_weights:
             res["weights"] = w[..., None]
         return res
-    lib = _lib.load()
     a = _lib.f32c(alphas[..., 0])
-    R, S = a.shape
-    dev = a.device
-    rgb_c, nrm_c, bins = _lib.f32c(rgb), _lib.f32c(normals), bins_of(ray_samples)
-    bg_mode, bg_t = _background(background, R, dev)
-    res = {"rgb": torch.empty(R, 3, device=dev), "depth": torch.empty(R, device=dev), "normal": torch.empty(R, 3, device=dev),
-           "accumulation": torch.empty(R, device=dev), "bg_transmittance": torch.empty(R, device=dev)}
-    w = torch.empty(R, S, device=dev) if want_weights else None
-    mm = _lib.steps_minmax_seed(dev).clone()
-    out = _lib.render_out(res["rgb"], res["depth"], res["normal"], res["accumulation"], mm)
-    _lib.check(lib.sdfb200_render_alphas(_lib.ptr(a), _lib.ptr(rgb_c), _lib.ptr(nrm_c), _lib.ptr(bins), _lib.ptr(bg_t), bg_mode, int(not training), R, S,
-                                         _lib.ptr(w), res["bg_transmittance"].data_ptr(), out, _lib.stream_ptr()), "sdfb200_render_alphas")
-    _lib.check(lib.sdfb200_depth_clip(out.depth, out.steps_minmax, R, _lib.stream_ptr()), "sdfb200_depth_clip")
-    res["depth"], res["accumulation"], res["bg_transmittance"] = res["depth"][:, None], res["accumulation"][:, None], res["bg_transmittance"][:, None]
+    R = a.shape[0]
+    bg_mode, bg_t = _background(background, R, a.device)
+    w, o_rgb, o_depth, o_nrm, o_acc, o_bgT, mm = _ag.launch_render_alphas(a, _lib.f32c(rgb), _lib.f32c(normals), bins_of(ray_samples), bg_t, bg_mode,
+                                                                           not training, want_weights)
+    _lib.check(_lib.load().sdfb200_depth_clip(_lib.ptr(o_depth), _lib.ptr(mm), R, _lib.stream_ptr()), "sdfb200_depth_clip")
+    res = {"rgb": o_rgb, "depth": o_depth[:, None], "normal": o_nrm, "accumulation": o_acc[:, None], "bg_transmittance": o_bgT[:, None]}
     if want_weights:
         res["weights"] = w[..., None]
     return res

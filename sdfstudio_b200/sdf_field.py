@@ -499,15 +499,7 @@ class SDFField(nn.Module):
             origins, directions, bins, shape = sample_geometry(ray_samples)
             o = self._run(origins, directions, bins, bins.shape[1] - 1, ("alpha",), apply_contraction=False)
             return o["alpha"].view(*shape, 1)
-        inv_s = self.deviation_network.get_variance()
-        d = ray_samples.frustums.directions
-        true_cos = (d * gradients).sum(-1, keepdim=True)
-        r = self._cos_anneal_ratio
-        iter_cos = -(torch.relu(-true_cos * 0.5 + 0.5) * (1.0 - r) + torch.relu(-true_cos) * r)
-        deltas = ray_samples.deltas
-        prev_cdf = torch.sigmoid((sdf - iter_cos * deltas * 0.5) * inv_s)
-        next_cdf = torch.sigmoid((sdf + iter_cos * deltas * 0.5) * inv_s)
-        return ((prev_cdf - next_cdf + 1e-5) / (prev_cdf + 1e-5)).clip(0.0, 1.0)
+        return _train.get_alpha(self, ray_samples, sdf, gradients)
 
     def _appearance(self, camera_indices, R, device):
         c = self.config

@@ -52,6 +52,13 @@ def _cases():
         yield f"from_alphas/{bn}", lambda bg=bg: sb.render_from_alphas(alphas, rgb, nrm, rs, bg)
         yield f"from_alphas_grad/{bn}", lambda bg=bg: grads(lambda a_, c_, n_: sb.render_from_alphas(a_, c_, n_, rs, bg, training=True), alphas, rgb, nrm)
     yield "render/no_rgb", lambda: renderers._render(w, bins=b, depth_method="expected", want_acc=True)
+    dens = torch.rand(R, S, 1, generator=g).to(dev) * 2.0
+    for tn, wt in (("", False), ("_T", True)):
+        as_dict = lambda r: dict(zip(("weights", "transmittance"), r)) if isinstance(r, tuple) else {"weights": r}  # noqa: E731
+        yield f"weights_alphas{tn}", lambda wt=wt: as_dict(sb.rays.weights_from_alphas(alphas, wt))
+        yield f"weights_alphas_grad{tn}", lambda wt=wt: grads(lambda a_: as_dict(sb.rays.weights_from_alphas(a_, wt)), alphas)
+        yield f"weights_density{tn}", lambda wt=wt: as_dict(sb.rays.weights_from_density(b, dens, wt))
+        yield f"weights_density_grad{tn}", lambda wt=wt: grads(lambda d_: as_dict(sb.rays.weights_from_density(b, d_, wt)), dens)
     idx = torch.arange(R, device=dev).repeat_interleave(S)
     for bn in ("color", "per_ray", "random"):
         yield f"packed/{bn}", lambda bn=bn: renderers._render_packed(w.reshape(-1), idx, R, rgb=rgb.reshape(-1, 3), normals=nrm.reshape(-1, 3), ray_samples=rs_pt,
@@ -63,6 +70,11 @@ def _cases():
     rs_cam = make_ray_samples(rb, b, b, None)
     for bn, bg in backgrounds.items():
         yield f"sdf_render/{bn}", lambda bg=bg: sdf.render(rs_cam, bg, sample_outputs=("sdf",))
+    for prec in ("bf16x3", "fp32"):    # the fused engine and the generic one: every per-sample head
+        torch.manual_seed(0)
+        cfg_p = sb.SDFFieldConfig(use_grid_feature=True, num_layers=2, num_layers_color=2, hidden_dim=256, log2_hashmap_size=14, precision=prec)
+        f = sb.SDFField(cfg_p, torch.tensor([[-1.0, -1, -1], [1, 1, 1]]), 8).to(dev).eval()
+        yield f"sdf_outputs/{prec}", lambda f=f: {str(k): v for k, v in f.get_outputs(rs_cam, return_alphas=True, return_occupancy=True).items()}
     for norm in ("linf", "l2", "none"):
         sd = None if norm == "none" else sb.SceneContraction(order=float("inf") if norm == "linf" else None)
         torch.manual_seed(1)
