@@ -10,6 +10,12 @@ constexpr int kEpiWarps = 8;                                 // two consumer war
 constexpr int kEpiThreads = kEpiWarps * 32;
 constexpr int kTcThreads = kEpiThreads + 128;                // + one producer warpgroup: warp 8 streams the weights, warps 9..11 encode
 constexpr int kEncThreads = 96;                              // encoder warps: the geo input, Jacobians and colour-static columns of tile n + 1
+// Staging items of a tile per encoder warp (with the heads: 512 grid, 128 PE, 128 colour-static).  Warp 0 runs two of the four 32-row
+// chunks of the heads of the tile before, warps 1 and 2 one each, so warp 0 stages fewer items.  Warp w takes items enc_item_begin(w)
+// .. enc_item_begin(w + 1) - 1 in order.  sdf-only mode (640 items, no heads) splits evenly: item i -> thread i % 96.
+constexpr int kEncItems0 = 288, kEncItems1 = 256, kEncItems2 = 224;
+static_assert(kEncItems0 + kEncItems1 + kEncItems2 == 768, "the encoder warps' items cover the tile");
+__host__ __device__ constexpr int enc_item_begin(int w) { return w == 0 ? 0 : w == 1 ? kEncItems0 : w == 2 ? kEncItems0 + kEncItems1 : 768; }
 // register split after setmaxnreg.  The launch gets 168 per thread (65536 / 384, rounded down to a multiple of 8); the consumers can
 // only take what the producer warpgroup gives back: 256 x (216 - 168) = 128 x (168 - 72)
 constexpr int kConsumerRegs = 216;
@@ -34,14 +40,15 @@ enum { PRM_B_G0 = 0, PRM_B_G1, PRM_W_G2 /* row 0 */, PRM_B_C0, PRM_B_C1, PRM_W_C
 enum { HS_SDF = 0, HS_GRAD /* x, y, z */, HS_RGB = HS_GRAD + 3 /* raw r, g, b */, kHsRows = HS_RGB + 3 };
 
 // Dynamic shared memory of k_field_tc: byte offsets from its 1024-aligned base
-struct TcSmem { size_t a, ring, prm, hs, coldesc, bytes; };
+struct TcSmem { size_t a, ring, prm, hs, coldesc, hx, bytes; };
 __host__ __device__ constexpr TcSmem tc_smem(int planes) {
   TcSmem s{};                                                  // a: A operand of every layer [P][32 chunks][128 rows][16 B]
   s.ring = s.a + (size_t)planes * kAPlane;                     // weight ring: kStages x one K-block
   s.prm = s.ring + (size_t)kStages * tc_stage_bytes(planes);   // epilogue parameters [kPrmRows][256] f32
   s.hs = s.prm + kPrmRows * 256 * 4;                           // head inputs by tile parity [2][kHsRows][128] f32
   s.coldesc = s.hs + 2 * kHsRows * 128 * 4;                    // EB0's view of the geo input columns 32..127 [96] float4 (ColDesc)
-  s.bytes = s.coldesc + 96 * 16;
+  s.hx = s.coldesc + 96 * 16;                                  // the heads' exclusive scan of a tile's rows [128] f64 (rays > 32 samples)
+  s.bytes = s.hx + 128 * 8;
   return s;
 }
 constexpr size_t kSmemPerBlock = 232448;  // H100: 227 KB of shared memory per block (dynamic + static)

@@ -20,8 +20,9 @@
 //   grad     d sdf/dx = gin_x + PE jacobian + grid jacobian / 4      (what autograd computes at sdf_field.py:647-654)
 //   C0 C1    relu MLP on [x, dir-enc, grad, geo feature, appearance] (misc columns first, h2 accumulated onto them);
 //            last 256->3 layer as fp32 dots; sigmoid + padding
-//   heads    (one encoder warp, a tile behind) Laplace density, NeuS alpha, occupancy, normals; optional per-sample outputs
-//   render   (fused mode, same warp) segmented prefix product over the rays of the tile in double, weights, per-ray sums
+//   heads    (the three encoder warps, a tile behind, 32-row chunks) Laplace density, NeuS alpha, occupancy, normals; optional
+//            per-sample outputs
+//   render   (fused mode, same warps) segmented prefix product over the rays of the tile in double, weights, per-ray sums
 // MMA = wgmma bf16 x bf16 -> fp32.  bf16x3: a0*w0 + a1*w0 + a0*w1 with a = a0+a1, w = w0+w1 (error ~2^-16 relative, fp32 accumulate).
 #pragma once
 #include "field_tc.h"
@@ -32,6 +33,7 @@ namespace sdfb200 {
 using namespace tc;
 
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+constexpr int kEncBar = 3;   // named barrier of the encoder warps (0 is __syncthreads, 1 and 2 belong to the consumer warpgroups)
 
 // sample position of point p (ray r, sample s): o + d * t_start, then SceneContraction (cameras/rays.py:61-73,
 // spatial_distortions.py:66-73).  Also returns the ray direction, the bin start and the bin width.
@@ -190,8 +192,11 @@ struct Slot {
 // (head inputs handed over), [18..23] end of the epilogues E0, E1, EB1, EB0, h2 reload, EC0 (before the SYNC_A that hands their A
 // operand to the next layer's MMAs); cycle sums over the tile of [9] consumer thread 0 waiting for weights (ring full), [10] the producer
 // waiting for a free ring slot (ring empty), [12] encoder thread 0 busy staging the tile, [13] encoder thread 0 waiting for its staging
-// slot (enc empty), [14] encoder thread 0 (heads warp) running the tile's heads / compositing, [16] consumer thread 0 waiting for the
-// tile's head-input buffer (hs empty), [17] the heads warp waiting for the tile's head inputs (hs full)
+// slot (enc empty), [14] encoder thread 0 running the tile's heads / compositing, [16] consumer thread 0 waiting for the tile's
+// head-input buffer (hs empty), [17] encoder thread 0 waiting for the tile's head inputs (hs full), [24] [25] lane 0 of encoder
+// warps 1, 2 busy staging the tile (warp 0: [12]), [26] [27] the same running the heads of the tile (warp 0: [14]), [28..30] encoder
+// thread 0's heads split: per-row heads (geometry, sdf -> alpha / sigma, per-sample outputs), transmittance scan and weights, sums and
+// the ray finish; [31] encoder thread 0 waiting at the encoder warps' barrier (kEncBar)
 __device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
 #define TC_PUT(tno, k, v)                                                                                            \
   do {                                                                                                               \
@@ -207,9 +212,9 @@ struct TcBars {
   Handoff<kStages> ring;  // weight ring, per K-block: full 1 + bytes, empty kEpiWarps
   Handoff<2> enc;         // staging slots: full kEncThreads (images written), empty kEpiThreads (after EB0; sdf-only: after a full)
   Handoff<1> a;           // A operand: full 1 + bytes (geo input landed), empty 2, one per consumer warpgroup (last layer has read A)
-  Handoff<2> hs;          // head inputs: full kEpiThreads (after EC1), empty 32 (the heads warp has read them); unused in sdf-only mode
+  Handoff<2> hs;          // head inputs: full kEpiThreads (after EC1), empty kEncThreads (the encoder warps are through the tile's heads);
+                          // unused in sdf-only mode
 };
-static_assert(sizeof(TcBars) + 4 * sizeof(double) <= kStaticSmem, "static shared memory of k_field_tc (kStaticSmem)");
 
 // Producer (one thread of the producer warpgroup).  Per tile: once the consumers have freed the A operand and the encoder has staged
 // the tile, bulk-copies the staged geo input image into A columns 0..95; then walks every K-block of every layer in consumption order
@@ -548,16 +553,39 @@ __device__ __forceinline__ void epi_ec1(const TileCtx& x, float (&acc)[4][32]) {
   }
 }
 
-// Per-point heads and, in fused mode, the per-ray compositing of one tile, run by one encoder warp on the head inputs `hs` that the
-// consumers left (sdf, gradient, raw rgb; the geometry is recomputed).  The warp walks the four 32-row chunks of the tile in order,
-// lane = row in the chunk.  A ray of S <= 32 samples lies in one chunk; a longer one spans S / 32 chunks: the chunk totals of its
-// transmittance scan go through `wtot` (chunk q -> wtot[q]) and its sums are carried from chunk to chunk in registers and written at
-// its last chunk, always in the same order.
-__device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float (*hs)[128], int tile, int lane, double* wtot) {
+// Per-point heads and, in fused mode, the per-ray compositing of a tile, spread over the three encoder warps.  They read the head
+// inputs `hs` that the consumers left (sdf, gradient, raw rgb; the geometry is recomputed).  Encoder warp ew takes the 32-row chunks
+// q = ew, ew + 3 of the tile (warp 0 two of the four), lane = row in the chunk.  A ray of S <= 32 samples lies in one chunk and is
+// finished there (heads_rows).  A longer one spans S / 32 chunks, in general of different warps, and takes three phases with a barrier
+// of the 96 encoder threads (kEncBar) between them:
+//   1 (heads_rows)       per-row heads, the chunk's segmented factor scan and its total wtot[q]; the row's exclusive scan goes to `hx`,
+//                        its alpha, normal and colour over its (already read) head inputs (HeadsRow)
+//   2 (composite_chunk)  excl x= wtot[first .. q - 1] in chunk order, T, w, the weights, and the chunk's eight sums to csum[q]
+//   3 (finish_rays)      the warp with the ray's last chunk adds the ray's chunk sums in chunk order, from 0, and finishes the ray
+// Every value sees the operations of one warp walking the chunks in order, so nothing depends on which warp runs which chunk.
+// wtot and csum are by tile parity: a warp may start phase 1 of the next tile while another still reads this tile's in phase 3.
+struct HeadsXfer { double wtot[2][4]; float csum[2][4][8]; };
+static_assert(sizeof(TcBars) + sizeof(HeadsXfer) <= kStaticSmem, "static shared memory of k_field_tc (kStaticSmem)");
+// the rows of `hs` that phase 1 leaves for phase 2 of a ray longer than 32 samples, over the head inputs of the same row
+enum { HR_ALPHA = HS_SDF /* alpha, or 1 - exp(-delta sigma) */, HR_NORMAL = HS_GRAD /* x, y, z */, HR_RGB = HS_RGB /* padded rgb */ };
+// the end of a ray that a warp's phase 2 found in its chunks (at most one per warp: a ray spans >= 2 of the 4 chunks)
+struct RayEnd { int q; double tot; float last[3]; };
+// encoder thread 0's cycles in the three kinds of heads work (timing build)
+struct HeadsClock { long long rows, scan, sums; };
+
+// (starts + ends) / 2 of point p (renderers.py:247), with the bin edges of point_geom
+__device__ __forceinline__ float sample_mid(const TcArgs& a, long long p) {
+  if (!a.has_bins) return 0.f;
+  const long long ray = p / a.n_samples;
+  const float* b = a.bins + ray * (a.n_samples + 1) + (p - ray * a.n_samples);
+  return __fdiv_rn(__fadd_rn(__ldg(b), __ldg(b + 1)), 2.0f);
+}
+
+// Phase 1 of chunk q (all of it for rays of S <= 32 samples and in unfused mode).  dmin / dmax: the thread's running depth range.
+__device__ __forceinline__ void heads_rows(const TcArgs& a, float (*hs)[128], double* hx, double* wtot, int tile, int q, int lane,
+                                           float& dmin, float& dmax, HeadsClock& clk) {
+  long long tc0 = TC_CLOCK();
   const float* b_c2 = reinterpret_cast<const float*>(a.blob + a.b_c2);
-  float csum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};     // sums of the chunks so far of a ray longer than 32 samples
-#pragma unroll 1
-  for (int q = 0; q < 4; ++q) {
   const int row = q * 32 + lane;
   const long long p_raw = (long long)tile * 128 + row;
   const bool valid = p_raw < a.n_points;
@@ -582,105 +610,169 @@ __device__ __forceinline__ void heads_and_composite(const TcArgs& a, const float
     if (a.out.occupancy) a.out.occupancy[p] = occupancy(sdf);
     if (a.out.alpha) a.out.alpha[p] = alpha;
   }
-  if (a.render) {
-    // ---------------- fused compositing: the tile holds 128 / S whole rays; row -> (ray, sample) = (row / S, row % S) ----------------
-    const int S = a.n_samples;
-    const int s_idx = row % S;
-    const bool dens = a.rnd.from_density != 0;
-    const bool multi = S > 32;                                // the ray spans chunks (warp-uniform)
-    const int first = multi ? (q * 32 / S) * (S / 32) : q;    // first chunk of the ray
-    const bool ray_end = !multi || q == first + S / 32 - 1;   // this chunk ends the ray (warp-uniform)
-    // factor by which the transmittance drops across this sample: 1 - alpha + 1e-7 (rays.py:204-206), or as an exponent
-    // delta * sigma for the density form (rays.py:160-170)
-    const float dd = valid ? __fmul_rn(delta, density) : 0.f;
-    double f = dens ? (double)dd : (valid ? (double)neus_trans_factor(alpha) : 1.0);
-    double incl = f;
-    // segmented by ray (s_idx >= d), so not the plain warp_scan_incl of common.cuh
+  { const long long c = TC_CLOCK(); clk.rows += c - tc0; tc0 = c; }
+  if (!a.render) return;
+  // ---------------- fused compositing: the tile holds 128 / S whole rays; row -> (ray, sample) = (row / S, row % S) ----------------
+  const int S = a.n_samples;
+  const int s_idx = row % S;
+  const bool dens = a.rnd.from_density != 0;
+  // factor by which the transmittance drops across this sample: 1 - alpha + 1e-7 (rays.py:204-206), or as an exponent
+  // delta * sigma for the density form (rays.py:160-170)
+  const float dd = valid ? __fmul_rn(delta, density) : 0.f;
+  double f = dens ? (double)dd : (valid ? (double)neus_trans_factor(alpha) : 1.0);
+  double incl = f;
+  // segmented by ray (s_idx >= d), so not the plain warp_scan_incl of common.cuh
 #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const double o = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d && s_idx >= d) incl = dens ? incl + o : incl * o;
-    }
-    double excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0 || s_idx == 0) excl = dens ? 0.0 : 1.0;
-    if (multi) {
-      __syncwarp();                                           // every lane is through its reads of wtot from the chunk before
-      if (lane == 31) wtot[q] = incl;
-      __syncwarp();
-      for (int w2 = first; w2 < q; ++w2) excl = dens ? excl + wtot[w2] : excl * wtot[w2];
-    }
-    const float T = dens ? expf(-(float)excl) : (float)excl;
-    const float al = dens ? __fsub_rn(1.0f, expf(-dd)) : alpha;
-    const float w = valid ? __fmul_rn(al, T) : 0.f;
-    const float mid = __fdiv_rn(__fadd_rn(pg.t0, pg.t1), 2.0f);            // (starts + ends) / 2, renderers.py:247
-    if (valid && a.rnd.weights) a.rnd.weights[p] = w;
-    float vs[8] = {w, w * rgbv[0], w * rgbv[1], w * rgbv[2], w * nx, w * ny, w * nz, w * mid};
-    float smin = valid ? mid : INFINITY, smax = valid ? mid : -INFINITY;
-    const int span = S < 32 ? S : 32;
+  for (int d = 1; d < 32; d <<= 1) {
+    const double o = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d && s_idx >= d) incl = dens ? incl + o : incl * o;
+  }
+  double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0 || s_idx == 0) excl = dens ? 0.0 : 1.0;
+  const float al = dens ? __fsub_rn(1.0f, expf(-dd)) : alpha;
+  const float mid = __fdiv_rn(__fadd_rn(pg.t0, pg.t1), 2.0f);            // (starts + ends) / 2, renderers.py:247
+  if (valid) { dmin = fminf(dmin, mid); dmax = fmaxf(dmax, mid); }      // the batch's steps.min() / max() (renderers.py:257)
+  if (S > 32) {                                                         // the ray spans chunks: phases 2 and 3 take it from here
+    if (lane == 31) wtot[q] = incl;
+    hx[row] = excl;
+    hs[HR_ALPHA][row] = al;
+    hs[HR_NORMAL][row] = nx; hs[HR_NORMAL + 1][row] = ny; hs[HR_NORMAL + 2][row] = nz;
+    hs[HR_RGB][row] = rgbv[0]; hs[HR_RGB + 1][row] = rgbv[1]; hs[HR_RGB + 2][row] = rgbv[2];
+    clk.scan += TC_CLOCK() - tc0;
+    return;
+  }
+  const float T = dens ? expf(-(float)excl) : (float)excl;
+  const float w = valid ? __fmul_rn(al, T) : 0.f;
+  if (valid && a.rnd.weights) a.rnd.weights[p] = w;
+  { const long long c = TC_CLOCK(); clk.scan += c - tc0; tc0 = c; }
+  float vs[8] = {w, w * rgbv[0], w * rgbv[1], w * rgbv[2], w * nx, w * ny, w * nz, w * mid};
 #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      if (d < span) {
+  for (int d = 1; d < 32; d <<= 1) {
+    if (d < S) {
 #pragma unroll
-        for (int k = 0; k < 8; ++k) vs[k] += __shfl_down_sync(0xffffffffu, vs[k], d);
-      }
-      smin = fminf(smin, __shfl_xor_sync(0xffffffffu, smin, d));
-      smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, d));
-    }
-    if (a.rnd.out.steps_minmax && lane == 0 && smin <= smax) { atomic_min_float(a.rnd.out.steps_minmax, smin); atomic_max_float(a.rnd.out.steps_minmax + 1, smax); }
-    // transmittance after the last sample (alphas: transmittance[:, -1] = bg_transmittance, neus.py:101) / before it (densities:
-    // volsdf.py:67-68), and the colour of the last sample
-    double tot;
-    float lr, lg, lb;
-    if (multi) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) { csum[k] += vs[k]; vs[k] = csum[k]; }   // lane 0: the chunk's sums, then the ray's so far
-      if (dens) {
-        tot = __shfl_sync(0xffffffffu, excl, 31);
-      } else {
-        tot = 1.0;
-        for (int w2 = first; w2 <= q; ++w2) tot *= wtot[w2];
-      }
-      lr = __shfl_sync(0xffffffffu, rgbv[0], 31); lg = __shfl_sync(0xffffffffu, rgbv[1], 31); lb = __shfl_sync(0xffffffffu, rgbv[2], 31);
-    } else {
-      const int last = (lane - s_idx) + S - 1;
-      tot = __shfl_sync(0xffffffffu, dens ? excl : incl, last);
-      lr = __shfl_sync(0xffffffffu, rgbv[0], last); lg = __shfl_sync(0xffffffffu, rgbv[1], last); lb = __shfl_sync(0xffffffffu, rgbv[2], last);
-    }
-    const long long ray = (long long)tile * (128 / S) + row / S;
-    if (ray_end && s_idx == (multi ? S - 32 : 0) && ray * S < a.n_points) {
-      const float last[3] = {lr, lg, lb};
-      finish_ray(ray, vs[0], {vs[1], vs[2], vs[3]}, {vs[4], vs[5], vs[6]}, vs[7], a.rnd.bg_mode, a.rnd.bg, last, a.rnd.clamp01, a.rnd.out.rgb,
-                 a.rnd.out.accumulation, a.rnd.out.normal, a.rnd.out.depth);
-      if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)tot) : (float)tot;
-    }
-    if (multi && ray_end) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) csum[k] = 0.f;
+      for (int k = 0; k < 8; ++k) vs[k] += __shfl_down_sync(0xffffffffu, vs[k], d);
     }
   }
+  // transmittance after the last sample (alphas: transmittance[:, -1] = bg_transmittance, neus.py:101) / before it (densities:
+  // volsdf.py:67-68), and the colour of the last sample
+  const int last = (lane - s_idx) + S - 1;
+  const double tot = __shfl_sync(0xffffffffu, dens ? excl : incl, last);
+  const float lc[3] = {__shfl_sync(0xffffffffu, rgbv[0], last), __shfl_sync(0xffffffffu, rgbv[1], last), __shfl_sync(0xffffffffu, rgbv[2], last)};
+  const long long ray = (long long)tile * (128 / S) + row / S;
+  if (s_idx == 0 && ray * S < a.n_points) {
+    finish_ray(ray, vs[0], {vs[1], vs[2], vs[3]}, {vs[4], vs[5], vs[6]}, vs[7], a.rnd.bg_mode, a.rnd.bg, lc, a.rnd.clamp01, a.rnd.out.rgb,
+               a.rnd.out.accumulation, a.rnd.out.normal, a.rnd.out.depth);
+    if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)tot) : (float)tot;
   }
+  clk.sums += TC_CLOCK() - tc0;
 }
 
-// The heads warp's part of a tile: wait for its head inputs, run the heads, hand the buffer back
-__device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no, int lane, TcBars& b, float (*hs)[128], double* wtot) {
-  long long waited = 0;
+// Phase 2 of chunk q of a ray longer than 32 samples: the scan totals of the ray's earlier chunks, the weights and the chunk's sums
+__device__ __forceinline__ void composite_chunk(const TcArgs& a, const float (*hs)[128], const double* hx, const double* wtot, float (*csum)[8],
+                                                int tile, int q, int lane, RayEnd& end, HeadsClock& clk) {
+  long long tc0 = TC_CLOCK();
+  const int row = q * 32 + lane;
+  const long long p_raw = (long long)tile * 128 + row;
+  const bool valid = p_raw < a.n_points;
+  const long long p = valid ? p_raw : a.n_points - 1;
+  const int S = a.n_samples;
+  const bool dens = a.rnd.from_density != 0;
+  const int first = (q * 32 / S) * (S / 32);                            // first chunk of the ray
+  double excl = hx[row];
+  for (int w2 = first; w2 < q; ++w2) excl = dens ? excl + wtot[w2] : excl * wtot[w2];
+  const float T = dens ? expf(-(float)excl) : (float)excl;
+  const float w = valid ? __fmul_rn(hs[HR_ALPHA][row], T) : 0.f;
+  if (valid && a.rnd.weights) a.rnd.weights[p] = w;
+  { const long long c = TC_CLOCK(); clk.scan += c - tc0; tc0 = c; }
+  const float rgbv[3] = {hs[HR_RGB][row], hs[HR_RGB + 1][row], hs[HR_RGB + 2][row]};
+  float vs[8] = {w, w * rgbv[0], w * rgbv[1], w * rgbv[2], w * hs[HR_NORMAL][row], w * hs[HR_NORMAL + 1][row], w * hs[HR_NORMAL + 2][row],
+                 w * sample_mid(a, p)};
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) vs[k] += __shfl_down_sync(0xffffffffu, vs[k], d);
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) csum[q][k] = vs[k];
+  }
+  if (q == first + S / 32 - 1) {                                        // the chunk ends the ray
+    end.q = q;
+    if (dens) {
+      end.tot = __shfl_sync(0xffffffffu, excl, 31);
+    } else {
+      end.tot = 1.0;
+      for (int w2 = first; w2 <= q; ++w2) end.tot *= wtot[w2];
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) end.last[c] = __shfl_sync(0xffffffffu, rgbv[c], 31);
+  }
+  clk.sums += TC_CLOCK() - tc0;
+}
+
+// Phase 3: the ray that ends in this warp's chunks, from its chunk sums added in chunk order
+__device__ __forceinline__ void finish_rays(const TcArgs& a, const float (*csum)[8], int tile, int lane, const RayEnd& end, HeadsClock& clk) {
+  const long long tc0 = TC_CLOCK();
+  const int S = a.n_samples;
+  const long long ray = (long long)tile * (128 / S) + end.q * 32 / S;
+  if (end.q >= 0 && lane == 0 && ray * S < a.n_points) {
+    float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int w2 = end.q + 1 - S / 32; w2 <= end.q; ++w2) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) s[k] += csum[w2][k];
+    }
+    finish_ray(ray, s[0], {s[1], s[2], s[3]}, {s[4], s[5], s[6]}, s[7], a.rnd.bg_mode, a.rnd.bg, end.last, a.rnd.clamp01, a.rnd.out.rgb,
+               a.rnd.out.accumulation, a.rnd.out.normal, a.rnd.out.depth);
+    const bool dens = a.rnd.from_density != 0;
+    if (a.rnd.bg_transmittance) a.rnd.bg_transmittance[ray] = dens ? expf(-(float)end.tot) : (float)end.tot;
+  }
+  clk.sums += TC_CLOCK() - tc0;
+}
+
+// An encoder warp's part of the heads of a tile: wait for the head inputs, run the warp's chunks, hand the buffer back
+__device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no, int et, TcBars& b, float (*hs)[128], double* hx, HeadsXfer& xf,
+                                         float& dmin, float& dmax) {
+  const int ew = et >> 5, lane = et & 31;
+  long long waited = 0, bar_waited = 0;
   b.hs.wait_full(tile_no, &waited);
   const long long t0 = TC_CLOCK();
-  heads_and_composite(a, hs + b.hs.slot(tile_no) * kHsRows, tile, lane, wtot);
+  float (*h)[128] = hs + b.hs.slot(tile_no) * kHsRows;
+  double* wtot = xf.wtot[tile_no & 1];
+  float (*csum)[8] = xf.csum[tile_no & 1];
+  HeadsClock clk{0, 0, 0};
+#pragma unroll 1
+  for (int q = ew; q < 4; q += kEncThreads / 32) heads_rows(a, h, hx, wtot, tile, q, lane, dmin, dmax, clk);
+  if (a.render && a.n_samples > 32) {
+    long long c = TC_CLOCK();
+    named_sync(kEncBar, kEncThreads);                 // every chunk's wtot is written
+    bar_waited += TC_CLOCK() - c;
+    RayEnd end{-1, 0.0, {0.f, 0.f, 0.f}};
+#pragma unroll 1
+    for (int q = ew; q < 4; q += kEncThreads / 32) composite_chunk(a, h, hx, wtot, csum, tile, q, lane, end, clk);
+    c = TC_CLOCK();
+    named_sync(kEncBar, kEncThreads);                 // every chunk's sums are written
+    bar_waited += TC_CLOCK() - c;
+    finish_rays(a, csum, tile, lane, end, clk);
+  }
   b.hs.arrive_empty(tile_no);
-  if (lane == 0) { TC_PUT(tile_no, 14, TC_CLOCK() - t0); TC_PUT(tile_no, 17, waited); }
+  if (lane == 0) TC_PUT(tile_no, ew == 0 ? 14 : 25 + ew, TC_CLOCK() - t0);
+  if (et == 0) { TC_PUT(tile_no, 17, waited); TC_PUT(tile_no, 28, clk.rows); TC_PUT(tile_no, 29, clk.scan); TC_PUT(tile_no, 30, clk.sums); TC_PUT(tile_no, 31, bar_waited); }
 }
 
 // Encoder warps (et = 0..95): walk the same tiles as the consumers and stage each one in its slot while the consumers run the tile
-// before it.  A tile is 768 items, 8 per thread: 512 (point, group of four hash levels), then 128 x (PE | x, point outputs) and, with
-// the colour MLP, 128 x colour-static columns.  Item i goes to thread i % 96, so each warp runs 32 consecutive items of one kind.
-// Except in sdf-only mode, the first encoder warp then runs the heads of the tile before (the one the consumers are finishing), and
-// those of the last tile after the loop.  Staging tile n + 1 and the heads of tile n - 1 both fit in the consumers' tile n: slot
-// n + 1 was freed at EB0 of tile n - 1, and the head inputs of tile n - 1 are ready when tile n starts.
+// before it.  A tile is 768 items: 512 (point, group of four hash levels), then 128 x (PE | x, point outputs) and, with the colour
+// MLP, 128 x colour-static columns.  Encoder warp ew takes items enc_item_begin(ew) .. enc_item_begin(ew + 1) - 1, lane = item mod 32:
+// warp 0, which runs two of the four chunks of the heads, takes fewer (field_tc.h).  In sdf-only mode (640 items, no heads) item i
+// goes to thread i % 96.  Except in sdf-only mode, the encoder warps then run the heads of the tile before (the one the consumers are
+// finishing), and those of the last tile after the loop.  Staging tile n + 1 and the heads of tile n - 1 both fit in the consumers'
+// tile n: slot n + 1 was freed at EB0 of tile n - 1, and the head inputs of tile n - 1 are ready when tile n starts.
 template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table, float (*hs)[128], double* wtot) {
-  const int n_items = a.mode != 0 ? 768 : 640;
-  const bool heads = a.mode != 0 && et < 32;     // the first encoder warp also runs the heads of the tile before
+__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table, float (*hs)[128], double* hx,
+                                           HeadsXfer& xf) {
+  const bool heads = a.mode != 0;
+  const int ew = et >> 5, lane = et & 31;
+  const int i_begin = heads ? enc_item_begin(ew) + lane : et, i_end = heads ? enc_item_begin(ew + 1) : 640, i_step = heads ? 32 : kEncThreads;
+  float dmin = INFINITY, dmax = -INFINITY;       // the midpoints of this thread's rows, over every tile of the CTA
   int tile_no = 0;
   for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
     long long waited = 0;
@@ -688,7 +780,7 @@ __device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots,
     const long long t0 = TC_CLOCK();
     const Slot<P> s(slots, b.enc.slot(tile_no));
 #pragma unroll 1
-    for (int i = et; i < n_items; i += kEncThreads) {
+    for (int i = i_begin; i < i_end; i += i_step) {
       const int row = i & 127;
       if (i < 512) encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jg(), pol_table);
       else if (i < 640) encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jpe());
@@ -697,9 +789,19 @@ __device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots,
     fence_async_global();                    // the geo image is read by the producer's bulk copy (async proxy)
     b.enc.arrive_full(tile_no);
     if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - t0); TC_PUT(tile_no, 13, waited); }
-    if (heads && tile_no > 0) heads_of(a, tile - (int)gridDim.x, tile_no - 1, et, b, hs, wtot);
+    else if (lane == 0) TC_PUT(tile_no, 23 + ew, TC_CLOCK() - t0);
+    if (heads && tile_no > 0) heads_of(a, tile - (int)gridDim.x, tile_no - 1, et, b, hs, hx, xf, dmin, dmax);
   }
-  if (heads && tile_no > 0) heads_of(a, blockIdx.x + (tile_no - 1) * (int)gridDim.x, tile_no - 1, et, b, hs, wtot);   // the last tile
+  if (heads && tile_no > 0) heads_of(a, blockIdx.x + (tile_no - 1) * (int)gridDim.x, tile_no - 1, et, b, hs, hx, xf, dmin, dmax);   // the last tile
+  // one depth-range update per warp and CTA: min and max are exact, so the result is that of any order of updates
+  if (heads && a.render && a.rnd.out.steps_minmax) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      dmin = fminf(dmin, __shfl_xor_sync(0xffffffffu, dmin, d));
+      dmax = fmaxf(dmax, __shfl_xor_sync(0xffffffffu, dmax, d));
+    }
+    if (lane == 0 && dmin <= dmax) { atomic_min_float(a.rnd.out.steps_minmax, dmin); atomic_max_float(a.rnd.out.steps_minmax + 1, dmax); }
+  }
 }
 
 template <int P, int LAYOUT>
@@ -712,8 +814,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   float (*prm)[256] = reinterpret_cast<float (*)[256]>(smem + sm.prm);
   float (*hs)[128] = reinterpret_cast<float (*)[128]>(smem + sm.hs);
   float4* coldesc = reinterpret_cast<float4*>(smem + sm.coldesc);
+  double* hx = reinterpret_cast<double*>(smem + sm.hx);
   __shared__ TcBars bars;
-  __shared__ double wtot[4];          // chunk totals of the compositing scan (heads warp)
+  __shared__ HeadsXfer hxf;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nlayers = a.mode == 0 ? 2 : L_COUNT;
@@ -722,7 +825,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   if (tid == 0) {
     bars.ring.init(1, kEpiWarps);
     bars.enc.init(kEncThreads, kEpiThreads);
-    bars.hs.init(kEpiThreads, 32);
+    bars.hs.init(kEpiThreads, kEncThreads);
     bars.a.init(1, 2);
     fence_barrier_init();
   }
@@ -741,7 +844,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   if (tid >= kEpiThreads) {
     setmaxnreg_dec<kProducerRegs>();
     if (tid == kEpiThreads) produce_all<P>(a, nlayers, abuf, ring, slots, bars);
-    else if (tid >= kTcThreads - kEncThreads) encode_all<P, LAYOUT>(a, tid - (kTcThreads - kEncThreads), slots, bars, l2_policy_evict_last(), hs, wtot);
+    else if (tid >= kTcThreads - kEncThreads) encode_all<P, LAYOUT>(a, tid - (kTcThreads - kEncThreads), slots, bars, l2_policy_evict_last(), hs, hx, hxf);
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();
@@ -791,7 +894,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     }
     {
       long long hs_waited = 0;
-      bars.hs.wait_empty(tile_no, &hs_waited); // the heads warp is done with the tile two before
+      bars.hs.wait_empty(tile_no, &hs_waited); // the encoder warps are done with the tile two before
       if (tid == 0) TC_PUT(tile_no, 16, hs_waited);
     }
     epi_e1<P>(x, tile, acc);
@@ -818,7 +921,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     LAYER(L_C1, true);
     if (t == 0) bars.a.arrive_empty(tile_no);  // the last layer has read A: the next tile's geo input may land
     epi_ec1(x, acc);
-    bars.hs.arrive_full(tile_no);              // the heads warp takes the tile from here
+    bars.hs.arrive_full(tile_no);              // the encoder warps take the tile from here
     TC_STAMP(15);
     if (tid == 0) TC_PUT(tile_no, 9, waited);
   }

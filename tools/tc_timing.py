@@ -1,6 +1,7 @@
 """Per-phase cycle breakdown of the fused tensor-core field kernel (CTA 0, consumer thread 0, first tiles): the wait for the staged geo
 input, every epilogue and every layer's MMAs apart, EC1, the cycles the consumers waited for weights and the producer for a
-free ring slot, the encoder warps' busy and slot-wait cycles per tile, and the heads warp's cycles on the tile's heads.  Uses the timing build of the kernel
+free ring slot, each encoder warp's cycles staging the tile and running its heads, encoder thread 0's heads split by kind of work and
+its slot and barrier waits.  Uses the timing build of the kernel
 inside libsdfb200_dbg.so (sdfstudio_b200/build.py).   usage: tools/tc_timing.py [precision] [log2T] [table dtype] [fused|unfused]"""
 import ctypes
 import os
@@ -58,9 +59,11 @@ assert lib.sdfb200_debug_tc_timing(buf) == 0
 # epilogue's cycles run from the end of the layer before it to its own stamp; a layer's MMA cycles from the end of the epilogue in front
 # of it (or the a_full stamp for G0) to the layer's stamp, so they include the warpgroup barrier and any wait for weights.  Cycle sums
 # over the tile: [9] consumer thread 0 waiting for weights, [10] producer waiting for a free ring slot, [12] encoder thread 0 busy
-# staging the tile, [13] encoder thread 0 waiting for the tile's staging slot (enc_empty), [14] encoder thread 0 (the heads warp)
-# running the tile's heads and compositing, [16] consumer thread 0 waiting for the tile's head-input buffer (hs_empty), [17] the heads
-# warp waiting for the tile's head inputs (hs_full).
+# staging the tile, [13] encoder thread 0 waiting for the tile's staging slot (enc_empty), [14] encoder thread 0 running the tile's
+# heads and compositing, [16] consumer thread 0 waiting for the tile's head-input buffer (hs_empty), [17] encoder thread 0 waiting for
+# the tile's head inputs (hs_full); per encoder warp w0 / w1 / w2 (lane 0): busy staging [12] [24] [25] and running
+# the tile's heads [14] [26] [27]; encoder thread 0's heads split [28] per-row heads, [29] transmittance scan + weights, [30] sums and
+# ray finish, and [31] its wait at the encoder warps' barrier.
 layers = ["G0", "G1", "B1", "B0", "C0 misc", "C0 h2", "C1"]
 epis = ["E0", "E1", "EB1", "EB0", "h2 reload", "EC0"]      # epis[L - 1] runs in front of layer L
 for t in (5, 10):
@@ -71,4 +74,7 @@ for t in (5, 10):
           + "  ".join(f"{n} {v}" for n, v in zip(epis + ["EC1"], epi))
           + f"  |  MMAs {sum(mma)}: " + "  ".join(f"{n} {v}" for n, v in zip(layers, mma))
           + f"  |  consumer weight wait {st[9]}  hs_empty wait {st[16]}  producer slot wait {st[10]}"
-          + f"  |  encoder busy {st[12]}  encoder slot wait {st[13]}  heads {st[14]}  heads wait {st[17]}")
+          + f"  |  encoder busy {st[12]}  encoder slot wait {st[13]}  heads {st[14]}  heads wait {st[17]}"
+          + f"  |  encoder warps w0/w1/w2: staging {st[12]}/{st[24]}/{st[25]}  heads {st[14]}/{st[26]}/{st[27]}"
+          + f"  busy {st[12] + st[14]}/{st[24] + st[26]}/{st[25] + st[27]}"
+          + f"  |  w0 heads: rows {st[28]}  scan+weights {st[29]}  sums+finish {st[30]}  barrier wait {st[31]}")
