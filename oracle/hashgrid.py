@@ -42,22 +42,26 @@ def hash_index(ix, iy, iz, table_size: int):
     return h % table_size
 
 
-def encode_torch_layout(x, table, scalings, table_size: int, smoothstep: bool, return_indices: bool = False):
+def encode_torch_layout(x, table, scalings, table_size: int, smoothstep: bool, return_indices: bool = False, fp32_positions: bool = False):
     """x [N,3] in [0,1] -> [N, L*F].  encodings.py:357-398 (+ smoothstep remap encodings.py:700-701).
 
     ``table`` is ``[L*T, F]``; ``scalings`` is the float32 per-level scale tensor.
     Blend order follows the reference: x-lerp (weight ``offset_x`` on the *ceil* corner), then y, then z.
+    ``fp32_positions``: ``x*scale`` takes its fp32 value (the reference's and the kernels' rounding) with the derivative of
+    ``x*scale``, so that an fp64 evaluation blends the same cell with the same offsets as the fp32 kernels.
     """
     dt = x.dtype
     L = scalings.shape[0]
     F = table.shape[1]
-    scaled = x[:, None, :] * scalings.view(-1, 1).to(dt)  # [N, L, 3]
+    scaled = x[:, None, :] * scalings.view(-1, 1).to(x.device, dt)  # [N, L, 3]
+    if fp32_positions:
+        scaled = scaled + ((x.detach().float()[:, None, :] * scalings.view(-1, 1).to(x.device, torch.float32)).to(dt) - scaled.detach())
     c = torch.ceil(scaled).to(torch.int32)
     f = torch.floor(scaled).to(torch.int32)
     off = scaled - f
     if smoothstep:
         off = off * off * (3.0 - 2.0 * off)
-    lvl_off = (torch.arange(L, dtype=torch.int64) * table_size).view(1, L)
+    lvl_off = (torch.arange(L, dtype=torch.int64, device=x.device) * table_size).view(1, L)
 
     def H(a, b, cc):
         return hash_index(a, b, cc, table_size) + lvl_off
@@ -103,27 +107,32 @@ def tcnn_grid_meta(n_levels: int, n_features: int, log2_hashmap_size: int, base_
     return {"scale": scales, "res": ress, "size": sizes, "offset": offsets[:-1], "total": offsets[-1], "hashed": hashed}
 
 
-def encode_tcnn_layout(x, params, meta, n_features: int, smoothstep: bool):
+def encode_tcnn_layout(x, params, meta, n_features: int, smoothstep: bool, return_indices: bool = False, fp32_positions: bool = False):
     """x [N,3] in [0,1] -> [N, L*F] (fp32 math; tcnn itself stores/returns fp16).  ``params`` is the flat table
     ``[total, F]``.  pos = x*scale + 0.5; cell = floor(pos); w = pos - cell (smoothstep: w^2(3-2w)); corner bit set ->
     cell+1 with weight w, else weight 1-w; dense index x + y*res + z*res^2, hashed index = spatial hash (uint32),
-    both ``% level_size``."""
+    both ``% level_size``.  Runs on ``x.device``.  ``return_indices``: also the [N, L, 8] rows of ``params`` of corner k
+    (bit 0 = x, 1 = y, 2 = z set -> cell + 1).  ``fp32_positions``: ``pos`` takes its fp32 value with the derivative of
+    ``x*scale``, as in ``encode_torch_layout``."""
     dt = x.dtype
     N = x.shape[0]
     L = len(meta["scale"])
-    out = torch.zeros(N, L, n_features, dtype=dt)
+    out = torch.zeros(N, L, n_features, dtype=dt, device=x.device)
+    rows = torch.empty(N, L, 8, dtype=torch.int64, device=x.device) if return_indices else None
     for l in range(L):
         scale, res, size, off, hashed = (meta[k][l] for k in ("scale", "res", "size", "offset", "hashed"))
         # tiny-cuda-nn computes pos with a fused multiply-add (one rounding); emulate it through float64
         pos = (x.double() * float(scale) + 0.5).to(dt)
+        if fp32_positions:
+            pos = pos + ((x.detach().double() * float(scale) + 0.5).float().to(dt) - pos.detach())
         cell = torch.floor(pos)
         w = pos - cell
         cell = cell.to(torch.int64)
         if smoothstep:
             w = w * w * (3.0 - 2.0 * w)
-        acc = torch.zeros(N, n_features, dtype=dt)
+        acc = torch.zeros(N, n_features, dtype=dt, device=x.device)
         for corner in range(8):
-            wt = torch.ones(N, dtype=dt)
+            wt = torch.ones(N, dtype=dt, device=x.device)
             cc = []
             for d in range(3):
                 if corner & (1 << d):
@@ -137,6 +146,10 @@ def encode_tcnn_layout(x, params, meta, n_features: int, smoothstep: bool):
             else:
                 idx = (cc[0] + cc[1] * res + cc[2] * res * res) & 0xFFFFFFFF
             idx = idx % size + off
+            if rows is not None:
+                rows[:, l, corner] = idx
             acc = acc + wt[:, None] * params[idx]
         out[:, l] = acc
+    if return_indices:
+        return out.reshape(N, L * n_features), rows
     return out.reshape(N, L * n_features)

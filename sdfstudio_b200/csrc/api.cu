@@ -83,6 +83,10 @@ static int check_field_call(const sdfb200_field_t* f, const void* packed, const 
   SDFB_REQUIRE(in->bins != nullptr || in->n_samples == 1, "point mode requires n_samples == 1");
   SDFB_REQUIRE(in->bins == nullptr || in->directions != nullptr, "ray mode requires directions");
   SDFB_REQUIRE(!f->use_grid_feature || table != nullptr, "grid table is NULL");
+  if (f->use_grid_feature) {
+    r = validate_grid_pointers(&f->grid, table, nullptr);
+    if (r) return r;
+  }
   SDFB_REQUIRE(workspace != nullptr, "workspace is NULL");
   if (rnd && rnd->out.rgb) SDFB_REQUIRE(rnd->bg_mode == SDFB200_BG_LAST_SAMPLE || rnd->bg != nullptr, "rgb output needs a background");
   if (rnd && rnd->out.depth) SDFB_REQUIRE(rnd->out.steps_minmax != nullptr, "depth output needs steps_minmax (pre-set to {+inf,-inf})");

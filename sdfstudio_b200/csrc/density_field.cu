@@ -69,6 +69,8 @@ extern "C" int sdfb200_density_field_forward(const sdfb200_grid_t* grid, const v
   SDFB_REQUIRE(table && weights && positions && density, "NULL pointer");
   SDFB_REQUIRE(n_hidden_layers >= 1 && n_hidden_layers <= 4, "n_hidden_layers out of range");
   SDFB_REQUIRE(grid->n_features == 2 || grid->n_features == 4 || grid->n_features == 1 || grid->n_features == 8, "n_features");
+  r = validate_grid_pointers(grid, table, nullptr);
+  if (r) return r;
   DensityArgs a;
   a.grid = *grid; a.table = table; a.weights = weights; a.positions = positions; a.aabb = aabb; a.contraction = contraction; a.n_hidden = n_hidden_layers;
   a.in_dim = grid->n_levels * grid->n_features; a.in_pad = (a.in_dim + 15) / 16 * 16; a.n = n; a.density = density; a.pre_activation = pre_activation;

@@ -10,6 +10,7 @@ namespace sdfb200 {
 
 // grid_encode.cu
 int validate_grid(const sdfb200_grid_t* g);
+int validate_grid_pointers(const sdfb200_grid_t* g, const void* table, const float* grad);   // grad: the table gradient, or NULL
 int grid_encode(const sdfb200_grid_t& g, const void* table, const float* x01, int64_t n, float* out, int64_t out_ld, float* dout_dx,
                 cudaStream_t st);
 

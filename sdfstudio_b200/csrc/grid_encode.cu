@@ -276,6 +276,17 @@ int validate_grid(const sdfb200_grid_t* g) {
   return 0;
 }
 
+// load_row reads a row with one vector load per 16 bytes (F * sizeof(T), capped at 16); atomic_add_row adds 16 (F % 4 == 0), 8 (F == 2)
+// or 4 bytes at once.  A pointer those instructions cannot take is refused before anything launches.  NULL pointers pass.
+int validate_grid_pointers(const sdfb200_grid_t* g, const void* table, const float* grad) {
+  const long long row = (long long)g->n_features * (g->table_dtype == SDFB200_DT_F16 ? 2 : 4);
+  const long long load = row < 16 ? row : 16;
+  const long long add = g->n_features % 4 == 0 ? 16 : g->n_features == 2 ? 8 : 4;
+  if ((uintptr_t)table % load) return fail(SDFB200_EINVAL, "grid table%s must be aligned to %lld bytes (its row loads)", "", load);
+  if ((uintptr_t)grad % add) return fail(SDFB200_EINVAL, "grid gradient%s must be aligned to %lld bytes (its vector atomics)", "", add);
+  return 0;
+}
+
 template <typename T, int F>
 static int launch_encode(const sdfb200_grid_t& g, const void* table, const float* x01, int64_t n, float* out, int64_t out_ld,
                          float* dout_dx, cudaStream_t st) {
@@ -354,6 +365,8 @@ extern "C" int sdfb200_grid_encode(const sdfb200_grid_t* grid, const void* table
   if (n == 0) return 0;
   SDFB_REQUIRE(table && x01 && out, "NULL pointer");
   SDFB_REQUIRE(out_ld >= (int64_t)grid->n_levels * grid->n_features, "out_ld too small");
+  r = validate_grid_pointers(grid, table, nullptr);
+  if (r) return r;
   return grid_encode(*grid, table, x01, n, out, out_ld, dout_dx, (cudaStream_t)stream);
 }
 
@@ -364,6 +377,8 @@ extern "C" int sdfb200_grid_encode_backward(const sdfb200_grid_t* grid, const vo
   SDFB_REQUIRE(n >= 0, "n < 0");
   if (n == 0) return 0;
   SDFB_REQUIRE(table && x01 && dout && (dtable || dx01), "NULL pointer");
+  r = validate_grid_pointers(grid, table, dtable);
+  if (r) return r;
   SDFB_DISPATCH_GRID(*grid, launch_encode_bwd, *grid, table, x01, dout, n, dtable, dx01, (cudaStream_t)stream);
 }
 
@@ -374,6 +389,8 @@ extern "C" int sdfb200_grid_encode_backward_backward(const sdfb200_grid_t* grid,
   SDFB_REQUIRE(n >= 0, "n < 0");
   if (n == 0) return 0;
   SDFB_REQUIRE(table && x01 && dout && g_dx01, "NULL pointer");
+  r = validate_grid_pointers(grid, table, g_table);
+  if (r) return r;
   SDFB_DISPATCH_GRID(*grid, launch_encode_bwd2, *grid, table, x01, dout, g_dx01, n, g_dout, g_table, g_x01, (cudaStream_t)stream);
 }
 
@@ -385,6 +402,8 @@ extern "C" int sdfb200_grid_encode_grouped(const sdfb200_grid_t* grid, const voi
   if (n == 0) return 0;
   SDFB_REQUIRE(table && x01 && out, "NULL pointer");
   SDFB_REQUIRE(out_ld >= (int64_t)grid->n_levels * grid->n_features, "out_ld too small");
+  r = validate_grid_pointers(grid, table, nullptr);
+  if (r) return r;
   SDFB_DISPATCH_GRID(*grid, launch_encode_grouped, *grid, table, x01, n / group, group, out, out_ld, (cudaStream_t)stream);
 }
 
@@ -395,5 +414,7 @@ extern "C" int sdfb200_grid_encode_backward_grouped(const sdfb200_grid_t* grid, 
   SDFB_REQUIRE(n >= 0 && group >= 1 && n % group == 0, "n must be a non-negative multiple of group");
   if (n == 0) return 0;
   SDFB_REQUIRE(x01 && dout && dtable, "NULL pointer");
+  r = validate_grid_pointers(grid, nullptr, dtable);
+  if (r) return r;
   SDFB_DISPATCH_GRID(*grid, launch_encode_bwd_grouped, *grid, x01, dout, n / group, group, dtable, (cudaStream_t)stream);
 }

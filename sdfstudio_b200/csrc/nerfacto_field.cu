@@ -31,6 +31,8 @@ extern "C" int sdfb200_nerfacto_field_forward(const sdfb200_grid_t* grid, const 
   const int64_t n = f->n_samples ? n_rays * f->n_samples : n_rays;
   if (n == 0) return 0;
   SDFB_REQUIRE(table && base_weights && origins && density, "NULL pointer");
+  r = validate_grid_pointers(grid, table, nullptr);
+  if (r) return r;
   SDFB_REQUIRE(f->n_samples == 0 || (bins != nullptr && directions != nullptr), "ray mode needs bins and directions (the midpoints use them)");
   if (rgb) SDFB_REQUIRE(head_weights != nullptr && directions != nullptr, "rgb needs head_weights and directions");
   NerfactoArgs a;

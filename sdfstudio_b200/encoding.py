@@ -17,8 +17,20 @@ from typing import Optional
 import numpy as np
 import torch
 from torch import nn
+from torch.optim.optimizer import register_optimizer_step_post_hook
 
 from . import _lib
+
+# Bumped after every optimizer step.  A fused optimizer step (torch.optim.Adam(fused=True)) writes the parameters without bumping their
+# version counter, so Encoding.compute_table keys its fp16 copy on this as well.
+_optimizer_steps = [0]
+
+
+def _count_optimizer_step(optimizer, args, kwargs):
+    _optimizer_steps[0] += 1
+
+
+register_optimizer_step_post_hook(_count_optimizer_step)
 
 
 def growth_factor(num_levels: int, base_res: int, max_res: float) -> float:
@@ -241,11 +253,16 @@ class Encoding(nn.Module):
         return self.hash_table if self.layout == "torch" else self.params
 
     def compute_table(self) -> torch.Tensor:
-        """the tensor the kernels gather from (the parameter itself, or its cached fp16 copy)."""
+        """the tensor the kernels gather from (the parameter itself, or its cached fp16 copy).
+
+        The fp16 copy is rebuilt when the parameter is reallocated, written in place (its version counter: optimizer steps with
+        ``foreach``, ``load_state_dict``, ``copy_`` under ``no_grad``) or after any optimizer step (fused steps do not bump the version
+        counter).  A write through ``.data`` is NOT seen: ``.data`` has a version counter of its own, so the kernels keep gathering the
+        old values until one of the events above.  Write under ``torch.no_grad()`` instead."""
         t = self.table
         if self.table_dtype == "fp32" or t.dtype == torch.float16:
             return t.detach()
-        key = (t.data_ptr(), t._version, str(t.device))
+        key = (t.data_ptr(), t._version, str(t.device), _optimizer_steps[0])
         if self._half_key != key:
             self._half_cache = t.detach().to(torch.float16)
             self._half_key = key

@@ -141,6 +141,8 @@ def test_field_calls_reject_invalid_inputs(preset, precision):
     assert forward(field_in(beta=None), field_out(density=0x90000)) == -1
     assert forward(field_in(beta_min=None), field_out(density=0x90000)) == -1
     assert forward(field_in(), field_out(sampled_sdf=0x90000)) == -1                           # numerical gradients only
+    if d.use_grid_feature:                                                                     # F = 2 fp32 rows are read 8 bytes at a time
+        assert forward(field_in(), field_out(sdf=0x90000), tb=table + 4) == -1 and b"aligned to 8 bytes" in lib.sdfb200_last_error_string()
 
     def render(fin, out=None, nbytes=big, from_density=0, **kw):
         rnd = _lib.FieldRender()
@@ -160,6 +162,58 @@ def test_field_calls_reject_invalid_inputs(preset, precision):
     assert render(field_in(variance=None)) == -1                                               # NeuS alphas
     assert render(field_in(beta=None), from_density=1) == -1                                   # Laplace density
     assert render(field_in(), field_out(sampled_sdf=0x90000)) == -1
+    if d.use_grid_feature:
+        assert lib.sdfb200_field_render(d, packed, table + 4, field_in(), None, C.byref(_lib.FieldRender()), ws, big, None) == -1
+        assert b"aligned to 8 bytes" in lib.sdfb200_last_error_string()
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason="the calls get sentinel device pointers, which a call that is not rejected would launch on")
+@pytest.mark.parametrize("table_dtype", ["fp32", "fp16"])
+@pytest.mark.parametrize("F", [1, 2, 4, 8])
+def test_grid_calls_refuse_misaligned_tables(F, table_dtype):
+    """The grid kernels read a table row with vector loads of min(F * sizeof(T), 16) bytes and scatter its gradient with 16-byte (F % 4 == 0),
+    8-byte (F == 2) or 4-byte atomics.  Every entry point over a grid refuses a pointer those loads and atomics cannot take, with -1 and a
+    message naming the alignment, before it launches anything.  The pointers are sentinels that a rejected call never dereferences."""
+    from sdfstudio_b200 import _lib
+    from sdfstudio_b200.encoding import make_grid_desc
+
+    lib = _lib.load()
+    dt = torch.float16 if table_dtype == "fp16" else torch.float32
+    load = min(F * (2 if table_dtype == "fp16" else 4), 16)
+    add = 16 if F % 4 == 0 else 8 if F == 2 else 4
+    g = make_grid_desc("tcnn", 4, F, 12, 4, 2.0, False, dt)
+    T0, X, DO, OUT, GDX = 0x100000, 0x200000, 0x300000, 0x400000, 0x500000
+    bad_tables = [T0 + off for off in range(1, load)]
+    bad_grads = [0x600000 + off for off in range(4, add, 4)]
+    assert len(bad_tables) == load - 1 and len(bad_grads) == add // 4 - 1
+
+    def refused(rc, what):
+        msg = lib.sdfb200_last_error_string()
+        return rc == -1 and what in msg and b"aligned" in msg
+
+    for t in bad_tables:
+        what = b"table"
+        assert refused(lib.sdfb200_grid_encode(g, t, X, 4, OUT, 4 * F, None, None), what)
+        assert refused(lib.sdfb200_grid_encode(g, t, X, 4, OUT, 4 * F, GDX, None), what)
+        assert refused(lib.sdfb200_grid_encode_grouped(g, t, X, 4, 2, OUT, 4 * F, None), what)
+        assert refused(lib.sdfb200_grid_encode_backward(g, t, X, DO, 4, None, GDX, None), what)
+        assert refused(lib.sdfb200_grid_encode_backward_backward(g, t, X, DO, GDX, 4, OUT, None, None, None), what)
+        assert refused(lib.sdfb200_density_field_forward(g, t, 0x700000, 16, 1, _lib.CONTRACT_LINF, None, X, 4, OUT, None, None), what)
+        if F == 2:
+            nd = _lib.NerfactoDesc(64, 1, 64, 2, 15, 0, _lib.CONTRACT_LINF, 0)
+            assert refused(lib.sdfb200_nerfacto_field_forward(g, nd, t, 0x700000, 0x800000, None, X, 0x900000, None, 4, None, 0, OUT, None, None,
+                                                              None, None), what)
+    for d in bad_grads:
+        what = b"gradient"
+        assert refused(lib.sdfb200_grid_encode_backward(g, T0, X, DO, 4, d, None, None), what)
+        assert refused(lib.sdfb200_grid_encode_backward(g, T0, X, DO, 4, d, GDX, None), what)
+        assert refused(lib.sdfb200_grid_encode_backward_grouped(g, X, DO, 4, 2, d, None), what)
+        assert refused(lib.sdfb200_grid_encode_backward_backward(g, T0, X, DO, GDX, 4, None, d, None, None), what)
+    assert lib.sdfb200_grid_encode(g, T0 + 1, X, 4, OUT, 4 * F, None, None) == -1
+    assert f"aligned to {load} bytes".encode() in lib.sdfb200_last_error_string()
+    if add > 4:
+        assert lib.sdfb200_grid_encode_backward(g, T0, X, DO, 4, 0x600004, None, None) == -1
+        assert f"aligned to {add} bytes".encode() in lib.sdfb200_last_error_string()
 
 
 def test_product_does_not_import_oracle():
