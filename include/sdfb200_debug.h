@@ -25,11 +25,11 @@ int sdfb200_debug_tc_linear(int32_t planes, int32_t epi, const float* X, int32_t
                             int32_t ldy, int64_t M, int32_t Np, int32_t Kp, const float* aux, int32_t ldaux, int32_t aux_cols,
                             void* scratch, void* stream);
 
-/* debug: copies the 16x32 clock64 phase stamps recorded by the fused tensor-core kernel (CTA 0, first 16 tiles; per tile: the
+/* debug: copies the 16x48 clock64 phase stamps recorded by the fused tensor-core kernel (CTA 0, first 16 tiles; per tile: the
  * consumers' phase ends and waits, the encoder warps' busy / wait cycles and the heads warp's cycles, layout in field_tc_kernel.cuh
- * next to TC_PUT) into a HOST buffer of 512 int64.  The stamps come from the debug library's own build of the bf16x3 / torch-layout instantiation, compiled with
+ * next to TC_PUT) into a HOST buffer of 768 int64.  The stamps come from the debug library's own build of the bf16x3 / torch-layout instantiation, compiled with
  * -DSDFB200_TC_TIMING (sdfstudio_b200/build.py); the product library records none. */
-int sdfb200_debug_tc_timing(long long* host_out_512);
+int sdfb200_debug_tc_timing(long long* host_out_768);
 
 #ifdef __cplusplus
 }

@@ -15,6 +15,7 @@ constexpr int kEncThreads = 96;                              // encoder warps: t
 // .. enc_item_begin(w + 1) - 1 in order.  sdf-only mode (640 items, no heads) splits evenly: item i -> thread i % 96.
 constexpr int kEncItems0 = 288, kEncItems1 = 256, kEncItems2 = 224;
 static_assert(kEncItems0 + kEncItems1 + kEncItems2 == 768, "the encoder warps' items cover the tile");
+static_assert(kEncItems0 % 32 == 0 && kEncItems1 % 32 == 0, "a warp stages whole 32-row batches (colour_static_tile shuffles across them)");
 __host__ __device__ constexpr int enc_item_begin(int w) { return w == 0 ? 0 : w == 1 ? kEncItems0 : w == 2 ? kEncItems0 + kEncItems1 : 768; }
 // register split after setmaxnreg.  The launch gets 168 per thread (65536 / 384, rounded down to a multiple of 8); the consumers can
 // only take what the producer warpgroup gives back: 256 x (216 - 168) = 128 x (168 - 72)
@@ -55,14 +56,14 @@ constexpr size_t kSmemPerBlock = 232448;  // H100: 227 KB of shared memory per b
 constexpr size_t kStaticSmem = 1024;      // the kernel's static shared memory (barriers): one 1024-byte slot, the dynamic part is 1024-aligned
 static_assert(tc_smem(2).bytes + kStaticSmem <= kSmemPerBlock, "shared memory of k_field_tc at two planes");
 
-// Per-CTA scratch of k_field_tc (caller workspace): byte offsets from the CTA's base.  sig and h2 are planes of [64 units][256 threads]
-// x 4 B (kFragWords) in the accumulator-fragment order of the thread that writes and later reads them.
+// Per-CTA scratch of k_field_tc (caller workspace): byte offsets from the CTA's base.  sig is a plane of [64 units][256 threads] x 4 B
+// (kFragWords) in the accumulator-fragment order of the thread that writes and later reads it.
 constexpr size_t kFragWords = 64 * 256;
 struct TcScratch { size_t sig, h2, slots, slot_bytes, geo, cs, jpe, jg, bytes; };
 __host__ __device__ constexpr TcScratch tc_scratch(int planes) {
   TcScratch s{};                                               // sig: softplus'(z1) as 2 x unorm16
-  s.h2 = s.sig + kFragWords * 4;                               // h2 as bf16x2 planes [P]
-  s.slots = s.h2 + (size_t)planes * kFragWords * 4;            // two staging slots (tile parity), slot_bytes apart, each with:
+  s.h2 = s.sig + kFragWords * 4;                               // h2 in the A operand's layout [P][32 chunks][128 rows][16 B]
+  s.slots = s.h2 + (size_t)planes * kAPlane;                   // two staging slots (tile parity), slot_bytes apart, each with:
   s.cs = s.geo + (size_t)planes * kImgPlane;                   //   geo input image [P][12 chunks][128 rows][16 B] at geo = 0 and the
   s.jpe = s.cs + (size_t)planes * kImgPlane;                   //   colour-static image (same layout, chunk 0 unused); PE jacobian
   s.jg = s.jpe + (size_t)kPeRows * 128 * 4;                    //   [kPeRows][128] f32, grid jacobian [kMaxGridDim * 3][128] f32

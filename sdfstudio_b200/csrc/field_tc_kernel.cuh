@@ -77,7 +77,9 @@ static __device__ __forceinline__ float sin_call(float x) { return sinf(x); }
 
 // Hash-grid part of the geo input of one tile, levels 4 grp .. 4 grp + 3 of one point (= operand chunk grp).  Outputs: bf16 planes
 // of the staged geo input image (`img`, planes `plane` bytes apart, kernel column order: four levels = one aligned 16-byte chunk)
-// and the grid jacobian Jg [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  One level at a time (smallest code).
+// and the grid jacobian Jg [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  The item's 32 corner rows are first requested
+// into L2 (no registers held), so that the level loop, one level at a time (smallest code, 8 gathers in flight), waits for L2 rather
+// than for HBM on its four dependent gather round trips.
 template <int P, int LAYOUT>
 __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int row, int grp, uint8_t* img, uint32_t plane, float* Jg,
                                                  uint64_t pol_table) {
@@ -85,12 +87,22 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
   const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
   const PointGeom g = point_geom(a, p);
   const float x01 = (g.px + 2.0f) * 0.25f, y01 = (g.py + 2.0f) * 0.25f, z01 = (g.pz + 2.0f) * 0.25f;   // sdf_field.py:384
-  // one level at a time, rolled (code size): 8 gathers in flight per thread, feature columns as 2-byte operand stores
+  const int l_end = min(4 * grp + 4, min(a.grid.n_levels, a.grid.active_levels));
+  if (a.use_grid && a.mode != 0) {   // sdf-only calls (the samplers' passes) measured slower with it
+#pragma unroll 1
+    for (int l = 4 * grp; l < l_end; ++l) {
+      LevelCtx c;
+      level_prepare<LAYOUT>(a.grid, l, x01, y01, z01, c);
+      if (a.grid.table_dtype == SDFB200_DT_F16) level_prefetch_l2<__half, 2>(a.table, c);
+      else level_prefetch_l2<float, 2>(a.table, c);
+    }
+  }
+  // feature columns as 2-byte operand stores
 #pragma unroll 1
   for (int l = 4 * grp; l < 4 * grp + 4; ++l) {
     float o[2] = {0.f, 0.f};
     float dj[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-    if (a.use_grid && l < a.grid.n_levels && l < a.grid.active_levels) {
+    if (a.use_grid && l < l_end) {
       LevelCtx c;
       float tv[8][2];
       level_prepare<LAYOUT>(a.grid, l, x01, y01, z01, c);
@@ -147,27 +159,34 @@ __device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int ro
   store_a<P>(img, plane, row, 32 + a.pe_dim + 2, pc[2]);
 }
 
+// direction-encoding value k (0..23) of direction d: sin(d_b 2^j) for k < 12, sin(d_b 2^j + pi/2) for k >= 12, b = (k mod 12) / 4,
+// j = k mod 4 (NeRFEncoding(4), encodings.py:167-208).  d_b 2^j is exact, so a contracted d_b 2^j + pi/2 rounds the same.
+__device__ __forceinline__ float dir_enc(const PointGeom& g, int k) {
+  const int i = k < 12 ? k : k - 12, b = i >> 2;
+  const float db = b == 0 ? g.dx : (b == 1 ? g.dy : g.dz);
+  const float arg = db * (float)(1 << (i & 3));
+  return sin_call(k < 12 ? arg : arg + kHalfPiF);
+}
+
 // static colour-operand columns of a tile (kernel columns 8..95 = chunks 1..11): x(3) | dir-enc(24) | dir(3) | appearance | 0, staged in
-// the same [plane][chunk][row][16 B] layout as the A operand; EB0 copies them over the A columns that B0 has consumed (chunk 0 =
-// [grad, n.v] comes from the epilogue)
+// the same [plane][chunk][row][16 B] layout as the A operand; colour_copy bulk-copies them over the A columns that B0 has consumed
+// (chunk 0 = [grad, n.v] comes from the epilogue).  Called by a whole warp for 32 consecutive rows (lane = row mod 32): when they are
+// all samples of one ray, lane k < 24 evaluates direction-encoding value k once for the warp (the same sinf of the same argument).
 template <int P>
 __device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, int row, uint8_t* img, uint32_t plane) {
   const long long p_raw = (long long)tile * 128 + row;
   const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
   const PointGeom g = point_geom(a, p);
+  const bool one_ray = __match_any_sync(0xffffffffu, g.ray) == 0xffffffffu;
+  const int lane = row & 31;
+  const float own = one_ray && lane < 24 ? dir_enc(g, lane) : 0.f;
   const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll 1
   for (int ch = 1; ch < kInK / 8; ++ch) store_a_chunk<P>(img, plane, row, ch, z4, z4);
   store_a<P>(img, plane, row, 8 + 0, g.px); store_a<P>(img, plane, row, 8 + 1, g.py); store_a<P>(img, plane, row, 8 + 2, g.pz);
-  // direction encoding: sin(d 2^k) | sin(d 2^k + pi/2), k = 0..3, then d itself (NeRFEncoding(4, include_input), encodings.py:167-208)
+  // direction encoding, then d itself (include_input)
 #pragma unroll 1
-  for (int i = 0; i < 12; ++i) {
-    const int b = i >> 2;
-    const float db = b == 0 ? g.dx : (b == 1 ? g.dy : g.dz);
-    const float arg = db * (float)(1 << (i & 3));
-    store_a<P>(img, plane, row, 8 + 3 + i, sin_call(arg));
-    store_a<P>(img, plane, row, 8 + 15 + i, sin_call(arg + kHalfPiF));
-  }
+  for (int k = 0; k < 24; ++k) store_a<P>(img, plane, row, 8 + 3 + k, one_ray ? __shfl_sync(0xffffffffu, own, k) : dir_enc(g, k));
   store_a<P>(img, plane, row, 8 + 27, g.dx); store_a<P>(img, plane, row, 8 + 28, g.dy); store_a<P>(img, plane, row, 8 + 29, g.dz);
   if (a.appearance != nullptr) {
 #pragma unroll 1
@@ -189,18 +208,19 @@ struct Slot {
 #ifdef SDFB200_TC_TIMING
 // CTA 0, first 16 tiles, row = tile: clock64() of consumer thread 0 at [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring
 // order), [8] the tile's geo input has landed (a full; [8] - [0] is the consumers' wait for the encoder), [15] tile end = end of EC1
-// (head inputs handed over), [18..23] end of the epilogues E0, E1, EB1, EB0, h2 reload, EC0 (before the SYNC_A that hands their A
+// (head inputs handed over), [18..23] end of the epilogues E0, E1, EB1, EB0, the late h2 copy issued, EC0 (before the SYNC_A that hands their A
 // operand to the next layer's MMAs); cycle sums over the tile of [9] consumer thread 0 waiting for weights (ring full), [10] the producer
 // waiting for a free ring slot (ring empty), [12] encoder thread 0 busy staging the tile, [13] encoder thread 0 waiting for its staging
 // slot (enc empty), [14] encoder thread 0 running the tile's heads / compositing, [16] consumer thread 0 waiting for the tile's
 // head-input buffer (hs empty), [17] encoder thread 0 waiting for the tile's head inputs (hs full), [24] [25] lane 0 of encoder
 // warps 1, 2 busy staging the tile (warp 0: [12]), [26] [27] the same running the heads of the tile (warp 0: [14]), [28..30] encoder
 // thread 0's heads split: per-row heads (geometry, sdf -> alpha / sigma, per-sample outputs), transmittance scan and weights, sums and
-// the ray finish; [31] encoder thread 0 waiting at the encoder warps' barrier (kEncBar)
-__device__ long long g_tc_timing[16 * 32];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
+// the ray finish; [31] encoder thread 0 waiting at the encoder warps' barrier (kEncBar); [32 + 3 w + k] lane 0 of encoder warp w
+// staging items of kind k (0 grid, 1 PE, 2 colour-static)
+__device__ long long g_tc_timing[16 * 48];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
 #define TC_PUT(tno, k, v)                                                                                            \
   do {                                                                                                               \
-    if (blockIdx.x == 0 && (tno) >= 0 && (tno) < 16) g_tc_timing[(tno) * 32 + (k)] = (v);                            \
+    if (blockIdx.x == 0 && (tno) >= 0 && (tno) < 16) g_tc_timing[(tno) * 48 + (k)] = (v);                            \
   } while (0)
 #else
 #define TC_PUT(tno, k, v) do { (void)(v); } while (0)
@@ -214,6 +234,8 @@ struct TcBars {
   Handoff<1> a;           // A operand: full 1 + bytes (geo input landed), empty 2, one per consumer warpgroup (last layer has read A)
   Handoff<2> hs;          // head inputs: full kEpiThreads (after EC1), empty kEncThreads (the encoder warps are through the tile's heads);
                           // unused in sdf-only mode
+  uint64_t cop[2][2];     // per consumer warpgroup, count 1 + bytes: [0] colour-static columns and h2 chunks 0..19 copied into A after
+                          // B0, [1] h2 chunks 20..31 copied after C0-misc (colour_copy); unused in sdf-only mode
 };
 
 // Producer (one thread of the producer warpgroup).  Per tile: once the consumers have freed the A operand and the encoder has staged
@@ -244,9 +266,12 @@ __device__ __forceinline__ void produce_all(const TcArgs& a, int nlayers, uint8_
 // 128 for B0: acc[0..1]), the weight K-blocks taken from the ring in order.  Every consumer warp releases a slot once its MMAs on it are
 // complete (empty barrier count = 8 warps).  Each block is drained before the next is issued: with the producer in its own warpgroup and
 // 5 stages, keeping one block in flight (wait_group 1) measured no faster.
+// C0-h2 reads h2 where colour_copy put it: K step j (h2 chunks 2j, 2j + 1) from A chunks (2j + kInK / 8) mod 32, and waits for the late
+// copy (`h2_late`, phase h2_parity) before the first K step it fills.  K order, weights and accumulation are those of any other layer.
+constexpr int kH2Early = 32 - kInK / 8;   // h2 chunks 0 .. kH2Early - 1 land in A chunks kInK / 8 .. 31, the others in A chunks 0 .. kInK / 8 - 1
 template <int P, int L>
 __device__ __forceinline__ void layer_mma(float (&acc)[4][32], bool zero, uint32_t a_base, const uint8_t* ring, Handoff<kStages>& rb, uint32_t& it,
-                                          int lane, long long& waited) {
+                                          int lane, long long& waited, uint64_t* h2_late, uint32_t h2_parity) {
   constexpr int N = tc_layer_np(L);
   constexpr int KSTEPS = tc_layer_kblk(L) / 16;              // K steps per ring stage
   constexpr uint32_t lbo_b = N * 16, plane_b = N * KSTEPS * 16 * 2;
@@ -257,6 +282,7 @@ __device__ __forceinline__ void layer_mma(float (&acc)[4][32], bool zero, uint32
   }
 #pragma unroll 1
   for (int kb = 0; kb < tc_layer_nkb(L); ++kb, ++it) {
+    if (L == L_C0H && kb * KSTEPS == kH2Early / 2) mbar_wait(h2_late, h2_parity);
     rb.wait_full(it, &waited);
     const uint32_t wbase = smem_u32(ring + (size_t)rb.slot(it) * tc_stage_bytes(P));
     wg_fence_acc(d);
@@ -264,7 +290,8 @@ __device__ __forceinline__ void layer_mma(float (&acc)[4][32], bool zero, uint32
 #pragma unroll
     for (int j = 0; j < KSTEPS; ++j) {
       const int kstep = kb * KSTEPS + j;
-      wgmma_kstep_wide_ss<P, N>(d, a_desc(a_base, kstep), a_desc(a_base + kAPlane, kstep), wbase + j * 2 * lbo_b, plane_b, lbo_b);
+      const int ka = L == L_C0H ? (kstep + kInK / 16) % 16 : kstep;
+      wgmma_kstep_wide_ss<P, N>(d, a_desc(a_base, ka), a_desc(a_base + kAPlane, ka), wbase + j * 2 * lbo_b, plane_b, lbo_b);
     }
     wg_commit();
     wg_wait<0>();
@@ -285,9 +312,9 @@ struct TileCtx {
   const float4* coldesc;     //   EB0's column table
   float sdf_bias;
   uint32_t* sig_s;           // per-CTA scratch (tc_scratch): softplus'(z1)
-  uint32_t* gf_s;            //   h2 planes
+  uint8_t* h2img;            //   h2 planes in the A operand's layout
   char* slots;               //   staging slots
-  // this thread's 4-byte unit for the accumulator pair (c, i) in a [64 units][256 threads] scratch plane (sig_s, gf_s)
+  // this thread's 4-byte unit for the accumulator pair (c, i) in a [64 units][256 threads] scratch plane (sig_s)
   __device__ __forceinline__ int unit(int c, int i) const { return (c * 16 + (i >> 1)) * kEpiThreads + tid; }
 };
 
@@ -344,7 +371,8 @@ __device__ __forceinline__ void epi_e0(const TileCtx& x, float (&acc)[4][32]) {
   }
 }
 
-// E1 (after G1): sdf = W2[0,:] . h2 + b (fp32) -> output / heads ; h2 -> scratch planes ; g2 = W2[0,:] * softplus'(z2) -> A
+// E1 (after G1): sdf = W2[0,:] . h2 + b (fp32) -> output / heads ; h2 -> scratch image (A layout, read back by colour_copy's bulk
+// copies) ; g2 = W2[0,:] * softplus'(z2) -> A
 template <int P>
 __device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, float (&acc)[4][32]) {
   const TcArgs& a = x.a;
@@ -369,15 +397,13 @@ __device__ __forceinline__ void epi_e1(const TileCtx& x, int tile, float (&acc)[
       sp = fmaf(w2.x, h0, sp);
       sp = fmaf(w2.y, h1, sp);
       if (a.mode != 0) {
-        uint32_t hi, lo;
-        split2(h0, h1, hi, lo);
-        const int u = x.unit(c, i);
-        x.gf_s[u] = hi;
-        if (P > 1) x.gf_s[kFragWords + u] = lo;
+        store_a_pair<P>(x.h2img, kAPlane, row, col, h0, h1);
         store_a_pair<P>(x.abuf, kAPlane, row, col, w2.x * s0, w2.y * s1);
       }
     }
   }
+  // hand-off: h2 (generic stores, global) -> colour_copy's bulk copies (async proxy), behind the warpgroup barriers up to B0
+  if (a.mode != 0) fence_async_global();
   sp0 = quad_sum(sp0);
   sp1 = quad_sum(sp1);
   if ((x.t & 3) < 2) {
@@ -431,23 +457,41 @@ __device__ __forceinline__ float4 col_desc(const TcArgs& a, int ip) {
   return make_float4(__int_as_float(jrow), ax == 0 ? 1.f : 0.f, ax == 1 ? 1.f : 0.f, ax == 2 ? 1.f : 0.f);
 }
 
-// EB0 (after B0): gin (96 cols, kernel order) . input jacobian -> d sdf / dx; then the colour misc operand over the (consumed) A columns
-// 0..95: chunk 0 = [grad(3), n.v, 0 x4] (sdf_field.py:572-584; columns re-ordered at pack time) from the thread pair that owns the row,
-// chunks 1..11 = [x, dir-enc, dir, appearance] copied from the tile's staging slot (16-byte units, the warpgroup's 64 rows)
+// Bulk copies of the colour MLP's A operand, issued by warp 0 of the warpgroup (lane 0 arms the barrier, every lane issues some of the
+// 1 KB copies: one plane of one chunk of the warpgroup's 64 rows).  Early (after B0, `cop[wg][0]`): the colour-static columns
+// (chunks 1..11 of the staging slot) into A chunks 1..11, h2 chunks 0..kH2Early - 1 into A chunks kInK / 8 .. 31.  Late (after C0-misc,
+// `cop[wg][1]`): the other h2 chunks into A chunks 0..kInK / 8 - 1.  A chunks are free once the layer before has read them (its MMAs are
+// complete and the warpgroup barrier is passed); earlier generic stores to them were fenced (SYNC_A).
+template <int P>
+__device__ __forceinline__ void copy_chunks(uint8_t* abuf, int a_chunk, const uint8_t* src, uint32_t src_plane, int src_chunk, int n, int wrow0,
+                                            uint64_t* bar, int lane) {
+  for (int k = lane; k < P * n; k += 32) {
+    const int pl = k / n, c = k - pl * n;
+    bulk_g2s(abuf + pl * kAPlane + (a_chunk + c) * kAChunk + wrow0 * 16, src + pl * src_plane + (src_chunk + c) * kAChunk + wrow0 * 16, 64 * 16, bar);
+  }
+}
+template <int P>
+__device__ __forceinline__ void colour_copy(const TileCtx& x, bool early, const uint8_t* cs, uint64_t* bar) {
+  constexpr int kMisc = kInK / 8;
+  const int lane = x.t & 31;
+  if (lane == 0) mbar_arrive_expect_tx(bar, (uint32_t)P * (early ? (kMisc - 1) + kH2Early : 32 - kH2Early) * 64 * 16);
+  __syncwarp();
+  if (early) {
+    copy_chunks<P>(x.abuf, 1, cs, kImgPlane, 1, kMisc - 1, x.wrow0, bar, lane);
+    copy_chunks<P>(x.abuf, kMisc, x.h2img, kAPlane, 0, kH2Early, x.wrow0, bar, lane);
+  } else {
+    copy_chunks<P>(x.abuf, 0, x.h2img, kAPlane, kH2Early, 32 - kH2Early, x.wrow0, bar, lane);
+  }
+}
+
+// EB0 (after B0): gin (96 cols, kernel order) . input jacobian -> d sdf / dx -> chunk 0 of the colour misc operand over the (consumed)
+// A columns: [grad(3), n.v, 0 x4] (sdf_field.py:572-584; columns re-ordered at pack time) from the thread pair that owns the row.  The
+// other chunks ([x, dir-enc, dir, appearance], h2) arrive by colour_copy.
 template <int P>
 __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P>& s, const float (&acc)[4][32]) {
   const TcArgs& a = x.a;
   const float* Jpe = s.jpe();
   const float* Jg = s.jg();
-  // colour-static units (below) loaded first, so that they are in flight together with the jacobian loads
-  // unit k: plane k / (11 * 64), chunk 1 + (k / 64) % 11, row wrow0 + k % 64
-  constexpr int kUnits = 11 * 64 * P, kPer = (kUnits + 127) / 128;
-  uint4 v[kPer];
-#pragma unroll
-  for (int j = 0; j < kPer; ++j) {
-    const int k = x.t + 128 * j, pl = k / (11 * 64), ch = 1 + (k - pl * 11 * 64) / 64, row = x.wrow0 + (k & 63);
-    if (k < kUnits) v[j] = *reinterpret_cast<const uint4*>(s.cs() + pl * kImgPlane + ch * kAChunk + row * 16);
-  }
   // d sdf / dx of rows r0 (g*0) and r0 + 8 (g*1), named scalars (see epi_e1).  Every column is accumulated the same way whatever its
   // kind, the kind coming from the column table (ColDesc): a zero factor adds +-0, which leaves the sum as it is, so the result is
   // the one of accumulating the live columns alone
@@ -486,25 +530,6 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
     const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? n.x * pg.dx + n.y * pg.dy + n.z * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
     store_a_chunk<P>(x.abuf, kAPlane, row, 0, c0v);
     x.hs[HS_GRAD][row] = grx; x.hs[HS_GRAD + 1][row] = gry; x.hs[HS_GRAD + 2][row] = grz;
-  }
-#pragma unroll
-  for (int j = 0; j < kPer; ++j) {
-    const int k = x.t + 128 * j, pl = k / (11 * 64), ch = 1 + (k - pl * 11 * 64) / 64, row = x.wrow0 + (k & 63);
-    if (k < kUnits) *reinterpret_cast<uint4*>(x.abuf + pl * kAPlane + ch * kAChunk + row * 16) = v[j];
-  }
-}
-
-// C0 h2 operand: h2 (bf16 planes, saved by E1) back from the scratch over the misc columns that C0's first part has consumed
-template <int P>
-__device__ __forceinline__ void reload_h2(const TileCtx& x) {
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const int col = frag_col(x.cq, c, i), row = frag_row(x.r0, i);
-      const int u = x.unit(c, i);
-      store_a_pair<P>(x.abuf, kAPlane, row, col, x.gf_s[u], x.gf_s[kFragWords + u]);
-    }
   }
 }
 
@@ -779,17 +804,20 @@ __device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots,
     b.enc.wait_empty(tile_no, &waited);
     const long long t0 = TC_CLOCK();
     const Slot<P> s(slots, b.enc.slot(tile_no));
+    long long kind_grid = 0, kind_pe = 0, kind_cs = 0;   // staging cycles by item kind (timing build)
 #pragma unroll 1
     for (int i = i_begin; i < i_end; i += i_step) {
       const int row = i & 127;
-      if (i < 512) encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jg(), pol_table);
-      else if (i < 640) encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jpe());
-      else colour_static_tile<P>(a, tile, row, s.cs(), kImgPlane);
+      const long long c0 = TC_CLOCK();
+      if (i < 512) { encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jg(), pol_table); kind_grid += TC_CLOCK() - c0; }
+      else if (i < 640) { encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jpe()); kind_pe += TC_CLOCK() - c0; }
+      else { colour_static_tile<P>(a, tile, row, s.cs(), kImgPlane); kind_cs += TC_CLOCK() - c0; }
     }
     fence_async_global();                    // the geo image is read by the producer's bulk copy (async proxy)
     b.enc.arrive_full(tile_no);
     if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - t0); TC_PUT(tile_no, 13, waited); }
     else if (lane == 0) TC_PUT(tile_no, 23 + ew, TC_CLOCK() - t0);
+    if (lane == 0) { TC_PUT(tile_no, 32 + 3 * ew, kind_grid); TC_PUT(tile_no, 33 + 3 * ew, kind_pe); TC_PUT(tile_no, 34 + 3 * ew, kind_cs); }
     if (heads && tile_no > 0) heads_of(a, tile - (int)gridDim.x, tile_no - 1, et, b, hs, hx, xf, dmin, dmax);
   }
   if (heads && tile_no > 0) heads_of(a, blockIdx.x + (tile_no - 1) * (int)gridDim.x, tile_no - 1, et, b, hs, hx, xf, dmin, dmax);   // the last tile
@@ -827,6 +855,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     bars.enc.init(kEncThreads, kEpiThreads);
     bars.hs.init(kEpiThreads, kEncThreads);
     bars.a.init(1, 2);
+    for (int w = 0; w < 2; ++w) { mbar_init(&bars.cop[w][0], 1); mbar_init(&bars.cop[w][1], 1); }
     fence_barrier_init();
   }
   {
@@ -856,7 +885,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   const uint32_t a_base = smem_u32(abuf) + wrow0 * 16;
   const float sdf_bias = __ldg(reinterpret_cast<const float*>(a.blob + a.b_g2));
   TileCtx x{a, tid, t, wg, wrow0, frag_row0(wrow0, t), frag_cq(t), abuf, prm, hs, coldesc, sdf_bias,
-            reinterpret_cast<uint32_t*>(cta_scr + scr.sig), reinterpret_cast<uint32_t*>(cta_scr + scr.h2), slots};
+            reinterpret_cast<uint32_t*>(cta_scr + scr.sig), reinterpret_cast<uint8_t*>(cta_scr + scr.h2), slots};
   uint32_t it = 0;
   long long waited = 0;
   float acc[4][32];
@@ -867,7 +896,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   } while (0)
 #define LAYER(L, zero)                                                                                 \
   do {                                                                                                 \
-    layer_mma<P, L>(acc, zero, a_base, ring, bars.ring, it, lane, waited);                             \
+    layer_mma<P, L>(acc, zero, a_base, ring, bars.ring, it, lane, waited, &bars.cop[wg][1], tile_no & 1); \
     named_sync(wg_bar, 128); /* every warp of the warpgroup is done reading this layer's A operand */  \
     TC_STAMP(1 + (L));                                                                                 \
   } while (0)
@@ -905,16 +934,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     TC_STAMP(20);
     SYNC_A();
     LAYER(L_B0, true);
-    bars.enc.wait_full(tile_no);               // (long complete: makes the encoder's jacobian / colour-static stores visible)
+    bars.enc.wait_full(tile_no);               // (long complete: the encoder's jacobian / colour-static stores are visible, and fenced
+                                               // for the async proxy)
+    if (t < 32) colour_copy<P>(x, true, s.cs(), &bars.cop[wg][0]);
     epi_eb0<P>(x, tile, s, acc);
-    bars.enc.arrive_empty(tile_no);
+    mbar_wait(&bars.cop[wg][0], tile_no & 1);  // the colour-static columns and early h2 chunks have landed
+    bars.enc.arrive_empty(tile_no);            // the slot's last reader (the early copy) is complete
     TC_STAMP(21);
     SYNC_A();
     LAYER(L_C0MISC, true);
-    reload_h2<P>(x);
+    if (t < 32) colour_copy<P>(x, false, nullptr, &bars.cop[wg][1]);
     TC_STAMP(22);
-    SYNC_A();
-    LAYER(L_C0H, false);                       // accumulates onto the misc columns' result
+    LAYER(L_C0H, false);                       // accumulates onto the misc columns' result; waits for the late h2 copy inside
     epi_ec0<P>(x, acc);
     TC_STAMP(23);
     SYNC_A();

@@ -6,8 +6,8 @@ int launch_field_tc_p2_torch(const TcArgs& a, int grid, size_t smem, cudaStream_
 }  // namespace sdfb200
 
 #ifdef SDFB200_TC_TIMING
-extern "C" int sdfb200_debug_tc_timing(long long* host_out_512) {
-  SDFB_CUDA(cudaMemcpyFromSymbol(host_out_512, sdfb200::g_tc_timing, sizeof(long long) * 512));
+extern "C" int sdfb200_debug_tc_timing(long long* host_out_768) {
+  SDFB_CUDA(cudaMemcpyFromSymbol(host_out_768, sdfb200::g_tc_timing, sizeof(sdfb200::g_tc_timing)));
   return 0;
 }
 #endif

@@ -139,6 +139,14 @@ __device__ __forceinline__ void level_fetch(const void* table, const LevelCtx& c
   for (int k = 0; k < 8; ++k) load_row<T, F, HINT>(table, c.base + c.idx[k], v[k], pol);
 }
 
+// the same rows requested into L2 (evict_last, the fused kernel's table policy) without waiting for them or holding registers
+template <typename T, int F>
+__device__ __forceinline__ void level_prefetch_l2(const void* table, const LevelCtx& c) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(reinterpret_cast<const T*>(table) + (c.base + c.idx[k]) * F));
+}
+
 // out[f] and dout[f][c] = d out[f] / d x01[c].  torch: the reference's expression tree (no FMA contraction on the value path).
 template <int F, int LAYOUT = -1>
 __device__ __forceinline__ void level_finish(const sdfb200_grid_t& g, const LevelCtx& c, const float (&v)[8][F], float (&out)[F], float (&dout)[F][3]) {

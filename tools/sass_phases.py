@@ -1,6 +1,6 @@
 """SASS of the fused field kernel's consumer phases, without a GPU.  Compiles one instantiation of k_field_tc with the flags of
 sdfstudio_b200/build.py, disassembles it with its inline line info and attributes every instruction to the call in the kernel body
-it was inlined from.  For each phase function called from the kernel body (epi_e0, epi_e1, epi_eb1, epi_eb0, reload_h2, epi_ec0,
+it was inlined from.  For each phase function called from the kernel body (epi_e0, epi_e1, epi_eb1, epi_eb0, colour_copy, epi_ec0,
 epi_ec1; one row per call site) it prints the instruction count, the main opcodes, and how many of the phase's loads are issued
 directly behind one of its stores, i.e. the loads whose preceding instruction in the phase is a store, and in how many batches its
 loads are issued (runs of loads with no store of the phase between them).  A load placed behind a store waits for whatever the
@@ -33,7 +33,7 @@ def phase_calls():
     start = next(i for i, ln in enumerate(lines) if re.search(r"__global__ .*\bk_field_tc\(", ln))
     calls = {}
     for i in range(start, len(lines)):
-        m = re.search(r"\b(epi_\w+|reload_h2)\s*(<[^>()]*>)?\s*\(", lines[i])
+        m = re.search(r"\b(epi_\w+|colour_copy)\s*(<[^>()]*>)?\s*\(", lines[i])
         if m:
             calls[i + 1] = m.group(1)
     return calls

@@ -51,11 +51,11 @@ with torch.no_grad():
 print(f"field call {sorted(ms)[len(ms)//2]:.3f} ms (median of 10, L2 flushed)")
 lib = _lib.load()
 lib.sdfb200_debug_tc_timing.argtypes = [ctypes.c_void_p]
-buf = (ctypes.c_longlong * 512)()
+buf = (ctypes.c_longlong * 768)()
 assert lib.sdfb200_debug_tc_timing(buf) == 0
 # stamps written by the kernel (field_tc_kernel.cuh, TC_STAMP / TC_PUT), consumer thread 0: [0] tile start, [8] the tile's geo input
 # has landed (a_full), [1 + L] end of layer L's MMAs in the order the kernel runs them, [18..23] end of the epilogues E0, E1, EB1, EB0,
-# h2 reload, EC0 (the epilogue in front of layers 1..6), [15] end of the tile (EC1 done, head inputs handed to the heads warp).  An
+# h2 operand (the late h2 bulk copy issued), EC0 (the epilogue in front of layers 1..6), [15] end of the tile (EC1 done, head inputs handed to the heads warp).  An
 # epilogue's cycles run from the end of the layer before it to its own stamp; a layer's MMA cycles from the end of the epilogue in front
 # of it (or the a_full stamp for G0) to the layer's stamp, so they include the warpgroup barrier and any wait for weights.  Cycle sums
 # over the tile: [9] consumer thread 0 waiting for weights, [10] producer waiting for a free ring slot, [12] encoder thread 0 busy
@@ -63,11 +63,12 @@ assert lib.sdfb200_debug_tc_timing(buf) == 0
 # heads and compositing, [16] consumer thread 0 waiting for the tile's head-input buffer (hs_empty), [17] encoder thread 0 waiting for
 # the tile's head inputs (hs_full); per encoder warp w0 / w1 / w2 (lane 0): busy staging [12] [24] [25] and running
 # the tile's heads [14] [26] [27]; encoder thread 0's heads split [28] per-row heads, [29] transmittance scan + weights, [30] sums and
-# ray finish, and [31] its wait at the encoder warps' barrier.
+# ray finish, and [31] its wait at the encoder warps' barrier; [32 + 3 w + k] encoder warp w's staging split by item kind k (grid,
+# PE, colour-static).
 layers = ["G0", "G1", "B1", "B0", "C0 misc", "C0 h2", "C1"]
-epis = ["E0", "E1", "EB1", "EB0", "h2 reload", "EC0"]      # epis[L - 1] runs in front of layer L
+epis = ["E0", "E1", "EB1", "EB0", "h2 operand", "EC0"]     # epis[L - 1] runs in front of layer L; "h2 operand": the late h2 copy is issued
 for t in (5, 10):
-    st = [buf[t * 32 + k] for k in range(32)]
+    st = [buf[t * 48 + k] for k in range(48)]
     epi = [st[18 + L] - st[1 + L] for L in range(6)] + [st[15] - st[7]]
     mma = [st[1] - st[8]] + [st[2 + L] - st[18 + L] for L in range(6)]
     print(f"tile {t}: total {st[15] - st[0]} cycles  a_full wait {st[8] - st[0]}  |  epilogues {sum(epi)}: "
@@ -77,4 +78,6 @@ for t in (5, 10):
           + f"  |  encoder busy {st[12]}  encoder slot wait {st[13]}  heads {st[14]}  heads wait {st[17]}"
           + f"  |  encoder warps w0/w1/w2: staging {st[12]}/{st[24]}/{st[25]}  heads {st[14]}/{st[26]}/{st[27]}"
           + f"  busy {st[12] + st[14]}/{st[24] + st[26]}/{st[25] + st[27]}"
-          + f"  |  w0 heads: rows {st[28]}  scan+weights {st[29]}  sums+finish {st[30]}  barrier wait {st[31]}")
+          + f"  |  w0 heads: rows {st[28]}  scan+weights {st[29]}  sums+finish {st[30]}  barrier wait {st[31]}"
+          + "  |  staging by kind (grid/PE/colour-static): "
+          + "  ".join(f"w{w} {st[32 + 3 * w]}/{st[33 + 3 * w]}/{st[34 + 3 * w]}" for w in range(3)))
