@@ -269,10 +269,19 @@ class SDFField(nn.Module):
         d.n_geo_linear = n_geo
         for i, v in enumerate(self._geo_dims):
             d.geo_dims[i] = v
-        d.geo_skip_layer = 4 if n_geo > 4 else -1
+        skip = 4 if n_geo > 4 else -1
+        d.geo_skip_layer = skip
         d.n_color_linear = self.num_layers_color - 1
         for i, v in enumerate(self._color_dims):
             d.color_dims[i] = v
+        # the packing reads every layer at the [N, K] the descriptor implies (make_field_plan, csrc/field_plan.h): the layer feeding the
+        # skip concat is narrower.  With num_layers = 3 the reference's skip_in = [4] narrows the LAST layer instead, which the descriptor
+        # cannot express, and a layer replaced by one of another shape would be read out of bounds just the same
+        gd, cd = self._geo_dims, self._color_dims
+        for l in range(n_geo):
+            self._check_layer_shape(f"glin{l}", gd[l + 1] - gd[0] if l + 1 == skip else gd[l + 1], gd[l])
+        for l in range(self.num_layers_color - 1):
+            self._check_layer_shape(f"clin{l}", cd[l + 1], cd[l])
         d.appearance_dim = c.appearance_embedding_dim
         d.use_diffuse_color, d.use_specular_tint = int(c.use_diffuse_color), int(c.use_specular_tint)
         d.use_reflections, d.use_n_dot_v = int(c.use_reflections), int(c.use_n_dot_v)
@@ -280,6 +289,19 @@ class SDFField(nn.Module):
         d.rgb_padding = c.rgb_padding
         d.precision = _lib.PRECISION[getattr(c, "precision", "fp32")]
         return d
+
+    def _check_layer_shape(self, name: str, n: int, k: int) -> None:
+        """ValueError unless Linear `name` holds an [n, k] weight (weight-normed: weight_v [n, k], weight_g [n, 1]) and an [n] bias.  Reads
+        the registered parameters directly: this runs on every call."""
+        p = self._modules[name]._parameters
+        v = p.get("weight_v")
+        if (p["weight"] if v is None else v).shape == (n, k) and p["bias"].shape == (n,) and (v is None or p["weight_g"].shape == (n, 1)):
+            return
+        have = (("weight", (n, k)),) if v is None else (("weight_v", (n, k)), ("weight_g", (n, 1)))
+        what, want = next((w, s) for w, s in have + (("bias", (n,)),) if p[w].shape != s)
+        raise ValueError(f"SDFField: {name}.{what} is {list(p[what].shape)}, but the field's layer dims make it {list(want)}"
+                         + (" (num_layers = 3 puts the reference's skip connection after the last geometric layer, which neither the "
+                            "reference nor this field can evaluate)" if self.num_layers == 5 and name == "glin3" else ""))
 
     def _mlp_params(self):
         """The MLPs' parameters, lazily (so that the engine choice touches none of them outside a training step)."""
@@ -352,9 +374,11 @@ class SDFField(nn.Module):
         return fin
 
     # ------------------------------------------------------------------ the kernel call
-    def _run(self, origins, directions, bins, n_samples: int, wants, apply_contraction: bool, appearance=None) -> Dict[str, torch.Tensor]:
+    def _run(self, origins, directions, bins, n_samples: int, wants, apply_contraction: bool, appearance=None,
+             analytic_gradients: bool = False) -> Dict[str, torch.Tensor]:
         """origins [R,3] (or points [N,3] in point mode), directions [R,3] | None, bins [R,S+1] | None.
-        `wants`: iterable of output names of sdfb200_field_out_t.  Returns flat tensors ([N] / [N,k])."""
+        `wants`: iterable of output names of sdfb200_field_out_t.  `analytic_gradients`: differentiate the network even when the field
+        uses numerical gradients.  Returns flat tensors ([N] / [N,k])."""
         lib = _lib.load()
         dev = self.aabb.device
         _lib.require_cuda(dev, "SDFField")
@@ -362,6 +386,11 @@ class SDFField(nn.Module):
         N = R * n_samples
         desc = self._field_desc()
         packed = self._packed_weights(desc)
+        if analytic_gradients and desc.use_numerical_gradients:
+            # a numerical-gradient field runs the exact-fp32 engine at every precision, and its packed weights are the fp32 section alone:
+            # the fp32 descriptor without numerical gradients evaluates the same network on the same blob
+            desc.use_numerical_gradients = 0
+            desc.precision = _lib.PRECISION["fp32"]
         ws = self._workspace_of(lib.sdfb200_field_workspace_bytes(desc, N), "sdfb200_field_workspace_bytes", dev)
         gf = self.config.geo_feat_dim
         shapes = {"sdf": (N,), "geo_feature": (N, gf), "gradients": (N, 3), "normals": (N, 3), "rgb": (N, 3), "density": (N,), "alpha": (N,),
@@ -496,8 +525,10 @@ class SDFField(nn.Module):
                 gradients = gradients.view(*ray_samples.frustums.shape, -1)
             return _train.get_alpha(self, ray_samples, sdf, gradients)
         if sdf is None or gradients is None:
+            # like the reference (and the training path), the gradient is autograd's at the un-contracted start positions, also when the
+            # field uses numerical gradients elsewhere
             origins, directions, bins, shape = sample_geometry(ray_samples)
-            o = self._run(origins, directions, bins, bins.shape[1] - 1, ("alpha",), apply_contraction=False)
+            o = self._run(origins, directions, bins, bins.shape[1] - 1, ("alpha",), apply_contraction=False, analytic_gradients=True)
             return o["alpha"].view(*shape, 1)
         return _train.get_alpha(self, ray_samples, sdf, gradients)
 

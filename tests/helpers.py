@@ -1,10 +1,11 @@
 """Shared helpers for the parity tests: build the *product* SDFField for a seeded oracle case."""
+import functools
 import os
 
 import numpy as np
 import torch
 
-from oracle import cases
+from oracle import cases, render, samplers
 from oracle.field import FieldSpec, OracleField, init_params
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -44,7 +45,7 @@ def product_field(spec: FieldSpec, params, kw, device="cuda", precision="fp32", 
         num_layers=spec.num_layers, hidden_dim=spec.hidden_dim, geo_feat_dim=spec.geo_feat_dim, num_layers_color=spec.num_layers_color,
         hidden_dim_color=spec.hidden_dim_color, appearance_embedding_dim=spec.appearance_embedding_dim,
         use_appearance_embedding=spec.use_appearance_embedding, bias=kw.get("bias", 0.5), inside_outside=kw.get("inside_outside", False),
-        use_grid_feature=spec.use_grid_feature, beta_init=kw.get("beta_init", 0.3), position_encoding_max_degree=spec.position_encoding_max_degree,
+        use_grid_feature=spec.use_grid_feature, weight_norm=spec.weight_norm, beta_init=kw.get("beta_init", 0.3), position_encoding_max_degree=spec.position_encoding_max_degree,
         use_diffuse_color=spec.use_diffuse_color, use_specular_tint=spec.use_specular_tint, use_reflections=spec.use_reflections,
         use_n_dot_v=spec.use_n_dot_v, rgb_padding=spec.rgb_padding, off_axis=spec.off_axis, use_numerical_gradients=spec.use_numerical_gradients,
         num_levels=spec.num_levels, max_res=spec.max_res, base_res=spec.base_res, log2_hashmap_size=spec.log2_hashmap_size,
@@ -92,6 +93,56 @@ def build_case(name, device="cuda", precision="fp32", table_dtype="fp32"):
         oracle.numerical_gradients_delta = kw["num_grad_delta"]
     field = product_field(spec, params, kw, device, precision, table_dtype)
     return spec, kw, o, d, cam, nears, fars, oracle, field
+
+
+@functools.lru_cache(maxsize=None)
+def generic_chunk_points():
+    """Points per pass of the generic field engine (kChunkPoints, csrc/field_plan.h), read off the library: the workspace of a generic-engine
+    call grows with the point count up to one chunk and then stays (every pass reuses it).  Host logic only."""
+    import sdfstudio_b200 as sb
+
+    lib = sb._lib.load()
+    d = sb.SDFField(sb.SDFFieldConfig(precision="fp32"), torch.tensor([[-1.0, -1, -1], [1, 1, 1]]), 1)._field_desc()
+    lo, hi = 1, 1 << 24
+    top = lib.sdfb200_field_workspace_bytes(d, hi)
+    assert top > 0 and lib.sdfb200_field_workspace_bytes(d, hi // 2) == top, "the workspace does not saturate: no chunked passes"
+    while lo < hi:                      # the first point count whose workspace is the whole chunk's
+        mid = (lo + hi) // 2
+        lo, hi = (lo, mid) if lib.sdfb200_field_workspace_bytes(d, mid) == top else (mid + 1, hi)
+    return lo
+
+
+def assert_straddles_chunk(R, S, sl):
+    """R rays of S samples cross the first chunk boundary of the generic engine, and the rays `sl` hold one that straddles it"""
+    chunk = generic_chunk_points()
+    assert R * S > chunk, f"{R * S} points fit in one {chunk}-point chunk"
+    assert chunk % S != 0 and sl.start <= chunk // S < sl.stop, f"no ray of {sl} straddles the {chunk}-point chunk boundary at S = {S}"
+
+
+def launches(fn):
+    """library kernel launches of one call, after a first call has packed the weights"""
+    from sdfstudio_b200 import _lib
+
+    fn()
+    torch.cuda.synchronize()
+    n0 = _lib.launch_count()
+    fn()
+    torch.cuda.synchronize()
+    return _lib.launch_count() - n0
+
+
+def oracle_render(e, eu, from_density):
+    """the renderers on the oracle's per-sample outputs `e` (OracleField.get_outputs on the euclidean bins `eu`): white background,
+    expected depth"""
+    ones = torch.ones(3, dtype=eu.dtype)
+    if from_density:
+        w, T = samplers.weights_from_density(eu[:, 1:] - eu[:, :-1], e["density"][..., 0])
+    else:
+        w, T = samplers.weights_from_alphas(e["alphas"][..., 0])
+    w = w[..., None]
+    return {"rgb": render.render_rgb(e["rgb"], w, ones), "depth": render.render_depth(w, eu[:, :-1, None], eu[:, 1:, None], "expected"),
+            "normal": render.render_semantics(e["normals"], w), "accumulation": render.render_accumulation(w), "bg_transmittance": T[:, -1:],
+            "weights": w}
 
 
 def make_bundle(o, d, cam, nears, fars, device="cuda"):

@@ -3,6 +3,8 @@ generic kernels launch one kernel per stage and GEMM, plus a weight pack per GEM
 import pytest
 import torch
 
+from helpers import launches
+
 pytestmark = pytest.mark.gpu
 
 SHAPES = {
@@ -35,30 +37,18 @@ def _field(shape, precision):
     return sb.SDFField(sb.SDFFieldConfig(**SHAPES[shape], precision=precision), torch.tensor([[-1.0, -1, -1], [1, 1, 1]]), 49).cuda().eval()
 
 
-def _launches(fn):
-    """library kernel launches of one call, after a first call has packed the weights"""
-    from sdfstudio_b200 import _lib
-
-    fn()
-    torch.cuda.synchronize()
-    n0 = _lib.launch_count()
-    fn()
-    torch.cuda.synchronize()
-    return _lib.launch_count() - n0
-
-
 def _forward_launches(shape, precision, wants=HEADS, n_samples=32):
     import sdfstudio_b200 as sb
 
     field, rs = _field(shape, precision), _samples(n_samples)
     origins, directions = sb.rays.rays_of(rs)
     bins = sb.rays.bins_of(rs)
-    return _launches(lambda: field._run(origins, directions, bins, n_samples, wants, True))
+    return launches(lambda: field._run(origins, directions, bins, n_samples, wants, True))
 
 
 def _render_launches(shape, precision, n_samples, clip_depth):
     field, rs = _field(shape, precision), _samples(n_samples)
-    return _launches(lambda: field.render(rs, torch.ones(3, device="cuda"), clip_depth=clip_depth))
+    return launches(lambda: field.render(rs, torch.ones(3, device="cuda"), clip_depth=clip_depth))
 
 
 @pytest.mark.parametrize("precision", ["bf16x3", "bf16"])

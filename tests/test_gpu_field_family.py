@@ -18,7 +18,7 @@ import torch
 from oracle import cases, render, samplers
 from oracle.field import FieldSpec, OracleField, init_params
 
-from helpers import assert_within_noise, build_case, load_golden, make_bundle, oracle64, product_field, rel_err
+from helpers import assert_within_noise, build_case, launches, load_golden, make_bundle, oracle64, oracle_render, product_field, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -123,18 +123,6 @@ def _reference(case, o, d, cam, rs, S):
     return res[0], res[1], eu
 
 
-def _launches(fn):
-    """library kernel launches of one call, after a first call has packed the weights"""
-    from sdfstudio_b200 import _lib
-
-    fn()
-    torch.cuda.synchronize()
-    n0 = _lib.launch_count()
-    fn()
-    torch.cuda.synchronize()
-    return _lib.launch_count() - n0
-
-
 def _assert_engine(case, precision, n, what):
     if case.fused(precision):
         assert n == 1, f"{case.name}/{precision}/{what}: {n} launches, the fused kernel is one"
@@ -162,8 +150,8 @@ def test_forward_get_sdf_and_point_mode_match_fp64_oracle(name, precision):
     o, d, cam, rs = c.samples(32)
     tag = f"{name}/{precision}"
     with torch.no_grad():
-        _assert_engine(c, precision, _launches(lambda: c.field(rs, return_alphas=True, return_occupancy=True)), "forward")
-        _assert_engine(c, precision, _launches(lambda: c.field.get_sdf(rs)), "get_sdf")
+        _assert_engine(c, precision, launches(lambda: c.field(rs, return_alphas=True, return_occupancy=True)), "forward")
+        _assert_engine(c, precision, launches(lambda: c.field.get_sdf(rs)), "get_sdf")
         out = c.field(rs, return_alphas=True, return_occupancy=True)
         sdf_u = c.field.get_sdf(rs)
     e32, e64, eu = _reference(c, o, d, cam, rs, 32)
@@ -190,19 +178,6 @@ def test_forward_get_sdf_and_point_mode_match_fp64_oracle(name, precision):
                             floor=1e-4 * _scale(g64))
 
 
-def _oracle_render(e, eu, from_density):
-    """the renderers on the oracle's per-sample outputs (white background, expected depth)"""
-    ones = torch.ones(3, dtype=eu.dtype)
-    if from_density:
-        w, T = samplers.weights_from_density(eu[:, 1:] - eu[:, :-1], e["density"][..., 0])
-    else:
-        w, T = samplers.weights_from_alphas(e["alphas"][..., 0])
-    w = w[..., None]
-    return {"rgb": render.render_rgb(e["rgb"], w, ones), "depth": render.render_depth(w, eu[:, :-1, None], eu[:, 1:, None], "expected"),
-            "normal": render.render_semantics(e["normals"], w), "accumulation": render.render_accumulation(w), "bg_transmittance": T[:, -1:],
-            "weights": w}
-
-
 def _check_render(name, precision, S, from_density):
     c = _Case(name, precision)
     o, d, cam, rs = c.samples(S)
@@ -210,14 +185,14 @@ def _check_render(name, precision, S, from_density):
     tag = f"{name}/{precision}/S={S}/{'density' if from_density else 'alpha'}"
     fused_render = c.fused(precision) and 128 % S == 0
     with torch.no_grad():
-        n = _launches(lambda: c.field.render(rs, bg, from_density=from_density, clip_depth=False))
+        n = launches(lambda: c.field.render(rs, bg, from_density=from_density, clip_depth=False))
         res = c.field.render(rs, bg, from_density=from_density)
     if fused_render:
         assert n == 1, f"{tag}: {n} launches, the fused render is one"
     elif precision != "fp32":
         assert n > 1, f"{tag}: one launch, but this render cannot be fused"
     e32, e64, eu = _reference(c, o, d, cam, rs, S)
-    r32, r64 = _oracle_render(e32, eu, from_density), _oracle_render(e64, eu.double(), from_density)
+    r32, r64 = oracle_render(e32, eu, from_density), oracle_render(e64, eu.double(), from_density)
     for k in ("rgb", "depth", "normal", "accumulation", "bg_transmittance", "weights"):
         assert_within_noise(res[k], r32[k], r64[k], f"{tag}/{k}", factor=4.0, floor=1e-4 * _scale(r64[k]))
 
@@ -246,15 +221,15 @@ def test_tcnn_layout_fast_mode(name):
     bg = torch.ones(3, device="cuda")
     H = sb.FieldHeadNames
     with torch.no_grad():
-        assert _launches(lambda: c.field(rs, return_alphas=True, return_occupancy=True)) == 1
-        assert _launches(lambda: c.field.render(rs, bg, clip_depth=False)) == 1
+        assert launches(lambda: c.field(rs, return_alphas=True, return_occupancy=True)) == 1
+        assert launches(lambda: c.field.render(rs, bg, clip_depth=False)) == 1
         out = c.field(rs, return_alphas=True, return_occupancy=True)
         res = c.field.render(rs, bg)
     _, e64, eu = _reference(c, o, d, cam, rs, 32)
     # bf16 rounds the MLP's operands, so its sdf error does not shrink where the sdf crosses zero: relative above |sdf| = 0.1
     assert rel_err(out[H.SDF], e64["sdf"], 1e-1) < 2e-2
     assert float((out[H.RGB].cpu().double() - e64["rgb"]).abs().max()) < 2e-2
-    mse = float(((res["rgb"].cpu().double() - _oracle_render(e64, eu.double(), False)["rgb"]) ** 2).mean())
+    mse = float(((res["rgb"].cpu().double() - oracle_render(e64, eu.double(), False)["rgb"]) ** 2).mean())
     psnr = -10.0 * torch.log10(torch.tensor(mse)).item()
     assert psnr > 55.0, f"{name}: fast-mode PSNR vs the fp64 oracle {psnr:.1f} dB"
 
@@ -317,7 +292,7 @@ def test_oracle_only_golden_on_the_tensor_core_engines(name):
     sb, G, spec, o, d, cam, rs, field, out, o64, e64 = _run_golden_case(name, "bf16x3")
     H = sb.FieldHeadNames
     with torch.no_grad():
-        n = _launches(lambda: field(rs, return_alphas=True, return_occupancy=True))
+        n = launches(lambda: field(rs, return_alphas=True, return_occupancy=True))
     assert (n == 1) == (name == "neusfacto_l2"), f"{name}: {n} launches"
     for key, gk in ((H.SDF, "sdf"), (H.RGB, "rgb"), (H.ALPHA, "alphas"), (H.DENSITY, "density"), (H.GRADIENT, "gradients"), (H.NORMAL, "normals")):
         assert_within_noise(out[key], G[gk], e64[gk], f"{name}/{gk}", factor=4.0, floor=3e-4 * _scale(e64[gk]))

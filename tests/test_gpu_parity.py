@@ -7,7 +7,7 @@ import torch
 from oracle import cases, hashgrid, render, samplers
 from oracle.field import FieldSpec, OracleField, init_params
 
-from helpers import assert_within_noise, build_case, cdf_consistency, load_golden, make_bundle, oracle64, product_field, rel_err
+from helpers import assert_straddles_chunk, assert_within_noise, build_case, cdf_consistency, load_golden, make_bundle, oracle64, product_field, rel_err
 
 pytestmark = pytest.mark.gpu
 RTOL = 1e-4
@@ -331,17 +331,18 @@ def test_empty_and_ragged_inputs():
 
 
 def test_large_batch_crosses_chunks():
-    """N > the internal chunk size: chunk boundaries must not show (compare a chunk-straddling slice with a small call)."""
+    """N > the generic engine's chunk: a slice of rays around the first chunk boundary, one of them straddling it, must match a small call
+    on that slice bit for bit."""
     import sdfstudio_b200 as sb
 
     spec, kw, o, d, cam, nears, fars, oracle, field = build_case("neusfacto_c1_init")
-    R, S = 1300, 64  # 83200 points > the 75776-point chunk (field_plan.h kChunkPoints); rays 1160..1210 straddle the boundary
+    R, S, sl = 1500, 50, slice(1330, 1380)      # 75 000 points
+    assert_straddles_chunk(R, S, sl)
     o, d, cam = cases.synthetic_rays(R, 123)
     nears, fars = torch.full((R, 1), 0.5), torch.full((R, 1), 4.5)
     rb = make_bundle(o, d, cam, nears, fars)
     rs = sb.UniformSampler(num_samples=S).eval()(rb)
     big = field(rs, return_alphas=True)
-    sl = slice(1160, 1210)
     rb2 = make_bundle(o[sl], d[sl], cam[sl], nears[sl], fars[sl])
     small = field(sb.UniformSampler(num_samples=S).eval()(rb2), return_alphas=True)
     for k in (sb.FieldHeadNames.RGB, sb.FieldHeadNames.SDF, sb.FieldHeadNames.ALPHA, sb.FieldHeadNames.GRADIENT):
