@@ -6,7 +6,7 @@ import numpy as np
 import torch
 
 from oracle import cases, render, samplers
-from oracle.field import FieldSpec, OracleField, init_params
+from oracle.field import FieldSpec, OracleField, folded_weight, init_params
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -168,6 +168,115 @@ def oracle64(spec, params, kw):
     if "num_grad_delta" in kw:
         o.numerical_gradients_delta = kw["num_grad_delta"]
     return o
+
+
+# the fp64 parity tables (test_gpu_field_family.py, test_gpu_field_generic.py): one configuration per row, one switch from a base
+# bias 0.9: the rays cross the zero level set or graze it, so the rendered accumulations spread over (0, 1) instead of all being ~0
+FIELD_INIT = dict(bias=0.9, beta_init=0.3, perturb=0.02, hash_init_scale=0.05, seed=41)
+RAY_SEED = 77
+POINTS = 2048                                                # samples per call: 16 tiles of 128
+UNBOUNDED = dict(near=0.2, far=30.0, spacing="piecewise")   # most samples lie outside the unit ball
+
+
+class FieldCase:
+    """One row of a configuration table: the product field at `precision` and the fp32 / fp64 oracles with the same parameters and
+    switches.  `row` = (FieldSpec changes to `base`, options).  Options: table_dtype, near / far / spacing of the rays, appearance ("mean":
+    eval mode with the mean embedding, "train": training mode with the per-camera rows), mask_level (update_mask), cos_anneal,
+    inside_outside, num_grad_delta (the numerical-gradient step)."""
+
+    _REF = {}
+
+    def __init__(self, base, row, name, precision, device="cuda"):
+        from dataclasses import replace
+
+        changes, opt = row
+        self.name, self.opt, self.precision = name, opt, precision
+        self.spec = replace(base, **changes)
+        self.kw = dict(FIELD_INIT, inside_outside=opt.get("inside_outside", False))
+        for k in ("mask_level", "num_grad_delta"):
+            if k in opt:
+                self.kw[k] = opt[k]
+        self.params = init_params(self.spec, **cases.init_kwargs(self.kw))
+        if not self.spec.weight_norm:
+            # a field without weight norm holds the folded weights as `{layer}.weight` (what the oracle then reads)
+            for layer in [k[: -len(".weight_v")] for k in self.params if k.endswith(".weight_v")]:
+                self.params[layer + ".weight"] = folded_weight(self.params, layer, True)
+                del self.params[layer + ".weight_v"], self.params[layer + ".weight_g"]
+        table_dtype = opt.get("table_dtype", "fp32")
+        if table_dtype == "fp16" and "hash_table" in self.params:
+            self.params["hash_table"] = self.params["hash_table"].half().float()   # the oracle holds the fp16-representable table
+        f = product_field(self.spec, self.params, self.kw, device=device, precision=precision, table_dtype=table_dtype)
+        f.set_cos_anneal_ratio(opt.get("cos_anneal", 1.0))
+        if opt.get("appearance") == "mean":
+            f.use_average_appearance_embedding = True
+        elif opt.get("appearance") == "train":
+            f.train()                                  # under no_grad: the inference kernels with the per-camera embedding rows
+        self.field = f
+
+    def oracle(self, dtype):
+        o = OracleField(self.spec, self.params, dtype=dtype)
+        if "mask_level" in self.kw:
+            o.update_mask(self.kw["mask_level"])
+        o.numerical_gradients_delta = self.kw.get("num_grad_delta", o.numerical_gradients_delta)
+        o.cos_anneal_ratio = self.opt.get("cos_anneal", 1.0)
+        o.use_average_appearance_embedding = self.opt.get("appearance") == "mean"
+        o.training = self.opt.get("appearance") == "train"
+        return o
+
+    def samples(self, S, R=None, seed=RAY_SEED):
+        """(origins, directions, camera indices, ray samples) of R rays (default: POINTS samples, or 48 rays) at S samples per ray"""
+        import sdfstudio_b200 as sb
+
+        R = R or (POINTS // S if POINTS % S == 0 else 48)
+        o, d, cam = cases.synthetic_rays(R, seed)
+        nears, fars = torch.full((R, 1), self.opt.get("near", 0.5)), torch.full((R, 1), self.opt.get("far", 4.5))
+        rs = sb.SpacedSampler(self.opt.get("spacing", "uniform"), None, num_samples=S).eval()(make_bundle(o, d, cam, nears, fars))
+        return o, d, cam, rs
+
+    def points(self):
+        """gradient() points (well outside the unit ball when the field contracts) and forward_geonetwork points"""
+        g = torch.Generator().manual_seed(5)
+        grad_pts = (torch.rand(200, 3, generator=g) * 2 - 1) * (4.0 if self.spec.contraction else 1.5)
+        return grad_pts, (torch.rand(POINTS, 3, generator=g) * 2 - 1) * 1.5
+
+    def reference(self, o, d, cam, rs):
+        """(fp32, fp64 oracle outputs, euclidean bins) on the product's own bins: cached per configuration and S, since every precision
+        samples the same bins"""
+        import sdfstudio_b200 as sb
+
+        eu = sb.rays.bins_of(rs).cpu()
+        key = (repr(self.spec), repr(sorted(self.opt.items())), eu.shape[1])
+        hit = FieldCase._REF.get(key)
+        if hit is not None and torch.equal(hit[0], eu):
+            return hit[1], hit[2], eu
+        res = []
+        for dt in (torch.float32, torch.float64):
+            e = eu.to(dt)
+            res.append(self.oracle(dt).get_outputs(o.to(dt), d.to(dt), e[:, :-1], e[:, 1:] - e[:, :-1], cam, return_alphas=True, return_occupancy=True))
+        FieldCase._REF[key] = (eu, res[0], res[1])
+        return res[0], res[1], eu
+
+
+def scale(t):
+    return float(t.abs().max())
+
+
+def head_pairs(sb):
+    """(product output key, oracle output key) of the per-sample heads of get_outputs, normals aside (see assert_heads_within_noise)"""
+    H = sb.FieldHeadNames
+    return ((H.SDF, "sdf"), (H.RGB, "rgb"), (H.DENSITY, "density"), (H.ALPHA, "alphas"), (H.OCCUPANCY, "occupancy"), (H.GRADIENT, "gradients"),
+            ("points_norm", "points_norm"))
+
+
+def assert_heads_within_noise(sb, out, e32, e64, tag, floor_rel):
+    """every per-sample head of get_outputs within 4x the fp32 oracle's noise, with a floor of `floor_rel` of the quantity's scale.  A
+    normal's error is its gradient's error over |grad sdf|, so normals are compared scaled by |grad sdf| under the gradients' floor (at
+    |grad sdf| = 0.27 the bf16x3 gradient error, 1e-5 of the gradients' scale, is a 1.1e-4 error of the unit normal)."""
+    for key, k in head_pairs(sb):
+        assert_within_noise(out[key], e32[k], e64[k], f"{tag}/{k}", factor=4.0, floor=floor_rel * scale(e64[k]))
+    gmag = e64["gradients"].norm(dim=-1, keepdim=True)
+    n_cu, n32, n64 = (t.detach().double().cpu() * gmag for t in (out[sb.FieldHeadNames.NORMAL], e32["normals"], e64["normals"]))
+    assert_within_noise(n_cu, n32, n64, f"{tag}/normals x |grad|", factor=4.0, floor=floor_rel * scale(e64["gradients"]))
 
 
 def assert_within_noise(cuda, ref32, ref64, what, factor=4.0, floor=2e-6):

@@ -10,27 +10,20 @@ rendered RGB and normal to 1e-4 relative instead, but their field is nearly tran
 surface, and the fp32 oracle itself then misses that relative bound: on these rays its rendered normal is 6e-4 (torch layout) to 4e-2
 (L-inf contraction) relative from the fp64 one, and its alpha-composited RGB 5e-3 relative behind the L-inf contraction, where the NeuS
 alpha divides two small sigmoids."""
-from dataclasses import replace
-
 import pytest
 import torch
 
 from oracle import cases, render, samplers
-from oracle.field import FieldSpec, OracleField, init_params
+from oracle.field import FieldSpec
 
-from helpers import assert_within_noise, build_case, launches, load_golden, make_bundle, oracle64, oracle_render, product_field, rel_err
+from helpers import (UNBOUNDED, FieldCase, assert_heads_within_noise, assert_within_noise, build_case, launches, load_golden, make_bundle, oracle64,
+                     oracle_render, rel_err, scale)
 
 pytestmark = pytest.mark.gpu
 
 BASE = FieldSpec(num_layers=2, num_layers_color=2, hidden_dim=256, use_grid_feature=True, log2_hashmap_size=15)
-# bias 0.9: the rays cross the zero level set or graze it, so the rendered accumulations spread over (0, 1) instead of all being ~0
-INIT = dict(bias=0.9, beta_init=0.3, perturb=0.02, hash_init_scale=0.05, seed=41)
-RAY_SEED = 77
-POINTS = 2048                                         # samples per call: 16 tiles of 128
-UNBOUNDED = dict(near=0.2, far=30.0, spacing="piecewise")   # most samples lie outside the unit ball
 
-# name -> (FieldSpec changes, options).  Options: table_dtype, near / far / spacing of the rays, appearance ("mean": eval mode with the
-# mean embedding, "train": training mode with the per-camera rows), mask_level (update_mask), cos_anneal, inside_outside.
+# name -> (FieldSpec changes, options of helpers.FieldCase)
 FAMILY = {
     "torch": ({}, {}),
     "tcnn": ({"grid_layout": "tcnn"}, {}),             # log2T = 15, base 16: the coarse levels are dense, the fine ones hashed
@@ -58,69 +51,12 @@ OUTSIDE = {
 CONFIGS = {**FAMILY, **OUTSIDE}
 
 
-class _Case:
-    """One configuration: the product field at `precision` and the fp32 / fp64 oracles with the same parameters and switches."""
-
+class _Case(FieldCase):
     def __init__(self, name, precision):
-        changes, opt = CONFIGS[name]
-        self.name, self.opt = name, opt
-        self.spec = replace(BASE, **changes)
-        self.kw = dict(INIT, inside_outside=opt.get("inside_outside", False))
-        if "mask_level" in opt:
-            self.kw["mask_level"] = opt["mask_level"]
-        self.params = init_params(self.spec, **cases.init_kwargs(self.kw))
-        table_dtype = opt.get("table_dtype", "fp32")
-        if table_dtype == "fp16" and "hash_table" in self.params:
-            self.params["hash_table"] = self.params["hash_table"].half().float()   # the oracle holds the fp16-representable table
-        f = product_field(self.spec, self.params, self.kw, precision=precision, table_dtype=table_dtype)
-        f.set_cos_anneal_ratio(opt.get("cos_anneal", 1.0))
-        if opt.get("appearance") == "mean":
-            f.use_average_appearance_embedding = True
-        elif opt.get("appearance") == "train":
-            f.train()                                  # under no_grad: the fused kernels with the per-camera embedding rows
-        self.field = f
-
-    def oracle(self, dtype):
-        o = OracleField(self.spec, self.params, dtype=dtype) if dtype == torch.float32 else oracle64(self.spec, self.params, self.kw)
-        if "mask_level" in self.opt:
-            o.update_mask(self.opt["mask_level"])
-        o.cos_anneal_ratio = self.opt.get("cos_anneal", 1.0)
-        o.use_average_appearance_embedding = self.opt.get("appearance") == "mean"
-        o.training = self.opt.get("appearance") == "train"
-        return o
-
-    def samples(self, S):
-        import sdfstudio_b200 as sb
-
-        R = POINTS // S if POINTS % S == 0 else 48
-        o, d, cam = cases.synthetic_rays(R, RAY_SEED)
-        nears, fars = torch.full((R, 1), self.opt.get("near", 0.5)), torch.full((R, 1), self.opt.get("far", 4.5))
-        rs = sb.SpacedSampler(self.opt.get("spacing", "uniform"), None, num_samples=S).eval()(make_bundle(o, d, cam, nears, fars))
-        return o, d, cam, rs
+        super().__init__(BASE, CONFIGS[name], name, precision)
 
     def fused(self, precision):
         return self.name in FAMILY and precision != "fp32"
-
-
-_REF = {}
-
-
-def _reference(case, o, d, cam, rs, S):
-    """fp32 and fp64 oracle outputs on the product's own bins (cached per configuration and S: every precision samples the same bins)"""
-    import sdfstudio_b200 as sb
-
-    eu = sb.rays.bins_of(rs).cpu()
-    hit = _REF.get((case.name, S))
-    if hit is not None and torch.equal(hit[0], eu):
-        return hit[1], hit[2], eu
-    res = []
-    for dt in (torch.float32, torch.float64):
-        e = eu.to(dt)
-        out = case.oracle(dt).get_outputs(o.to(dt), d.to(dt), e[:, :-1], e[:, 1:] - e[:, :-1], cam, return_alphas=True, return_occupancy=True)
-        out.pop("geo_feature")
-        res.append(out)
-    _REF[(case.name, S)] = (eu, res[0], res[1])
-    return res[0], res[1], eu
 
 
 def _assert_engine(case, precision, n, what):
@@ -128,16 +64,6 @@ def _assert_engine(case, precision, n, what):
         assert n == 1, f"{case.name}/{precision}/{what}: {n} launches, the fused kernel is one"
     elif precision != "fp32":
         assert n > 1, f"{case.name}/{precision}/{what}: one launch, but the configuration is outside the fused family"
-
-
-def _scale(t):
-    return float(t.abs().max())
-
-
-def _heads(sb):
-    H = sb.FieldHeadNames
-    return ((H.SDF, "sdf"), (H.RGB, "rgb"), (H.DENSITY, "density"), (H.ALPHA, "alphas"), (H.OCCUPANCY, "occupancy"), (H.GRADIENT, "gradients"),
-            (H.NORMAL, "normals"), ("points_norm", "points_norm"))
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -154,28 +80,20 @@ def test_forward_get_sdf_and_point_mode_match_fp64_oracle(name, precision):
         _assert_engine(c, precision, launches(lambda: c.field.get_sdf(rs)), "get_sdf")
         out = c.field(rs, return_alphas=True, return_occupancy=True)
         sdf_u = c.field.get_sdf(rs)
-    e32, e64, eu = _reference(c, o, d, cam, rs, 32)
-    for key, k in _heads(sb):
-        if k != "normals":
-            assert_within_noise(out[key], e32[k], e64[k], f"{tag}/{k}", factor=4.0, floor=1e-4 * _scale(e64[k]))
-    # a normal's error is its gradient's error over |grad sdf|, so normals are compared scaled by |grad sdf| under the gradients' floor (at
-    # |grad sdf| = 0.27 the bf16x3 gradient error, 1e-5 of the gradients' scale, is a 1.1e-4 error of the unit normal)
-    gmag = e64["gradients"].norm(dim=-1, keepdim=True)
-    n_cu, n32, n64 = (t.detach().double().cpu() * gmag for t in (out[sb.FieldHeadNames.NORMAL], e32["normals"], e64["normals"]))
-    assert_within_noise(n_cu, n32, n64, f"{tag}/normals x |grad|", factor=4.0, floor=1e-4 * _scale(e64["gradients"]))
+    e32, e64, eu = c.reference(o, d, cam, rs)
+    assert_heads_within_noise(sb, out, e32, e64, tag, 1e-4)
     # sdf-only mode: un-contracted start positions
     o32, o64 = c.oracle(torch.float32), c.oracle(torch.float64)
     s32, s64 = o32.get_sdf(o, d, eu[:, :-1]), o64.get_sdf(o.double(), d.double(), eu[:, :-1].double())
-    assert_within_noise(sdf_u[..., 0], s32, s64, f"{tag}/get_sdf", factor=4.0, floor=1e-4 * _scale(s64))
+    assert_within_noise(sdf_u[..., 0], s32, s64, f"{tag}/get_sdf", factor=4.0, floor=1e-4 * scale(s64))
     # point mode: gradient() with and without the contraction (points well outside the unit ball when the field contracts)
-    g = torch.Generator().manual_seed(5)
-    pts = (torch.rand(200, 3, generator=g) * 2 - 1) * (4.0 if c.spec.contraction else 1.5)
+    pts, _ = c.points()
     for skip in (False, True):
         with torch.no_grad():
             gp = c.field.gradient(pts.cuda(), skip_spatial_distortion=skip)
         g64 = o64.gradient(pts.double(), skip_spatial_distortion=skip)
         assert_within_noise(gp, o32.gradient(pts, skip_spatial_distortion=skip), g64, f"{tag}/gradient(skip={skip})", factor=4.0,
-                            floor=1e-4 * _scale(g64))
+                            floor=1e-4 * scale(g64))
 
 
 def _check_render(name, precision, S, from_density):
@@ -191,10 +109,10 @@ def _check_render(name, precision, S, from_density):
         assert n == 1, f"{tag}: {n} launches, the fused render is one"
     elif precision != "fp32":
         assert n > 1, f"{tag}: one launch, but this render cannot be fused"
-    e32, e64, eu = _reference(c, o, d, cam, rs, S)
+    e32, e64, eu = c.reference(o, d, cam, rs)
     r32, r64 = oracle_render(e32, eu, from_density), oracle_render(e64, eu.double(), from_density)
     for k in ("rgb", "depth", "normal", "accumulation", "bg_transmittance", "weights"):
-        assert_within_noise(res[k], r32[k], r64[k], f"{tag}/{k}", factor=4.0, floor=1e-4 * _scale(r64[k]))
+        assert_within_noise(res[k], r32[k], r64[k], f"{tag}/{k}", factor=4.0, floor=1e-4 * scale(r64[k]))
 
 
 @pytest.mark.parametrize("from_density", [False, True])
@@ -225,7 +143,7 @@ def test_tcnn_layout_fast_mode(name):
         assert launches(lambda: c.field.render(rs, bg, clip_depth=False)) == 1
         out = c.field(rs, return_alphas=True, return_occupancy=True)
         res = c.field.render(rs, bg)
-    _, e64, eu = _reference(c, o, d, cam, rs, 32)
+    _, e64, eu = c.reference(o, d, cam, rs)
     # bf16 rounds the MLP's operands, so its sdf error does not shrink where the sdf crosses zero: relative above |sdf| = 0.1
     assert rel_err(out[H.SDF], e64["sdf"], 1e-1) < 2e-2
     assert float((out[H.RGB].cpu().double() - e64["rgb"]).abs().max()) < 2e-2
@@ -295,7 +213,7 @@ def test_oracle_only_golden_on_the_tensor_core_engines(name):
         n = launches(lambda: field(rs, return_alphas=True, return_occupancy=True))
     assert (n == 1) == (name == "neusfacto_l2"), f"{name}: {n} launches"
     for key, gk in ((H.SDF, "sdf"), (H.RGB, "rgb"), (H.ALPHA, "alphas"), (H.DENSITY, "density"), (H.GRADIENT, "gradients"), (H.NORMAL, "normals")):
-        assert_within_noise(out[key], G[gk], e64[gk], f"{name}/{gk}", factor=4.0, floor=3e-4 * _scale(e64[gk]))
+        assert_within_noise(out[key], G[gk], e64[gk], f"{name}/{gk}", factor=4.0, floor=3e-4 * scale(e64[gk]))
     # rendered RGB against the reference's own fp32 render (7e-4 relative from the fp64 one for neusfacto_l2, see above)
     w = rs.get_weights_from_alphas(out[H.ALPHA])
     img = sb.render_all(w, out[H.RGB], out[H.NORMAL], rs, torch.ones(3, device="cuda"))

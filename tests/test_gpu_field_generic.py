@@ -12,30 +12,25 @@ bf16; the exact GEMMs, and so fp32's bits, whenever the field uses numerical gra
 The descriptor-against-weights checks at the end run without a GPU."""
 import contextlib
 import math
-from dataclasses import replace
 
 import pytest
 import torch
 
 from oracle import cases
-from oracle.field import FieldSpec, OracleField, folded_weight, init_params
+from oracle.field import FieldSpec
 
-from helpers import assert_straddles_chunk, assert_within_noise, launches, make_bundle, oracle_render, product_field, rel_err
+from helpers import (POINTS, RAY_SEED, UNBOUNDED, FieldCase, assert_heads_within_noise, assert_straddles_chunk, assert_within_noise, launches,
+                     make_bundle, oracle_render, rel_err, scale)
 
 gpu = pytest.mark.gpu
 
 # in_dim = 3 + 36 (PE) + 32 (grid) = 71: a layer feeding the skip concat has a 57-wide output, a multiple of no tile
 BASE = FieldSpec(num_layers=2, hidden_dim=128, geo_feat_dim=64, num_layers_color=2, hidden_dim_color=128, use_grid_feature=True, log2_hashmap_size=15)
-INIT = dict(bias=0.9, beta_init=0.3, perturb=0.02, hash_init_scale=0.05, seed=41)   # the rays reach the surface (test_gpu_field_family.py)
-RAY_SEED = 77
-POINTS = 2048
-UNBOUNDED = dict(near=0.2, far=30.0, spacing="piecewise")
 NUMGRAD = dict(num_grad_delta=0.002)
 FLOOR = {"fp32": 1e-4, "bf16x3": 3e-4}
 
-# name -> (FieldSpec changes, options).  Options: table_dtype, near / far / spacing of the rays, appearance ("mean" | "train"), mask_level,
-# cos_anneal, inside_outside, num_grad_delta (the field's numerical-gradient step).  The reference's skip concat (skip_in = [4]) feeds geo
-# layer 4, which exists from num_layers = 4 on.
+# name -> (FieldSpec changes, options of helpers.FieldCase).  The reference's skip concat (skip_in = [4]) feeds geo layer 4, which exists
+# from num_layers = 4 on.
 CONFIGS = {
     "base": ({}, {}),
     # depth
@@ -91,67 +86,13 @@ CONFIGS = {
 ANALYTIC = [n for n, (ch, _) in CONFIGS.items() if not ch.get("use_numerical_gradients")]
 
 
-def _params(spec, kw):
-    p = init_params(spec, **cases.init_kwargs(kw))
-    if not spec.weight_norm:
-        # a field without weight norm holds the folded weights as `{layer}.weight` (what the oracle then reads)
-        for name in [k[: -len(".weight_v")] for k in p if k.endswith(".weight_v")]:
-            p[name + ".weight"] = folded_weight(p, name, True)
-            del p[name + ".weight_v"], p[name + ".weight_g"]
-    return p
-
-
-class _Case:
-    """One configuration: the product field at `precision` and the fp32 / fp64 oracles with the same parameters and switches."""
-
+class _Case(FieldCase):
     def __init__(self, name, precision, device="cuda"):
-        changes, opt = CONFIGS[name]
-        self.name, self.opt, self.precision = name, opt, precision
-        self.spec = replace(BASE, **changes)
-        self.kw = dict(INIT, inside_outside=opt.get("inside_outside", False))
-        for k in ("mask_level", "num_grad_delta"):
-            if k in opt:
-                self.kw[k] = opt[k]
-        self.params = _params(self.spec, self.kw)
-        table_dtype = opt.get("table_dtype", "fp32")
-        if table_dtype == "fp16" and "hash_table" in self.params:
-            self.params["hash_table"] = self.params["hash_table"].half().float()   # the oracle holds the fp16-representable table
-        f = product_field(self.spec, self.params, self.kw, device=device, precision=precision, table_dtype=table_dtype)
-        f.set_cos_anneal_ratio(opt.get("cos_anneal", 1.0))
-        if opt.get("appearance") == "mean":
-            f.use_average_appearance_embedding = True
-        elif opt.get("appearance") == "train":
-            f.train()                                  # under no_grad: the inference kernels with the per-camera embedding rows
-        self.field = f
+        super().__init__(BASE, CONFIGS[name], name, precision, device)
 
     @property
     def numerical(self):
         return self.spec.use_numerical_gradients
-
-    def oracle(self, dtype):
-        o = OracleField(self.spec, self.params, dtype=dtype)
-        if "mask_level" in self.opt:
-            o.update_mask(self.opt["mask_level"])
-        o.numerical_gradients_delta = self.opt.get("num_grad_delta", o.numerical_gradients_delta)
-        o.cos_anneal_ratio = self.opt.get("cos_anneal", 1.0)
-        o.use_average_appearance_embedding = self.opt.get("appearance") == "mean"
-        o.training = self.opt.get("appearance") == "train"
-        return o
-
-    def samples(self, S, R=None, seed=RAY_SEED):
-        import sdfstudio_b200 as sb
-
-        R = R or (POINTS // S if POINTS % S == 0 else 48)
-        o, d, cam = cases.synthetic_rays(R, seed)
-        nears, fars = torch.full((R, 1), self.opt.get("near", 0.5)), torch.full((R, 1), self.opt.get("far", 4.5))
-        rs = sb.SpacedSampler(self.opt.get("spacing", "uniform"), None, num_samples=S).eval()(make_bundle(o, d, cam, nears, fars))
-        return o, d, cam, rs
-
-    def points(self):
-        """gradient() points (well outside the unit ball when the field contracts) and forward_geonetwork points"""
-        g = torch.Generator().manual_seed(5)
-        grad_pts = (torch.rand(200, 3, generator=g) * 2 - 1) * (4.0 if self.spec.contraction else 1.5)
-        return grad_pts, (torch.rand(POINTS, 3, generator=g) * 2 - 1) * 1.5
 
 
 def _calls(field, rs, grad_pts, geo_pts):
@@ -172,25 +113,6 @@ def _tensors(x):
     if isinstance(x, dict):
         return [v for v in x.values() if v is not None]
     return list(x) if isinstance(x, tuple) else [x]
-
-
-_REF = {}
-
-
-def _reference(case, o, d, cam, rs, S):
-    """fp32 and fp64 oracle outputs on the product's own bins (cached per configuration and S: every precision samples the same bins)"""
-    import sdfstudio_b200 as sb
-
-    eu = sb.rays.bins_of(rs).cpu()
-    hit = _REF.get((case.name, S))
-    if hit is not None and torch.equal(hit[0], eu):
-        return hit[1], hit[2], eu
-    res = []
-    for dt in (torch.float32, torch.float64):
-        e = eu.to(dt)
-        res.append(case.oracle(dt).get_outputs(o.to(dt), d.to(dt), e[:, :-1], e[:, 1:] - e[:, :-1], cam, return_alphas=True, return_occupancy=True))
-    _REF[(case.name, S)] = (eu, res[0], res[1])
-    return res[0], res[1], eu
 
 
 def _at_starts(of, o, d, eu):
@@ -226,16 +148,6 @@ def _point_reference(case, o, d, eu, grad_pts, geo_pts):
         res[dt] = r
     _POINT_REF[case.name] = (eu, res)
     return res
-
-
-def _scale(t):
-    return float(t.abs().max())
-
-
-def _heads(sb):
-    H = sb.FieldHeadNames
-    return ((H.SDF, "sdf"), (H.RGB, "rgb"), (H.DENSITY, "density"), (H.ALPHA, "alphas"), (H.OCCUPANCY, "occupancy"), (H.GRADIENT, "gradients"),
-            ("points_norm", "points_norm"))
 
 
 def _check_engine(c, counts, got, rs, grad_pts, geo_pts):
@@ -278,18 +190,13 @@ def test_outputs_and_point_mode_match_fp64_oracle(name, precision):
 
     tag, fl = f"{name}/{precision}", FLOOR[precision]
 
-    def close(cu, r32, r64, what, scale_of=None):
-        assert_within_noise(cu, r32, r64, f"{tag}/{what}", factor=4.0, floor=fl * _scale(r64 if scale_of is None else scale_of))
+    def close(cu, r32, r64, what):
+        assert_within_noise(cu, r32, r64, f"{tag}/{what}", factor=4.0, floor=fl * scale(r64))
 
     # get_outputs: every per-sample head
-    e32, e64, eu = _reference(c, o, d, cam, rs, 32)
+    e32, e64, eu = c.reference(o, d, cam, rs)
     out = got["get_outputs"]
-    for key, k in _heads(sb):
-        close(out[key], e32[k], e64[k], k)
-    # a normal's error is its gradient's error over |grad sdf|: normals are compared scaled by |grad sdf| under the gradients' floor
-    gmag = e64["gradients"].norm(dim=-1, keepdim=True)
-    n_cu, n32, n64 = (t.detach().double().cpu() * gmag for t in (out[sb.FieldHeadNames.NORMAL], e32["normals"], e64["normals"]))
-    close(n_cu, n32, n64, "normals x |grad|", scale_of=e64["gradients"])
+    assert_heads_within_noise(sb, out, e32, e64, tag, fl)
     if c.numerical:
         close(out["sampled_sdf"], e32["sampled_sdf"], e64["sampled_sdf"], "sampled_sdf")
     else:
@@ -321,7 +228,7 @@ def test_render_matches_fp64_oracle(name, precision, S):
     c = _Case(name, precision)
     o, d, cam, rs = c.samples(S)
     bg = torch.ones(3, device="cuda")
-    e32, e64, eu = _reference(c, o, d, cam, rs, S)
+    e32, e64, eu = c.reference(o, d, cam, rs)
     for from_density in (False, True):
         tag = f"{name}/{precision}/S={S}/{'density' if from_density else 'alpha'}"
         with torch.no_grad():
@@ -330,7 +237,7 @@ def test_render_matches_fp64_oracle(name, precision, S):
         assert n > 1, f"{tag}: one launch, but the configuration is outside the fused kernel's family"
         r32, r64 = oracle_render(e32, eu, from_density), oracle_render(e64, eu.double(), from_density)
         for k in ("rgb", "depth", "normal", "accumulation", "bg_transmittance", "weights"):
-            assert_within_noise(res[k], r32[k], r64[k], f"{tag}/{k}", factor=4.0, floor=FLOOR[precision] * _scale(r64[k]))
+            assert_within_noise(res[k], r32[k], r64[k], f"{tag}/{k}", factor=4.0, floor=FLOOR[precision] * scale(r64[k]))
 
 
 @contextlib.contextmanager
@@ -370,7 +277,7 @@ def test_single_pass_bf16_within_fast_mode_bounds(name):
         out = fwd(c.field)
         res = c.field.render(rs, bg)
     assert n > n32 > 1, f"{name}: {n} launches at bf16, {n32} at fp32: the GEMMs did not run on the tensor cores"
-    _, e64, eu = _reference(c, o, d, cam, rs, 32)
+    _, e64, eu = c.reference(o, d, cam, rs)
     e = eu.float()
     with _bf16_operands():
         eb = c.oracle(torch.float32).get_outputs(o, d, e[:, :-1], e[:, 1:] - e[:, :-1], cam, return_alphas=True, return_occupancy=True)
