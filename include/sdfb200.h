@@ -512,8 +512,11 @@ int sdfb200_interlevel_loss(const float* fine_bins, const float* fine_weights, i
  * closed under differentiation (each one's backward is the other two), which is what the eikonal term's double backward needs
  * (sdf_field.py:646-655, create_graph=True).  P = number of points (the long dimension); N, K = layer widths.  Buffers of width N / K
  * must be allocated with their row padded to a multiple of 16 floats (ld >= pad16(width)); padding columns of outputs are written
- * (zeros for epilogue 0), padding columns of inputs are ignored.  workspace >= sdfb200_gemm_workspace_bytes().
- * epilogue: 0 none, 1 softplus(beta = 100), 2 relu.  bias [pad16(N)] or NULL.
+ * (zeros for epilogue 0 without bias, epilogue(bias) otherwise), padding columns of inputs are ignored.
+ * workspace >= sdfb200_gemm_workspace_bytes(), aligned to 16 bytes.  W is [N, K] with ldw >= K in all three; tn needs lda >= N,
+ * ldb >= K and ldc >= K.  nt / nn read X 16 bytes at a time and bias / Y 8 bytes at a time: X must be aligned to 16 bytes, Y and bias
+ * to 8 (ldx, ldy multiples of 4 keep every row so).  A call that breaks one of these, or has P < 0, returns -1 before any launch.
+ * epilogue: 0 none, 1 softplus(beta = 100), 2 relu.  bias [pad16(N)] or NULL (NULL only with epilogue 0).
  * ------------------------------------------------------------------------------------------------------------- */
 size_t sdfb200_gemm_workspace_bytes(void);
 /* Y[P, N] = epilogue(X[P, K] W[N, K]^T + bias) */

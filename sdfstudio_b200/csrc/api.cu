@@ -241,12 +241,25 @@ extern "C" int sdfb200_field_render(const sdfb200_field_t* f, const void* packed
 // ---------------------------------------------------------------------------------------------------------------------
 extern "C" size_t sdfb200_gemm_workspace_bytes(void) { return tc_wgrad_workspace_bytes() + kTcGemmScratchBytes + 256; }
 
+// What k_tc_linear's memory accesses need of the caller's buffers: X rows are read 16 bytes at a time (float4), bias and Y 8 bytes at a
+// time (float2), and the packed weights are bulk-copied out of the workspace, which needs 16-byte alignment.  Checked before any launch.
+static int check_gemm_buffers(const char* name, const float* X, const float* bias, const float* Y, const void* workspace, int64_t P) {
+  if (P < 0) return fail(SDFB200_EINVAL, "%s: negative point count P (%lld)", name, (long long)P);
+  if ((uintptr_t)X % 16) return fail(SDFB200_EINVAL, "%s: X must be aligned to %lld bytes (its float4 loads)", name, 16);
+  if ((uintptr_t)Y % 8) return fail(SDFB200_EINVAL, "%s: Y must be aligned to %lld bytes (its float2 loads and stores)", name, 8);
+  if ((uintptr_t)bias % 8) return fail(SDFB200_EINVAL, "%s: bias must be aligned to %lld bytes (its float2 loads)", name, 8);
+  if ((uintptr_t)workspace % 16) return fail(SDFB200_EINVAL, "%s: workspace must be aligned to %lld bytes (bulk copies of the packed weights)", name, 16);
+  return 0;
+}
+
 extern "C" int sdfb200_gemm_nt(int32_t precision, const float* X, int64_t ldx, const float* W, int64_t ldw, int32_t N, int32_t K, const float* bias,
                                int32_t epilogue, float* Y, int64_t ldy, int64_t P, void* workspace, size_t workspace_bytes, void* stream) {
   SDFB_REQUIRE(precision == SDFB200_PRECISION_BF16X3 || precision == SDFB200_PRECISION_BF16, "gemm: precision must be bf16x3 or bf16");
   SDFB_REQUIRE(X && W && Y && workspace && workspace_bytes >= kTcGemmScratchBytes, "gemm_nt: NULL pointer / workspace too small");
   SDFB_REQUIRE(epilogue == TCL_NONE || epilogue == TCL_SOFTPLUS || epilogue == TCL_RELU, "gemm_nt: epilogue");
   SDFB_REQUIRE(N >= 1 && K >= 1 && ldx >= pad16(K) && ldy >= pad16(N) && ldx % 4 == 0 && ldy % 4 == 0, "gemm_nt: X / Y must hold the dims padded to 16");
+  SDFB_REQUIRE(ldw >= K, "gemm_nt: W rows must hold K (ldw >= K)");
+  if (int r = check_gemm_buffers("gemm_nt", X, bias, Y, workspace, P)) return r;
   return tc_gemm_ex(tc_planes(precision), epilogue, X, (int)ldx, W, (int)ldw, 0, N, K, bias, Y, (int)ldy, P, pad16(N), pad16(K), nullptr, 0, 0, workspace,
                     (cudaStream_t)stream);
 }
@@ -256,6 +269,8 @@ extern "C" int sdfb200_gemm_nn(int32_t precision, const float* X, int64_t ldx, c
   SDFB_REQUIRE(precision == SDFB200_PRECISION_BF16X3 || precision == SDFB200_PRECISION_BF16, "gemm: precision must be bf16x3 or bf16");
   SDFB_REQUIRE(X && W && Y && workspace && workspace_bytes >= kTcGemmScratchBytes, "gemm_nn: NULL pointer / workspace too small");
   SDFB_REQUIRE(N >= 1 && K >= 1 && ldx >= pad16(N) && ldy >= pad16(K) && ldx % 4 == 0 && ldy % 4 == 0, "gemm_nn: X / Y must hold the dims padded to 16");
+  SDFB_REQUIRE(ldw >= K, "gemm_nn: W rows must hold K (ldw >= K)");
+  if (int r = check_gemm_buffers("gemm_nn", X, nullptr, Y, workspace, P)) return r;
   // Y[P, K] = X[P, N] W[N, K]  ==  X (W^T)^T : the weight tile is packed from the transposed view
   return tc_gemm_ex(tc_planes(precision), TCL_NONE, X, (int)ldx, W, (int)ldw, 1, K, N, nullptr, Y, (int)ldy, P, pad16(K), pad16(N), nullptr, 0, 0, workspace,
                     (cudaStream_t)stream);

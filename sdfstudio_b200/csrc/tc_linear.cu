@@ -194,6 +194,8 @@ int tc_gemm_ex(int planes, int epi, const float* X, int ldx, const float* W, int
   SDFB_REQUIRE(planes == 1 || planes == 2, "tc_gemm: planes");
   SDFB_REQUIRE(Np % 16 == 0 && Kp % 16 == 0 && ldx % 4 == 0 && ldy % 4 == 0, "tc_gemm: dims must be padded to 16");
   SDFB_REQUIRE(scratch != nullptr, "tc_gemm: scratch is NULL");
+  SDFB_REQUIRE(M >= 0, "tc_gemm: negative row count");
+  SDFB_REQUIRE(epi == TCL_MUL_DSOFTPLUS || epi == TCL_NONE || bias != nullptr, "tc_gemm: bias is NULL");
   if (M == 0) return 0;
   const unsigned grid = (unsigned)ceil_div(M, 128);
   for (int n0 = 0; n0 < Np; n0 += 256) {
@@ -209,7 +211,6 @@ int tc_gemm_ex(int planes, int epi, const float* X, int ldx, const float* W, int
       a.X = X + k0; a.ldx = ldx; a.M = M; a.Kc32 = Kc32; a.Kvalid = kv; a.Wp = (const __nv_bfloat16*)scratch; a.Ncp = Nc; a.Np64 = Np64;
       a.bias = bias ? bias + n0 : nullptr; a.Y = Y; a.ldy = ldy; a.n0 = n0; a.accumulate = k0 > 0; a.final_chunk = k0 + 256 >= Kp;
       a.aux = aux; a.ldaux = ldaux; a.aux_cols = aux_cols;
-      if (epi != TCL_MUL_DSOFTPLUS && epi != TCL_NONE) SDFB_REQUIRE(bias != nullptr, "tc_gemm: bias is NULL");
       const size_t smem = (size_t)planes * kAPlaneL + kRingBytesL + 1024;
       const int r = planes == 2 ? launch_linear<2>(epi, a, smem, grid, st) : launch_linear<1>(epi, a, smem, grid, st);
       if (r) return r;

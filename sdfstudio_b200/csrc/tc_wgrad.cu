@@ -150,6 +150,8 @@ int tc_wgrad(int planes, const float* A, long long lda, const float* B, long lon
   SDFB_REQUIRE(A && B && C && workspace, "tc_wgrad: NULL pointer");
   SDFB_REQUIRE(workspace_bytes >= tc_wgrad_workspace_bytes(), "tc_wgrad: workspace too small");
   SDFB_REQUIRE(N >= 1 && K >= 1 && P >= 0, "tc_wgrad: bad sizes");
+  SDFB_REQUIRE(lda >= N && ldb >= K && ldc >= K, "tc_wgrad: row strides must hold the widths (lda >= N, ldb >= K, ldc >= K)");
+  if ((uintptr_t)workspace % 16) return fail(SDFB200_EINVAL, "tc_wgrad: workspace must be aligned to %s%lld bytes (float2 partial sums)", "", 16);
   const long long nblk = (P + kWgPts - 1) / kWgPts;
   const int ctas = persistent_ctas();
   const int grid = (int)(nblk < ctas ? (nblk > 0 ? nblk : 1) : ctas);

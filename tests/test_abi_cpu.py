@@ -216,6 +216,63 @@ def test_grid_calls_refuse_misaligned_tables(F, table_dtype):
         assert f"aligned to {add} bytes".encode() in lib.sdfb200_last_error_string()
 
 
+@pytest.mark.skipif(torch.cuda.is_available(), reason="the calls get sentinel device pointers, which a call that is not rejected would launch on")
+@pytest.mark.parametrize("precision", ["bf16x3", "bf16"])
+def test_gemm_calls_refuse_misaligned_buffers_and_bad_sizes(precision):
+    """sdfb200_gemm_nt / _nn / _tn: k_tc_linear reads X with 16-byte loads and bias / Y with 8-byte ones, the packed weights are
+    bulk-copied out of the workspace (16 bytes) and k_tc_wgrad writes 8-byte partial sums into it.  A pointer those accesses cannot take,
+    P < 0, or a row stride below the width it holds is refused with -1 and a message naming the alignment or the size, before anything is
+    launched (the launch counter does not move).  The pointers are sentinels that a rejected call never dereferences."""
+    from sdfstudio_b200 import _lib
+
+    lib = _lib.load()
+    prec = _lib.PRECISION[precision]
+    X, W, B, Y, WS = 0x100000, 0x200000, 0x300000, 0x400000, 0x500000
+    nbytes = lib.sdfb200_gemm_workspace_bytes()
+    N, K, P = 40, 24, 1000                                    # pad16: 48 and 32
+
+    def nt(x=X, ldx=32, w=W, ldw=K, bias=B, epi=1, y=Y, ldy=48, p=P, ws=WS, n=N, k=K):
+        return lib.sdfb200_gemm_nt(prec, x, ldx, w, ldw, n, k, bias, epi, y, ldy, p, ws, nbytes, None)
+
+    def nn(x=X, ldx=48, w=W, ldw=K, y=Y, ldy=32, p=P, ws=WS):
+        return lib.sdfb200_gemm_nn(prec, x, ldx, w, ldw, N, K, y, ldy, p, ws, nbytes, None)
+
+    def tn(a=X, lda=N, b=W, ldb=K, c=Y, ldc=K, p=P, ws=WS):
+        return lib.sdfb200_gemm_tn(prec, a, lda, b, ldb, c, ldc, p, N, K, ws, nbytes, None)
+
+    def refused(rc, *words):
+        msg = lib.sdfb200_last_error_string()
+        return rc == -1 and all(w in msg for w in words)
+
+    before = _lib.launch_count()
+    for off in (4, 8, 12):
+        assert refused(nt(x=X + off), b"X", b"aligned to 16 bytes")
+        assert refused(nn(x=X + off), b"X", b"aligned to 16 bytes")
+        assert refused(nt(ws=WS + off), b"workspace", b"aligned to 16 bytes")
+        assert refused(nn(ws=WS + off), b"workspace", b"aligned to 16 bytes")
+        assert refused(tn(ws=WS + off), b"workspace", b"aligned to 16 bytes")
+    for off in (4, 12):
+        assert refused(nt(y=Y + off), b"Y", b"aligned to 8 bytes")
+        assert refused(nn(y=Y + off), b"Y", b"aligned to 8 bytes")
+        assert refused(nt(bias=B + off), b"bias", b"aligned to 8 bytes")
+        assert refused(nt(bias=B + off, epi=0), b"bias", b"aligned to 8 bytes")
+    for p in (-1, -1000, -(1 << 40)):
+        assert refused(nt(p=p), b"P")
+        assert refused(nn(p=p), b"P")
+        assert refused(tn(p=p), b"sizes")
+    assert refused(nt(ldw=K - 1), b"ldw")
+    assert refused(nn(ldw=K - 1), b"ldw")
+    assert refused(tn(lda=N - 1), b"lda")
+    assert refused(tn(ldb=K - 1), b"ldb")
+    assert refused(tn(ldc=K - 1), b"ldc")
+    assert refused(nt(ldx=16), b"padded to 16")                                               # ldx < pad16(K)
+    assert refused(nt(ldy=44), b"padded to 16")                                               # ldy < pad16(N)
+    for epi in (1, 2):                                                                         # bias is NULL: refused before the weights are packed
+        assert refused(nt(bias=None, epi=epi), b"bias is NULL")
+    assert refused(nt(epi=3), b"epilogue")
+    assert _lib.launch_count() == before                                                       # no refusal launched anything
+
+
 def test_product_does_not_import_oracle():
     pkg = os.path.join(ROOT, "sdfstudio_b200")
     for dirpath, _, files in os.walk(pkg):
