@@ -458,6 +458,31 @@ int sdfb200_marching_cubes(const float* volume, const int64_t* dims, float level
                            const float* spacing, const int64_t* offsets, int32_t* counts, float* verts, float* normals, int32_t* faces,
                            void* stream);
 
+/* Texture export (nerfstudio/exporter/texture_utils.py).  A texel grid is [height, width] in row-major order; its centres are
+ * (linspace_w[j], linspace_h[i]) with the two vectors of get_texture_image (:59-75) on the device.  face [P] int32 and bary [P,3] fp32
+ * (w0, w1, w2), P = width * height, are each texel's face and barycentric weights; the weights are rounded op by op as the reference's
+ * ATen ops round them (IEEE division, no FMA contraction), so face and bary are bit-identical to the reference's.
+ *
+ * sdfb200_uv_rasterize: unwrap_mesh_with_xatlas' search (:265-301) over texture_coordinates [n_faces,3,2] fp32 in chunks of `chunk`
+ * faces; only faces 0 .. floor(n_faces / chunk) * chunk - 1 take part.  In a chunk, the face with the smallest |w0|+|w1|+|w2| wins (lowest
+ * index on ties), and a chunk that gives the texel a NaN contributes nothing; a chunk replaces the texel's face only with a strictly
+ * smaller value, starting from FLT_MAX.  Texels no chunk claims keep face 0 and weights 0.  Deterministic (no atomics). */
+int sdfb200_uv_rasterize(const float* texture_coordinates, int64_t n_faces, int32_t chunk, const float* linspace_w, int32_t width,
+                         const float* linspace_h, int32_t height, int32_t* face, float* bary, void* stream);
+/* sdfb200_uv_unwrap_grid: unwrap_mesh_per_uv_triangle (:100-192).  square_uv [6,2] fp32 = the two triangles of the first rectangle,
+ * lr [2] fp32 = the rectangle's extent in UV; rectangle s holds faces 2s and 2s + 1 at column s % squares_per_side_w and row
+ * s / squares_per_side_w, each (px_per_uv_triangle + 3) x px_per_uv_triangle texels.  Writes texture_coordinates [n_faces,3,2] and each
+ * texel's face (clamped to n_faces - 1, so padding texels extrapolate from the last face) and bary. */
+int sdfb200_uv_unwrap_grid(const float* square_uv, const float* lr, int64_t n_faces, int32_t squares_per_side_w, int32_t px_per_uv_triangle,
+                           const float* linspace_w, int32_t width, const float* linspace_h, int32_t height, float* texture_coordinates,
+                           int32_t* face, float* bary, void* stream);
+/* sdfb200_uv_texel_rays (:194-205, :303-321, :391): per texel, origin = v0 w0 + v1 w1 + v2 w2 and direction = -normalize(n0 w0 + n1 w1 +
+ * n2 w2) (F.normalize's eps) over the corners faces[face] (int64 [F,3]) of vertices / vertex_normals [V,3] fp32, then origin -= 0.5 raylen
+ * direction.  raylen is a DEVICE fp32 scalar; origins / directions [P,3] and fars [P] = raylen are written.  With raylen NULL the origins
+ * are not shifted and fars is not written. */
+int sdfb200_uv_texel_rays(const float* vertices, const float* vertex_normals, const int64_t* faces, const int32_t* face, const float* bary,
+                          const float* raylen, int64_t n_texels, float* origins, float* directions, float* fars, void* stream);
+
 /* Training path: backward of sdfb200_render (expected depth) / sdfb200_render_alphas' compositing w.r.t. the per-sample
  * inputs (autograd over renderers.py:42-295 in the reference).  `accumulation`, `depth` = forward outputs (depth BEFORE the
  * global clip).  g_rgb [R,3], g_depth [R], g_normal [R,3], g_accumulation [R], g_weights_in [R,S]: incoming gradients, each
