@@ -483,6 +483,27 @@ int sdfb200_uv_unwrap_grid(const float* square_uv, const float* lr, int64_t n_fa
 int sdfb200_uv_texel_rays(const float* vertices, const float* vertex_normals, const int64_t* faces, const int32_t* face, const float* bary,
                           const float* raylen, int64_t n_texels, float* origins, float* directions, float* fars, void* stream);
 
+/* TSDF fusion: TSDF.integrate_tsdf (nerfstudio/exporter/tsdf_utils.py:168-270) of n_cams images, in order, into n_voxels voxels.
+ * voxel_coords [3,N] fp32 (world x, y, z planes); cams [B,18] fp32 = rows 0-2 of inverse(c2w) (12 floats, row-major), then rows 0-1 of
+ * K (6 floats; K's third row is never used); depth [B,H,W]; color [B,3,H,W] or NULL; truncation is a DEVICE fp32 scalar.  values,
+ * weights [N] and colors [N,3] (untouched when color is NULL) are read once and written once.  Per voxel and image, every operation
+ * rounded on its own (no FMA contraction, IEEE division and square root):
+ *   x, y, z = ((m0 x + m1 y) + m2 z) + m3 for rows 0, 1, 2 of inverse(c2w); then y = -y, z = -z
+ *   voxel_depth = sqrt((x^2 + y^2) + z^2);  u = x / z, v = y / z, w = z / z
+ *   px = (k00 u + k01 v) + k02 w, py = (k10 u + k11 v) + k12 w
+ *   g = (2 px) / W - 1;  ix = nearbyint(((g + 1) W - 1) / 2)   (ATen's CUDA unnormalisation; half to even), likewise iy from py and H
+ *   sampled = depth[b, iy, ix], or 0 when the pixel lies outside the image or the coordinate is not finite (the reference's result for
+ *             a non-finite coordinate depends on the grid_sample backend; here such a voxel is outside)
+ *   dist = sampled - voxel_depth;  valid = voxel_depth > 0 && sampled > 0 && dist > -truncation   (a NaN depth is never valid)
+ *   if valid: total = weight + 1;  value = (value weight + clamp(dist / truncation, -1, 1)) / total;
+ *             color_c = (color_c weight + color[b, c, iy, ix]) / total;  weight = min(total, 1)
+ * Kept from the reference: voxels behind a camera (z < 0) project through the mirrored point and fuse when they land in the image; the
+ * depth images are compared with the Euclidean voxel_depth.  One thread per voxel, no atomics: the result depends only on the order
+ * of the images, not on how they are split into calls, and reruns are bit-identical. */
+int sdfb200_tsdf_integrate(const float* voxel_coords, int64_t n_voxels, const float* cams, int32_t n_cams, const float* depth,
+                           const float* color, int32_t height, int32_t width, const float* truncation, float* values, float* weights,
+                           float* colors, void* stream);
+
 /* Training path: backward of sdfb200_render (expected depth) / sdfb200_render_alphas' compositing w.r.t. the per-sample
  * inputs (autograd over renderers.py:42-295 in the reference).  `accumulation`, `depth` = forward outputs (depth BEFORE the
  * global clip).  g_rgb [R,3], g_depth [R], g_normal [R,3], g_accumulation [R], g_weights_in [R,S]: incoming gradients, each

@@ -37,6 +37,22 @@ class Cameras:
     def __len__(self):
         return self.camera_to_worlds.shape[0]
 
+    def get_intrinsics_matrices(self) -> torch.Tensor:
+        """[C,3,3] fp32 pinhole intrinsics (cameras/cameras.py:733-745)."""
+        K = torch.zeros((len(self), 3, 3), dtype=torch.float32, device=self.device)
+        K[:, 0, 0], K[:, 1, 1], K[:, 0, 2], K[:, 1, 2], K[:, 2, 2] = self.fx, self.fy, self.cx, self.cy, 1.0
+        return K
+
+    def rescale_output_resolution(self, scaling_factor: Union[float, int]) -> None:
+        """Scales fx, fy, cx, cy (fp32 products) and the image size (cameras/cameras.py:747-771); height and width are truncated as
+        ``.to(torch.int64)`` truncates the fp32 product.  The cameras share one image size, so the factor is one number."""
+        if not isinstance(scaling_factor, (float, int)):
+            raise ValueError("Scaling factor must be a float or an int (the cameras share one image size).")
+        s = torch.tensor([scaling_factor], dtype=torch.float32, device=self.device)
+        self.fx, self.fy, self.cx, self.cy = self.fx * s, self.fy * s, self.cx * s, self.cy * s
+        self.height = int((torch.tensor([self.height]) * s.cpu()).to(torch.int64))
+        self.width = int((torch.tensor([self.width]) * s.cpu()).to(torch.int64))
+
     def get_image_coords(self, pixel_offset: float = 0.5) -> torch.Tensor:
         """[H, W, 2] (y, x) pixel centres (cameras/cameras.py:268-293)."""
         ys = torch.arange(self.height, device=self.device, dtype=torch.float32) + pixel_offset

@@ -156,17 +156,25 @@ class Mesh:
         self.vertices = v[keep].cpu().numpy()
         self.vertex_normals = self.vertex_normals[keep.cpu().numpy()]
 
-    def export(self, path):
-        """binary little-endian PLY: float x, y, z, nx, ny, nz per vertex, uchar-counted int lists per face."""
-        v = np.empty(len(self.vertices), dtype=[(n, "<f4") for n in ("x", "y", "z", "nx", "ny", "nz")])
+    def export(self, path, vertex_colors=None):
+        """binary little-endian PLY: float x, y, z, nx, ny, nz per vertex, uchar-counted int lists per face.  With ``vertex_colors``
+        [V,3] in [0, 1], each vertex also carries uchar red, green, blue = floor(clip(c, 0, 1) * 255 + 0.5) (in fp32) and alpha = 255."""
+        props = [(n, "<f4") for n in ("x", "y", "z", "nx", "ny", "nz")]
+        if vertex_colors is not None:
+            props += [(n, "u1") for n in ("red", "green", "blue", "alpha")]
+        v = np.empty(len(self.vertices), dtype=props)
         for a, n in enumerate("xyz"):
             v[n] = self.vertices[:, a]
             v["n" + n] = self.vertex_normals[:, a]
+        if vertex_colors is not None:
+            c = np.asarray(vertex_colors, dtype=np.float32).reshape(len(v), 3)
+            q = np.floor(np.clip(c, 0.0, 1.0) * np.float32(255.0) + np.float32(0.5)).astype(np.uint8)
+            v["red"], v["green"], v["blue"], v["alpha"] = q[:, 0], q[:, 1], q[:, 2], 255
         f = np.empty(len(self.faces), dtype=[("n", "u1"), ("i", "<i4", (3,))])
         f["n"] = 3
         f["i"] = self.faces
         header = ("ply\nformat binary_little_endian 1.0\n"
-                  f"element vertex {len(v)}\n" + "".join(f"property float {n}\n" for n in ("x", "y", "z", "nx", "ny", "nz")) +
+                  f"element vertex {len(v)}\n" + "".join(f"property {'float' if t == '<f4' else 'uchar'} {n}\n" for n, t in props) +
                   f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
         with open(path, "wb") as fh:
             fh.write(header.encode("ascii"))
