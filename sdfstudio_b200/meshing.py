@@ -7,13 +7,14 @@ copies each block's volume to the host for ``skimage.measure.marching_cubes`` an
 is generated on the device (sdfb200_lattice_points), only the SDF head is evaluated (the fused kernel's sdf-only mode when
 ``precision != "fp32"``), the pyramid and masks stay torch ops on the device, and marching cubes is the library's two-pass kernel
 (sdfb200_marching_cubes): the volume never goes to the host, only the mesh does.  ``Mesh`` stands in for the few ``trimesh.Trimesh``
-members the reference uses.
+members the reference uses.  ``write_ply`` and ``read_ply`` are the package's one PLY writer and reader, for every exporter.
 
 Kept from the reference, quirks included: ``level`` is overwritten with 0 in both sliding variants, ``coarse_mask`` is permuted in
 get_surface_sliding only, ``merge_vertices`` runs on the file path of get_surface_sliding and always in the contraction variant.
 get_surface_occupancy also returns its mesh when ``return_mesh`` is set (the reference ignores the flag; it still writes the file).
 """
 import ctypes as C
+import importlib
 from pathlib import Path
 from typing import Callable, Sequence
 
@@ -28,6 +29,11 @@ CROP_N = 512                 # lattice points per block side of the sliding vari
 avg_pool_3d = torch.nn.AvgPool3d(2, stride=2)
 upsample = torch.nn.Upsample(scale_factor=2, mode="nearest")
 max_pool_3d = torch.nn.MaxPool3d(3, stride=1, padding=1)
+
+
+def work_device() -> torch.device:
+    """Where host-side mesh work (welding, normals) runs as torch ops: the GPU when there is one."""
+    return torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
 
 
 def sdf_fn(field, level: float = 0.0) -> Callable[[torch.Tensor], torch.Tensor]:
@@ -54,22 +60,25 @@ def lattice_points(bbox_min: Sequence[float], bbox_max: Sequence[float], resolut
     return out
 
 
+def _lattice_values(fn, bbox_min, bbox_max, res, chunk: int, device) -> torch.Tensor:
+    """``fn`` on the lattice of ``res`` = (rx, ry, rz) points, called on ``chunk`` points at a time -> float32 [rx * ry * rz]."""
+    total = res[0] * res[1] * res[2]
+    out = torch.empty(total, device=device, dtype=torch.float32)
+    for start in range(0, total, chunk):
+        n = min(chunk, total - start)
+        out[start:start + n] = fn(lattice_points(bbox_min, bbox_max, res, start, n, device))
+    return out
+
+
 @torch.no_grad()
 def evaluate_sdf_grid(field, resolution, bbox_min=(-1.0, -1.0, -1.0), bbox_max=(1.0, 1.0, 1.0), chunk: int = 1 << 22) -> torch.Tensor:
     """SDF on the dense lattice -> float32 tensor [rx, ry, rz] (what ``evaluate(points).reshape(N, N, N)`` is in the reference)."""
     res = (resolution,) * 3 if isinstance(resolution, int) else tuple(int(r) for r in resolution)
-    total = res[0] * res[1] * res[2]
-    dev = field.aabb.device
-    out = torch.empty(total, device=dev, dtype=torch.float32)
-    f = sdf_fn(field)
-    for start in range(0, total, chunk):
-        n = min(chunk, total - start)
-        out[start:start + n] = f(lattice_points(bbox_min, bbox_max, res, start, n, dev))
-    return out.view(*res)
+    return _lattice_values(sdf_fn(field), bbox_min, bbox_max, res, chunk, field.aabb.device).view(*res)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------
-# marching cubes and the mesh
+# marching cubes, the mesh and its files
 # ---------------------------------------------------------------------------------------------------------------------------------
 @torch.no_grad()
 def marching_cubes(volume: torch.Tensor, level: float = 0.0, spacing=(1.0, 1.0, 1.0), mask: torch.Tensor = None):
@@ -141,7 +150,7 @@ class Mesh:
         first occurrence, and re-indexes the faces.  torch ops, on the GPU when there is one."""
         if len(self.vertices) == 0:
             return
-        dev = torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
+        dev = work_device()
         v = torch.from_numpy(self.vertices).to(dev)
         key = torch.round(v * (10.0 ** digits_vertex)).to(torch.int64)
         _, inverse = torch.unique(key, dim=0, return_inverse=True)
@@ -157,29 +166,99 @@ class Mesh:
         self.vertex_normals = self.vertex_normals[keep.cpu().numpy()]
 
     def export(self, path, vertex_colors=None):
-        """binary little-endian PLY: float x, y, z, nx, ny, nz per vertex, uchar-counted int lists per face.  With ``vertex_colors``
-        [V,3] in [0, 1], each vertex also carries uchar red, green, blue = floor(clip(c, 0, 1) * 255 + 0.5) (in fp32) and alpha = 255."""
-        props = [(n, "<f4") for n in ("x", "y", "z", "nx", "ny", "nz")]
-        if vertex_colors is not None:
-            props += [(n, "u1") for n in ("red", "green", "blue", "alpha")]
-        v = np.empty(len(self.vertices), dtype=props)
-        for a, n in enumerate("xyz"):
-            v[n] = self.vertices[:, a]
-            v["n" + n] = self.vertex_normals[:, a]
-        if vertex_colors is not None:
-            c = np.asarray(vertex_colors, dtype=np.float32).reshape(len(v), 3)
-            q = np.floor(np.clip(c, 0.0, 1.0) * np.float32(255.0) + np.float32(0.5)).astype(np.uint8)
-            v["red"], v["green"], v["blue"], v["alpha"] = q[:, 0], q[:, 1], q[:, 2], 255
-        f = np.empty(len(self.faces), dtype=[("n", "u1"), ("i", "<i4", (3,))])
-        f["n"] = 3
-        f["i"] = self.faces
-        header = ("ply\nformat binary_little_endian 1.0\n"
-                  f"element vertex {len(v)}\n" + "".join(f"property {'float' if t == '<f4' else 'uchar'} {n}\n" for n, t in props) +
-                  f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
-        with open(path, "wb") as fh:
-            fh.write(header.encode("ascii"))
-            fh.write(v.tobytes())
-            fh.write(f.tobytes())
+        """:func:`write_ply` of the mesh."""
+        write_ply(path, self.vertices, self.faces, self.vertex_normals, vertex_colors)
+
+
+def write_ply(path, vertices, faces, normals, vertex_colors=None):
+    """binary little-endian PLY of numpy ``vertices`` [V,3], ``faces`` [F,3] and ``normals`` [V,3]: float x, y, z, nx, ny, nz per vertex,
+    uchar-counted int lists per face.  With ``vertex_colors`` [V,3] in [0, 1], each vertex also carries uchar red, green, blue =
+    floor(clip(c, 0, 1) * 255 + 0.5) (in fp32) and alpha = 255."""
+    props = [(n, "<f4") for n in ("x", "y", "z", "nx", "ny", "nz")]
+    if vertex_colors is not None:
+        props += [(n, "u1") for n in ("red", "green", "blue", "alpha")]
+    v = np.empty(len(vertices), dtype=props)
+    for a, n in enumerate("xyz"):
+        v[n] = vertices[:, a]
+        v["n" + n] = normals[:, a]
+    if vertex_colors is not None:
+        c = np.asarray(vertex_colors, dtype=np.float32).reshape(len(v), 3)
+        q = np.floor(np.clip(c, 0.0, 1.0) * np.float32(255.0) + np.float32(0.5)).astype(np.uint8)
+        v["red"], v["green"], v["blue"], v["alpha"] = q[:, 0], q[:, 1], q[:, 2], 255
+    f = np.empty(len(faces), dtype=[("n", "u1"), ("i", "<i4", (3,))])
+    f["n"] = 3
+    f["i"] = faces
+    header = ("ply\nformat binary_little_endian 1.0\n"
+              f"element vertex {len(v)}\n" + "".join(f"property {'float' if t == '<f4' else 'uchar'} {n}\n" for n, t in props) +
+              f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(v.tobytes())
+        fh.write(f.tobytes())
+
+
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "<i2", "int16": "<i2", "ushort": "<u2", "uint16": "<u2",
+              "int": "<i4", "int32": "<i4", "uint": "<u4", "uint32": "<u4", "float": "<f4", "float32": "<f4", "double": "<f8",
+              "float64": "<f8"}
+
+
+def read_ply(filename):
+    """(vertices [V,3] fp32, faces [F,3] int64, normals [V,3] fp32 or None) of a binary little-endian PLY of triangles, such as
+    :func:`write_ply` writes."""
+    with open(filename, "rb") as fh:
+        data = fh.read()
+    end = data.find(b"end_header\n")
+    if not data.startswith(b"ply\n") or end < 0:
+        raise ValueError(f"{filename}: not a PLY file")
+    elements, fmt = [], None
+    for line in data[:end].decode("ascii").splitlines()[1:]:
+        tok = line.split()
+        if not tok or tok[0] in ("comment", "obj_info"):
+            continue
+        if tok[0] == "format":
+            fmt = tok[1]
+        elif tok[0] == "element":
+            elements.append((tok[1], int(tok[2]), []))
+        elif tok[0] == "property":
+            elements[-1][2].append(tok[1:])
+    if fmt != "binary_little_endian":
+        raise ValueError(f"{filename}: only binary_little_endian PLY is read, not {fmt}")
+    pos, out = end + len(b"end_header\n"), {}
+    for name, count, props in elements:
+        if any(p[0] == "list" for p in props):
+            if name != "face" or len(props) != 1:
+                raise ValueError(f"{filename}: unsupported list element {name}")
+            _, ct, it, _ = props[0]
+            dt = np.dtype([("n", _PLY_TYPES[ct]), ("i", _PLY_TYPES[it], (3,))])
+            rec = np.frombuffer(data, dtype=dt, count=count, offset=pos)
+            if count and (rec["n"] != 3).any():
+                raise ValueError(f"{filename}: only triangle faces are read")
+            out[name] = rec["i"].astype(np.int64)
+        else:
+            dt = np.dtype([(p[1], _PLY_TYPES[p[0]]) for p in props])
+            out[name] = np.frombuffer(data, dtype=dt, count=count, offset=pos)
+        pos += count * dt.itemsize
+    v = out["vertex"]
+    vertices = np.stack([v[c] for c in "xyz"], axis=1).astype(np.float32)
+    normals = np.stack([v[c] for c in ("nx", "ny", "nz")], axis=1).astype(np.float32) if "nx" in v.dtype.names else None
+    return vertices, out.get("face", np.zeros((0, 3), np.int64)), normals
+
+
+def import_optional(name: str, message: str):
+    """The module ``name``, or an ImportError with ``message`` (what needed it and what to do instead) when it is not installed."""
+    try:
+        return importlib.import_module(name)
+    except ImportError as e:
+        raise ImportError(message) from e
+
+
+def decimate(filename, target_num_faces: int, message: str):
+    """pymeshlab's quadric edge collapse of the mesh file ``filename`` to ``target_num_faces`` faces: the MeshSet holding the result.
+    ``message``: the ImportError's text when pymeshlab is not installed."""
+    ms = import_optional("pymeshlab", message).MeshSet()
+    ms.load_new_mesh(str(filename))
+    ms.meshing_decimation_quadric_edge_collapse(targetfacenum=target_num_faces)
+    return ms
 
 
 def _block_mesh(volume, level, spacing, mask, offset) -> Mesh:
@@ -193,13 +272,7 @@ def _write(combined: Mesh, output_path, simplify_mesh: bool):
     filename_simplify = str(output_path).replace(".ply", "-simplify.ply")
     combined.export(filename)
     if simplify_mesh:
-        try:
-            import pymeshlab
-        except ImportError as e:
-            raise ImportError(f"simplify_mesh=True needs pymeshlab, which is not installed; the unsimplified mesh is at {filename}") from e
-        ms = pymeshlab.MeshSet()
-        ms.load_new_mesh(filename)
-        ms.meshing_decimation_quadric_edge_collapse(targetfacenum=2000000)
+        ms = decimate(filename, 2000000, f"simplify_mesh=True needs pymeshlab, which is not installed; the unsimplified mesh is at {filename}")
         ms.save_current_mesh(filename_simplify, save_face_color=False)
 
 
@@ -213,8 +286,29 @@ def _outside(z, level) -> bool:
     return lo > level or hi < level
 
 
-def _block_bounds(bounding_box_min, bounding_box_max, N):
-    return [np.linspace(bounding_box_min[a], bounding_box_max[a], N + 1) for a in range(3)]
+def _blocks(bounding_box_min, bounding_box_max, resolution, device):
+    """The sliding variants' CROP_N^3-point blocks, i then j then k: (lower corner, upper corner, the block's lattice points [CROP_N^3, 3])
+    for each, the corners from np.linspace over the box in float64."""
+    N = resolution // CROP_N
+    xs, ys, zs = [np.linspace(bounding_box_min[a], bounding_box_max[a], N + 1) for a in range(3)]
+    for i in range(N):
+        for j in range(N):
+            for k in range(N):
+                lo, hi = (xs[i], ys[j], zs[k]), (xs[i + 1], ys[j + 1], zs[k + 1])
+                yield lo, hi, lattice_points(lo, hi, CROP_N, 0, CROP_N**3, device)
+
+
+def _crossing_block_mesh(z, level, mask, lo, hi):
+    """The mesh of block ``z`` [CROP_N]^3 between corners ``lo`` and ``hi``, or None unless ``level`` crosses both the values under
+    ``mask`` (when there is one) and the whole block."""
+    if mask is not None:
+        valid_z = z[mask]
+        if valid_z.shape[0] <= 0 or _outside(valid_z, level):
+            return None
+    if _outside(z, level):
+        return None
+    spacing = tuple((hi[a] - lo[a]) / (CROP_N - 1) for a in range(3))
+    return _block_mesh(z, level, spacing, mask, lo)
 
 
 @torch.no_grad()
@@ -237,61 +331,48 @@ def get_surface_sliding(
         coarse_mask = coarse_mask.permute(2, 1, 0)[None, None].to(dev).float()
     cropN = CROP_N
     level = 0
-    N = resolution // cropN
-    xs, ys, zs = _block_bounds(bounding_box_min, bounding_box_max, N)
     meshes = []
-    for i in range(N):
-        for j in range(N):
-            for k in range(N):
-                x_min, x_max = xs[i], xs[i + 1]
-                y_min, y_max = ys[j], ys[j + 1]
-                z_min, z_max = zs[k], zs[k + 1]
-                points = lattice_points((x_min, y_min, z_min), (x_max, y_max, z_max), cropN, 0, cropN**3, dev)
-                points = points.reshape(cropN, cropN, cropN, 3).permute(3, 0, 1, 2)
+    for lo, hi, points in _blocks(bounding_box_min, bounding_box_max, resolution, dev):
+        points = points.reshape(cropN, cropN, cropN, 3).permute(3, 0, 1, 2)
+        if coarse_mask is not None:
+            current_mask = torch.nn.functional.grid_sample(coarse_mask, points.permute(1, 2, 3, 0)[None])
+            current_mask = (current_mask > 0.0)[0, 0]
+        else:
+            current_mask = None
+
+        points_pyramid = [points]
+        for _ in range(3):
+            points = avg_pool_3d(points[None])[0]
+            points_pyramid.append(points)
+        points_pyramid = points_pyramid[::-1]
+
+        mask = None
+        threshold = 2 * (hi[0] - lo[0]) / cropN * 8
+        for pid, pts in enumerate(points_pyramid):
+            coarse_N = pts.shape[-1]
+            pts = pts.reshape(3, -1).permute(1, 0).contiguous()
+            if mask is None:
                 if coarse_mask is not None:
-                    current_mask = torch.nn.functional.grid_sample(coarse_mask, points.permute(1, 2, 3, 0)[None])
-                    current_mask = (current_mask > 0.0)[0, 0]
+                    pts_sdf = torch.ones_like(pts[:, 1])
+                    valid_mask = torch.nn.functional.grid_sample(coarse_mask, pts[None, None, None])[0, 0, 0, 0] > 0
+                    if valid_mask.any():
+                        pts_sdf[valid_mask] = _evaluate(sdf, pts[valid_mask].contiguous())
                 else:
-                    current_mask = None
+                    pts_sdf = _evaluate(sdf, pts)
+            else:
+                mask = mask.reshape(-1)
+                pts_to_eval = pts[mask]
+                if pts_to_eval.shape[0] > 0:
+                    pts_sdf[mask] = _evaluate(sdf, pts_to_eval.contiguous())
+            if pid < 3:
+                mask = torch.abs(pts_sdf) < threshold
+                mask = upsample(mask.reshape(coarse_N, coarse_N, coarse_N)[None, None].float()).bool()
+                pts_sdf = upsample(pts_sdf.reshape(coarse_N, coarse_N, coarse_N)[None, None]).reshape(-1)
+            threshold /= 2.0
 
-                points_pyramid = [points]
-                for _ in range(3):
-                    points = avg_pool_3d(points[None])[0]
-                    points_pyramid.append(points)
-                points_pyramid = points_pyramid[::-1]
-
-                mask = None
-                threshold = 2 * (x_max - x_min) / cropN * 8
-                for pid, pts in enumerate(points_pyramid):
-                    coarse_N = pts.shape[-1]
-                    pts = pts.reshape(3, -1).permute(1, 0).contiguous()
-                    if mask is None:
-                        if coarse_mask is not None:
-                            pts_sdf = torch.ones_like(pts[:, 1])
-                            valid_mask = torch.nn.functional.grid_sample(coarse_mask, pts[None, None, None])[0, 0, 0, 0] > 0
-                            if valid_mask.any():
-                                pts_sdf[valid_mask] = _evaluate(sdf, pts[valid_mask].contiguous())
-                        else:
-                            pts_sdf = _evaluate(sdf, pts)
-                    else:
-                        mask = mask.reshape(-1)
-                        pts_to_eval = pts[mask]
-                        if pts_to_eval.shape[0] > 0:
-                            pts_sdf[mask] = _evaluate(sdf, pts_to_eval.contiguous())
-                    if pid < 3:
-                        mask = torch.abs(pts_sdf) < threshold
-                        mask = upsample(mask.reshape(coarse_N, coarse_N, coarse_N)[None, None].float()).bool()
-                        pts_sdf = upsample(pts_sdf.reshape(coarse_N, coarse_N, coarse_N)[None, None]).reshape(-1)
-                    threshold /= 2.0
-
-                z = pts_sdf.reshape(cropN, cropN, cropN)
-                if current_mask is not None:
-                    valid_z = z[current_mask]
-                    if valid_z.shape[0] <= 0 or _outside(valid_z, level):
-                        continue
-                if not _outside(z, level):
-                    spacing = ((x_max - x_min) / (cropN - 1), (y_max - y_min) / (cropN - 1), (z_max - z_min) / (cropN - 1))
-                    meshes.append(_block_mesh(z, level, spacing, current_mask, (x_min, y_min, z_min)))
+        mesh = _crossing_block_mesh(pts_sdf.reshape(cropN, cropN, cropN), level, current_mask, lo, hi)
+        if mesh is not None:
+            meshes.append(mesh)
 
     combined = Mesh.concatenate(meshes)
     if return_mesh:
@@ -315,11 +396,7 @@ def get_surface_occupancy(
     grid_min, grid_max = bounding_box_min, bounding_box_max
     N = resolution
     dev = torch.device("cuda") if device is None else torch.device(device)
-    total = N**3
-    z = torch.empty(total, device=dev, dtype=torch.float32)
-    for start in range(0, total, EVAL_CHUNK):
-        n = min(EVAL_CHUNK, total - start)
-        z[start:start + n] = occupancy_fn(lattice_points(grid_min, grid_max, N, start, n, dev).contiguous()).contiguous()
+    z = _lattice_values(occupancy_fn, grid_min, grid_max, (N, N, N), EVAL_CHUNK, dev)
     if _outside(z, level):
         print("=================================================no surface skip")
         return None
@@ -351,37 +428,24 @@ def get_surface_sliding_with_contraction(
     coarse_mask = coarse_mask.to(dev)
     cropN = CROP_N
     level = 0
-    N = resolution // cropN
-    xs, ys, zs = _block_bounds(bounding_box_min, bounding_box_max, N)
     meshes = []
-    for i in range(N):
-        for j in range(N):
-            for k in range(N):
-                x_min, x_max = xs[i], xs[i + 1]
-                y_min, y_max = ys[j], ys[j + 1]
-                z_min, z_max = zs[k], zs[k + 1]
-                points = lattice_points((x_min, y_min, z_min), (x_max, y_max, z_max), cropN, 0, cropN**3, dev)
-                points = points.reshape(cropN, cropN, cropN, 3)
-                current_mask = torch.nn.functional.grid_sample(coarse_mask, points[None] * 0.5)   # [-2, 2] -> [-1, 1]
-                points = points.reshape(-1, 3)
-                valid_mask = current_mask.reshape(-1) > 0
-                pts_to_eval = points[valid_mask]
-                pts_sdf = torch.ones_like(points[..., 0]) * 100.0
-                if pts_to_eval.shape[0] > 0:
-                    pts_sdf[valid_mask.reshape(-1)] = _evaluate(sdf, pts_to_eval.contiguous())
-                # min-pooling removes the artefacts of masked marching cubes
-                min_sdf = max_pool_3d(pts_sdf.reshape(1, 1, cropN, cropN, cropN) * -1.0) * -1.0
-                min_mask = (current_mask > 0.0).float()
-                pts_sdf = pts_sdf.reshape(1, 1, cropN, cropN, cropN) * min_mask + min_sdf * (1.0 - min_mask)
+    for lo, hi, points in _blocks(bounding_box_min, bounding_box_max, resolution, dev):
+        points = points.reshape(cropN, cropN, cropN, 3)
+        current_mask = torch.nn.functional.grid_sample(coarse_mask, points[None] * 0.5)   # [-2, 2] -> [-1, 1]
+        points = points.reshape(-1, 3)
+        valid_mask = current_mask.reshape(-1) > 0
+        pts_to_eval = points[valid_mask]
+        pts_sdf = torch.ones_like(points[..., 0]) * 100.0
+        if pts_to_eval.shape[0] > 0:
+            pts_sdf[valid_mask.reshape(-1)] = _evaluate(sdf, pts_to_eval.contiguous())
+        # min-pooling removes the artefacts of masked marching cubes
+        min_sdf = max_pool_3d(pts_sdf.reshape(1, 1, cropN, cropN, cropN) * -1.0) * -1.0
+        min_mask = (current_mask > 0.0).float()
+        pts_sdf = pts_sdf.reshape(1, 1, cropN, cropN, cropN) * min_mask + min_sdf * (1.0 - min_mask)
 
-                z = pts_sdf.reshape(cropN, cropN, cropN)
-                current_mask = (current_mask > 0.0)[0, 0]
-                valid_z = z[current_mask]
-                if valid_z.shape[0] <= 0 or _outside(valid_z, level):
-                    continue
-                if not _outside(z, level):
-                    spacing = ((x_max - x_min) / (cropN - 1), (y_max - y_min) / (cropN - 1), (z_max - z_min) / (cropN - 1))
-                    meshes.append(_block_mesh(z, level, spacing, current_mask, (x_min, y_min, z_min)))
+        mesh = _crossing_block_mesh(pts_sdf.reshape(cropN, cropN, cropN), level, (current_mask > 0.0)[0, 0], lo, hi)
+        if mesh is not None:
+            meshes.append(mesh)
 
     combined = Mesh.concatenate(meshes)
     combined.merge_vertices(digits_vertex=6)

@@ -19,7 +19,7 @@ from typing import Optional
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, meshing
 
 MTL_LINES = ("# Generated with nerfstudio", "newmtl material_0", "Ka 1.000 1.000 1.000", "Kd 1.000 1.000 1.000", "Ks 0.000 0.000 0.000",
              "d 1.0", "illum 2", "Ns 1.00000000", "map_Kd material_0.png")
@@ -135,12 +135,8 @@ def unwrap_mesh_per_uv_triangle(vertices, faces, vertex_normals, px_per_uv_trian
 
 
 def _import_xatlas():
-    try:
-        import xatlas
-    except ImportError as e:
-        raise ImportError('unwrap_method="xatlas" needs the xatlas package, which is not installed; '
-                          'install it or use unwrap_method="custom"') from e
-    return xatlas
+    return meshing.import_optional("xatlas", 'unwrap_method="xatlas" needs the xatlas package, which is not installed; '
+                                             'install it or use unwrap_method="custom"')
 
 
 def _xatlas_texture_coordinates(vertices, faces, vertex_normals):
@@ -220,6 +216,12 @@ def _mesh_tensors(mesh, device):
             torch.as_tensor(normals).to(device, torch.float32))
 
 
+def model_and_device(pipeline):
+    """(model, device) of the reference's Pipeline (its ``.model`` and ``.device``) or of a renderer (itself, where its parameters are)."""
+    model = getattr(pipeline, "model", pipeline)
+    return model, (pipeline.device if hasattr(pipeline, "device") else next(model.parameters()).device)
+
+
 def _ray_bundle_class(model):
     from .surface_model import SurfaceRenderer
 
@@ -243,8 +245,7 @@ def export_textured_mesh(mesh, pipeline, output_dir: Path, px_per_uv_triangle: O
         raise ValueError('unwrap_method="custom" needs px_per_uv_triangle')
     if unwrap_method == "xatlas":
         _import_xatlas()
-    model = getattr(pipeline, "model", pipeline)
-    device = pipeline.device if hasattr(pipeline, "device") else next(model.parameters()).device
+    model, device = model_and_device(pipeline)
     vertices, faces, vertex_normals = _mesh_tensors(mesh, device)
     _check_mesh(vertices, faces, vertex_normals)
     if unwrap_method == "xatlas":
@@ -272,53 +273,6 @@ def export_textured_mesh(mesh, pipeline, output_dir: Path, px_per_uv_triangle: O
 # ---------------------------------------------------------------------------------------------------------------------------------
 # mesh input and scripts/texture.py
 # ---------------------------------------------------------------------------------------------------------------------------------
-_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "<i2", "int16": "<i2", "ushort": "<u2", "uint16": "<u2",
-              "int": "<i4", "int32": "<i4", "uint": "<u4", "uint32": "<u4", "float": "<f4", "float32": "<f4", "double": "<f8",
-              "float64": "<f8"}
-
-
-def read_ply(filename):
-    """(vertices [V,3] fp32, faces [F,3] int64, normals [V,3] fp32 or None) of a binary little-endian PLY of triangles, such as
-    ``meshing.Mesh.export`` writes."""
-    with open(filename, "rb") as fh:
-        data = fh.read()
-    end = data.find(b"end_header\n")
-    if not data.startswith(b"ply\n") or end < 0:
-        raise ValueError(f"{filename}: not a PLY file")
-    elements, fmt = [], None
-    for line in data[:end].decode("ascii").splitlines()[1:]:
-        tok = line.split()
-        if not tok or tok[0] in ("comment", "obj_info"):
-            continue
-        if tok[0] == "format":
-            fmt = tok[1]
-        elif tok[0] == "element":
-            elements.append((tok[1], int(tok[2]), []))
-        elif tok[0] == "property":
-            elements[-1][2].append(tok[1:])
-    if fmt != "binary_little_endian":
-        raise ValueError(f"{filename}: only binary_little_endian PLY is read, not {fmt}")
-    pos, out = end + len(b"end_header\n"), {}
-    for name, count, props in elements:
-        if any(p[0] == "list" for p in props):
-            if name != "face" or len(props) != 1:
-                raise ValueError(f"{filename}: unsupported list element {name}")
-            _, ct, it, _ = props[0]
-            dt = np.dtype([("n", _PLY_TYPES[ct]), ("i", _PLY_TYPES[it], (3,))])
-            rec = np.frombuffer(data, dtype=dt, count=count, offset=pos)
-            if count and (rec["n"] != 3).any():
-                raise ValueError(f"{filename}: only triangle faces are read")
-            out[name] = rec["i"].astype(np.int64)
-        else:
-            dt = np.dtype([(p[1], _PLY_TYPES[p[0]]) for p in props])
-            out[name] = np.frombuffer(data, dtype=dt, count=count, offset=pos)
-        pos += count * dt.itemsize
-    v = out["vertex"]
-    vertices = np.stack([v[c] for c in "xyz"], axis=1).astype(np.float32)
-    normals = np.stack([v[c] for c in ("nx", "ny", "nz")], axis=1).astype(np.float32) if "nx" in v.dtype.names else None
-    return vertices, out.get("face", np.zeros((0, 3), np.int64)), normals
-
-
 def vertex_normals_area_weighted(vertices: torch.Tensor, faces: torch.Tensor) -> torch.Tensor:
     """Unit vertex normals: the sum of the adjacent faces' cross products (each twice the face's area), normalised."""
     fv = vertices[faces]
@@ -330,22 +284,16 @@ def vertex_normals_area_weighted(vertices: torch.Tensor, faces: torch.Tensor) ->
 def get_mesh_from_filename(filename, target_num_faces: Optional[int] = None) -> Mesh:
     """exporter_utils.py:75-83.  Reads a binary little-endian PLY; without normals in the file, area-weighted vertex normals are computed
     (on the GPU when there is one).  Decimating to ``target_num_faces`` needs pymeshlab, as in the reference."""
-    vertices, faces, normals = read_ply(filename)
+    vertices, faces, normals = meshing.read_ply(filename)
     if target_num_faces is not None and target_num_faces < len(faces):
-        try:
-            import pymeshlab
-        except ImportError as e:
-            raise ImportError(f"reducing {filename} from {len(faces)} to {target_num_faces} faces needs pymeshlab, which is not installed; "
-                              "pass target_num_faces=None to texture the mesh as it is") from e
-        ms = pymeshlab.MeshSet()
-        ms.load_new_mesh(str(filename))
-        ms.meshing_decimation_quadric_edge_collapse(targetfacenum=target_num_faces)
-        m = ms.current_mesh()
+        m = meshing.decimate(filename, target_num_faces,
+                             f"reducing {filename} from {len(faces)} to {target_num_faces} faces needs pymeshlab, which is not installed; "
+                             "pass target_num_faces=None to texture the mesh as it is").current_mesh()
         return Mesh(torch.from_numpy(m.vertex_matrix()).float(), torch.from_numpy(m.face_matrix()).long(),
                     torch.from_numpy(np.copy(m.vertex_normal_matrix())).float())
     v, f = torch.from_numpy(vertices), torch.from_numpy(faces)
     if normals is None:
-        dev = torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
+        dev = meshing.work_device()
         n = vertex_normals_area_weighted(v.to(dev), f.to(dev)).cpu()
     else:
         n = torch.from_numpy(normals)

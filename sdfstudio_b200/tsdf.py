@@ -5,7 +5,7 @@ The reference fuses depth images into a truncated signed distance volume with wh
 transform alone is 21.5 GB at 512^3 and a batch of 10) and then a masked gather and scatter per image; it meshes the volume with
 skimage on the host and writes it with pymeshlab.  Here the fusion of every image is one kernel over the voxels
 (sdfb200_tsdf_integrate: the images in order, the update in registers, the volume read and written once), the mesh comes from the
-package's marching-cubes kernel (``meshing.marching_cubes``), and the PLY from ``meshing.Mesh.export``.  Depth and rgb images stay on
+package's marching-cubes kernel (``meshing.marching_cubes``), and the PLY from ``meshing.write_ply``.  Depth and rgb images stay on
 the device.
 
 Kept from the reference, quirks included: the weight stored after an update is clamped to 1, colours mix with the old weight, voxels
@@ -88,9 +88,9 @@ class TSDF:
     @classmethod
     def export_mesh(cls, mesh, filename: str):
         """Binary PLY with per-vertex normals and colours (uchar red, green, blue, alpha = 255; each channel
-        floor(clip(c, 0, 1) * 255 + 0.5)), written by ``meshing.Mesh.export``."""
+        floor(clip(c, 0, 1) * 255 + 0.5)), written by ``meshing.write_ply``."""
         colors = None if mesh.colors is None else mesh.colors.cpu().numpy()
-        meshing.Mesh(mesh.vertices.cpu().numpy(), mesh.faces.cpu().numpy(), mesh.normals.cpu().numpy()).export(filename, vertex_colors=colors)
+        meshing.write_ply(filename, mesh.vertices.cpu().numpy(), mesh.faces.cpu().numpy(), mesh.normals.cpu().numpy(), colors)
 
     def integrate_tsdf(self, c2w: torch.Tensor, K: torch.Tensor, depth_images: torch.Tensor, color_images: Optional[torch.Tensor] = None,
                        mask_images: Optional[torch.Tensor] = None):
@@ -220,8 +220,7 @@ def tsdf_mesh(renderer, cameras: Cameras, output_dir, downscale_factor: int = 2,
         raise ValueError(f"texture_method must be 'tsdf' or 'nerf', not {texture_method!r}")
     output_dir = Path(output_dir)
     output_dir.mkdir(parents=True, exist_ok=True)
-    model = getattr(renderer, "model", renderer)
-    device = renderer.device if hasattr(renderer, "device") else next(model.parameters()).device
+    model, device = texturing.model_and_device(renderer)
     _export(model, device, cameras, torch.tensor([bounding_box_min, bounding_box_max]), output_dir, downscale_factor, depth_output_name,
             rgb_output_name, volume_dims_of(resolution))
     if texture_method == "nerf":

@@ -1,9 +1,10 @@
 """CPU: the generated marching-cubes table, the numpy restatement of the kernel (oracle/marching_cubes.py) on analytic volumes, the
 restatement of the reference's mesh-extraction functions against the golden minted from the unmodified reference, the drop-ins'
-signatures, and the Mesh container."""
+signatures, the Mesh container, and the PLY writer and reader every exporter shares."""
 import inspect
 import json
 import os
+import struct
 from collections import Counter
 from pathlib import Path
 
@@ -256,7 +257,7 @@ def test_dropin_signatures_match_reference():
 
 
 # ---------------------------------------------------------------------------------------------------------------------------------
-# Mesh
+# Mesh and PLY files
 # ---------------------------------------------------------------------------------------------------------------------------------
 def read_ply(path):
     with open(path, "rb") as fh:
@@ -290,3 +291,47 @@ def test_mesh_export_roundtrip_concatenate_and_merge(tmp_path):
     w.merge_vertices(digits_vertex=6)
     assert np.array_equal(w.vertices, a.vertices) and np.array_equal(w.faces, np.concatenate([F, F]))
     assert Mesh.concatenate([]).faces.shape == (0, 3)
+
+
+def test_ply_reader_rejects_ascii_and_polygons(tmp_path):
+    from sdfstudio_b200 import meshing
+
+    (tmp_path / "a.ply").write_bytes(b"ply\nformat ascii 1.0\nelement vertex 0\nend_header\n")
+    with pytest.raises(ValueError, match="binary_little_endian"):
+        meshing.read_ply(tmp_path / "a.ply")
+    fr = np.zeros(1, dtype=[("n", "u1"), ("i", "<i4", (3,))])
+    fr["n"] = 4
+    (tmp_path / "q.ply").write_bytes(b"ply\nformat binary_little_endian 1.0\nelement vertex 0\nproperty float x\nproperty float y\n"
+                                     b"property float z\nelement face 1\nproperty list uchar int vertex_indices\nend_header\n" + fr.tobytes())
+    with pytest.raises(ValueError, match="triangle"):
+        meshing.read_ply(tmp_path / "q.ply")
+
+
+def test_coloured_ply_round_trip_and_uncoloured_bytes(tmp_path):
+    """Mesh.export with vertex colours reads back through meshing.read_ply with its colours quantised as the texture PNG's; without
+    colours the file is byte for byte the float-only PLY."""
+    from sdfstudio_b200 import meshing
+
+    g = np.random.default_rng(0)
+    v, n, f = g.normal(size=(7, 3)), g.normal(size=(7, 3)), g.integers(0, 7, size=(5, 3))
+    c = np.array([[0.0, 1.0, 0.5], [-0.2, 1.3, 0.499], [0.5 / 255, 1.5 / 255, 2.5 / 255], [np.nan, 0.25, 0.75], [0.1, 0.2, 0.3],
+                  [0.998, 0.002, 0.0], [1.0, 1.0, 1.0]], np.float32)
+    meshing.Mesh(v, f, n).export(tmp_path / "c.ply", vertex_colors=c)
+    rv, rf, rn = meshing.read_ply(tmp_path / "c.ply")
+    assert np.array_equal(rv, v.astype(np.float32)) and np.array_equal(rf, f) and np.array_equal(rn, n.astype(np.float32))
+    data = (tmp_path / "c.ply").read_bytes()
+    head, body = data.split(b"end_header\n")
+    assert head.endswith(b"property uchar red\nproperty uchar green\nproperty uchar blue\nproperty uchar alpha\nelement face 5\n"
+                         b"property list uchar int vertex_indices\n")
+    rec = np.frombuffer(body, dtype=[("p", "<f4", (6,)), ("c", "u1", (4,))], count=7)
+    with np.errstate(invalid="ignore"):
+        want = np.floor(np.clip(c, 0, 1) * np.float32(255) + np.float32(0.5)).astype(np.uint8)
+    assert np.array_equal(rec["c"][:, :3][~np.isnan(c).any(1)], want[~np.isnan(c).any(1)]) and (rec["c"][:, 3] == 255).all()
+    assert rec["c"][2, :3].tolist() == [1, 2, 3] and rec["c"][0].tolist() == [0, 255, 128, 255]
+
+    meshing.Mesh(v, f, n).export(tmp_path / "u.ply")
+    vert = b"".join(struct.pack("<6f", *v[i], *n[i]) for i in range(7))
+    face = b"".join(struct.pack("<B3i", 3, *f[i]) for i in range(5))
+    header = ("ply\nformat binary_little_endian 1.0\nelement vertex 7\n" + "".join(f"property float {p}\n" for p in ("x", "y", "z", "nx", "ny", "nz"))
+              + "element face 5\nproperty list uchar int vertex_indices\nend_header\n").encode()
+    assert (tmp_path / "u.ply").read_bytes() == header + vert + face

@@ -191,20 +191,6 @@ def test_ply_without_normals_gets_area_weighted_normals(tmp_path):
     assert np.allclose(mesh.normals.numpy(), acc, atol=1e-6)
 
 
-def test_ply_reader_rejects_ascii_and_polygons(tmp_path):
-    from sdfstudio_b200 import texturing
-
-    (tmp_path / "a.ply").write_bytes(b"ply\nformat ascii 1.0\nelement vertex 0\nend_header\n")
-    with pytest.raises(ValueError, match="binary_little_endian"):
-        texturing.read_ply(tmp_path / "a.ply")
-    fr = np.zeros(1, dtype=[("n", "u1"), ("i", "<i4", (3,))])
-    fr["n"] = 4
-    (tmp_path / "q.ply").write_bytes(b"ply\nformat binary_little_endian 1.0\nelement vertex 0\nproperty float x\nproperty float y\n"
-                                     b"property float z\nelement face 1\nproperty list uchar int vertex_indices\nend_header\n" + fr.tobytes())
-    with pytest.raises(ValueError, match="triangle"):
-        texturing.read_ply(tmp_path / "q.ply")
-
-
 @pytest.mark.skipif(importlib.util.find_spec("pymeshlab") is not None, reason="pymeshlab is installed")
 def test_decimation_without_pymeshlab_is_an_import_error(tmp_path):
     from sdfstudio_b200 import meshing, texturing

@@ -1,6 +1,6 @@
 """CPU: the two restatements of the reference's TSDF fusion (oracle/tsdf.py) against the golden minted from the unmodified reference
 (oracle/make_golden_tsdf.py), and the host side of sdfstudio_b200/tsdf.py: signatures and defaults, the Cameras additions, the
-coloured PLY, the argument errors and the C-ABI error codes.
+argument errors and the C-ABI error codes.
 
 (b), the kernel's op order in numpy float32, differs from (a), the reference's ATen ops, in the summation order inside ``bmm`` and in
 the CPU ``grid_sample``'s unnormalisation.  The camera coordinates then differ by a few ulp of their magnitude, so the voxel depth does
@@ -11,7 +11,6 @@ import dataclasses
 import inspect
 import json
 import os
-import struct
 import types
 
 import numpy as np
@@ -234,36 +233,6 @@ def test_resolution_quirk_and_argument_errors(tmp_path):
         t.integrate_tsdf(c2w, K, depth)
     with pytest.raises(ValueError):
         tsdf.tsdf_mesh(None, None, tmp_path, texture_method="poisson")
-
-
-def test_coloured_ply_round_trip_and_uncoloured_bytes(tmp_path):
-    """Mesh.export with vertex colours reads back through texturing.read_ply with its colours quantised as the texture PNG's; without
-    colours the file is byte for byte the float-only PLY."""
-    from sdfstudio_b200 import meshing, texturing
-
-    g = np.random.default_rng(0)
-    v, n, f = g.normal(size=(7, 3)), g.normal(size=(7, 3)), g.integers(0, 7, size=(5, 3))
-    c = np.array([[0.0, 1.0, 0.5], [-0.2, 1.3, 0.499], [0.5 / 255, 1.5 / 255, 2.5 / 255], [np.nan, 0.25, 0.75], [0.1, 0.2, 0.3],
-                  [0.998, 0.002, 0.0], [1.0, 1.0, 1.0]], np.float32)
-    meshing.Mesh(v, f, n).export(tmp_path / "c.ply", vertex_colors=c)
-    rv, rf, rn = texturing.read_ply(tmp_path / "c.ply")
-    assert np.array_equal(rv, v.astype(np.float32)) and np.array_equal(rf, f) and np.array_equal(rn, n.astype(np.float32))
-    data = (tmp_path / "c.ply").read_bytes()
-    head, body = data.split(b"end_header\n")
-    assert head.endswith(b"property uchar red\nproperty uchar green\nproperty uchar blue\nproperty uchar alpha\nelement face 5\n"
-                         b"property list uchar int vertex_indices\n")
-    rec = np.frombuffer(body, dtype=[("p", "<f4", (6,)), ("c", "u1", (4,))], count=7)
-    with np.errstate(invalid="ignore"):
-        want = np.floor(np.clip(c, 0, 1) * np.float32(255) + np.float32(0.5)).astype(np.uint8)
-    assert np.array_equal(rec["c"][:, :3][~np.isnan(c).any(1)], want[~np.isnan(c).any(1)]) and (rec["c"][:, 3] == 255).all()
-    assert rec["c"][2, :3].tolist() == [1, 2, 3] and rec["c"][0].tolist() == [0, 255, 128, 255]
-
-    meshing.Mesh(v, f, n).export(tmp_path / "u.ply")
-    vert = b"".join(struct.pack("<6f", *v[i], *n[i]) for i in range(7))
-    face = b"".join(struct.pack("<B3i", 3, *f[i]) for i in range(5))
-    header = ("ply\nformat binary_little_endian 1.0\nelement vertex 7\n" + "".join(f"property float {p}\n" for p in ("x", "y", "z", "nx", "ny", "nz"))
-              + "element face 5\nproperty list uchar int vertex_indices\nend_header\n").encode()
-    assert (tmp_path / "u.ply").read_bytes() == header + vert + face
 
 
 def test_c_abi_error_codes():

@@ -7,9 +7,7 @@ over their kernel time, against the H100 SXM's 3.35 TB/s.  Prints one JSON line 
 """
 import argparse
 import ctypes as C
-import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -18,6 +16,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import sdfstudio_b200 as sb  # noqa: E402
+from bench_common import header, report  # noqa: E402
 from sdfstudio_b200 import _lib, meshing, synthetic  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
@@ -153,12 +152,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("mesh_bench needs a CUDA device")
     field = make_field(args.precision)
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                               capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        power = f"unavailable ({e})"
-    result = dict(tool="mesh_bench", device=torch.cuda.get_device_name(), power_limit=power, precision=args.precision, runs=[])
+    result = dict(header("mesh_bench"), precision=args.precision, runs=[])
     with tempfile.TemporaryDirectory() as tmp:
         for res in (int(r) for r in args.resolutions.split(",")):
             run(field, res, tmp)                                         # warm-up of every shape this resolution uses
@@ -168,12 +162,7 @@ def main():
             r["marching_cubes_kernels_last_block"] = kernel_passes(vol, mask)
             result["runs"].append(r)
             del calls
-    line = json.dumps(result)
-    print(line)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    report(result, args.out)
 
 
 if __name__ == "__main__":

@@ -12,9 +12,7 @@ Prints one JSON line and writes it to --out.
     python tools/texture_bench.py [--out profiles/r14_texture_bench.json]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -23,24 +21,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import sdfstudio_b200 as sb  # noqa: E402
+from bench_common import cuda_ms, header, report  # noqa: E402
 from oracle import texture as otex  # noqa: E402
 from sdfstudio_b200 import synthetic, texturing  # noqa: E402
 from test_gpu_texture import random_charts  # noqa: E402
 
 CHUNK = 10
 ORACLE_CHUNKS = 200
-
-
-def cuda_ms(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(reps):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / reps
 
 
 def rasterize_run(n_faces, n, reps):
@@ -67,12 +54,7 @@ def main():
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "texture_bench needs a GPU"
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                               capture_output=True, text=True, check=True).stdout.strip()
-    except (OSError, subprocess.CalledProcessError) as e:
-        power = f"unavailable ({e})"
-    result = dict(tool="texture_bench", device=torch.cuda.get_device_name(), power_limit=power)
+    result = header("texture_bench")
     result["rasterize"] = [rasterize_run(50000, 2048, 3), rasterize_run(5000, 1024, 10)]
     ppt, nf = 4, 50000
     g = torch.Generator().manual_seed(0)
@@ -100,11 +82,7 @@ def main():
         result["texel_render"] = dict(rays=o.shape[0], ms=cuda_ms(lambda: renderer.get_outputs_for_camera_ray_bundle(bundle), 2))
 
     result["oracle_aten_loop"] = [oracle_run(5000, 1024, 10 ** 9), oracle_run(50000, 2048, ORACLE_CHUNKS)]
-    line = json.dumps(result)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    report(result, args.out)
 
 
 if __name__ == "__main__":

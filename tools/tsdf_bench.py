@@ -14,9 +14,7 @@ Prints one JSON line and writes it to --out.
     python tools/tsdf_bench.py [--out profiles/r15_tsdf_bench.json]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -27,6 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import sdfstudio_b200 as sb  # noqa: E402
+from bench_common import cuda_ms, header, report  # noqa: E402
 from oracle import tsdf as ot  # noqa: E402
 from oracle.make_golden_tsdf import intrinsics, look_at, on_sphere, sphere_images  # noqa: E402
 from sdfstudio_b200 import synthetic, tsdf  # noqa: E402
@@ -35,18 +34,6 @@ from sdfstudio_b200.cameras import Cameras  # noqa: E402
 N_CAMS, HW = 49, 192
 BYTES_PER_VOXEL = 52
 AABB = torch.tensor([[-1.0, -1, -1], [1, 1, 1]])
-
-
-def cuda_ms(fn, reps):
-    fn()
-    torch.cuda.synchronize()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(reps):
-        fn()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / reps
 
 
 def images():
@@ -121,21 +108,12 @@ def main():
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "tsdf_bench needs a GPU"
-    try:
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                               capture_output=True, text=True, check=True).stdout.strip()
-    except (OSError, subprocess.CalledProcessError) as e:
-        power = f"unavailable ({e})"
-    result = dict(tool="tsdf_bench", device=torch.cuda.get_device_name(), power_limit=power)
+    result = header("tsdf_bench")
     c2w, K, depth, color = images()
     result["kernel"] = [kernel_run(r, c2w, K, depth, color, reps) for r, reps in ((128, 50), (256, 20), (512, 5))]
     result["reference_ops_batch10"] = [reference_run(r, c2w, K, depth, color) for r in (128, 256, 512)]
     result["tsdf_mesh_export"] = export_breakdown()
-    line = json.dumps(result)
-    print(line)
-    if args.out:
-        with open(args.out, "w") as fh:
-            fh.write(line + "\n")
+    report(result, args.out)
 
 
 if __name__ == "__main__":
