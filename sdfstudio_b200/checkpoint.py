@@ -52,6 +52,17 @@ def load_field_checkpoint(field, loaded_state, prefix: str = FIELD_PREFIX, stric
     return missing, list(unexpected)
 
 
+def load_flat_params(flats: Dict[str, Tuple[torch.nn.Parameter, torch.Tensor]], owner: str, knobs: Dict[str, str]) -> None:
+    """Copy tiny-cuda-nn flat ``params`` vectors (fp16-stored ones cast to fp32) into their parameters: `flats` maps a name to
+    (parameter, vector).  Every length is checked before anything is copied; a mismatch names the constructor arguments to check."""
+    for key, (p, v) in flats.items():
+        if v.numel() != p.numel():
+            raise ValueError(f"{key} has {v.numel()} entries, {owner} needs {p.numel()} (check {knobs[key]})")
+    with torch.no_grad():
+        for p, v in flats.values():
+            p.copy_(v.reshape(-1).to(device=p.device, dtype=torch.float32))
+
+
 def load_density_field_checkpoint(density_field, loaded_state, index: int = 0, strict: bool = True):
     """Load ``_model.proposal_networks.{index}.mlp_base.params`` (tiny-cuda-nn ``NetworkWithInputEncoding``: FullyFusedMLP weights then the
     HashGrid table, nerfstudio/fields/density_fields.py:89-96) of a reference neus-facto / bakedsdf checkpoint into a
@@ -63,13 +74,8 @@ def load_density_field_checkpoint(density_field, loaded_state, index: int = 0, s
     key = "mlp_base.params"
     if key not in sd:
         raise KeyError(f"{key} not found under _model.proposal_networks.{index}.")
-    flat = sd[key].reshape(-1).to(torch.float32)
-    nb = density_field.mlp_base
-    if flat.numel() != nb.params.numel():
-        raise ValueError(f"mlp_base.params has {flat.numel()} entries, this proposal network needs {nb.params.numel()} "
-                         "(check num_levels / log2_hashmap_size / max_res / hidden_dim / num_layers)")
-    with torch.no_grad():
-        nb.params.copy_(flat.to(nb.params.device))
+    load_flat_params({key: (density_field.mlp_base.params, sd[key])}, "this proposal network",
+                     {key: "num_levels / log2_hashmap_size / max_res / hidden_dim / num_layers"})
     extra = [k for k in sd if k not in (key, "aabb")]
     if strict and extra:
         raise RuntimeError(f"unexpected entries for the proposal network: {extra}")
@@ -99,23 +105,14 @@ def load_background_field_checkpoint(field, loaded_state, prefix: str = BACKGROU
         if strict and (missing or unexpected):
             raise RuntimeError(f"checkpoint does not match the background field: missing {list(missing)}, unexpected {list(unexpected)}")
         return list(missing), list(unexpected)
-    flats = {}
-    for key, knobs in _FLAT_KNOBS.items():
+    for key in _FLAT_KNOBS:
         if key not in sd:
             raise KeyError(f"{key} not found under {prefix}")
-        flat = sd.pop(key).reshape(-1).to(torch.float32)
-        need = field.get_parameter(key).numel()
-        if flat.numel() != need:
-            raise ValueError(f"{key} has {flat.numel()} entries, this background field needs {need} (check {knobs})")
-        flats[key] = flat
     for key in _EMPTY_PARAMS:
         v = sd.pop(key, None)
         if v is not None and v.numel() != 0:
             raise ValueError(f"{key} has {v.numel()} entries, the parameter-free encoding has none")
-    with torch.no_grad():
-        for key, flat in flats.items():
-            p = field.get_parameter(key)
-            p.copy_(flat.to(p.device))
+    load_flat_params({key: (field.get_parameter(key), sd.pop(key)) for key in _FLAT_KNOBS}, "this background field", _FLAT_KNOBS)
     missing, unexpected = field.load_state_dict(sd, strict=False)
     missing = [m for m in missing if m not in _FLAT_KNOBS and m not in _EMPTY_PARAMS and m != "aabb"]
     if strict and (missing or unexpected):

@@ -51,15 +51,28 @@ def fully_fused_weights(g: torch.Generator, in_dim: int, hidden_dim: int, n_hidd
     return torch.cat(ws)
 
 
-def relu_mlp(x: torch.Tensor, w: torch.Tensor, in_dim: int, in_pad: int, hidden_dim: int, n_hidden_layers: int):
-    """The hidden layers of a FullyFusedMLP over the flat weights `w` (layout of fully_fused_weights), through ATen on views of `w` so
-    that autograd reaches it: returns the last hidden activations [N, hidden] and the rest of `w` (the output matrix)."""
+def fully_fused_mlp(x: torch.Tensor, w: torch.Tensor, in_dim: int, in_pad: int, hidden_dim: int, n_hidden_layers: int, n_output_dims: int):
+    """A FullyFusedMLP over the flat weights `w` (layout of fully_fused_weights), through ATen on views of `w` so that autograd reaches
+    it: [N, in_dim] -> the live output rows [N, n_output_dims] (no output activation)."""
     o = hidden_dim * in_pad
     h = torch.relu(x @ w[:o].view(hidden_dim, in_pad)[:, :in_dim].t())
     for _ in range(n_hidden_layers - 1):
         h = torch.relu(h @ w[o: o + hidden_dim * hidden_dim].view(hidden_dim, hidden_dim).t())
         o += hidden_dim * hidden_dim
-    return h, w[o:]
+    return h @ w[o: o + 16 * hidden_dim].view(16, hidden_dim)[:n_output_dims].t()
+
+
+def normalized_positions(positions: torch.Tensor, aabb: torch.Tensor, spatial_distortion) -> torch.Tensor:
+    """Positions -> the grid's unit cube: SceneContraction then (x + 2) / 4 when there is a spatial distortion, else
+    SceneBox.get_normalized_positions."""
+    if spatial_distortion is not None:
+        return (spatial_distortion(positions) + 2.0) / 4.0
+    return (positions - aabb[0]) / (aabb[1] - aabb[0])
+
+
+def kernel_aabb(aabb: torch.Tensor, code: int) -> Optional[torch.Tensor]:
+    """The aabb of a field kernel call with contraction `code`: the kernels normalise with it only when there is no contraction."""
+    return _lib.f32c(aabb.detach()) if code == _lib.CONTRACT_NONE else None
 
 
 class _NetworkWithInputEncoding(nn.Module):
@@ -91,6 +104,16 @@ class _NetworkWithInputEncoding(nn.Module):
     def table(self):
         return self.params[self.n_net:]
 
+    def kernel_desc(self) -> "_lib.GridDesc":
+        """The grid descriptor of a kernel call on this network's table: every level active, fp32."""
+        self.desc.active_levels, self.desc.table_dtype = self.desc.n_levels, _lib.DT_F32
+        return self.desc
+
+    def forward(self, x01: torch.Tensor) -> torch.Tensor:
+        """The differentiable pass: [N, 3] in [0, 1] -> [N, n_output_dims] (no output activation)."""
+        feat = _GridFn.apply(x01, self.params, self)
+        return fully_fused_mlp(feat, self.params[: self.n_net], self.in_dim, self.in_pad, self.hidden_dim, self.n_hidden_layers, self.n_output_dims)
+
 
 class HashMLPDensityField(nn.Module):
     """density_fields.py:40-121."""
@@ -118,15 +141,12 @@ class HashMLPDensityField(nn.Module):
         dens = torch.empty(n, device=pos.device, dtype=torch.float32)
         pre = torch.empty_like(dens) if return_pre_activation else None
         code = contraction_code(self.spatial_distortion)
-        aabb = _lib.f32c(self.aabb.detach()) if code == _lib.CONTRACT_NONE else None
+        aabb = kernel_aabb(self.aabb, code)
         nb = self.mlp_base
         p = nb.params.detach()
-        w, table = p[: nb.n_net], p[nb.n_net:]
-        desc = nb.desc
-        desc.active_levels = desc.n_levels
-        desc.table_dtype = _lib.DT_F32
-        _lib.check(lib.sdfb200_density_field_forward(desc, table.data_ptr(), w.data_ptr(), nb.hidden_dim, nb.n_hidden_layers, code, _lib.ptr(aabb),
-                                                     _lib.ptr(pos), n, _lib.ptr(dens), _lib.ptr(pre), _lib.stream_ptr()), "sdfb200_density_field_forward")
+        _lib.check(lib.sdfb200_density_field_forward(nb.kernel_desc(), p[nb.n_net:].data_ptr(), p.data_ptr(), nb.hidden_dim, nb.n_hidden_layers, code,
+                                                     _lib.ptr(aabb), _lib.ptr(pos), n, _lib.ptr(dens), _lib.ptr(pre), _lib.stream_ptr()),
+                   "sdfb200_density_field_forward")
         dens = dens.view(*positions.shape[:-1], 1)
         return (dens, pre.view(*positions.shape[:-1], 1)) if return_pre_activation else dens
 
@@ -134,15 +154,8 @@ class HashMLPDensityField(nn.Module):
         """Training path (the interlevel loss trains the proposal networks, models/neus_facto.py): the hash grid through this package's
         twice-differentiable operator (sdfb200_grid_encode / _backward), the width-16..64 ReLU MLP through ATen, trunc_exp with the
         reference's clipped backward (field_components/activations.py:24-42)."""
-        nb = self.mlp_base
-        x = positions.reshape(-1, 3)
-        if self.spatial_distortion is not None:
-            x01 = (self.spatial_distortion(x) + 2.0) / 4.0
-        else:
-            x01 = (x - self.aabb[0]) / (self.aabb[1] - self.aabb[0])                  # SceneBox.get_normalized_positions
-        feat = _GridFn.apply(x01, nb.params, nb)
-        h, wo = relu_mlp(feat, nb.params[: nb.n_net], nb.in_dim, nb.in_pad, nb.hidden_dim, nb.n_hidden_layers)
-        pre = (h @ wo[: nb.hidden_dim]).view(*positions.shape[:-1], 1)
+        x01 = normalized_positions(positions.reshape(-1, 3), self.aabb, self.spatial_distortion)
+        pre = self.mlp_base(x01).view(*positions.shape[:-1], 1)
         dens = _TruncExp.apply(pre)
         return (dens, pre) if return_pre_activation else dens
 

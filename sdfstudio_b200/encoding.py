@@ -178,11 +178,9 @@ class _GridFn(torch.autograd.Function):
         lib = _lib.load()
         x = _lib.f32c(x01)
         n = x.shape[0]
-        desc = nb.desc
-        desc.active_levels, desc.table_dtype = desc.n_levels, _lib.DT_F32
         out = torch.empty(n, nb.in_dim, device=x.device, dtype=torch.float32)
         table = params.detach()[nb.n_net:]
-        _lib.check(lib.sdfb200_grid_encode(desc, table.data_ptr(), _lib.ptr(x), n, _lib.ptr(out), nb.in_dim, None, _lib.stream_ptr()), "sdfb200_grid_encode")
+        _lib.check(lib.sdfb200_grid_encode(nb.kernel_desc(), table.data_ptr(), _lib.ptr(x), n, _lib.ptr(out), nb.in_dim, None, _lib.stream_ptr()), "sdfb200_grid_encode")
         ctx.save_for_backward(x, params)
         ctx.nb = nb
         return out

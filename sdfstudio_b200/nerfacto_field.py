@@ -32,8 +32,7 @@ from torch import nn
 
 from . import _lib
 from .autograd_ops import training_step
-from .density_fields import _NetworkWithInputEncoding, _TruncExp, fully_fused_weights, relu_mlp
-from .encoding import _GridFn
+from .density_fields import _NetworkWithInputEncoding, _TruncExp, fully_fused_mlp, fully_fused_weights, kernel_aabb, normalized_positions
 from .field_heads import FieldHeadNames
 from .rays import point_or_ray_inputs
 from .sdf_field import _Embedding
@@ -78,8 +77,7 @@ class _Network(nn.Module):
 
     def forward(self, x):
         """[N, in_dim] -> [N, n_output_dims] (no output activation)."""
-        h, wo = relu_mlp(x, self.params, self.in_dim, self.in_pad, self.hidden_dim, self.n_hidden_layers)
-        return h @ wo.view(16, self.hidden_dim)[: self.n_output_dims].t()
+        return fully_fused_mlp(x, self.params, self.in_dim, self.in_pad, self.hidden_dim, self.n_hidden_layers, self.n_output_dims)
 
 
 class TCNNNerfactoField(nn.Module):
@@ -125,29 +123,17 @@ class TCNNNerfactoField(nn.Module):
         access.  The composition path stores them like the reference."""
         if self._locations is None and self._positions_of_last_call is not None:
             with torch.no_grad():
-                self._locations = self._normalize(self._positions_of_last_call())
+                self._locations = normalized_positions(self._positions_of_last_call(), self.aabb, self.spatial_distortion)
         return self._locations
 
     def _contraction_code(self) -> int:
         return contraction_code(self.spatial_distortion)
 
     # ------------------------------------------------------------------ differentiable composition
-    def _normalize(self, positions):
-        if self.spatial_distortion is not None:
-            return (self.spatial_distortion(positions) + 2.0) / 4.0
-        return (positions - self.aabb[0]) / (self.aabb[1] - self.aabb[0])   # SceneBox.get_normalized_positions
-
-    def _base(self, x01):
-        """mlp_base: [N,3] in [0,1] -> [N, 1 + geo_feat_dim]."""
-        nb = self.mlp_base
-        feat = _GridFn.apply(x01, nb.params, nb)
-        h, wo = relu_mlp(feat, nb.params[: nb.n_net], nb.in_dim, nb.in_pad, nb.hidden_dim, nb.n_hidden_layers)
-        return h @ wo.view(16, nb.hidden_dim)[: nb.n_output_dims].t()
-
     def _density_from_positions(self, positions):
-        x01 = self._normalize(positions)
+        x01 = normalized_positions(positions, self.aabb, self.spatial_distortion)
         self._locations, self._positions_of_last_call = x01, None
-        h = self._base(x01.reshape(-1, 3)).view(*positions.shape[:-1], -1)
+        h = self.mlp_base(x01.reshape(-1, 3)).view(*positions.shape[:-1], -1)
         density_before_activation, base_mlp_out = torch.split(h, [1, self.geo_feat_dim], dim=-1)
         self._density_before_activation = density_before_activation
         return _TruncExp.apply(density_before_activation), base_mlp_out
@@ -222,11 +208,9 @@ class TCNNNerfactoField(nn.Module):
         pre = torch.empty(N, device=dev, dtype=torch.float32)
         nb, nh = self.mlp_base, self.mlp_head
         p = nb.params.detach()
-        desc = nb.desc
-        desc.active_levels, desc.table_dtype = desc.n_levels, _lib.DT_F32
-        code = self._contraction_code()
-        aabb = _lib.f32c(self.aabb.detach()) if code == _lib.CONTRACT_NONE else None
-        _lib.check(lib.sdfb200_nerfacto_field_forward(desc, self._desc(S), p[nb.n_net:].data_ptr(), p.data_ptr(), nh.params.detach().data_ptr(),
+        nd = self._desc(S)
+        aabb = kernel_aabb(self.aabb, nd.contraction)
+        _lib.check(lib.sdfb200_nerfacto_field_forward(nb.kernel_desc(), nd, p[nb.n_net:].data_ptr(), p.data_ptr(), nh.params.detach().data_ptr(),
                                                       _lib.ptr(aabb), _lib.ptr(origins), _lib.ptr(directions), _lib.ptr(bins), n_rows, _lib.ptr(app),
                                                       stride, density.data_ptr(), rgb.data_ptr(), pre.data_ptr(), None, _lib.stream_ptr()),
                    "sdfb200_nerfacto_field_forward")

@@ -1,4 +1,4 @@
-"""The nerfacto background field on the GPU (csrc/nerfacto_field.cu, sdfstudio_b200/nerfacto_field.py) against the fp64 oracle
+"""The nerfacto background field on the GPU (csrc/hash_mlp.cuh, sdfstudio_b200/nerfacto_field.py) against the fp64 oracle
 (oracle/nerfacto.py): the eval kernel across normalisations, table types, widths, appearance modes and sizes, the C-ABI's error paths, the
 differentiable training composition, and an angelo-shaped step with the reference's background merge."""
 import math
