@@ -504,6 +504,39 @@ int sdfb200_tsdf_integrate(const float* voxel_coords, int64_t n_voxels, const fl
                            const float* color, int32_t height, int32_t width, const float* truncation, float* values, float* weights,
                            float* colors, void* stream);
 
+/* Exact k nearest neighbours of every point of a cloud among all its points, itself included at distance 0 (open3d's SearchKNN, as
+ * PointCloud::RemoveStatisticalOutliers and EstimateNormals call it from exporter_utils.generate_point_cloud,
+ * nerfstudio/exporter/exporter_utils.py:86-205).  The caller buckets the cloud on a grid of cells of edge h = 2^log2_cell:
+ *   box [6] (HOST fp32) = min x, y, z, max x, y, z of the cloud, read back by the caller (the box sets the grid dimensions)
+ *   cell_min_a = floor(box_min_a 2^-log2_cell), dims_a = floor(box_max_a 2^-log2_cell) - cell_min_a + 1 (computed in double; exact)
+ *   cell of p: c_a = floor(double(p_a) 2^-log2_cell) - cell_min_a;  key = (c_z dims_y + c_y) dims_x + c_x
+ *   points [N,3] fp32 = the cloud sorted by key; order [N] int32 = the original index of each sorted point;
+ *   cell_start [cells + 1] int32 = the first sorted position of each key (cell_start[cells] = N)
+ * Per pair, in double (fp32 converted as open3d's Vector3dVector does), every operation rounded on its own:
+ *   dx = double(a_x) - double(b_x) (likewise dy, dz);  d2 = (dx dx + dy dy) + dz dz
+ * The neighbours of a point are the k_eff = min(k, N) smallest (d2, original index) pairs, in that order: ties in d2 go to the lower
+ * index, so the lists are fully defined and do not depend on the bucketing.  The search visits Chebyshev shells of cells around the
+ * point's cell and stops once k_eff are held and the k-th d2 is at most (1 - 2^-48) times the squared distance to the nearest wall with
+ * unvisited cells beyond it (the factor covers the rounding of both sides, so the result is exact).
+ * Outputs, indexed by original index, either may be NULL (not both):
+ *   mean_dist [N] double = (sqrt(d2_0) + sqrt(d2_1) + ... + sqrt(d2_{k_eff-1})) / k_eff, added in ascending order (__dsqrt_rn,
+ *                          __dadd_rn, __ddiv_rn)
+ *   indices [N,k] int32 = the neighbour list; entries k_eff..k-1 (only when N < k) are -1.  Offsets are int64.
+ * Refused with SDFB200_EINVAL before any launch: k outside [1, 32], N outside [0, 2^31), both outputs NULL, a NULL input (N > 0), a
+ * non-finite box (any non-finite point makes the box non-finite), box min > max, more than 2^31 - 2 cells. */
+int sdfb200_knn(const float* points, const int32_t* order, int64_t n_points, const int32_t* cell_start, const float* box, int32_t log2_cell,
+                int32_t k, double* mean_dist, int32_t* indices, void* stream);
+
+/* Normals by PCA over given neighbour lists (open3d's EstimateNormals without its orientation step).  points [N,3] fp32 in original
+ * order, indices [N,k] int32 (entries < 0 are skipped), normals [N,3] fp32.  Per point, in double, every operation rounded on its own:
+ *   cumulants x, y, z, xx, xy, xz, yy, yz, zz summed over the list in list order, each divided by the count n;
+ *   cov_ab = E[ab] - E[a] E[b]   (open3d's cumulant form)
+ * then cyclic Jacobi rotations on (0,1), (0,2), (1,2) until the off-diagonal is zero, and the eigenvector of the smallest eigenvalue
+ * (the first axis on ties), written as fp32.  Sign (the package's own rule; open3d's is not pinned): the component of largest
+ * magnitude of the fp32 vector is positive, the first axis on ties.  A zero covariance, or an empty list, gives (0, 0, 1).
+ * Refused with SDFB200_EINVAL: k outside [1, 32], N outside [0, 2^31), a NULL pointer (N > 0). */
+int sdfb200_point_normals(const float* points, int64_t n_points, const int32_t* indices, int32_t k, float* normals, void* stream);
+
 /* Training path: backward of sdfb200_render (expected depth) / sdfb200_render_alphas' compositing w.r.t. the per-sample
  * inputs (autograd over renderers.py:42-295 in the reference).  `accumulation`, `depth` = forward outputs (depth BEFORE the
  * global clip).  g_rgb [R,3], g_depth [R], g_normal [R,3], g_accumulation [R], g_weights_in [R,S]: incoming gradients, each

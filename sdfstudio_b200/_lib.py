@@ -121,6 +121,8 @@ _PROTOS = {
     "sdfb200_uv_unwrap_grid": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp]),
     "sdfb200_uv_texel_rays": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "sdfb200_tsdf_integrate": (C.c_int, [_vp, _i64, _vp, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "sdfb200_knn": (C.c_int, [_vp, _vp, _i64, _vp, C.POINTER(C.c_float), _i32, _i32, _vp, _vp, _vp]),
+    "sdfb200_point_normals": (C.c_int, [_vp, _i64, _vp, _i32, _vp, _vp]),
     "sdfb200_field_packed_bytes": (_sz, [C.POINTER(FieldDesc)]),
     "sdfb200_field_pack": (C.c_int, [C.POINTER(FieldDesc), C.POINTER(FieldParams), _vp, _vp]),
     "sdfb200_field_workspace_bytes": (_sz, [C.POINTER(FieldDesc), _i64]),

@@ -173,28 +173,34 @@ class Mesh:
 def write_ply(path, vertices, faces, normals, vertex_colors=None):
     """binary little-endian PLY of numpy ``vertices`` [V,3], ``faces`` [F,3] and ``normals`` [V,3]: float x, y, z, nx, ny, nz per vertex,
     uchar-counted int lists per face.  With ``vertex_colors`` [V,3] in [0, 1], each vertex also carries uchar red, green, blue =
-    floor(clip(c, 0, 1) * 255 + 0.5) (in fp32) and alpha = 255."""
-    props = [(n, "<f4") for n in ("x", "y", "z", "nx", "ny", "nz")]
+    floor(clip(c, 0, 1) * 255 + 0.5) (in fp32) and alpha = 255.  ``normals`` None leaves out nx, ny, nz; ``faces`` None leaves out the
+    face element (a point cloud)."""
+    props = [(n, "<f4") for n in ("x", "y", "z")]
+    if normals is not None:
+        props += [(n, "<f4") for n in ("nx", "ny", "nz")]
     if vertex_colors is not None:
         props += [(n, "u1") for n in ("red", "green", "blue", "alpha")]
     v = np.empty(len(vertices), dtype=props)
     for a, n in enumerate("xyz"):
         v[n] = vertices[:, a]
-        v["n" + n] = normals[:, a]
+        if normals is not None:
+            v["n" + n] = normals[:, a]
     if vertex_colors is not None:
         c = np.asarray(vertex_colors, dtype=np.float32).reshape(len(v), 3)
         q = np.floor(np.clip(c, 0.0, 1.0) * np.float32(255.0) + np.float32(0.5)).astype(np.uint8)
         v["red"], v["green"], v["blue"], v["alpha"] = q[:, 0], q[:, 1], q[:, 2], 255
-    f = np.empty(len(faces), dtype=[("n", "u1"), ("i", "<i4", (3,))])
-    f["n"] = 3
-    f["i"] = faces
     header = ("ply\nformat binary_little_endian 1.0\n"
-              f"element vertex {len(v)}\n" + "".join(f"property {'float' if t == '<f4' else 'uchar'} {n}\n" for n, t in props) +
-              f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+              f"element vertex {len(v)}\n" + "".join(f"property {'float' if t == '<f4' else 'uchar'} {n}\n" for n, t in props))
+    if faces is not None:
+        f = np.empty(len(faces), dtype=[("n", "u1"), ("i", "<i4", (3,))])
+        f["n"] = 3
+        f["i"] = faces
+        header += f"element face {len(f)}\nproperty list uchar int vertex_indices\n"
     with open(path, "wb") as fh:
-        fh.write(header.encode("ascii"))
+        fh.write((header + "end_header\n").encode("ascii"))
         fh.write(v.tobytes())
-        fh.write(f.tobytes())
+        if faces is not None:
+            fh.write(f.tobytes())
 
 
 _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "<i2", "int16": "<i2", "ushort": "<u2", "uint16": "<u2",
@@ -204,7 +210,7 @@ _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short":
 
 def read_ply(filename):
     """(vertices [V,3] fp32, faces [F,3] int64, normals [V,3] fp32 or None) of a binary little-endian PLY of triangles, such as
-    :func:`write_ply` writes."""
+    :func:`write_ply` writes.  A file without a face element (a point cloud) gives no faces."""
     with open(filename, "rb") as fh:
         data = fh.read()
     end = data.find(b"end_header\n")
