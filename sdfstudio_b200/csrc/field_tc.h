@@ -39,6 +39,9 @@ __host__ __device__ constexpr uint32_t tc_stage_bytes(int planes) { return (uint
 enum { PRM_B_G0 = 0, PRM_B_G1, PRM_W_G2 /* row 0 */, PRM_B_C0, PRM_B_C1, PRM_W_C2 /* rows 0..2 */, kPrmRows = PRM_W_C2 + 3 };
 // rows of the head inputs `hs` of one tile ([kHsRows][128] f32, one column per tile row)
 enum { HS_SDF = 0, HS_GRAD /* x, y, z */, HS_RGB = HS_GRAD + 3 /* raw r, g, b */, kHsRows = HS_RGB + 3 };
+// rows of a staging slot's point geometry ([kGeomRows][128] f32, one column per tile row, then the rays [128] i64): the contracted
+// position and the ray direction of every row of the tile, computed once per tile by the encoder warps
+enum { GEOM_PX = 0, GEOM_PY, GEOM_PZ, GEOM_DX, GEOM_DY, GEOM_DZ, kGeomRows };
 
 // Dynamic shared memory of k_field_tc: byte offsets from its 1024-aligned base
 struct TcSmem { size_t a, ring, prm, hs, coldesc, hx, bytes; };
@@ -59,15 +62,17 @@ static_assert(tc_smem(2).bytes + kStaticSmem <= kSmemPerBlock, "shared memory of
 // Per-CTA scratch of k_field_tc (caller workspace): byte offsets from the CTA's base.  sig is a plane of [64 units][256 threads] x 4 B
 // (kFragWords) in the accumulator-fragment order of the thread that writes and later reads it.
 constexpr size_t kFragWords = 64 * 256;
-struct TcScratch { size_t sig, h2, slots, slot_bytes, geo, cs, jpe, jg, bytes; };
+struct TcScratch { size_t sig, h2, slots, slot_bytes, geo, cs, jpe, jg, geom, ray, bytes; };
 __host__ __device__ constexpr TcScratch tc_scratch(int planes) {
   TcScratch s{};                                               // sig: softplus'(z1) as 2 x unorm16
   s.h2 = s.sig + kFragWords * 4;                               // h2 in the A operand's layout [P][32 chunks][128 rows][16 B]
   s.slots = s.h2 + (size_t)planes * kAPlane;                   // two staging slots (tile parity), slot_bytes apart, each with:
   s.cs = s.geo + (size_t)planes * kImgPlane;                   //   geo input image [P][12 chunks][128 rows][16 B] at geo = 0 and the
   s.jpe = s.cs + (size_t)planes * kImgPlane;                   //   colour-static image (same layout, chunk 0 unused); PE jacobian
-  s.jg = s.jpe + (size_t)kPeRows * 128 * 4;                    //   [kPeRows][128] f32, grid jacobian [kMaxGridDim * 3][128] f32
-  s.slot_bytes = s.jg + (size_t)kMaxGridDim * 3 * 128 * 4;
+  s.jg = s.jpe + (size_t)kPeRows * 128 * 4;                    //   [kPeRows][128] f32, grid jacobian [kMaxGridDim * 3][128] f32,
+  s.geom = s.jg + (size_t)kMaxGridDim * 3 * 128 * 4;           //   point geometry [kGeomRows][128] f32 and the rows' rays
+  s.ray = s.geom + (size_t)kGeomRows * 128 * 4;                //   [128] i64
+  s.slot_bytes = s.ray + 128 * 8;
   s.bytes = s.slots + 2 * s.slot_bytes;                        // per CTA
   return s;
 }

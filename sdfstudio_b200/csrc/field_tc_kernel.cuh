@@ -35,18 +35,31 @@ using namespace tc;
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 constexpr int kEncBar = 3;   // named barrier of the encoder warps (0 is __syncthreads, 1 and 2 belong to the consumer warpgroups)
 
-// sample position of point p (ray r, sample s): o + d * t_start, then SceneContraction (cameras/rays.py:61-73,
-// spatial_distortions.py:66-73).  Also returns the ray direction, the bin start and the bin width.
+// Point p = tile * 128 + row of a call with bins (the last point for a row past the end): its ray p / n_samples and sample
+// p mod n_samples, from those of the tile's first point (one 64-bit division) and a 32-bit division of the row's offset.  Returns the
+// point's first bin edge (bins + ray * (n_samples + 1) + sample).
+__device__ __forceinline__ const float* point_bin(const TcArgs& a, int tile, int row, long long& ray) {
+  const long long p0 = (long long)tile * 128;
+  const long long ray0 = p0 / a.n_samples;
+  const int s = (int)(p0 - ray0 * a.n_samples) + (int)(min(p0 + row, a.n_points - 1) - p0);
+  ray = ray0 + s / a.n_samples;
+  return a.bins + ray * (a.n_samples + 1) + s % a.n_samples;
+}
+
+// sample position of point p = tile * 128 + row (the last point for a row past the end; ray r, sample s): o + d * t_start, then
+// SceneContraction (cameras/rays.py:61-73, spatial_distortions.py:66-73).  Also returns the ray direction, the bin start and the bin
+// width.
 struct PointGeom { float px, py, pz, dx, dy, dz, delta, t0, t1; long long ray; };
-__device__ __forceinline__ PointGeom point_geom(const TcArgs& a, long long p) {
+__device__ __forceinline__ PointGeom point_geom(const TcArgs& a, int tile, int row) {
+  const long long p = min((long long)tile * 128 + row, a.n_points - 1);
   PointGeom g;
   g.dx = g.dy = g.dz = 0.f; g.delta = 0.f; g.t0 = g.t1 = 0.f;
-  g.ray = a.has_bins ? p / a.n_samples : p;
+  g.ray = p;
   if (a.has_bins) {
-    const int smp = (int)(p - g.ray * a.n_samples);
-    const float t0 = __ldg(a.bins + g.ray * (a.n_samples + 1) + smp);
+    const float* bin = point_bin(a, tile, row, g.ray);
+    const float t0 = __ldg(bin);
     g.t0 = t0;
-    g.t1 = __ldg(a.bins + g.ray * (a.n_samples + 1) + smp + 1);
+    g.t1 = __ldg(bin + 1);
     g.delta = __fsub_rn(g.t1, t0);
     g.dx = __ldg(a.directions + g.ray * 3); g.dy = __ldg(a.directions + g.ray * 3 + 1); g.dz = __ldg(a.directions + g.ray * 3 + 2);
     g.px = __fadd_rn(__ldg(a.origins + g.ray * 3 + 0), __fmul_rn(g.dx, t0));
@@ -75,18 +88,43 @@ __device__ __forceinline__ PointGeom point_geom(const TcArgs& a, long long p) {
 static __device__ __forceinline__ void sincos_call(float x, float* s, float* c) { sincosf(x, s, c); }
 static __device__ __forceinline__ float sin_call(float x) { return sinf(x); }
 
+// Staging slot s of the per-CTA scratch (tc_scratch)
+template <int P>
+struct Slot {
+  uint8_t* base;
+  __device__ __forceinline__ Slot(char* slots, uint32_t s) : base(reinterpret_cast<uint8_t*>(slots) + s * tc_scratch(P).slot_bytes) {}
+  __device__ __forceinline__ uint8_t* geo() const { return base + tc_scratch(P).geo; }
+  __device__ __forceinline__ uint8_t* cs() const { return base + tc_scratch(P).cs; }
+  __device__ __forceinline__ float* jpe() const { return reinterpret_cast<float*>(base + tc_scratch(P).jpe); }
+  __device__ __forceinline__ float* jg() const { return reinterpret_cast<float*>(base + tc_scratch(P).jg); }
+  __device__ __forceinline__ float (*geom() const)[128] { return reinterpret_cast<float (*)[128]>(base + tc_scratch(P).geom); }
+  __device__ __forceinline__ long long* ray() const { return reinterpret_cast<long long*>(base + tc_scratch(P).ray); }
+};
+
+// The point geometry of every row of a tile into its slot, rows et, et + 96 of encoder thread et: the staging items and EB0 read
+// it from there instead of recomputing it (8 loads, and the contraction's divisions, per point and reader)
+template <int P>
+__device__ __forceinline__ void stage_geom(const TcArgs& a, int tile, int et, const Slot<P>& s) {
+  float (*gm)[128] = s.geom();
+#pragma unroll 1
+  for (int row = et; row < 128; row += kEncThreads) {
+    const PointGeom g = point_geom(a, tile, row);
+    gm[GEOM_PX][row] = g.px; gm[GEOM_PY][row] = g.py; gm[GEOM_PZ][row] = g.pz;
+    gm[GEOM_DX][row] = g.dx; gm[GEOM_DY][row] = g.dy; gm[GEOM_DZ][row] = g.dz;
+    s.ray()[row] = g.ray;
+  }
+}
+
 // Hash-grid part of the geo input of one tile, levels 4 grp .. 4 grp + 3 of one point (= operand chunk grp).  Outputs: bf16 planes
-// of the staged geo input image (`img`, planes `plane` bytes apart, kernel column order: four levels = one aligned 16-byte chunk)
-// and the grid jacobian Jg [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  The item's 32 corner rows are first requested
-// into L2 (no registers held), so that the level loop, one level at a time (smallest code, 8 gathers in flight), waits for L2 rather
-// than for HBM on its four dependent gather round trips.
+// of the staged geo input image (`img`, planes `plane` bytes apart, kernel column order: four levels = one aligned 16-byte chunk,
+// written once per plane) and the grid jacobian Jg [(col*3 + d)][row] (with the 1/4 of (x+2)/4 folded in).  The item's 32 corner
+// rows are first requested into L2 (no registers held), so that the level loop, one level at a time (smallest code, 8 gathers in
+// flight), waits for L2 rather than for HBM on its four dependent gather round trips.
 template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int row, int grp, uint8_t* img, uint32_t plane, float* Jg,
-                                                 uint64_t pol_table) {
-  const long long p_raw = (long long)tile * 128 + row;
-  const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
-  const PointGeom g = point_geom(a, p);
-  const float x01 = (g.px + 2.0f) * 0.25f, y01 = (g.py + 2.0f) * 0.25f, z01 = (g.pz + 2.0f) * 0.25f;   // sdf_field.py:384
+__device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int row, int grp, const Slot<P>& s, uint64_t pol_table) {
+  const float (*gm)[128] = s.geom();
+  float* Jg = s.jg();
+  const float x01 = (gm[GEOM_PX][row] + 2.0f) * 0.25f, y01 = (gm[GEOM_PY][row] + 2.0f) * 0.25f, z01 = (gm[GEOM_PZ][row] + 2.0f) * 0.25f;   // sdf_field.py:384
   const int l_end = min(4 * grp + 4, min(a.grid.n_levels, a.grid.active_levels));
   if (a.use_grid && a.mode != 0) {   // sdf-only calls (the samplers' passes) measured slower with it
 #pragma unroll 1
@@ -97,7 +135,8 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
       else level_prefetch_l2<float, 2>(a.table, c);
     }
   }
-  // feature columns as 2-byte operand stores
+  // the chunk's four (level) words per plane, shifted in level by level
+  uint32_t h0 = 0u, h1 = 0u, h2 = 0u, h3 = 0u, l0 = 0u, l1 = 0u, l2 = 0u, l3 = 0u;
 #pragma unroll 1
   for (int l = 4 * grp; l < 4 * grp + 4; ++l) {
     float o[2] = {0.f, 0.f};
@@ -110,8 +149,10 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
       else level_fetch<float, 2, true>(a.table, c, tv, pol_table);
       level_finish<2, LAYOUT>(a.grid, c, tv, o, dj);
     }
-    store_a<P>(img, plane, row, 2 * l, o[0]);
-    store_a<P>(img, plane, row, 2 * l + 1, o[1]);
+    uint32_t hi, lo;
+    split2(o[0], o[1], hi, lo);
+    h0 = h1; h1 = h2; h2 = h3; h3 = hi;
+    l0 = l1; l1 = l2; l2 = l3; l3 = lo;
     if (a.mode != 0 && l < a.grid.n_levels) {
 #pragma unroll
       for (int f = 0; f < 2; ++f) {
@@ -122,48 +163,52 @@ __device__ __forceinline__ void encode_tile_grid(const TcArgs& a, int tile, int 
       }
     }
   }
+  store_a_chunk<P>(s.geo(), kImgPlane, row, grp, make_uint4(h0, h1, h2, h3), make_uint4(l0, l1, l2, l3));
 }
 
 // PE | x | zero padding: chunks 4..11 of the geo input.  Kernel column 32 + i holds PE_i, 32 + pe_dim + j holds x_j.  Also the
 // point outputs (contracted position and its norm) of a valid row, and the PE jacobian Jpe [i][row].
 template <int P>
-__device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int row, uint8_t* img, uint32_t plane, float* Jpe) {
-  const long long p_raw = (long long)tile * 128 + row;
-  const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
-  const PointGeom g = point_geom(a, p);
-  if (p_raw < a.n_points) {
-    if (a.out.points_norm) a.out.points_norm[p] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(g.px, g.px), __fmul_rn(g.py, g.py)), __fmul_rn(g.pz, g.pz)));
-    if (a.out.points) { a.out.points[p * 3] = g.px; a.out.points[p * 3 + 1] = g.py; a.out.points[p * 3 + 2] = g.pz; }
+__device__ __forceinline__ void encode_tile_pe(const TcArgs& a, int tile, int row, const Slot<P>& s) {
+  const long long p = (long long)tile * 128 + row;
+  const float (*gm)[128] = s.geom();
+  const float px = gm[GEOM_PX][row], py = gm[GEOM_PY][row], pz = gm[GEOM_PZ][row];
+  if (p < a.n_points) {
+    if (a.out.points_norm) a.out.points_norm[p] = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
+    if (a.out.points) { a.out.points[p * 3] = px; a.out.points[p * 3 + 1] = py; a.out.points[p * 3 + 2] = pz; }
   }
   const int deg = a.pe_degree, half = 3 * deg;
-  const float pc[3] = {g.px, g.py, g.pz};
-  // zero the chunks first (padding columns), then the live columns as 2-byte stores (same thread: program order)
+  uint8_t* img = s.geo();
+  float* Jpe = s.jpe();
+  // zero the chunks first (padding columns), then the live columns as 2-byte stores (same thread: program order).  Building whole
+  // chunks in registers instead measured slower: every padding column then costs a pass of the column loop.
   const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll 1
-  for (int ch = 4; ch < kInK / 8; ++ch) store_a_chunk<P>(img, plane, row, ch, z4, z4);
+  for (int ch = 4; ch < kInK / 8; ++ch) store_a_chunk<P>(img, kImgPlane, row, ch, z4, z4);
 #pragma unroll 1
   for (int i = 0; i < a.pe_dim; ++i) {                       // sin(x 2^k) | sin(x 2^k + pi/2)   (encodings.py:194-198)
     const int ia = i >= half ? i - half : i;
     const int b = ia / deg, k = ia - b * deg;
     const float fr = (float)(1 << k);
-    const float xb = b == 0 ? pc[0] : (b == 1 ? pc[1] : pc[2]);
+    const float xb = b == 0 ? px : (b == 1 ? py : pz);
     const float arg = i >= half ? xb * fr + kHalfPiF : xb * fr;
     float sv, cv;
     sincos_call(arg, &sv, &cv);
-    store_a<P>(img, plane, row, 32 + i, a.use_pe ? sv : 0.f);
+    store_a<P>(img, kImgPlane, row, 32 + i, a.use_pe ? sv : 0.f);
     // autograd of sin on the forward's own fp32 arguments: d/dx_b = 2^k cos(arg)
     if (a.mode != 0) Jpe[i * 128 + row] = a.use_pe ? fr * cv : 0.f;
   }
-  store_a<P>(img, plane, row, 32 + a.pe_dim + 0, pc[0]);
-  store_a<P>(img, plane, row, 32 + a.pe_dim + 1, pc[1]);
-  store_a<P>(img, plane, row, 32 + a.pe_dim + 2, pc[2]);
+  store_a<P>(img, kImgPlane, row, 32 + a.pe_dim + 0, px);
+  store_a<P>(img, kImgPlane, row, 32 + a.pe_dim + 1, py);
+  store_a<P>(img, kImgPlane, row, 32 + a.pe_dim + 2, pz);
 }
 
-// direction-encoding value k (0..23) of direction d: sin(d_b 2^j) for k < 12, sin(d_b 2^j + pi/2) for k >= 12, b = (k mod 12) / 4,
-// j = k mod 4 (NeRFEncoding(4), encodings.py:167-208).  d_b 2^j is exact, so a contracted d_b 2^j + pi/2 rounds the same.
-__device__ __forceinline__ float dir_enc(const PointGeom& g, int k) {
+// direction-encoding value k (0..23) of direction (dx, dy, dz): sin(d_b 2^j) for k < 12, sin(d_b 2^j + pi/2) for k >= 12,
+// b = (k mod 12) / 4, j = k mod 4 (NeRFEncoding(4), encodings.py:167-208).  d_b 2^j is exact, so a contracted d_b 2^j + pi/2 rounds
+// the same.
+__device__ __forceinline__ float dir_enc(float dx, float dy, float dz, int k) {
   const int i = k < 12 ? k : k - 12, b = i >> 2;
-  const float db = b == 0 ? g.dx : (b == 1 ? g.dy : g.dz);
+  const float db = b == 0 ? dx : (b == 1 ? dy : dz);
   const float arg = db * (float)(1 << (i & 3));
   return sin_call(k < 12 ? arg : arg + kHalfPiF);
 }
@@ -173,37 +218,31 @@ __device__ __forceinline__ float dir_enc(const PointGeom& g, int k) {
 // (chunk 0 = [grad, n.v] comes from the epilogue).  Called by a whole warp for 32 consecutive rows (lane = row mod 32): when they are
 // all samples of one ray, lane k < 24 evaluates direction-encoding value k once for the warp (the same sinf of the same argument).
 template <int P>
-__device__ __forceinline__ void colour_static_tile(const TcArgs& a, int tile, int row, uint8_t* img, uint32_t plane) {
-  const long long p_raw = (long long)tile * 128 + row;
-  const long long p = p_raw < a.n_points ? p_raw : a.n_points - 1;
-  const PointGeom g = point_geom(a, p);
-  const bool one_ray = __match_any_sync(0xffffffffu, g.ray) == 0xffffffffu;
+__device__ __forceinline__ void colour_static_tile(const TcArgs& a, int row, const Slot<P>& s) {
+  const float (*gm)[128] = s.geom();
+  const float px = gm[GEOM_PX][row], py = gm[GEOM_PY][row], pz = gm[GEOM_PZ][row];
+  const float dx = gm[GEOM_DX][row], dy = gm[GEOM_DY][row], dz = gm[GEOM_DZ][row];
+  const long long ray = s.ray()[row];
+  const bool one_ray = __match_any_sync(0xffffffffu, ray) == 0xffffffffu;
   const int lane = row & 31;
-  const float own = one_ray && lane < 24 ? dir_enc(g, lane) : 0.f;
+  const float own = one_ray && lane < 24 ? dir_enc(dx, dy, dz, lane) : 0.f;
+  uint8_t* img = s.cs();
   const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll 1
-  for (int ch = 1; ch < kInK / 8; ++ch) store_a_chunk<P>(img, plane, row, ch, z4, z4);
-  store_a<P>(img, plane, row, 8 + 0, g.px); store_a<P>(img, plane, row, 8 + 1, g.py); store_a<P>(img, plane, row, 8 + 2, g.pz);
+  for (int ch = 1; ch < kInK / 8; ++ch) store_a_chunk<P>(img, kImgPlane, row, ch, z4, z4);
+  store_a<P>(img, kImgPlane, row, 8 + 0, px); store_a<P>(img, kImgPlane, row, 8 + 1, py); store_a<P>(img, kImgPlane, row, 8 + 2, pz);
   // direction encoding, then d itself (include_input)
 #pragma unroll 1
-  for (int k = 0; k < 24; ++k) store_a<P>(img, plane, row, 8 + 3 + k, one_ray ? __shfl_sync(0xffffffffu, own, k) : dir_enc(g, k));
-  store_a<P>(img, plane, row, 8 + 27, g.dx); store_a<P>(img, plane, row, 8 + 28, g.dy); store_a<P>(img, plane, row, 8 + 29, g.dz);
+  for (int k = 0; k < 24; ++k) {
+    const float shared = __shfl_sync(0xffffffffu, own, k);
+    store_a<P>(img, kImgPlane, row, 8 + 3 + k, one_ray ? shared : dir_enc(dx, dy, dz, k));
+  }
+  store_a<P>(img, kImgPlane, row, 8 + 27, dx); store_a<P>(img, kImgPlane, row, 8 + 28, dy); store_a<P>(img, kImgPlane, row, 8 + 29, dz);
   if (a.appearance != nullptr) {
 #pragma unroll 1
-    for (int j = 0; j < a.app_dim; ++j) store_a<P>(img, plane, row, 8 + 30 + j, __ldg(a.appearance + g.ray * a.app_dim + j));
+    for (int j = 0; j < a.app_dim; ++j) store_a<P>(img, kImgPlane, row, 8 + 30 + j, __ldg(a.appearance + ray * a.app_dim + j));
   }
 }
-
-// Staging slot s of the per-CTA scratch (tc_scratch)
-template <int P>
-struct Slot {
-  uint8_t* base;
-  __device__ __forceinline__ Slot(char* slots, uint32_t s) : base(reinterpret_cast<uint8_t*>(slots) + s * tc_scratch(P).slot_bytes) {}
-  __device__ __forceinline__ uint8_t* geo() const { return base + tc_scratch(P).geo; }
-  __device__ __forceinline__ uint8_t* cs() const { return base + tc_scratch(P).cs; }
-  __device__ __forceinline__ float* jpe() const { return reinterpret_cast<float*>(base + tc_scratch(P).jpe); }
-  __device__ __forceinline__ float* jg() const { return reinterpret_cast<float*>(base + tc_scratch(P).jg); }
-};
 
 #ifdef SDFB200_TC_TIMING
 // CTA 0, first 16 tiles, row = tile: clock64() of consumer thread 0 at [0] tile start, [1..7] end of the MMAs of layer 0..6 (ring
@@ -216,7 +255,8 @@ struct Slot {
 // warps 1, 2 busy staging the tile (warp 0: [12]), [26] [27] the same running the heads of the tile (warp 0: [14]), [28..30] encoder
 // thread 0's heads split: per-row heads (geometry, sdf -> alpha / sigma, per-sample outputs), transmittance scan and weights, sums and
 // the ray finish; [31] encoder thread 0 waiting at the encoder warps' barrier (kEncBar); [32 + 3 w + k] lane 0 of encoder warp w
-// staging items of kind k (0 grid, 1 PE, 2 colour-static)
+// staging items of kind k (0 grid, 1 PE, 2 colour-static); [41 + w] lane 0 of encoder warp w staging the tile's point geometry,
+// barrier included
 __device__ long long g_tc_timing[16 * 48];   // only the timing build of ONE instantiation defines SDFB200_TC_TIMING
 #define TC_PUT(tno, k, v)                                                                                            \
   do {                                                                                                               \
@@ -465,9 +505,12 @@ __device__ __forceinline__ float4 col_desc(const TcArgs& a, int ip) {
 template <int P>
 __device__ __forceinline__ void copy_chunks(uint8_t* abuf, int a_chunk, const uint8_t* src, uint32_t src_plane, int src_chunk, int n, int wrow0,
                                             uint64_t* bar, int lane) {
-  for (int k = lane; k < P * n; k += 32) {
-    const int pl = k / n, c = k - pl * n;
-    bulk_g2s(abuf + pl * kAPlane + (a_chunk + c) * kAChunk + wrow0 * 16, src + pl * src_plane + (src_chunk + c) * kAChunk + wrow0 * 16, 64 * 16, bar);
+  for (int k0 = 0; k0 < P * n; k0 += 32) {   // a warp-uniform trip count: the warp is converged again after the loop
+    const int k = k0 + lane;
+    if (k < P * n) {
+      const int pl = k / n, c = k - pl * n;
+      bulk_g2s(abuf + pl * kAPlane + (a_chunk + c) * kAChunk + wrow0 * 16, src + pl * src_plane + (src_chunk + c) * kAChunk + wrow0 * 16, 64 * 16, bar);
+    }
   }
 }
 template <int P>
@@ -488,7 +531,7 @@ __device__ __forceinline__ void colour_copy(const TileCtx& x, bool early, const 
 // A columns: [grad(3), n.v, 0 x4] (sdf_field.py:572-584; columns re-ordered at pack time) from the thread pair that owns the row.  The
 // other chunks ([x, dir-enc, dir, appearance], h2) arrive by colour_copy.
 template <int P>
-__device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P>& s, const float (&acc)[4][32]) {
+__device__ __forceinline__ void epi_eb0(const TileCtx& x, const Slot<P>& s, const float (&acc)[4][32]) {
   const TcArgs& a = x.a;
   const float* Jpe = s.jpe();
   const float* Jg = s.jg();
@@ -523,11 +566,11 @@ __device__ __forceinline__ void epi_eb0(const TileCtx& x, int tile, const Slot<P
   g1x = quad_sum(g1x); g1y = quad_sum(g1y); g1z = quad_sum(g1z);
   if ((x.t & 3) < 2) {
     const int h = x.t & 1, row = x.r0 + 8 * h;
-    const long long p_raw = (long long)tile * 128 + row;
-    const PointGeom pg = point_geom(a, p_raw < a.n_points ? p_raw : a.n_points - 1);
+    const float (*gm)[128] = s.geom();
     const float grx = h ? g1x : g0x, gry = h ? g1y : g0y, grz = h ? g1z : g0z;
     const float3 n = normalize_eps(grx, gry, grz);
-    const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? n.x * pg.dx + n.y * pg.dy + n.z * pg.dz : 0.f, 0.f, 0.f, 0.f, 0.f};
+    const float c0v[8] = {grx, gry, grz, a.use_n_dot_v ? n.x * gm[GEOM_DX][row] + n.y * gm[GEOM_DY][row] + n.z * gm[GEOM_DZ][row] : 0.f,
+                          0.f, 0.f, 0.f, 0.f};
     store_a_chunk<P>(x.abuf, kAPlane, row, 0, c0v);
     x.hs[HS_GRAD][row] = grx; x.hs[HS_GRAD + 1][row] = gry; x.hs[HS_GRAD + 2][row] = grz;
   }
@@ -598,11 +641,11 @@ struct RayEnd { int q; double tot; float last[3]; };
 // encoder thread 0's cycles in the three kinds of heads work (timing build)
 struct HeadsClock { long long rows, scan, sums; };
 
-// (starts + ends) / 2 of point p (renderers.py:247), with the bin edges of point_geom
-__device__ __forceinline__ float sample_mid(const TcArgs& a, long long p) {
+// (starts + ends) / 2 of point tile * 128 + row (renderers.py:247), with the bin edges of point_geom
+__device__ __forceinline__ float sample_mid(const TcArgs& a, int tile, int row) {
   if (!a.has_bins) return 0.f;
-  const long long ray = p / a.n_samples;
-  const float* b = a.bins + ray * (a.n_samples + 1) + (p - ray * a.n_samples);
+  long long ray;
+  const float* b = point_bin(a, tile, row, ray);
   return __fdiv_rn(__fadd_rn(__ldg(b), __ldg(b + 1)), 2.0f);
 }
 
@@ -615,7 +658,7 @@ __device__ __forceinline__ void heads_rows(const TcArgs& a, float (*hs)[128], do
   const long long p_raw = (long long)tile * 128 + row;
   const bool valid = p_raw < a.n_points;
   const long long p = valid ? p_raw : a.n_points - 1;
-  const PointGeom pg = point_geom(a, p);
+  const PointGeom pg = point_geom(a, tile, row);
   const float dirx = pg.dx, diry = pg.dy, dirz = pg.dz, delta = pg.delta;
   const float sdf = hs[HS_SDF][row], grx = hs[HS_GRAD][row], gry = hs[HS_GRAD + 1][row], grz = hs[HS_GRAD + 2][row];
   const float3 nv = normalize_eps(grx, gry, grz);
@@ -711,7 +754,7 @@ __device__ __forceinline__ void composite_chunk(const TcArgs& a, const float (*h
   { const long long c = TC_CLOCK(); clk.scan += c - tc0; tc0 = c; }
   const float rgbv[3] = {hs[HR_RGB][row], hs[HR_RGB + 1][row], hs[HR_RGB + 2][row]};
   float vs[8] = {w, w * rgbv[0], w * rgbv[1], w * rgbv[2], w * hs[HR_NORMAL][row], w * hs[HR_NORMAL + 1][row], w * hs[HR_NORMAL + 2][row],
-                 w * sample_mid(a, p)};
+                 w * sample_mid(a, tile, row)};
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
 #pragma unroll
@@ -755,9 +798,8 @@ __device__ __forceinline__ void finish_rays(const TcArgs& a, const float (*csum)
 }
 
 // An encoder warp's part of the heads of a tile: wait for the head inputs, run the warp's chunks, hand the buffer back
-__device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no, int et, TcBars& b, float (*hs)[128], double* hx, HeadsXfer& xf,
-                                         float& dmin, float& dmax) {
-  const int ew = et >> 5, lane = et & 31;
+__device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no, int ew, int lane, TcBars& b, float (*hs)[128], double* hx,
+                                         HeadsXfer& xf, float& dmin, float& dmax) {
   long long waited = 0, bar_waited = 0;
   b.hs.wait_full(tile_no, &waited);
   const long long t0 = TC_CLOCK();
@@ -781,22 +823,24 @@ __device__ __forceinline__ void heads_of(const TcArgs& a, int tile, int tile_no,
   }
   b.hs.arrive_empty(tile_no);
   if (lane == 0) TC_PUT(tile_no, ew == 0 ? 14 : 25 + ew, TC_CLOCK() - t0);
-  if (et == 0) { TC_PUT(tile_no, 17, waited); TC_PUT(tile_no, 28, clk.rows); TC_PUT(tile_no, 29, clk.scan); TC_PUT(tile_no, 30, clk.sums); TC_PUT(tile_no, 31, bar_waited); }
+  if (ew == 0 && lane == 0) { TC_PUT(tile_no, 17, waited); TC_PUT(tile_no, 28, clk.rows); TC_PUT(tile_no, 29, clk.scan); TC_PUT(tile_no, 30, clk.sums); TC_PUT(tile_no, 31, bar_waited); }
 }
 
-// Encoder warps (et = 0..95): walk the same tiles as the consumers and stage each one in its slot while the consumers run the tile
-// before it.  A tile is 768 items: 512 (point, group of four hash levels), then 128 x (PE | x, point outputs) and, with the colour
-// MLP, 128 x colour-static columns.  Encoder warp ew takes items enc_item_begin(ew) .. enc_item_begin(ew + 1) - 1, lane = item mod 32:
-// warp 0, which runs two of the four chunks of the heads, takes fewer (field_tc.h).  In sdf-only mode (640 items, no heads) item i
-// goes to thread i % 96.  Except in sdf-only mode, the encoder warps then run the heads of the tile before (the one the consumers are
+// Encoder warps (ew = 0..2, et = 32 ew + lane): walk the same tiles as the consumers and stage each one in its slot while the consumers
+// run the tile before it.  A tile's staging starts with its point geometry (stage_geom, then the encoder warps' barrier), then 768
+// items: 512 (point, group of four hash levels), then 128 x (PE | x, point outputs) and, with the colour MLP, 128 x colour-static
+// columns.  Encoder warp ew takes items enc_item_begin(ew) .. enc_item_begin(ew + 1) - 1, lane = item mod 32: warp 0, which runs two
+// of the four chunks of the heads, takes fewer (field_tc.h).  In sdf-only mode (640 items, no heads) item i goes to thread i % 96.
+// Either way a warp walks whole 32-item batches, 32-aligned, so the kind of item is the same across the warp and ptxas, given the
+// warp index as warp-uniform (k_field_tc), sees the shuffles of the colour-static items and of the heads as converged.  Except in sdf-only mode, the encoder warps then run the heads of the tile before (the one the consumers are
 // finishing), and those of the last tile after the loop.  Staging tile n + 1 and the heads of tile n - 1 both fit in the consumers'
 // tile n: slot n + 1 was freed at EB0 of tile n - 1, and the head inputs of tile n - 1 are ready when tile n starts.
 template <int P, int LAYOUT>
-__device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots, TcBars& b, uint64_t pol_table, float (*hs)[128], double* hx,
-                                           HeadsXfer& xf) {
+__device__ __forceinline__ void encode_all(const TcArgs& a, int ew, int lane, char* slots, TcBars& b, uint64_t pol_table, float (*hs)[128],
+                                           double* hx, HeadsXfer& xf) {
   const bool heads = a.mode != 0;
-  const int ew = et >> 5, lane = et & 31;
-  const int i_begin = heads ? enc_item_begin(ew) + lane : et, i_end = heads ? enc_item_begin(ew + 1) : 640, i_step = heads ? 32 : kEncThreads;
+  const int et = ew * 32 + lane;
+  const int i_begin = heads ? enc_item_begin(ew) : ew * 32, i_end = heads ? enc_item_begin(ew + 1) : 640, i_step = heads ? 32 : kEncThreads;
   float dmin = INFINITY, dmax = -INFINITY;       // the midpoints of this thread's rows, over every tile of the CTA
   int tile_no = 0;
   for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x, ++tile_no) {
@@ -804,23 +848,29 @@ __device__ __forceinline__ void encode_all(const TcArgs& a, int et, char* slots,
     b.enc.wait_empty(tile_no, &waited);
     const long long t0 = TC_CLOCK();
     const Slot<P> s(slots, b.enc.slot(tile_no));
-    long long kind_grid = 0, kind_pe = 0, kind_cs = 0;   // staging cycles by item kind (timing build)
+    long long kind_grid = 0, kind_pe = 0, kind_cs = 0, geom = 0;   // staging cycles by item kind (timing build)
+    stage_geom<P>(a, tile, et, s);
+    named_sync(kEncBar, kEncThreads);        // every row's geometry is in the slot
+    geom = TC_CLOCK() - t0;
 #pragma unroll 1
-    for (int i = i_begin; i < i_end; i += i_step) {
-      const int row = i & 127;
+    for (int ib = i_begin; ib < i_end; ib += i_step) {   // the warp's batch of items ib .. ib + 31
+      const int row = (ib & 127) + lane;
       const long long c0 = TC_CLOCK();
-      if (i < 512) { encode_tile_grid<P, LAYOUT>(a, tile, row, i >> 7, s.geo(), kImgPlane, s.jg(), pol_table); kind_grid += TC_CLOCK() - c0; }
-      else if (i < 640) { encode_tile_pe<P>(a, tile, row, s.geo(), kImgPlane, s.jpe()); kind_pe += TC_CLOCK() - c0; }
-      else { colour_static_tile<P>(a, tile, row, s.cs(), kImgPlane); kind_cs += TC_CLOCK() - c0; }
+      if (ib < 512) { encode_tile_grid<P, LAYOUT>(a, row, ib >> 7, s, pol_table); kind_grid += TC_CLOCK() - c0; }
+      else if (ib < 640) { encode_tile_pe<P>(a, tile, row, s); kind_pe += TC_CLOCK() - c0; }
+      else { colour_static_tile<P>(a, row, s); kind_cs += TC_CLOCK() - c0; }
     }
     fence_async_global();                    // the geo image is read by the producer's bulk copy (async proxy)
     b.enc.arrive_full(tile_no);
     if (et == 0) { TC_PUT(tile_no, 12, TC_CLOCK() - t0); TC_PUT(tile_no, 13, waited); }
     else if (lane == 0) TC_PUT(tile_no, 23 + ew, TC_CLOCK() - t0);
-    if (lane == 0) { TC_PUT(tile_no, 32 + 3 * ew, kind_grid); TC_PUT(tile_no, 33 + 3 * ew, kind_pe); TC_PUT(tile_no, 34 + 3 * ew, kind_cs); }
-    if (heads && tile_no > 0) heads_of(a, tile - (int)gridDim.x, tile_no - 1, et, b, hs, hx, xf, dmin, dmax);
+    if (lane == 0) {
+      TC_PUT(tile_no, 32 + 3 * ew, kind_grid); TC_PUT(tile_no, 33 + 3 * ew, kind_pe); TC_PUT(tile_no, 34 + 3 * ew, kind_cs);
+      TC_PUT(tile_no, 41 + ew, geom);
+    }
+    if (heads && tile_no > 0) heads_of(a, tile - (int)gridDim.x, tile_no - 1, ew, lane, b, hs, hx, xf, dmin, dmax);
   }
-  if (heads && tile_no > 0) heads_of(a, blockIdx.x + (tile_no - 1) * (int)gridDim.x, tile_no - 1, et, b, hs, hx, xf, dmin, dmax);   // the last tile
+  if (heads && tile_no > 0) heads_of(a, blockIdx.x + (tile_no - 1) * (int)gridDim.x, tile_no - 1, ew, lane, b, hs, hx, xf, dmin, dmax);   // the last tile
   // one depth-range update per warp and CTA: min and max are exact, so the result is that of any order of updates
   if (heads && a.render && a.rnd.out.steps_minmax) {
 #pragma unroll
@@ -846,7 +896,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   __shared__ TcBars bars;
   __shared__ HeadsXfer hxf;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // the warp index as the canonical warp-uniform value (a shuffle from lane 0): the role dispatch below branches on it, so that ptxas
+  // sees every role's shuffles as converged rather than wrapping each in a WARPSYNC.COLLECTIVE loop
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int nlayers = a.mode == 0 ? 2 : L_COUNT;
   char* cta_scr = a.scratch + (size_t)blockIdx.x * scr.bytes;
   char* slots = cta_scr + scr.slots;
@@ -870,10 +922,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
   __syncthreads();
 
   // ============ producer warpgroup: one thread streams the weights and the geo input, warps 9..11 encode the tile ahead ============
-  if (tid >= kEpiThreads) {
+  constexpr int kEncWarp0 = (kTcThreads - kEncThreads) / 32;
+  if (warp >= kEpiWarps) {
     setmaxnreg_dec<kProducerRegs>();
-    if (tid == kEpiThreads) produce_all<P>(a, nlayers, abuf, ring, slots, bars);
-    else if (tid >= kTcThreads - kEncThreads) encode_all<P, LAYOUT>(a, tid - (kTcThreads - kEncThreads), slots, bars, l2_policy_evict_last(), hs, hx, hxf);
+    if (warp == kEpiWarps) {
+      if (lane == 0) produce_all<P>(a, nlayers, abuf, ring, slots, bars);
+    } else if (warp >= kEncWarp0) {
+      encode_all<P, LAYOUT>(a, warp - kEncWarp0, lane, slots, bars, l2_policy_evict_last(), hs, hx, hxf);
+    }
     return;
   }
   setmaxnreg_inc<kConsumerRegs>();
@@ -936,14 +992,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) k_field_tc(const __grid_constan
     LAYER(L_B0, true);
     bars.enc.wait_full(tile_no);               // (long complete: the encoder's jacobian / colour-static stores are visible, and fenced
                                                // for the async proxy)
-    if (t < 32) colour_copy<P>(x, true, s.cs(), &bars.cop[wg][0]);
-    epi_eb0<P>(x, tile, s, acc);
+    if ((warp & 3) == 0) colour_copy<P>(x, true, s.cs(), &bars.cop[wg][0]);
+    epi_eb0<P>(x, s, acc);
     mbar_wait(&bars.cop[wg][0], tile_no & 1);  // the colour-static columns and early h2 chunks have landed
     bars.enc.arrive_empty(tile_no);            // the slot's last reader (the early copy) is complete
     TC_STAMP(21);
     SYNC_A();
     LAYER(L_C0MISC, true);
-    if (t < 32) colour_copy<P>(x, false, nullptr, &bars.cop[wg][1]);
+    if ((warp & 3) == 0) colour_copy<P>(x, false, nullptr, &bars.cop[wg][1]);
     TC_STAMP(22);
     LAYER(L_C0H, false);                       // accumulates onto the misc columns' result; waits for the late h2 copy inside
     epi_ec0<P>(x, acc);

@@ -64,7 +64,7 @@ assert lib.sdfb200_debug_tc_timing(buf) == 0
 # the tile's head inputs (hs_full); per encoder warp w0 / w1 / w2 (lane 0): busy staging [12] [24] [25] and running
 # the tile's heads [14] [26] [27]; encoder thread 0's heads split [28] per-row heads, [29] transmittance scan + weights, [30] sums and
 # ray finish, and [31] its wait at the encoder warps' barrier; [32 + 3 w + k] encoder warp w's staging split by item kind k (grid,
-# PE, colour-static).
+# PE, colour-static); [41 + w] encoder warp w's staging of the tile's point geometry (with the encoder warps' barrier after it).
 layers = ["G0", "G1", "B1", "B0", "C0 misc", "C0 h2", "C1"]
 epis = ["E0", "E1", "EB1", "EB0", "h2 operand", "EC0"]     # epis[L - 1] runs in front of layer L; "h2 operand": the late h2 copy is issued
 for t in (5, 10):
@@ -80,4 +80,5 @@ for t in (5, 10):
           + f"  busy {st[12] + st[14]}/{st[24] + st[26]}/{st[25] + st[27]}"
           + f"  |  w0 heads: rows {st[28]}  scan+weights {st[29]}  sums+finish {st[30]}  barrier wait {st[31]}"
           + "  |  staging by kind (grid/PE/colour-static): "
-          + "  ".join(f"w{w} {st[32 + 3 * w]}/{st[33 + 3 * w]}/{st[34 + 3 * w]}" for w in range(3)))
+          + "  ".join(f"w{w} {st[32 + 3 * w]}/{st[33 + 3 * w]}/{st[34 + 3 * w]}" for w in range(3))
+          + "  |  point geometry w0/w1/w2: " + "/".join(str(st[41 + w]) for w in range(3)))
