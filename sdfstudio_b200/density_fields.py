@@ -125,6 +125,10 @@ class HashMLPDensityField(nn.Module):
             raise NotImplementedError("use_linear=True (encoding + nn.Linear) is not used by any SDF preset")
         if hidden_dim not in (16, 32, 64):
             raise NotImplementedError("hidden_dim must be 16, 32 or 64")
+        if num_layers not in (2, 3, 4, 5):
+            raise NotImplementedError("num_layers must be 2, 3, 4 or 5")
+        if features_per_level not in (1, 2, 4, 8):
+            raise NotImplementedError("features_per_level must be 1, 2, 4 or 8")
         self.aabb = nn.Parameter(torch.as_tensor(aabb, dtype=torch.float32), requires_grad=False)
         self.spatial_distortion = spatial_distortion
         self.use_linear = use_linear

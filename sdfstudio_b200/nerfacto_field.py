@@ -95,7 +95,7 @@ class TCNNNerfactoField(nn.Module):
             raise NotImplementedError("hidden_dim and hidden_dim_color must be 16, 32 or 64")
         if num_layers not in (2, 3, 4) or num_layers_color not in (2, 3, 4):
             raise NotImplementedError("num_layers and num_layers_color must be 2, 3 or 4")
-        if not 0 <= geo_feat_dim <= 15 or SH_DIM + geo_feat_dim + appearance_embedding_dim > 64:
+        if not 0 <= geo_feat_dim <= 15 or appearance_embedding_dim < 0 or SH_DIM + geo_feat_dim + appearance_embedding_dim > 64:
             raise NotImplementedError("needs geo_feat_dim <= 15 and 16 + geo_feat_dim + appearance_embedding_dim <= 64")
         self.aabb = nn.Parameter(torch.as_tensor(aabb, dtype=torch.float32), requires_grad=False)
         self.geo_feat_dim = geo_feat_dim
@@ -161,13 +161,18 @@ class TCNNNerfactoField(nn.Module):
         d = sh4(directions.reshape(-1, 3) * 2.0 - 1.0)                      # tcnn maps its [0,1] input back with 2x - 1
         mode = self._appearance_mode()
         A = self.appearance_embedding_dim
-        if mode == "camera":
+        if mode == "camera" and A > 0:
             app = self.embedding_appearance(ray_samples.camera_indices.squeeze())
+        elif mode == "camera":
+            # no lookup into an empty embedding: the CUDA backward of nn.Embedding with embedding_dim = 0 takes the weight's row stride (1)
+            # as its feature count and reads and writes one element per index out of bounds
+            app = torch.zeros((*shape, 0), device=directions.device)
         elif mode == "mean":
             app = torch.ones((*shape, A), device=directions.device) * self.embedding_appearance.mean(dim=0)
         else:
             app = torch.zeros((*shape, A), device=directions.device)
-        h = torch.cat([d, density_embedding.reshape(-1, self.geo_feat_dim), app.reshape(-1, A)], dim=-1)
+        n = d.shape[0]   # explicit row counts: geo_feat_dim or A may be 0, and reshape(-1, 0) cannot infer the rows
+        h = torch.cat([d, density_embedding.reshape(n, self.geo_feat_dim), app.reshape(n, A)], dim=-1)
         rgb = torch.sigmoid(self.mlp_head(h)).view(*shape, -1)
         return {FieldHeadNames.RGB: rgb}
 

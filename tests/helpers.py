@@ -261,6 +261,44 @@ def scale(t):
     return float(t.abs().max())
 
 
+# the rounding of one hash-grid level lookup (csrc/grid.cuh, level_prepare / encode_level), restated in fp64 for the element-wise bounds
+# of the grid operator (test_gpu_grid_operator.py) and of the hash-MLP fields (test_gpu_hash_mlp.py)
+def kernel_positions(x32, scales, layout):
+    """[N, L, 3] fp32 positions exactly as level_prepare rounds them (CPU-checkable: torch's fp32 multiply, fma through fp64).  `scales`
+    [L] fp32 are the descriptor's level scales, `layout` "torch" or "tcnn"."""
+    s = scales.to(x32.device)
+    if layout == "torch":
+        return x32[:, None, :] * s[None, :, None]
+    return (x32.double()[:, None, :] * s.double()[None, :, None] + 0.5).float()
+
+
+def geometry(x32, scales, layout, smooth):
+    """per (point, level, axis) in fp64: w, the magnitude of dw/dx and of d2w/dx2 ((6 + 12t) s^2).
+
+    t = p - floor(p) is exact in fp32 except for p in (-1, 0) (points just below the grid), where floor(p) = -1 and the kernel rounds
+    t (by <= u t).  dw = 6t(1 - t) then inherits 6|1 - 2t| u t from it, which its magnitude includes there."""
+    p = kernel_positions(x32, scales, layout)
+    t32 = p - torch.floor(p)
+    t = p.double() - torch.floor(p).double()
+    rounded = (t32.double() != t).double()
+    s = scales.double().to(x32.device)[None, :, None]
+    if smooth:
+        return t * t * (3 - 2 * t), (6 * t * (1 - t) + 6 * (1 - 2 * t).abs() * t * rounded) * s, (6 + 12 * t) * s * s
+    return t, torch.ones_like(t) * s, torch.zeros_like(t)
+
+
+def corner_factors(w):
+    """[N, L, 8, 3]: |per-axis weight factor| of corner k"""
+    bits = torch.tensor([[(k >> d) & 1 for d in range(3)] for k in range(8)], device=w.device, dtype=torch.bool)
+    return torch.where(bits[None, None], w[:, :, None, :], 1 - w[:, :, None, :]).abs()
+
+
+def weight_mag(a):
+    """|W_k| + sum of the 2-factor sub-products: the weight and the absolute rounding of each factor"""
+    a0, a1, a2 = a.unbind(-1)
+    return a0 * a1 * a2 + a1 * a2 + a0 * a2 + a0 * a1
+
+
 def head_pairs(sb):
     """(product output key, oracle output key) of the per-sample heads of get_outputs, normals aside (see assert_heads_within_noise)"""
     H = sb.FieldHeadNames

@@ -418,6 +418,17 @@ def test_proposal_network_checkpoint_layout_loads():
         checkpoint.load_density_field_checkpoint(wrong, ckpt, index=0)
 
 
+@pytest.mark.parametrize("kw", [{"num_layers": 1}, {"num_layers": 6}, {"features_per_level": 3}, {"hidden_dim": 48}], ids=str)
+def test_proposal_network_refuses_what_its_kernel_cannot_run(kw):
+    """the density kernel runs 1..4 hidden layers (num_layers 2..5), 1, 2, 4 or 8 features per level and widths 16, 32, 64: anything else
+    is refused at construction instead of training and then failing on its first evaluation (num_layers = 1 would also split the
+    parameters with a negative hidden-layer count)"""
+    import sdfstudio_b200 as sb
+
+    with pytest.raises(NotImplementedError):
+        sb.HashMLPDensityField(torch.tensor([[-1.0, -1, -1], [1, 1, 1]]), num_levels=5, max_res=64, log2_hashmap_size=12, **kw)
+
+
 def test_foreign_tensordataclasses_pass_through_the_host_side():
     """Inside sdfstudio the modules receive the reference's own RayBundle / RaySamples (TensorDataclass objects, cameras/rays.py:233-339),
     not this package's classes.  Local stand-ins with the same fields and the same memory layout (a camera bundle [H, W, k]; starts / ends as

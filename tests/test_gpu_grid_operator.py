@@ -25,6 +25,8 @@ import torch
 
 from oracle import hashgrid
 
+from helpers import corner_factors, geometry, kernel_positions, weight_mag
+
 pytestmark = pytest.mark.gpu
 
 U = 2.0**-24
@@ -81,41 +83,6 @@ def oracle(enc, x64, t64):
     return hashgrid.encode_tcnn_layout(x64, t64, meta, F, smooth, return_indices=True, fp32_positions=True)
 
 
-def kernel_positions(enc, x32):
-    """[N, L, 3] fp32 positions exactly as level_prepare rounds them (CPU-checkable: torch's fp32 multiply, fma through fp64)."""
-    s = scales(enc).to(x32.device)
-    if enc.layout == "torch":
-        return x32[:, None, :] * s[None, :, None]
-    return (x32.double()[:, None, :] * s.double()[None, :, None] + 0.5).float()
-
-
-def geometry(enc, x32):
-    """per (point, level, axis) in fp64: w, the magnitude of dw/dx and of d2w/dx2 ((6 + 12t) s^2).
-
-    t = p - floor(p) is exact in fp32 except for p in (-1, 0) (points just below the grid), where floor(p) = -1 and the kernel rounds
-    t (by <= u t).  dw = 6t(1 - t) then inherits 6|1 - 2t| u t from it, which its magnitude includes there."""
-    p = kernel_positions(enc, x32)
-    t32 = p - torch.floor(p)
-    t = p.double() - torch.floor(p).double()
-    rounded = (t32.double() != t).double()
-    s = scales(enc).double().to(x32.device)[None, :, None]
-    if enc.interpolation == "Smoothstep":
-        return t * t * (3 - 2 * t), (6 * t * (1 - t) + 6 * (1 - 2 * t).abs() * t * rounded) * s, (6 + 12 * t) * s * s
-    return t, torch.ones_like(t) * s, torch.zeros_like(t)
-
-
-def corner_factors(w):
-    """[N, L, 8, 3]: |per-axis weight factor| of corner k"""
-    bits = torch.tensor([[(k >> d) & 1 for d in range(3)] for k in range(8)], device=w.device, dtype=torch.bool)
-    return torch.where(bits[None, None], w[:, :, None, :], 1 - w[:, :, None, :]).abs()
-
-
-def weight_mag(a):
-    """|W_k| + sum of the 2-factor sub-products: the weight and the absolute rounding of each factor"""
-    a0, a1, a2 = a.unbind(-1)
-    return a0 * a1 * a2 + a1 * a2 + a0 * a2 + a0 * a1
-
-
 def deriv_mag(a, dws):
     """[N, L, 8, 3]: magnitude of dW_k / dx_d (|dw_d s| times the other two factors, each with its absolute error)"""
     out = []
@@ -149,7 +116,7 @@ class Ref:
         self.x64 = x32.double().requires_grad_(True)
         self.tab = self.t64.clone().requires_grad_(True)
         self.out, self.rows = oracle(enc, self.x64, self.tab)
-        w, dws, d2m = geometry(enc, x32)
+        w, dws, d2m = geometry(x32, scales(enc), enc.layout, enc.interpolation == "Smoothstep")
         self.a = corner_factors(w)
         self.dws, self.d2m = dws, d2m
         self.vabs = self.t64.abs()[self.rows]                        # [N, L, 8, F]
@@ -207,7 +174,7 @@ def lattice_points(enc, gen):
                     raise AssertionError(f"no fp32 lattice point for level {l}")
             pts.append(p)
     x = torch.tensor(np.stack(pts))
-    q = kernel_positions(enc, x)
+    q = kernel_positions(x, scales(enc), enc.layout)
     lv = torch.arange(enc.n_levels).repeat_interleave(3)
     qi = q[torch.arange(len(x)), lv]
     n_on = (qi == torch.floor(qi)).sum(1)

@@ -76,7 +76,8 @@ def test_signature_state_dict_and_parameter_counts_match_reference():
 
 def test_unsupported_options_raise():
     for kw in ({"use_transient_embedding": True}, {"use_semantics": True}, {"use_pred_normals": True}, {"hidden_dim": 128}, {"hidden_dim_color": 8},
-               {"num_layers": 5}, {"num_layers_color": 1}, {"geo_feat_dim": 16}, {"appearance_embedding_dim": 40}):
+               {"num_layers": 5}, {"num_layers_color": 1}, {"geo_feat_dim": 16}, {"geo_feat_dim": -1}, {"appearance_embedding_dim": 40},
+               {"appearance_embedding_dim": -1}):
         with pytest.raises(NotImplementedError):
             _default_field(**kw)
 
