@@ -537,6 +537,63 @@ int sdfb200_knn(const float* points, const int32_t* order, int64_t n_points, con
  * Refused with SDFB200_EINVAL: k outside [1, 32], N outside [0, 2^31), a NULL pointer (N > 0). */
 int sdfb200_point_normals(const float* points, int64_t n_points, const int32_t* indices, int32_t k, float* normals, void* stream);
 
+/* Poisson surface reconstruction (the mesh of open3d's TriangleMesh.create_from_point_cloud_poisson, which the reference's
+ * ns-export poisson calls), as a screened Poisson problem on a dense grid.  The discretisation:
+ *   cube   c = the centre of the box of the points that take part, W = scale * (largest box extent), scale = 1.1; n = 2^depth cells per
+ *          side, h = W / n, origin o = c - W / 2, (n+1)^3 nodes at o + h (i, j, k), depth in [1, 10].  Node (i, j, k) has linear index
+ *          (i (n+1) + j) (n+1) + k and cell (x, y, z) key (x n + y) n + z (z fastest, the layout of sdfb200_marching_cubes).
+ *   point  t = (p - o) / h in double, cell = clamp(floor(t), 0, n-1), u = t - cell; corner l = (lx, ly, lz) = 4 lx + 2 ly + lz of the
+ *          cell has hat phi_l = prod (l_a ? u_a : 1 - u_a).  Points with a zero or non-finite normal take no part in anything; normals
+ *          are normalised before use.
+ *   system (L + alpha a S) x = a b, chi = sum x_i phi_i (Q1 hats):
+ *          L   the Q1 stiffness matrix with natural boundaries: element entries h/3 (same node), 0 (differ in one axis), -h/12 (two or
+ *              three); interior stencil 8h/3 centre, 0 face, -h/6 edge, -h/12 corner neighbours; zero row sums.
+ *          b_i = sum_p n_p . grad(phi_i)(p)          S_ij = sum_p phi_i(p) phi_j(p)
+ *          alpha = SDFB200_POISSON_POINT_WEIGHT,  a = h^2 (cells holding a point) / N, N the points that take part.
+ *   iso    the mean over the points of chi(p), summed in double in a fixed order.
+ *   density / colour: the hats' sums sum_p phi_i(p) and sum_p phi_i(p) rgb_p on the grid of depth max(depth - 2, 0), interpolated at the
+ *          mesh vertices; colour = colour sum / density, 0 where the density is 0.
+ * S enters as per-cell 8x8 blocks M_c = sum_{p in c} phi phi^T (row = corner).  Every sum runs over the points of one cell in the
+ * caller's bucket order (a stable sort by cell key), then over a node's <= 8 adjacent cells in the order x, then y, then z offset, low
+ * first; accumulation is in double, results are stored as fp32.  No floating-point atomics anywhere: reruns are bit-identical.
+ *
+ * sdfb200_poisson_cells: for the n_cells occupied cells of the grid 2^level (keys cell_key [n_cells] int64, points of cell s at
+ * cell_start[s] .. cell_start[s+1]-1 of points [*,3] fp32), with normals [*,3]: mat [n_cells,8,8] = M_c and rhs [n_cells,8] = the cell's
+ * part of b; with colors [*,3] instead: splat [n_cells,8,4] = per corner (sum phi, sum phi r, sum phi g, sum phi b).  origin (double[3])
+ * and h are the level's, on the host.
+ * sdfb200_poisson_coarsen: mat of the occupied cells of level `level` (cell_key) from the blocks of level + 1 (fine_slot [(2n)^3] int32,
+ * -1 for an empty cell, fine_mat): M_C = sum over the 8 children (x, y, z offset order) of Q^T M_c Q, Q the coarse hats on the child.
+ * This is S evaluated with the coarse hats; the coarse L is the stiffness at the coarse h.
+ * sdfb200_poisson_gather: node_vals [(n+1)^3, channels] fp32 = per node the sum over its adjacent occupied cells (cell_slot [n^3]) of
+ * cell_vals[slot * cell_stride + corner * corner_stride + ch], corner the node's corner of that cell.
+ * sdfb200_poisson_sample: out [n_points, channels] double = the trilinear interpolation of node_vals at the points.
+ * sdfb200_poisson_apply: y = (L + alpha_a S) x at level `level` with cell size h.
+ * sdfb200_poisson_solve: x = the solution of (L + alpha_a S) x = rhs at `depth` (rhs = a b, caller-owned; x written).  cell_slot[l] and
+ * mat[l], l = 1 .. depth (host arrays of device pointers, index l), are each level's slots and blocks.  Conjugate gradients
+ * preconditioned by one V-cycle per iteration: two l1-Jacobi sweeps x += 1.4 (f - A x) / (l1 row sum of A) before and after, the Q1
+ * transfer operators, a dense Cholesky solve on the 3^3 nodes of level 1.  Stops when ||rhs - A x||_2 <= tol ||rhs||_2 (the true
+ * residual, recomputed whenever the recurrence says so) or after max_cycles; *cycles and *rel_residual (host) report the iterations and
+ * the final true relative residual.  Synchronises `stream` once per reduction.  workspace: sdfb200_poisson_workspace_bytes(depth) bytes.
+ * sdfb200_poisson_sum: *out (device) = the sum of values [n] double over a fixed partition (partial: 1024 doubles of scratch).
+ * All refuse bad arguments with SDFB200_EINVAL before any launch. */
+#define SDFB200_POISSON_POINT_WEIGHT 4.0
+int sdfb200_poisson_cells(const float* points, const float* normals, const float* colors, int64_t n_cells, const int64_t* cell_key,
+                          const int64_t* cell_start, int32_t level, const double* origin, double h, float* mat, float* rhs, float* splat,
+                          void* stream);
+int sdfb200_poisson_coarsen(int32_t level, const int32_t* fine_slot, const float* fine_mat, int64_t n_cells, const int64_t* cell_key,
+                            float* mat, void* stream);
+int sdfb200_poisson_gather(int32_t level, const int32_t* cell_slot, const float* cell_vals, int32_t cell_stride, int32_t corner_stride,
+                           int32_t channels, float* node_vals, void* stream);
+int sdfb200_poisson_sample(const float* points, int64_t n_points, int32_t level, const double* origin, double h, const float* node_vals,
+                           int32_t channels, double* out, void* stream);
+int sdfb200_poisson_apply(int32_t level, double h, const int32_t* cell_slot, const float* mat, double alpha_a, const float* x, float* y,
+                          void* stream);
+size_t sdfb200_poisson_workspace_bytes(int32_t depth);
+int sdfb200_poisson_solve(int32_t depth, double h, const int32_t* const* cell_slot, const float* const* mat, double alpha_a,
+                          const float* rhs, float* x, int32_t max_cycles, double tol, void* workspace, size_t workspace_bytes,
+                          int32_t* cycles, double* rel_residual, void* stream);
+int sdfb200_poisson_sum(const double* values, int64_t n, double* partial, double* out, void* stream);
+
 /* Training path: backward of sdfb200_render (expected depth) / sdfb200_render_alphas' compositing w.r.t. the per-sample
  * inputs (autograd over renderers.py:42-295 in the reference).  `accumulation`, `depth` = forward outputs (depth BEFORE the
  * global clip).  g_rgb [R,3], g_depth [R], g_normal [R,3], g_accumulation [R], g_weights_in [R,S]: incoming gradients, each

@@ -123,6 +123,15 @@ _PROTOS = {
     "sdfb200_tsdf_integrate": (C.c_int, [_vp, _i64, _vp, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "sdfb200_knn": (C.c_int, [_vp, _vp, _i64, _vp, C.POINTER(C.c_float), _i32, _i32, _vp, _vp, _vp]),
     "sdfb200_point_normals": (C.c_int, [_vp, _i64, _vp, _i32, _vp, _vp]),
+    "sdfb200_poisson_cells": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _i32, C.POINTER(C.c_double), C.c_double, _vp, _vp, _vp, _vp]),
+    "sdfb200_poisson_coarsen": (C.c_int, [_i32, _vp, _vp, _i64, _vp, _vp, _vp]),
+    "sdfb200_poisson_gather": (C.c_int, [_i32, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "sdfb200_poisson_sample": (C.c_int, [_vp, _i64, _i32, C.POINTER(C.c_double), C.c_double, _vp, _i32, _vp, _vp]),
+    "sdfb200_poisson_apply": (C.c_int, [_i32, C.c_double, _vp, _vp, C.c_double, _vp, _vp, _vp]),
+    "sdfb200_poisson_workspace_bytes": (_sz, [_i32]),
+    "sdfb200_poisson_solve": (C.c_int, [_i32, C.c_double, C.POINTER(_vp), C.POINTER(_vp), C.c_double, _vp, _vp, _i32, C.c_double, _vp, _sz,
+                                        C.POINTER(C.c_int32), C.POINTER(C.c_double), _vp]),
+    "sdfb200_poisson_sum": (C.c_int, [_vp, _i64, _vp, _vp, _vp]),
     "sdfb200_field_packed_bytes": (_sz, [C.POINTER(FieldDesc)]),
     "sdfb200_field_pack": (C.c_int, [C.POINTER(FieldDesc), C.POINTER(FieldParams), _vp, _vp]),
     "sdfb200_field_workspace_bytes": (_sz, [C.POINTER(FieldDesc), _i64]),
