@@ -537,6 +537,51 @@ int sdfb200_knn(const float* points, const int32_t* order, int64_t n_points, con
  * Refused with SDFB200_EINVAL: k outside [1, 32], N outside [0, 2^31), a NULL pointer (N > 0). */
 int sdfb200_point_normals(const float* points, int64_t n_points, const int32_t* indices, int32_t k, float* normals, void* stream);
 
+/* Mesh rendering (scripts/render_mesh.py of the reference, which draws with open3d's OpenGL visualizer): a triangle rasterizer and a
+ * shader for B frames of one mesh.
+ *   vertices [V,3] fp32, faces [F,3] int64 (indices in [0, V); the caller checks them), cams [B,18] fp32 = rows 0-2 of inverse(c2w)
+ *   (12 floats, row-major; c2w in nerfstudio's OpenGL axes: x right, y up, looking along -z), then rows 0-1 of K (6 floats: fx at 0,
+ *   cx at 2, fy at 4, cy at 5; the skew and K's third row are not read).  keys [B,H,W] uint64.
+ * Per (frame, face), in double from the fp32 inputs, every operation rounded on its own (__dmul_rn, __dadd_rn, __dsub_rn, __ddiv_rn):
+ *   v_k = ((m0 x + m1 y) + m2 z) + m3 for rows 0, 1, 2 of inverse(c2w)     (camera space of vertex k = 0, 1, 2)
+ *   a x b = (a_y b_z - a_z b_y, a_z b_x - a_x b_z, a_x b_y - a_y b_x);  a . b = (a_x b_x + a_y b_y) + a_z b_z
+ *   E_0 = v_1 x v_2, E_1 = v_2 x v_0, E_2 = v_0 x v_1;  det = v_0 . E_0
+ *   the face is front-facing (counter-clockwise as seen from the camera) and non-degenerate iff det < 0; only then may it cover a
+ *   pixel.  Then e_k = -E_k and num = -det (exact negations).
+ * Per pixel (i, j), the ray through its centre, d = ((i + 0.5 - cx) / fx, -((j + 0.5 - cy) / fy), -1):
+ *   w_k = (d_x e_k.x + d_y e_k.y) - e_k.z;  S = (w_0 + w_1) + w_2;  depth = num / S   (the view depth, -z, of the hit on the plane)
+ *   the face covers the pixel iff w_0 >= 0, w_1 >= 0, w_2 >= 0, S > 0 and depth >= z_near  (edges and vertices included; NaN never
+ *   covers).  key = (bits of (float)depth << 32) | face; depth > 0, so the keys order like the depths.
+ * The homogeneous test needs no clipping: a face across the camera plane covers exactly the pixels whose rays meet it in front of the
+ * camera, and one wholly behind it covers none.  Adjacent faces share their edge's E with opposite signs, exactly, so a closed mesh
+ * leaves no holes.  keys is set to all ones (background) and every covering pair does atomicMin: the result does not depend on the
+ * schedule, the binning, the order of faces of equal depth or how frames are batched, and ties go to the smaller face id.
+ * Per (frame, face), a pixel box bounds the work: faces whose largest vertex depth is below z_near / 2 are skipped, and the others
+ * walk the box of the projected corners of the face clipped at view depth z_near / 2 (every hit that may cover lies in that part),
+ * widened by one pixel (a margin that dwarfs the rounding of the test and of the clipping).  One thread walks a box of at most SDFB200_MESH_LARGE_TRIANGLE_PIXELS pixels; a larger box is queued in
+ * shared memory and walked by the whole block, one pixel per thread.
+ * Refused with SDFB200_EINVAL before any launch: n_frames < 0, height or width outside [1, SDFB200_MESH_MAX_SIDE], F outside
+ * [0, 2^31 - 1), z_near not finite and > 0, a NULL or misaligned pointer (vertices and cams 4 bytes, faces and keys 8) when
+ * n_frames > 0 (vertices and faces may be NULL when F = 0). */
+#define SDFB200_MESH_LARGE_TRIANGLE_PIXELS 256
+#define SDFB200_MESH_MAX_SIDE 32768
+int sdfb200_mesh_rasterize(const float* vertices, const int64_t* faces, int64_t n_faces, const float* cams, int32_t n_frames, int32_t height,
+                           int32_t width, float z_near, uint64_t* keys, void* stream);
+/* Shading of the keys of sdfb200_mesh_rasterize (same vertices, faces and cams) into rgb and / or normal [B,H,W,3] uint8 (either may
+ * be NULL, not both).  vertex_normals [V,3] fp32 (world space).  light_positions [B,4,3] fp32 (DEVICE): each frame's four lights in
+ * its camera space.  light_params [27] fp32 (HOST): per light k = 0..3 colour r, g, b, diffuse, specular, shininess, then the ambient
+ * colour r, g, b.  Background pixels are white (255).  Per covered pixel, in double: the face's v_k, e_k, w_k, S and depth exactly as
+ * the rasterizer computes them, barycentrics b_k = w_k / S, hit p = depth d, and the vertex normals in camera space n_k = R n (R the
+ * rotation rows of inverse(c2w)).
+ *   normal: n = normalize((b_0 n_0 + b_1 n_1) + b_2 n_2), colour n / 2 + 1/2
+ *   rgb:    each n_k with n_k . (-v_k) < 0 is negated first; n as above, e = normalize(-p); per light, l = normalize(L_k - p),
+ *           r = 2 (n . l) n - l, colour = ambient + sum_k colour_k (diffuse_k max(0, n . l) + specular_k max(0, e . r)^shininess_k)
+ *   byte = floor(clamp(colour, 0, 1) 255 + 0.5).
+ * Refused as sdfb200_mesh_rasterize, and when both outputs are NULL. */
+int sdfb200_mesh_shade(const uint64_t* keys, int32_t n_frames, int32_t height, int32_t width, const float* vertices, const float* vertex_normals,
+                       const int64_t* faces, int64_t n_faces, const float* cams, const float* light_positions, const float* light_params,
+                       uint8_t* rgb, uint8_t* normal, void* stream);
+
 /* Poisson surface reconstruction (the mesh of open3d's TriangleMesh.create_from_point_cloud_poisson, which the reference's
  * ns-export poisson calls), as a screened Poisson problem on a dense grid.  The discretisation:
  *   cube   c = the centre of the box of the points that take part, W = scale * (largest box extent), scale = 1.1; n = 2^depth cells per

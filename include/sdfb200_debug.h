@@ -31,6 +31,12 @@ int sdfb200_debug_tc_linear(int32_t planes, int32_t epi, const float* X, int32_t
  * -DSDFB200_TC_TIMING (sdfstudio_b200/build.py); the product library records none. */
 int sdfb200_debug_tc_timing(long long* host_out_768);
 
+/* debug: sdfb200_mesh_rasterize with the box size above which a (frame, face) is walked by the whole block as an argument instead of
+ * SDFB200_MESH_LARGE_TRIANGLE_PIXELS (0: every face on the block path; INT64_MAX: every face on its own thread).  The keys do not depend
+ * on it. */
+int sdfb200_debug_mesh_rasterize(const float* vertices, const int64_t* faces, int64_t n_faces, const float* cams, int32_t n_frames,
+                                 int32_t height, int32_t width, float z_near, uint64_t* keys, int64_t large_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,12 +13,14 @@ Host side mirrors the reference's plug points (SURVEY.md section 8b):
   tsdf.*                       <- nerfstudio.exporter.tsdf_utils (TSDF fusion and the ns-export tsdf mesh)
   pointcloud.*                 <- nerfstudio.exporter.exporter_utils.generate_point_cloud (the ns-export pointcloud cloud)
   poisson.*                    <- open3d's create_from_point_cloud_poisson as ns-export poisson calls it (the Poisson mesh)
+  render_mesh.*                <- scripts/render_mesh.py (ns-render-mesh) and nerfstudio.cameras.camera_paths
 All arithmetic runs in libsdfb200.so (CUDA, sm_90a) behind the C ABI of include/sdfb200.h.  No CPU / PyTorch fallback.
 """
 from . import _lib  # noqa: F401
-from . import cameras, losses, meshing, packed, pointcloud, poisson, tsdf  # noqa: F401
+from . import cameras, losses, meshing, packed, pointcloud, poisson, render_mesh, tsdf  # noqa: F401
 from .pointcloud import PointCloud, estimate_normals, generate_point_cloud, point_cloud, remove_statistical_outlier  # noqa: F401
 from .poisson import create_from_point_cloud_poisson, poisson_mesh, remove_vertices_by_mask  # noqa: F401
+from .render_mesh import render_frames, render_trajectory_video  # noqa: F401  (render_mesh.render_mesh: the module keeps the name)
 from .density_fields import HashMLPDensityField  # noqa: F401
 from .encoding import Encoding, HashEncoding  # noqa: F401
 from .field_heads import FieldHeadNames  # noqa: F401

@@ -123,6 +123,8 @@ _PROTOS = {
     "sdfb200_tsdf_integrate": (C.c_int, [_vp, _i64, _vp, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "sdfb200_knn": (C.c_int, [_vp, _vp, _i64, _vp, C.POINTER(C.c_float), _i32, _i32, _vp, _vp, _vp]),
     "sdfb200_point_normals": (C.c_int, [_vp, _i64, _vp, _i32, _vp, _vp]),
+    "sdfb200_mesh_rasterize": (C.c_int, [_vp, _vp, _i64, _vp, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "sdfb200_mesh_shade": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i64, _vp, _vp, C.POINTER(C.c_float), _vp, _vp, _vp]),
     "sdfb200_poisson_cells": (C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, _i32, C.POINTER(C.c_double), C.c_double, _vp, _vp, _vp, _vp]),
     "sdfb200_poisson_coarsen": (C.c_int, [_i32, _vp, _vp, _i64, _vp, _vp, _vp]),
     "sdfb200_poisson_gather": (C.c_int, [_i32, _vp, _vp, _i32, _i32, _i32, _vp, _vp]),
@@ -176,6 +178,7 @@ EXPORTED_SYMBOLS = tuple(_PROTOS)
 _DEBUG_PROTOS = {
     "sdfb200_debug_tc_linear": (C.c_int, [_i32, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _i32, _i32, _vp, _vp]),
     "sdfb200_debug_tc_gemm": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "sdfb200_debug_mesh_rasterize": (C.c_int, [_vp, _vp, _i64, _vp, _i32, _i32, _i32, _f32, _vp, _i64, _vp]),
 }
 _dbg = None
 

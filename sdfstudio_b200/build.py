@@ -7,8 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsdfb200.so")
 LIB_DEBUG = os.path.join(HERE, "libsdfb200_dbg.so")   # product objects + the building-block validation hooks (tests only)
-SOURCES = ["api.cu", "grid_encode.cu", "field_simt.cu", "field_tc.cu", "field_tc_p2_torch.cu", "field_tc_p2_tcnn.cu", "field_tc_p1_torch.cu", "field_tc_p1_tcnn.cu", "tc_linear.cu", "tc_wgrad.cu", "samplers.cu", "render.cu", "render_backward.cu", "hash_mlp_field.cu", "hash_mlp_field_f16.cu", "nerf_field_tc.cu", "rays_gen.cu", "occupancy.cu", "marching_cubes.cu", "texture.cu", "tsdf.cu", "pointcloud.cu", "poisson.cu", "losses.cu"]
-DEBUG_SOURCES = ["tc_test.cu"]
+SOURCES = ["api.cu", "grid_encode.cu", "field_simt.cu", "field_tc.cu", "field_tc_p2_torch.cu", "field_tc_p2_tcnn.cu", "field_tc_p1_torch.cu", "field_tc_p1_tcnn.cu", "tc_linear.cu", "tc_wgrad.cu", "samplers.cu", "render.cu", "render_backward.cu", "hash_mlp_field.cu", "hash_mlp_field_f16.cu", "nerf_field_tc.cu", "rays_gen.cu", "occupancy.cu", "marching_cubes.cu", "texture.cu", "tsdf.cu", "pointcloud.cu", "poisson.cu", "mesh_render.cu", "losses.cu"]
+DEBUG_SOURCES = ["tc_test.cu", "mesh_render_debug.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
          "-Xptxas", "-v"]

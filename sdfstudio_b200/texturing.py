@@ -186,9 +186,14 @@ def obj_text(vertices: np.ndarray, faces: np.ndarray, vertex_normals: np.ndarray
 
 def png_bytes(image: np.ndarray) -> bytes:
     """8-bit RGB PNG of an [H,W,3] float image in [0,1]: floor(clip(x, 0, 1) * 255 + 0.5), unfiltered rows, one zlib stream."""
-    img = np.floor(np.clip(np.asarray(image, dtype=np.float32), 0.0, 1.0) * 255.0 + 0.5).astype(np.uint8)
-    if img.ndim != 3 or img.shape[2] != 3:
-        raise ValueError(f"expected an [H, W, 3] image, got {img.shape}")
+    return png_bytes_u8(np.floor(np.clip(np.asarray(image, dtype=np.float32), 0.0, 1.0) * 255.0 + 0.5).astype(np.uint8))
+
+
+def png_bytes_u8(img: np.ndarray) -> bytes:
+    """8-bit RGB PNG of an [H,W,3] uint8 image: unfiltered rows, one zlib stream (zlib releases the GIL, so threads encode in parallel)."""
+    img = np.ascontiguousarray(img)
+    if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+        raise ValueError(f"expected an [H, W, 3] uint8 image, got {img.dtype} {img.shape}")
     h, w = img.shape[:2]
     raw = np.concatenate([np.zeros((h, 1), np.uint8), img.reshape(h, w * 3)], axis=1).tobytes()
 
